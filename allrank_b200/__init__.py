@@ -1,4 +1,4 @@
-"""allrank_b200 -- B200-native (sm_100a) scoring + listwise-loss + metric path behind allRank's call surfaces.
+"""allrank_b200 -- H100-native (sm_90a) scoring + listwise-loss + metric path behind allRank's call surfaces.
 
     from allrank_b200 import losses, metrics          # same names/signatures as allrank.models.{losses,metrics}
     from allrank_b200.model import make_model         # same surface as allrank.models.model.make_model

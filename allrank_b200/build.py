@@ -1,9 +1,9 @@
-"""In-tree build of the C-ABI CUDA library (sm_100a only).  (The oracle is pure Python / PyTorch: nothing to compile.)
+"""In-tree build of the C-ABI CUDA library (sm_90a only).  (The oracle is pure Python / PyTorch: nothing to compile.)
 
     python -m allrank_b200.build            # or __graft_entry__.build()
 
-nvcc cross-compiles without a GPU.  The resulting liballrank_b200.so stays in-tree (git-ignored) so it
-travels to the GPU box with the gpurun snapshot.
+nvcc cross-compiles without a GPU.  The resulting liballrank_b200.so stays in-tree (git-ignored), so the package is
+importable from the repository tree.
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, "liballrank_b200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 

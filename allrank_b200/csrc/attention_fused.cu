@@ -1,20 +1,18 @@
 // Fused self-attention core for slates of up to 256 items:  ctx = softmax(mask(Q K^T / sqrt(dk))) V
-// in ONE kernel, the [S,S] score / probability tile living only in tensor memory.
+// in ONE kernel, the [S,S] score / probability tile living only in registers.
 //
 // Reference: attention() allrank/models/transformer.py:137-156 (+ the head split / concat of
 // MultiHeadedAttention.forward :193-202, which here are just TMA coordinates).
 //
-// One CTA = one (slate b, head, 128-query tile).  Q (128 x dk), K and V (S x dk) are staged by TMA straight
-// out of the packed [B*S, 3*d_model] QKV activation (4-D tensor maps: dk, item, head, slate).
-//   warp 0    : TMA producer
-//   warp 1    : TMEM allocation + tcgen05.mma issue
-//                 S[128 x S]  = Q K^T          (kind::tf32, A/B from shared memory, accumulator in TMEM cols 0..S)
-//                 O[128 x dk] = P V            (A = P read back from TMEM, B = V as an MN-major smem operand)
-//   warps 2-5 : one thread per query row (= one TMEM lane): key mask, row max, exp2, row sum, P written back to
-//               TMEM in place (rounded to tf32), then the O epilogue (1/rowsum) and a TMA store into the
-//               concatenated-heads layout.
-// Nothing of size S^2 touches HBM: per (slate, head) the kernel reads 3*S*dk*4 bytes and writes S*dk*4 (+ 8*S
-// of softmax statistics for the backward pass) -- versus ~5*S^2*4 bytes for the unfused sequence.
+// One CTA = one (slate b, head, 128-query tile).  Q (128 x dk), K and V (up to 256 x dk, in 128-key boxes) are staged
+// by TMA straight out of the packed [B*S, 3*d_model] QKV activation (4-D tensor maps: dk, item, head, slate).
+// Eight warps, each owning 16 query rows, run the whole attention on the tensor cores (mma.sync m16n8k8 tf32):
+//   pass A  S = Q K^T, one 8-key block at a time, keeping only the masked row maximum;
+//   pass B  the same blocks again: P = exp2((S - max) / sqrt(dk) * log2 e) (key mask, dropout), rounded to tf32 and
+//           fed straight from the accumulator registers into O += P V.
+// The O epilogue (1/rowsum) is staged in swizzled shared memory and TMA-stored into the concatenated-heads layout.
+// Nothing of size S^2 touches HBM or shared memory: per (slate, head) the kernel reads 3*S*dk*4 bytes and writes
+// S*dk*4 (+ 8*S of softmax statistics for the backward pass) -- versus ~5*S^2*4 bytes for the unfused sequence.
 #include <cstdint>
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -22,255 +20,57 @@
 
 #include "attention_fused.h"
 #include "common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace arb {
 
-constexpr int ATT_THREADS = 192;
-constexpr int ATT2_SOFTMAX = 256;              // two-pass kernel: 8 softmax warps, two per TMEM lane quadrant
-constexpr int ATT2_THREADS = 64 + ATT2_SOFTMAX;
+constexpr int ATT_THREADS = 256;               // 8 warps x 16 query rows
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t round_tf32(float x) {
+__device__ __forceinline__ float round_tf32(float x) {
   // round-to-nearest (ties away) to tf32 as "+ half an ulp of the 10-bit mantissa, then let the tensor core ignore the
-  // low 13 bits" -- one integer add instead of cvt.rna.tf32.f32, which ptxas expands to three instructions here.
-  // Same result as cvt.rna for every finite value (probabilities and their gradients are finite).
-  return __float_as_uint(x) + 0x1000u;
+  // low 13 bits" -- one integer add instead of cvt.rna.tf32.f32.  Same result as cvt.rna for every finite value
+  // (probabilities are finite).
+  return __uint_as_float(__float_as_uint(x) + 0x1000u);
 }
 
 template <int DK>
 struct AttFwdSmem {
-  static constexpr int NKB = (DK + 31) / 32;            // 32-wide k-blocks of the Q K^T contraction / V slabs
-  static constexpr int Q_BYTES = NKB * 128 * 128;       // [kb][128 rows][128 B]
-  static constexpr int K_BYTES = NKB * 256 * 128;       // [kb][256 rows][128 B]
-  static constexpr int V_BYTES = NKB * 256 * 128;       // [slab][256 key rows][128 B]
-  static constexpr int O_BYTES = NKB * 128 * 128;       // staging [slab][128 rows][128 B]
-  static constexpr int total() { return Q_BYTES + K_BYTES + V_BYTES + O_BYTES + 256 + 1024; }
+  static constexpr int NKB = (DK + 31) / 32;            // 32-wide column blocks of the head (one 128-byte row each)
+  static constexpr int TILE = 128 * 128;                // one [128 rows][128 B] box
+  static constexpr int Q_BYTES = NKB * TILE;            // [kb]
+  static constexpr int KV_BYTES = 2 * NKB * TILE;       // [128-key chunk][kb]
+  static constexpr int O_BYTES = NKB * TILE;            // staging [kb][128 rows][128 B]
+  static constexpr int total() { return Q_BYTES + 2 * KV_BYTES + O_BYTES + 256 + 1024; }
 };
 
-template <int DK, bool DROP>
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ,
-                                                                  const __grid_constant__ CUtensorMap tmK,
-                                                                  const __grid_constant__ CUtensorMap tmV,
-                                                                  const __grid_constant__ CUtensorMap tmO,
-                                                                  const uint8_t* __restrict__ mask,
-                                                                  float* __restrict__ stat_max,
-                                                                  float* __restrict__ stat_sum, int S, int n_heads,
-                                                                  float scale_log2e, DropSite drop,
-                                                                  const int* __restrict__ extent,
-                                                                  const int* __restrict__ pack_off) {
-  (void)extent; (void)pack_off;   // the single-pass kernel always covers the whole (dense) slate
+template <int DK, bool DROP, bool OUT16 = false>
+__global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ,
+                                                               const __grid_constant__ CUtensorMap tmK,
+                                                               const __grid_constant__ CUtensorMap tmV,
+                                                               const __grid_constant__ CUtensorMap tmO,
+                                                               const uint8_t* __restrict__ mask,
+                                                               float* __restrict__ stat_max,
+                                                               float* __restrict__ stat_sum, int S, int n_heads,
+                                                               float scale_log2e, DropSite drop,
+                                                               const int* __restrict__ extent,
+                                                               const int* __restrict__ pack_off, int rnd) {
   using L = AttFwdSmem<DK>;
   constexpr int NKB = L::NKB;
+  constexpr int KS = DK / 8;                 // k8 steps over the head width
+  static_assert(!OUT16 || DK <= 32, "bf16 context: one 64-byte row per query");
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* q_s = smem;
   uint8_t* k_s = q_s + L::Q_BYTES;
-  uint8_t* v_s = k_s + L::K_BYTES;
-  uint8_t* o_s = v_s + L::V_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(o_s + L::O_BYTES);
-  uint64_t* load_bar = bars;        // Q, K, V landed
-  uint64_t* s_bar = bars + 1;       // S = Q K^T complete
-  uint64_t* p_bar = bars + 2;       // P written to TMEM by all 128 softmax threads
-  uint64_t* o_bar = bars + 3;       // O = P V complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-  uint32_t* mask_bits = tmem_slot + 2;   // 8 words: bit j of word w = key 32w+j is a real (unpadded, < S) item
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * 128, head = blockIdx.y, b = blockIdx.z;
-  const int S16 = (S + 15) & ~15;       // UMMA N of the score tile
-  const int S8 = (S + 7) & ~7;          // contraction length of P V
-
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmQ); ptx::prefetch_tmap(&tmK); ptx::prefetch_tmap(&tmV); ptx::prefetch_tmap(&tmO);
-    ptx::mbar_init(load_bar, 1);
-    ptx::mbar_init(s_bar, 1);
-    ptx::mbar_init(p_bar, 128);
-    ptx::mbar_init(o_bar, 1);
-    ptx::fence_barrier_init();
-  }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  arb_pdl_wait();
-  if (warp >= 2) {
-    const int et = threadIdx.x - 64;
-    if (et < 8) {
-      uint32_t w = 0;
-      for (int j = 0; j < 32; ++j) {
-        const int key = 32 * et + j;
-        if (key < S && mask[size_t(b) * S + key] == 0) w |= (1u << j);
-      }
-      mask_bits[et] = w;
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;            // columns [0, 256)
-  const uint32_t tmem_O = tmem_base + 256;      // columns [256, 256 + DK)
-
-  if (warp == 0) {
-    if (lane == 0) {
-      ptx::mbar_expect_tx(load_bar, L::Q_BYTES + L::K_BYTES + L::V_BYTES);
-      for (int kb = 0; kb < NKB; ++kb) {
-        ptx::tma_load_4d(q_s + kb * (128 * 128), &tmQ, load_bar, 32 * kb, m0, head, b);
-        ptx::tma_load_4d(k_s + kb * (256 * 128), &tmK, load_bar, 32 * kb, 0, head, b);
-        ptx::tma_load_4d(v_s + kb * (256 * 128), &tmV, load_bar, 32 * kb, 0, head, b);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      ptx::mbar_wait(load_bar, 0);
-      ptx::tc_fence_after();
-      // ---- S = Q K^T
-      const uint32_t idesc_s = ptx::idesc_tf32(128, S16, 0, 0);
-      uint32_t acc = 0;
-      for (int kb = 0; kb < NKB; ++kb) {
-        const int ksteps = (DK - 32 * kb >= 32) ? 4 : (DK - 32 * kb + 7) / 8;
-        const uint32_t qa = ptx::smem_u32(q_s + kb * (128 * 128));
-        const uint32_t ka = ptx::smem_u32(k_s + kb * (256 * 128));
-        for (int k = 0; k < ksteps; ++k) {
-          ptx::mma_tf32_ss(tmem_S, ptx::smem_desc_sw128<2>(qa + k * 32, 16, 1024),
-                           ptx::smem_desc_sw128<2>(ka + k * 32, 16, 1024), idesc_s, acc);
-          acc = 1;
-        }
-      }
-      ptx::mma_commit(s_bar);
-      // ---- O = P V   (A = P from TMEM, B = V MN-major: 8 key rows = 1024 B per K step, 4-row swizzle atoms)
-      ptx::mbar_wait(p_bar, 0);
-      ptx::tc_fence_after();
-      const uint32_t idesc_o = ptx::idesc_tf32(128, DK < 16 ? 16 : DK, 0, 1);
-      const uint32_t va = ptx::smem_u32(v_s);
-      for (int i = 0; i < S8 / 8; ++i) {
-        ptx::mma_tf32_ts(tmem_O, tmem_S + 8 * i, ptx::smem_desc_sw128<1>(va + i * 1024, 256 * 128, 512), idesc_o,
-                         i > 0 ? 1u : 0u);
-      }
-      ptx::mma_commit(o_bar);
-    }
-  } else {
-    // ===================== softmax + epilogue: thread = query row =====================
-    const int q = warp & 3;
-    const int row = 32 * q + lane;
-    const int qidx = m0 + row;
-    const uint32_t lane_addr = uint32_t(32 * q) << 16;
-    ptx::mbar_wait(s_bar, 0);
-    ptx::tc_fence_after();
-    const int nchunks = (S8 + 31) / 32;
-    float mx = -CUDART_INF_F;
-    for (int c = 0; c < nchunks; ++c) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(tmem_S + lane_addr + 32 * c, v);
-      ptx::tmem_ld_wait();
-      const uint32_t bits = mask_bits[c];
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (bits & (1u << j)) mx = fmaxf(mx, __uint_as_float(v[j]));
-    }
-    float sum = 0.f;
-    const float mxs = mx * scale_log2e;
-    for (int c = 0; c < nchunks; ++c) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(tmem_S + lane_addr + 32 * c, v);
-      ptx::tmem_ld_wait();
-      const uint32_t bits = mask_bits[c];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        // exp((s - max)/sqrt(dk)) as exp2; padded keys contribute exactly 0.  An all-padded slate gives
-        // (-inf) - (-inf) = NaN like the reference (quirk Q2).
-        float e = (bits & (1u << j)) ? ex2_approx(fmaf(__uint_as_float(v[j]), scale_log2e, -mxs)) : 0.0f;
-        sum += e;                       // softmax normalises BEFORE dropout (transformer.py:153-155)
-        if constexpr (DROP) {
-          const unsigned long long idx =
-              ((unsigned long long)(b * n_heads + head) * S + qidx) * (unsigned long long)S + (32 * c + j);
-          e = drop_keep(idx, drop.seed, drop.thresh) ? e * drop.scale : 0.0f;
-        }
-        v[j] = round_tf32(e);
-      }
-      ptx::tmem_st_32x32(tmem_S + lane_addr + 32 * c, v);
-    }
-    ptx::tmem_st_wait();
-    ptx::tc_fence_before();
-    ptx::mbar_arrive(p_bar);
-    if (qidx < S) {
-      const size_t so = (size_t(b) * n_heads + head) * S + qidx;
-      stat_max[so] = mx;
-      stat_sum[so] = sum;
-    }
-    const float inv = 1.0f / sum;
-    ptx::mbar_wait(o_bar, 0);
-    ptx::tc_fence_after();
-#pragma unroll
-    for (int sl = 0; sl < NKB; ++sl) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(tmem_O + lane_addr + 32 * sl, v);
-      ptx::tmem_ld_wait();
-      uint8_t* slab_row = o_s + sl * (128 * 128) + row * 128;
-#pragma unroll
-      for (int piece = 0; piece < 8; ++piece) {
-        float4 o;
-        o.x = __uint_as_float(v[piece * 4 + 0]) * inv;
-        o.y = __uint_as_float(v[piece * 4 + 1]) * inv;
-        o.z = __uint_as_float(v[piece * 4 + 2]) * inv;
-        o.w = __uint_as_float(v[piece * 4 + 3]) * inv;
-        *reinterpret_cast<float4*>(slab_row + ((piece ^ (row & 7)) << 4)) = o;
-      }
-    }
-    ptx::fence_proxy_async_smem();
-    ptx::named_bar_sync(1, 128);
-    if (threadIdx.x == 64) {
-      for (int sl = 0; sl < NKB; ++sl) ptx::tma_store_4d(&tmO, o_s + sl * (128 * 128), 32 * sl, m0, head, b);
-      ptx::tma_store_commit();
-      ptx::tma_store_wait_all();
-    }
-    ptx::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<512>(tmem_base);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------ two-pass variant
-// Same result, organised so that TWO CTAs fit on an SM (the kernel above needs S(<=256)+O columns = a 512-column TMEM
-// allocation, i.e. one CTA per SM, and is latency-bound at 7 % tensor pipe).  Here the score tile is produced in
-// 128-key chunks into a 128-column TMEM window, twice: pass A only takes the row maximum, pass B recomputes the chunk
-// (K = dk, a handful of MMAs), exponentiates against the final maximum, writes P in place and accumulates O += P V.
-// TMEM: S chunk [0,128) + O [128,128+DK) -> 256 columns; shared memory 96 KB -> two co-resident CTAs overlap each
-// other's load / MMA / softmax phases.  Head width <= 32.  Eight softmax warps per CTA: a warp may only touch the 32
-// TMEM lanes of its quadrant, so two warps share each quadrant and split every 32-key chunk 16 / 16; the two partial
-// row maxima (after pass A) and row sums (after pass B) are combined through shared memory.
-template <int DK, bool DROP, bool OUT16 = false>
-__global__ void __launch_bounds__(ATT2_THREADS, 2) attn_fwd2_kernel(const __grid_constant__ CUtensorMap tmQ,
-                                                                   const __grid_constant__ CUtensorMap tmK,
-                                                                   const __grid_constant__ CUtensorMap tmV,
-                                                                   const __grid_constant__ CUtensorMap tmO,
-                                                                   const uint8_t* __restrict__ mask,
-                                                                   float* __restrict__ stat_max,
-                                                                   float* __restrict__ stat_sum, int S, int n_heads,
-                                                                   float scale_log2e, DropSite drop,
-                                                                   const int* __restrict__ extent,
-                                                                   const int* __restrict__ pack_off) {
-  static_assert(DK <= 32, "two-pass forward kernel: head width <= 32");
-  using L = AttFwdSmem<DK>;
-  extern __shared__ uint8_t smem_dyn[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_s = smem;
-  uint8_t* k_s = q_s + L::Q_BYTES;
-  uint8_t* v_s = k_s + L::K_BYTES;
-  uint8_t* o_s = v_s + L::V_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(o_s + L::O_BYTES);
-  uint64_t* load_bar = bars;
-  uint64_t* s_bar = bars + 1;       // a score chunk is complete            (one phase per step)
-  uint64_t* t_bar = bars + 2;       // the 256 softmax threads are done with the chunk (one phase per step)
-  uint64_t* o_bar = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-  uint32_t* mask_bits = tmem_slot + 2;
+  uint8_t* v_s = k_s + L::KV_BYTES;
+  uint8_t* o_s = v_s + L::KV_BYTES;
+  uint64_t* load_bar = reinterpret_cast<uint64_t*>(o_s + L::O_BYTES);
+  uint32_t* mask_bits = reinterpret_cast<uint32_t*>(load_bar + 1);   // 8 words: bit j of word w = key 32w+j is real
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * 128, head = blockIdx.y, b = blockIdx.z;
@@ -283,238 +83,180 @@ __global__ void __launch_bounds__(ATT2_THREADS, 2) attn_fwd2_kernel(const __grid
   const int row_base = packed ? __ldg(pack_off + b) : 0;
   const int bc = packed ? 0 : b;
   if (packed && m0 >= ((__ldg(extent + b) + 15) & ~15)) return;   // no packed query rows in this tile (or an empty slate)
+  // keys at or beyond the slate's extent are all masked (probability exactly 0): the products, the softmax and the
+  // K / V loads stop there.  At least one key block is always processed, so an all-padded slate still produces the
+  // reference's NaN rows.
+  const int kext = extent ? max(1, min(S, __ldg(extent + b))) : S;
+  const int S8 = (kext + 7) & ~7;
+  const int nkc = (S8 + 127) / 128;          // 128-key chunks
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmQ); ptx::prefetch_tmap(&tmK); ptx::prefetch_tmap(&tmV); ptx::prefetch_tmap(&tmO);
     ptx::mbar_init(load_bar, 1);
-    ptx::mbar_init(s_bar, 1);
-    ptx::mbar_init(t_bar, ATT2_SOFTMAX);
-    ptx::mbar_init(o_bar, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<256>(tmem_slot);
   arb_pdl_wait();
-  // keys at or beyond the slate's extent are all masked (probability exactly 0): the score / P V products, the softmax
-  // loop and the K / V loads stop there.  At least one key column group is always processed, so an all-padded slate
-  // still produces the reference's NaN rows.
-  const int kext = extent ? max(1, min(S, __ldg(extent + b))) : S;
-  const int S16 = (kext + 15) & ~15, S8 = (kext + 7) & ~7;
-  const int nkc = (S16 + 127) / 128;          // key chunks
-  const int nsteps = 1 + nkc;                 // one pass-A step over the whole score row + one pass-B step per chunk
-  if (warp == 0 && lane == 0) {
-    // The loads go out right here -- the thread that initialised the barriers needs nobody else -- so that they run
-    // behind the TMEM allocation, the mask read and the block-wide barrier below instead of after them.
-    // K and V arrive as 128-key boxes: only the chunks that hold keys below the extent are fetched
-    ptx::mbar_expect_tx(load_bar, L::Q_BYTES + nkc * 2 * (128 * 128));
-    ptx::tma_load_4d(q_s, &tmQ, load_bar, 0, row_base + m0, head, bc);
-    for (int kc = 0; kc < nkc; ++kc) {
-      ptx::tma_load_4d(k_s + kc * 16384, &tmK, load_bar, 0, row_base + 128 * kc, head, bc);
-      ptx::tma_load_4d(v_s + kc * 16384, &tmV, load_bar, 0, row_base + 128 * kc, head, bc);
+  if (threadIdx.x == 0) {
+    ptx::mbar_expect_tx(load_bar, L::Q_BYTES + nkc * 2 * NKB * L::TILE);
+    for (int kb = 0; kb < NKB; ++kb) {
+      ptx::tma_load_4d(q_s + kb * L::TILE, &tmQ, load_bar, 32 * kb, row_base + m0, head, bc);
+      for (int kc = 0; kc < nkc; ++kc) {
+        ptx::tma_load_4d(k_s + (kc * NKB + kb) * L::TILE, &tmK, load_bar, 32 * kb, row_base + 128 * kc, head, bc);
+        ptx::tma_load_4d(v_s + (kc * NKB + kb) * L::TILE, &tmV, load_bar, 32 * kb, row_base + 128 * kc, head, bc);
+      }
     }
   }
-  if (warp >= 2) {      // key mask as 8 words: one key per softmax thread, one ballot per warp
-    const int key = threadIdx.x - 64;
+  {                     // key mask as 8 words: one key per thread, one ballot per warp
+    const int key = threadIdx.x;
     const uint32_t w = __ballot_sync(0xffffffffu, key < S && mask[size_t(b) * S + key] == 0);
-    if (lane == 0) mask_bits[warp - 2] = w;
+    if (lane == 0) mask_bits[warp] = w;
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;
-  const uint32_t tmem_O = tmem_base + 128;
+  ptx::mbar_wait(load_bar, 0);
 
-  if (warp == 0) {
-    // (the producer's loads were issued above)
-  } else if (warp == 1) {
-    if (lane == 0) {
-      ptx::mbar_wait(load_bar, 0);
-      ptx::tc_fence_after();
-      constexpr int KSTEPS = (DK + 7) / 8;
-      const uint32_t qa = ptx::smem_u32(q_s), ka = ptx::smem_u32(k_s), va = ptx::smem_u32(v_s);
-      const uint32_t idesc_o = ptx::idesc_tf32(128, DK < 16 ? 16 : DK, 0, 1);
-      auto issue_pv = [&](int kc) {
-        const int keys = min(128, S8 - 128 * kc);
-        for (int i = 0; i < keys / 8; ++i)
-          ptx::mma_tf32_ts(tmem_O, tmem_S + 8 * i, ptx::smem_desc_sw128<1>(va + kc * 16384 + i * 1024, 256 * 128, 512),
-                           idesc_o, (kc > 0 || i > 0) ? 1u : 0u);
-      };
-      // step 0 (pass A): the WHOLE score row block S = Q K^T, N = S16 <= 256 columns, in one issue -- it may spill over
-      // the O columns, which pass B only starts to use after every softmax thread has taken its row maximum
-      {
-        const uint32_t idesc_a = ptx::idesc_tf32(128, S16, 0, 0);
-        for (int k = 0; k < KSTEPS; ++k)
-          ptx::mma_tf32_ss(tmem_S, ptx::smem_desc_sw128<2>(qa + k * 32, 16, 1024),
-                           ptx::smem_desc_sw128<2>(ka + k * 32, 16, 1024), idesc_a, k > 0);
-        ptx::mma_commit(s_bar);
-      }
-      // steps 1..nkc (pass B): recompute one 128-key chunk into the 128-column window; the previous chunk's P V runs
-      // first (P sits in the window until then)
-      for (int st = 1; st < nsteps; ++st) {
-        const int kc = st - 1;
-        ptx::mbar_wait(t_bar, (st - 1) & 1);
-        ptx::tc_fence_after();
-        if (kc > 0) issue_pv(kc - 1);
-        const int nc = min(128, S16 - 128 * kc);
-        const uint32_t idesc_s = ptx::idesc_tf32(128, nc, 0, 0);
-        for (int k = 0; k < KSTEPS; ++k)
-          ptx::mma_tf32_ss(tmem_S, ptx::smem_desc_sw128<2>(qa + k * 32, 16, 1024),
-                           ptx::smem_desc_sw128<2>(ka + kc * 16384 + k * 32, 16, 1024), idesc_s, k > 0);
-        ptx::mma_commit(s_bar);
-      }
-      ptx::mbar_wait(t_bar, (nsteps - 1) & 1);
-      ptx::tc_fence_after();
-      issue_pv(nkc - 1);
-      ptx::mma_commit(o_bar);
-    }
-  } else {
-    const int q = warp & 3;                     // TMEM lane quadrant
-    const int sub = (warp - 2) >> 2;            // which 16 keys of every 32-key chunk this warp handles
-    const int row = 32 * q + lane;
-    const int qidx = m0 + row;
-    const uint32_t lane_addr = uint32_t(32 * q) << 16;
-    float* xch_max = reinterpret_cast<float*>(o_s);     // [2][128] partial maxima (the O staging is idle until the end)
-    float* xch_sum = reinterpret_cast<float*>(k_s);     // [2][128] partial sums   (K is dead after the last score chunk)
-    float mx = -CUDART_INF_F, sum = 0.f, mxs = 0.f;
-    for (int st = 0; st < nsteps; ++st) {
-      const bool pass_b = st > 0;
-      const int kc = pass_b ? st - 1 : 0;
-      if (st == 1) {                            // pass A done: combine the two partial row maxima
-        xch_max[sub * 128 + row] = mx;
-        ptx::named_bar_sync(1, ATT2_SOFTMAX);
-        mx = fmaxf(xch_max[row], xch_max[128 + row]);
-        mxs = mx * scale_log2e;
-      }
-      ptx::mbar_wait(s_bar, st & 1);
-      ptx::tc_fence_after();
-      // pass A walks every 32-key group of the row block, pass B the groups of its chunk
-      const int keys = pass_b ? min(128, S8 - 128 * kc) : S8;
-      const int nch = (keys + 31) / 32;
-      for (int c = 0; c < nch; ++c) {
-        uint32_t v[16];
-        const int col = 32 * c + 16 * sub;
-        ptx::tmem_ld_32x16(tmem_S + lane_addr + col, v);
-        ptx::tmem_ld_wait();
-        const uint32_t bits = mask_bits[4 * kc + c] >> (16 * sub);
-        if (!pass_b) {
+  const int g = lane >> 2, t = lane & 3;
+  const int rA = 16 * warp + g, rB = rA + 8;        // this thread's two query rows of the tile
+  auto kv_at = [&](const uint8_t* base, int key, int e) -> uint32_t {
+    const float x = ptx::ld_f32(base + ((key >> 7) * NKB + (e >> 5)) * L::TILE, key & 127, e & 31);
+    return rnd ? ptx::cvt_tf32(x) : __float_as_uint(x);
+  };
+  uint32_t qa[KS][4];
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (bits & (1u << j)) mx = fmaxf(mx, __uint_as_float(v[j]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float e = (bits & (1u << j)) ? ex2_approx(fmaf(__uint_as_float(v[j]), scale_log2e, -mxs)) : 0.0f;
-            sum += e;
-            if constexpr (DROP) {
-              const unsigned long long idx =
-                  ((unsigned long long)(b * n_heads + head) * S + qidx) * (unsigned long long)S + (128 * kc + col + j);
-              e = drop_keep(idx, drop.seed, drop.thresh) ? e * drop.scale : 0.0f;
-            }
-            v[j] = round_tf32(e);
-          }
-          ptx::tmem_st_32x16(tmem_S + lane_addr + col, v);
-        }
-      }
-      if (pass_b) ptx::tmem_st_wait();
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(t_bar);
-    }
-    xch_sum[sub * 128 + row] = sum;             // every score MMA has completed: the K tile is free
-    ptx::named_bar_sync(1, ATT2_SOFTMAX);
-    sum = xch_sum[row] + xch_sum[128 + row];
-    if (sub == 0 && qidx < S) {
-      const size_t so = (size_t(b) * n_heads + head) * S + qidx;
-      stat_max[so] = mx;
-      stat_sum[so] = sum;
-    }
-    const float inv = 1.0f / sum;
-    ptx::mbar_wait(o_bar, 0);
-    ptx::tc_fence_after();
-    {
-      uint32_t v[16];                           // this warp's 16 of the (up to) 32 output columns
-      ptx::tmem_ld_32x16(tmem_O + lane_addr + 16 * sub, v);
-      ptx::tmem_ld_wait();
-      if constexpr (OUT16) {
-        // bf16 mode: the context only feeds the output projection -- stage it as dense bfloat16 rows (32 columns =
-        // 64 bytes, unswizzled tensor map); this warp's 16 columns are bytes [32 sub, 32 sub + 32)
-        uint4* dst = reinterpret_cast<uint4*>(o_s + row * 64 + sub * 32);
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          uint4 pk;
-          pk.x = ptx::pack_bf16(__uint_as_float(v[8 * k + 0]) * inv, __uint_as_float(v[8 * k + 1]) * inv);
-          pk.y = ptx::pack_bf16(__uint_as_float(v[8 * k + 2]) * inv, __uint_as_float(v[8 * k + 3]) * inv);
-          pk.z = ptx::pack_bf16(__uint_as_float(v[8 * k + 4]) * inv, __uint_as_float(v[8 * k + 5]) * inv);
-          pk.w = ptx::pack_bf16(__uint_as_float(v[8 * k + 6]) * inv, __uint_as_float(v[8 * k + 7]) * inv);
-          dst[k] = pk;
-        }
-      } else {
-        uint8_t* slab_row = o_s + row * 128;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int piece = 4 * sub + k;
-          float4 o;
-          o.x = __uint_as_float(v[k * 4 + 0]) * inv;
-          o.y = __uint_as_float(v[k * 4 + 1]) * inv;
-          o.z = __uint_as_float(v[k * 4 + 2]) * inv;
-          o.w = __uint_as_float(v[k * 4 + 3]) * inv;
-          *reinterpret_cast<float4*>(slab_row + ((piece ^ (row & 7)) << 4)) = o;
-        }
-      }
-    }
-    ptx::fence_proxy_async_smem();
-    ptx::named_bar_sync(1, ATT2_SOFTMAX);
-    if (threadIdx.x == 64) {
-      if (packed) {       // 16-row boxes up to the slate's last packed row (the staged rows are 128 / 64 bytes wide)
-        const int n16 = (min(128, S16 - m0) + 15) >> 4;
-        for (int i = 0; i < n16; ++i)
-          ptx::tma_store_4d(&tmO, o_s + i * (OUT16 ? 1024 : 2048), 0, row_base + m0 + 16 * i, head, 0);
-      } else {
-        ptx::tma_store_4d(&tmO, o_s, 0, m0, head, b);
-      }
-      ptx::tma_store_commit();
-      ptx::tma_store_wait_read();
-    }
-    ptx::tc_fence_before();
+  for (int ks = 0; ks < KS; ++ks) {
+    const int e0 = 8 * ks + t, e1 = e0 + 4;
+    const uint8_t* qt = q_s + (e0 >> 5) * L::TILE;
+    auto qv = [&](int r, int e) { const float x = ptx::ld_f32(qt, r, e & 31); return rnd ? ptx::cvt_tf32(x) : __float_as_uint(x); };
+    qa[ks][0] = qv(rA, e0); qa[ks][1] = qv(rB, e0); qa[ks][2] = qv(rA, e1); qa[ks][3] = qv(rB, e1);
   }
+  // raw scores of keys 8j + 2t, 8j + 2t + 1 for rows rA, rB
+  auto scores = [&](int j, float (&s)[4]) {
+    s[0] = s[1] = s[2] = s[3] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      const uint32_t kb2[2] = {kv_at(k_s, 8 * j + g, 8 * ks + t), kv_at(k_s, 8 * j + g, 8 * ks + t + 4)};
+      ptx::mma_tf32(s, qa[ks], kb2);
+    }
+  };
+  const int nj = S8 / 8;
+  // ---- pass A: masked row maxima
+  float mxA = -CUDART_INF_F, mxB = -CUDART_INF_F;
+  for (int j = 0; j < nj; ++j) {
+    float s[4];
+    scores(j, s);
+    const int k0 = 8 * j + 2 * t;
+    const uint32_t bits = mask_bits[k0 >> 5] >> (k0 & 31);
+    if (bits & 1u) { mxA = fmaxf(mxA, s[0]); mxB = fmaxf(mxB, s[2]); }
+    if (bits & 2u) { mxA = fmaxf(mxA, s[1]); mxB = fmaxf(mxB, s[3]); }
+  }
+  mxA = fmaxf(mxA, __shfl_xor_sync(0xffffffffu, mxA, 1)); mxA = fmaxf(mxA, __shfl_xor_sync(0xffffffffu, mxA, 2));
+  mxB = fmaxf(mxB, __shfl_xor_sync(0xffffffffu, mxB, 1)); mxB = fmaxf(mxB, __shfl_xor_sync(0xffffffffu, mxB, 2));
+  // ---- pass B: probabilities and O = P V
+  const float mxsA = mxA * scale_log2e, mxsB = mxB * scale_log2e;
+  const int qA = m0 + rA, qB = m0 + rB;
+  float sumA = 0.f, sumB = 0.f;
+  float o[KS][4];
+#pragma unroll
+  for (int nt = 0; nt < KS; ++nt) o[nt][0] = o[nt][1] = o[nt][2] = o[nt][3] = 0.f;
+  for (int j = 0; j < nj; ++j) {
+    float s[4];
+    scores(j, s);
+    const int k0 = 8 * j + 2 * t;
+    const uint32_t bits = mask_bits[k0 >> 5] >> (k0 & 31);
+    // exp((s - max)/sqrt(dk)) as exp2; padded keys contribute exactly 0.  An all-padded slate gives
+    // (-inf) - (-inf) = NaN like the reference (quirk Q2).
+    float p[4];
+    p[0] = (bits & 1u) ? ex2_approx(fmaf(s[0], scale_log2e, -mxsA)) : 0.0f;
+    p[1] = (bits & 2u) ? ex2_approx(fmaf(s[1], scale_log2e, -mxsA)) : 0.0f;
+    p[2] = (bits & 1u) ? ex2_approx(fmaf(s[2], scale_log2e, -mxsB)) : 0.0f;
+    p[3] = (bits & 2u) ? ex2_approx(fmaf(s[3], scale_log2e, -mxsB)) : 0.0f;
+    sumA += p[0] + p[1];                 // softmax normalises BEFORE dropout (transformer.py:153-155)
+    sumB += p[2] + p[3];
+    if constexpr (DROP) {
+      const unsigned long long base = (unsigned long long)(b * n_heads + head) * S;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const unsigned long long idx = (base + (i < 2 ? qA : qB)) * (unsigned long long)S + (k0 + (i & 1));
+        p[i] = drop_keep(idx, drop.seed, drop.thresh) ? p[i] * drop.scale : 0.0f;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) p[i] = round_tf32(p[i]);
+    uint32_t pa[4];
+    ptx::acc_to_a_tf32(p, pa, lane);
+#pragma unroll
+    for (int nt = 0; nt < KS; ++nt) {
+      const uint32_t vb[2] = {kv_at(v_s, 8 * j + t, 8 * nt + g), kv_at(v_s, 8 * j + t + 4, 8 * nt + g)};
+      ptx::mma_tf32(o[nt], pa, vb);
+    }
+  }
+  sumA += __shfl_xor_sync(0xffffffffu, sumA, 1); sumA += __shfl_xor_sync(0xffffffffu, sumA, 2);
+  sumB += __shfl_xor_sync(0xffffffffu, sumB, 1); sumB += __shfl_xor_sync(0xffffffffu, sumB, 2);
+  if (t == 0) {
+    const size_t so = (size_t(b) * n_heads + head) * S;
+    if (qA < S) { stat_max[so + qA] = mxA; stat_sum[so + qA] = sumA; }
+    if (qB < S) { stat_max[so + qB] = mxB; stat_sum[so + qB] = sumB; }
+  }
+  const float invA = 1.0f / sumA, invB = 1.0f / sumB;
+#pragma unroll
+  for (int nt = 0; nt < KS; ++nt) {
+    const int e = 8 * nt + 2 * t;
+    if constexpr (OUT16) {
+      // bf16 mode: the context only feeds the output projection -- stage it as dense bfloat16 rows (32 columns =
+      // 64 bytes, unswizzled tensor map)
+      *reinterpret_cast<uint32_t*>(o_s + rA * 64 + 2 * e) = ptx::pack_bf16(o[nt][0] * invA, o[nt][1] * invA);
+      *reinterpret_cast<uint32_t*>(o_s + rB * 64 + 2 * e) = ptx::pack_bf16(o[nt][2] * invB, o[nt][3] * invB);
+    } else {
+      uint8_t* ot = o_s + (e >> 5) * L::TILE;
+      *reinterpret_cast<float2*>(ot + ptx::sw128(rA, 4 * (e & 31))) = make_float2(o[nt][0] * invA, o[nt][1] * invA);
+      *reinterpret_cast<float2*>(ot + ptx::sw128(rB, 4 * (e & 31))) = make_float2(o[nt][2] * invB, o[nt][3] * invB);
+    }
+  }
+  ptx::fence_proxy_async_smem();
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<256>(tmem_base);
+  if (threadIdx.x == 0) {
+    constexpr int OSLABS = OUT16 ? 1 : NKB;
+    for (int sl = 0; sl < OSLABS; ++sl) {
+      if (packed) {       // 16-row boxes up to the slate's last packed row (the staged rows are 128 / 64 bytes wide)
+        const int ext16 = (__ldg(extent + b) + 15) & ~15;
+        const int n16 = (min(128, ext16 - m0) + 15) >> 4;
+        for (int i = 0; i < n16; ++i)
+          ptx::tma_store_4d(&tmO, o_s + sl * L::TILE + i * (OUT16 ? 1024 : 2048), 32 * sl, row_base + m0 + 16 * i, head, 0);
+      } else {
+        ptx::tma_store_4d(&tmO, o_s + sl * L::TILE, 32 * sl, m0, head, b);
+      }
+    }
+    ptx::tma_store_commit();
+    ptx::tma_store_wait_all();
   }
 }
 
-static int g_attn_fwd_two_pass = 1;
-void set_attn_fwd_two_pass(int on) { g_attn_fwd_two_pass = on; }
+// Both settings run attn_fwd_kernel; the switch is kept for the C ABI (arb_set_attention_fwd_two_pass).
+void set_attn_fwd_two_pass(int) {}
 
 template <int DK>
 static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   using L = AttFwdSmem<DK>;
   alignas(64) CUtensorMap tQ, tK, tV, tO;
   int rc;
-  if ((rc = make_tmap_4d(&tQ, a.q, TmapBox{{32, 128, 1, 1}}, 0, 1))) return rc;
-  const uint32_t kv_rows = (DK <= 32 && g_attn_fwd_two_pass) ? 128u : 256u;   // two-pass kernel: one box per key chunk
-  if ((rc = make_tmap_4d(&tK, a.k, TmapBox{{32, kv_rows, 1, 1}}, 0, 1))) return rc;
-  if ((rc = make_tmap_4d(&tV, a.v, TmapBox{{32, kv_rows, 1, 1}}, 1, 1))) return rc;
+  if ((rc = make_tmap_4d(&tQ, a.q, TmapBox{{32, 128, 1, 1}}, 0))) return rc;
+  if ((rc = make_tmap_4d(&tK, a.k, TmapBox{{32, 128, 1, 1}}, 0))) return rc;
+  if ((rc = make_tmap_4d(&tV, a.v, TmapBox{{32, 128, 1, 1}}, 0))) return rc;
   const bool out16 = a.o.bf16 != 0;
-  if (out16 && !(DK <= 32 && g_attn_fwd_two_pass)) { arb_set_error("attn_fwd: a bf16 context needs the two-pass kernel (head width <= 32)"); return ARB_E_UNSUPPORTED; }
+  if (out16 && DK > 32) { arb_set_error("attn_fwd: a bf16 context needs head width <= 32"); return ARB_E_UNSUPPORTED; }
   const bool packed = a.pack_off != nullptr;
-  if (packed && !(DK <= 32 && g_attn_fwd_two_pass && a.extent)) { arb_set_error("attn_fwd: packed rows need the two-pass kernel and the slate extents"); return ARB_E_UNSUPPORTED; }
-  if ((rc = make_tmap_4d(&tO, a.o, TmapBox{{32, packed ? 16u : 128u, 1, 1}}, out16 ? 2 : 0, 0))) return rc;
+  if (packed && !a.extent) { arb_set_error("attn_fwd: packed rows need the slate extents"); return ARB_E_UNSUPPORTED; }
+  if ((rc = make_tmap_4d(&tO, a.o, TmapBox{{32, packed ? 16u : 128u, 1, 1}}, out16 ? 1 : 0))) return rc;
   const bool drop = a.drop.thresh != 0;
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, const uint8_t*, float*, float*, int, int, float,
-               DropSite, const int*, const int*);
+               DropSite, const int*, const int*, int);
   if constexpr (DK <= 32) {
-    if (g_attn_fwd_two_pass) {
-      if (out16) kern = drop ? attn_fwd2_kernel<DK, true, true> : attn_fwd2_kernel<DK, false, true>;
-      else kern = drop ? attn_fwd2_kernel<DK, true> : attn_fwd2_kernel<DK, false>;
-    } else {
-      kern = drop ? attn_fwd_kernel<DK, true> : attn_fwd_kernel<DK, false>;
-    }
+    if (out16) kern = drop ? attn_fwd_kernel<DK, true, true> : attn_fwd_kernel<DK, false, true>;
+    else kern = drop ? attn_fwd_kernel<DK, true> : attn_fwd_kernel<DK, false>;
   } else {
     kern = drop ? attn_fwd_kernel<DK, true> : attn_fwd_kernel<DK, false>;
   }
-  static bool configured[ARB_MAX_DEVICES][8] = {};
-  const int slot = (drop ? 1 : 0) + ((DK <= 32 && g_attn_fwd_two_pass) ? 2 : 0) + (out16 ? 4 : 0);
+  static bool configured[ARB_MAX_DEVICES][4] = {};
+  const int slot = (drop ? 1 : 0) + (out16 ? 2 : 0);
   const int dev = arb_device_slot();
   if (!configured[dev][slot]) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total()) != cudaSuccess) {
@@ -527,10 +269,9 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   {
     ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 4.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                  (packed ? arb_row_frac() : 1.0) * 4.0 * double(a.B) * a.h * a.S * ((out16 ? 3.5 : 4.0) * a.dk + 2.0),
-                 (DK <= 32 && g_attn_fwd_two_pass) ? "attn_fwd2_kernel" : "attn_fwd_kernel");
-    const int threads = (DK <= 32 && g_attn_fwd_two_pass) ? ATT2_THREADS : ATT_THREADS;
-    arb_launch(kern, grid, dim3(threads), size_t(L::total()), st, tQ, tK, tV, tO, a.mask, a.stat_max, a.stat_sum, a.S, a.h,
-               a.scale * 1.4426950408889634f, a.drop, a.extent, a.pack_off);
+                 "attn_fwd_kernel");
+    arb_launch(kern, grid, dim3(ATT_THREADS), size_t(L::total()), st, tQ, tK, tV, tO, a.mask, a.stat_max, a.stat_sum, a.S,
+               a.h, a.scale * 1.4426950408889634f, a.drop, a.extent, a.pack_off, tf32_round_on_load());
   }
   arb_count_launch();
   cudaError_t e = cudaGetLastError();

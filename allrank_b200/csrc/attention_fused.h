@@ -22,7 +22,7 @@ struct AttnFwdArgs {
 };
 
 bool attn_fused_supported(int S, int dk);
-void set_attn_fwd_two_pass(int on);   // 1 (default): two-pass 128-key-chunk forward kernel, two CTAs per SM
+void set_attn_fwd_two_pass(int on);   // accepted for the C ABI; every setting runs the same kernel
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st);
 
 }  // namespace arb

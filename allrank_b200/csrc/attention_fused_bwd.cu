@@ -2,28 +2,7 @@
 //
 // Reference: autograd of attention() allrank/models/transformer.py:137-156.  Given d ctx it produces dQ, dK, dV
 // without ever materialising the S x S probabilities in HBM: they are recomputed from Q, K and the row statistics
-// (max, sum) the fused forward kernel saved.
-//
-// One CTA = one (slate, head).  Everything is computed in the TRANSPOSED orientation (TMEM lane = key), because the
-// tensor core takes its A operand from TMEM with lane = M:
-//     S^T  = K Q^T   , dP^T = V dO^T                       (tcgen05.mma kind::tf32, smem x smem -> TMEM)
-//     P^T  = exp2(S^T c - m_q c - log2 l_q)                 (one thread per key row; statistics per query column)
-//     dS^T = P^T * (dP^T - delta_q),  delta_q = sum_e dO[q,e] O[q,e]
-//     dV  += P^T  dO        (A = P^T  from TMEM, B = dO as MN-major smem operand)
-//     dK  += dS^T Q  * a    (A = dS^T from TMEM, B = Q  as MN-major smem operand)
-//     dQ  += dS   K  * a    (A = dS^T staged to smem and read as an MN-major A operand, B = K MN-major)
-// over 128-key tiles (outer) and 128-query chunks (inner); dV/dK accumulate in TMEM across query chunks, the two dQ
-// chunks accumulate in TMEM across key tiles.  TMEM columns: S^T [0,128) dP^T [128,256) dV [256..) dK [320..)
-// dQ0 [384..) dQ1 [448..).
-//   warp 0: TMA producer   warp 1: TMEM alloc + MMA issue   warps 2-17: 512 compute/epilogue threads
-//   (warp w owns TMEM lanes 32*(w%4).., and 16 of the 64 query columns of each half: sub = (w-2)/4; four warps per
-//   scheduler hide the TMEM / shared-memory / MUFU latencies of the element-wise work).
-//
-// Each 128-query chunk is processed as two 64-column HALVES (a, b) that are software-pipelined against each other:
-// while the 512 compute threads turn half b's S^T / dP^T into P^T / dS^T, the tensor core runs half a's dV / dK
-// products and already produces half a's S^T / dP^T of the NEXT iteration in the columns that just became free; the
-// dQ product (which contracts over all 128 keys and needs both halves staged) trails half b.  The compute threads
-// therefore never sit behind an MMA round trip except in the pipeline prologue.
+// (max, sum) the fused forward kernel saved.  See attn_bwd_kernel for the organisation.
 #include <cstdint>
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -33,12 +12,11 @@
 #include "block_utils.cuh"
 #include "common.h"
 #include "defaults.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace arb {
 
-constexpr int BWD_COMPUTE = 512;              // 16 compute warps: four per TMEM lane quadrant
-constexpr int BWD_THREADS = 64 + BWD_COMPUTE;
+constexpr int BWD_THREADS = 256;          // 8 warps x 16 rows of a 128-row tile
 constexpr int TILE_BYTES = 128 * 128;     // one [128 rows][128 B] operand tile
 
 __device__ __forceinline__ float ex2_approx_b(float x) {
@@ -46,11 +24,11 @@ __device__ __forceinline__ float ex2_approx_b(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t round_tf32_b(float x) {
+__device__ __forceinline__ float round_tf32_b(float x) {
   // round-to-nearest (ties away) to tf32 as "+ half an ulp of the 10-bit mantissa, then let the tensor core ignore the
-  // low 13 bits" -- one integer add instead of cvt.rna.tf32.f32, which ptxas expands to three instructions here.
+  // low 13 bits" -- one integer add instead of cvt.rna.tf32.f32.
   // Same result as cvt.rna for every finite value (probabilities and their gradients are finite).
-  return __float_as_uint(x) + 0x1000u;
+  return __uint_as_float(__float_as_uint(x) + 0x1000u);
 }
 
 // delta[b,h,q] = sum_e dO[b,q,h,e] * O[b,q,h,e]: one warp per row of the [B*S, d_model] activations, 128-bit loads,
@@ -104,490 +82,304 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
 }
 
 struct BwdSmem {
-  // operand tiles (DK <= 32 -> one 32-wide k-block / slab each)
-  static constexpr int K_KM = 0;                    // K tile, K-major   (A of S^T)
-  static constexpr int K_MN = 1;                    // K tile, MN-major  (B of dQ)
-  static constexpr int V_KM = 2;                    // V tile, K-major   (A of dP^T)
-  static constexpr int Q_KM = 3;                    // Q chunk, K-major  (B of S^T)
-  static constexpr int Q_MN = 4;                    // Q chunk, MN-major (B of dK)
-  static constexpr int DO_KM = 5;                   // dO chunk, K-major (B of dP^T)
-  static constexpr int DO_MN = 6;                   // dO chunk, MN-major(B of dV)
-  static constexpr int N_TILES = 7;
-  static constexpr int STAGE_OFF = N_TILES * TILE_BYTES;          // dS^T staging: 4 slabs x [128 key rows][128 B]
-  static constexpr int STAGE_BYTES = 4 * TILE_BYTES;
-  // Output staging: dV -> slab 2, dK -> slab 3 of the dS^T staging (idle between the previous dQ product and this
-  // iteration's half-b staging), dQ -> one extra tile.  Slabs 0 / 1 are NOT used, so the half-a staging that follows
-  // an epilogue does not have to wait for the TMA stores to drain.
-  static constexpr int OUT_OFF = STAGE_OFF + STAGE_BYTES;
-  static constexpr int STATS_OFF = OUT_OFF + TILE_BYTES;          // float2 {nm_q, delta_q} x 128, double-buffered
-  static constexpr int BARS_OFF = STATS_OFF + 2 * 128 * 8;
-  static constexpr int total() { return BARS_OFF + 256 + 1024; }
+  // operand tiles: Q, K, V, dO of the whole slate (up to 256 rows = two 128-row boxes each, DK <= 32 -> one 128-byte
+  // row per item), then the output staging tiles dV | dK | dQ
+  static constexpr int OPS = 4 * 2 * TILE_BYTES;
+  static constexpr int OUT_OFF = OPS;
+  static constexpr int STATS_OFF = OUT_OFF + 3 * TILE_BYTES;    // float2 {nm_q, delta_q} x 256
+  static constexpr int BITS_OFF = STATS_OFF + 256 * 8;          // 8 words: key is a real item
+  static constexpr int BARS_OFF = BITS_OFF + 64;
+  static constexpr int BIAS_OFF = BARS_OFF + 64;                // float [3 * d_model]: this CTA's QKV bias gradient
+  static int total(int d_model) { return BIAS_OFF + 12 * d_model + 1024; }
 };
 
-// One unit of work of the kernel below: (slate, head) `item`, key tile jt, query chunk qc.  A CTA walks the items
-// item0, item0 + stride, ... and, inside an item, its n_kt x n_kt (key tile, query chunk) iterations; the three roles
-// (TMA producer, MMA issuer, compute warps) each advance their own copy.
-struct BwdIter {
-  int item, b, head, jt, qc, n_kt, ext16, q_lim, row_base;
-  int q_live;     // queries at or beyond it contribute nothing (the dense layout's padding has zero d ctx rows; packed
-                  // rows: the slate has no such queries): a 64-query half that starts there is skipped
-  __device__ __forceinline__ bool half_b_live() const { return 128 * qc + 64 < q_live; }
-};
-struct BwdWalk {
-  int n_items, stride, n_heads, S;
-  const int* extent;
-  const int* pack_off;
-  // position `it` on the first iteration of the first item at or after it.item that has work
-  __device__ __forceinline__ bool seek(BwdIter& it) const {
-    for (; it.item < n_items; it.item += stride) {
-      it.b = it.item / n_heads;
-      it.head = it.item - it.b * n_heads;
-      int e = extent ? __ldg(extent + it.b) : S;
-      if (pack_off && e <= 0) continue;           // packed rows: an empty slate holds no rows
-      e = max(1, min(S, e));
-      it.n_kt = (e + 127) / 128;                  // active key tiles == active query chunks
-      it.ext16 = (e + 15) & ~15;
-      it.q_lim = pack_off ? min(S, it.ext16) : S; // queries at or beyond it do not exist in this slate
-      it.q_live = pack_off ? it.q_lim : (extent ? e : S);
-      it.row_base = pack_off ? __ldg(pack_off + it.b) : 0;
-      it.jt = it.qc = 0;
-      return true;
-    }
-    return false;
-  }
-  __device__ __forceinline__ bool next(BwdIter& it) const {
-    if (++it.qc < it.n_kt) return true;
-    it.qc = 0;
-    if (++it.jt < it.n_kt) return true;
-    it.item += stride;
-    return seek(it);
-  }
-};
-
-// The grid is either one CTA per (slate, head) or -- persistent -- one CTA per SM walking many of them: the barrier
-// phases, the operand tiles and the TMEM accumulators form ONE stream of iterations across items, so the loads and the
-// S^T / dP^T products of an item's first iteration run behind the previous item's last iteration, and its epilogue
-// behind the next item's first arithmetic.  (One CTA per item pays the prologue -- first loads, first products -- and
-// the output drain, about 4.7 us, for 4.2 us of work per iteration; most slates need a single iteration.)
+// One CTA walks the (slate, head) items item0, item0 + gridDim.x, ...  (one CTA per item, or -- persistent -- one per
+// SM).  Per item, eight warps run two phases on the tensor cores (mma.sync m16n8k8 tf32), each keeping its products
+// in registers:
+//   phase 1, per 128-key tile (warp = 16 keys):  S^T = K Q^T, dP^T = V dO^T over 8-query blocks,
+//            P^T = exp2(S^T c + nm_q) (key mask, dropout), dS^T = P^T * (dP^T - delta_q),
+//            dV += P^T dO,  dK += dS^T Q   (P^T / dS^T go straight from the accumulators into the next product)
+//   phase 2, per 128-query tile (warp = 16 queries):  S = Q K^T, dP = dO V^T over 8-key blocks, dS as above,
+//            dQ += dS K
+// with nm_q = -max_q c - log2 l_q from the forward's row statistics and c = log2(e) / sqrt(dk).  Outputs are staged in
+// shared memory and TMA-stored (+ the QKV bias column sums).
 template <int DK, bool DROP, bool OUT16 = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
-    const __grid_constant__ CUtensorMap tmQk, const __grid_constant__ CUtensorMap tmQm,
-    const __grid_constant__ CUtensorMap tmKk, const __grid_constant__ CUtensorMap tmKm,
-    const __grid_constant__ CUtensorMap tmVk, const __grid_constant__ CUtensorMap tmDOk,
-    const __grid_constant__ CUtensorMap tmDOm, const __grid_constant__ CUtensorMap tmDQ,
-    const __grid_constant__ CUtensorMap tmDK, const __grid_constant__ CUtensorMap tmDV,
-    const uint8_t* __restrict__ mask, const float* __restrict__ stat_max, const float* __restrict__ stat_sum,
-    const float* __restrict__ delta, int S, int n_heads, float scale, DropSite drop, float* __restrict__ dbias_qkv,
-    int d_model, const int* __restrict__ extent, const int* __restrict__ pack_off, int n_items) {
+    const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+    const __grid_constant__ CUtensorMap tmDQ, const __grid_constant__ CUtensorMap tmDK,
+    const __grid_constant__ CUtensorMap tmDV, const uint8_t* __restrict__ mask, const float* __restrict__ stat_max,
+    const float* __restrict__ stat_sum, const float* __restrict__ delta, int S, int n_heads, float scale, DropSite drop,
+    float* __restrict__ dbias_qkv, int d_model, const int* __restrict__ extent, const int* __restrict__ pack_off,
+    int n_items, int rnd) {
+  constexpr int KS = DK / 8;
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-  auto tile = [&](int t) { return smem + t * TILE_BYTES; };
-  uint8_t* stage = smem + BwdSmem::STAGE_OFF;
+  uint8_t* q_s = smem;
+  uint8_t* k_s = smem + 2 * TILE_BYTES;
+  uint8_t* v_s = smem + 4 * TILE_BYTES;
+  uint8_t* do_s = smem + 6 * TILE_BYTES;
+  auto out_tile = [&](int which) { return smem + BwdSmem::OUT_OFF + which * TILE_BYTES; };   // 0 dV, 1 dK, 2 dQ
   float2* qstats = reinterpret_cast<float2*>(smem + BwdSmem::STATS_OFF);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BwdSmem::BARS_OFF);
-  uint64_t* kv_bar = bars;          // K-major K/V tiles of a key tile landed      (one phase per key tile of the stream)
-  uint64_t* q_bar = bars + 1;       // K-major Q/dO tiles of an iteration landed   (one phase per iteration)
-  uint64_t* s_bar = bars + 2;       // [2] S^T and dP^T of half a / b complete     (per iteration)
-  uint64_t* p_bar = bars + 4;       // [2] P^T / dS^T of half a / b written by the 512 compute threads (per iteration)
-  uint64_t* mma_bar = bars + 6;     // all trailing MMAs (dV, dK, dQ) of the iteration complete
-  uint64_t* qm_bar = bars + 7;      // MN-major Q/dO tiles of an iteration landed  (one phase per iteration)
-  uint64_t* km_bar = bars + 8;      // MN-major K tile of a key tile landed        (one phase per key tile)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
+  uint32_t* key_bits = reinterpret_cast<uint32_t*>(smem + BwdSmem::BITS_OFF);
+  uint64_t* load_bar = reinterpret_cast<uint64_t*>(smem + BwdSmem::BARS_OFF);
+  float* bias_acc = reinterpret_cast<float*>(smem + BwdSmem::BIAS_OFF);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   // Rows at or beyond a slate's extent are masked keys (probability exactly 0) whose d ctx rows are exactly zero:
-  // neither their key tiles nor their query chunks contribute anything, and their dQ / dK / dV rows are zero.  Only
+  // neither their key tiles nor their query tiles contribute anything, and their dQ / dK / dV rows are zero.  Only
   // the tiles below the extent are processed; in the dense layout the rest is written as zeros.
-  // Packed rows (see attn_fwd2_kernel): slate b holds its first ext16 = round_up(extent, 16) rows at row pack_off[b] of
+  // Packed rows (see attn_fwd_kernel): slate b holds its first ext16 = round_up(extent, 16) rows at row pack_off[b] of
   // one long tensor.  Tiles that overrun the slate read other slates' rows: as keys they are masked, as queries their
-  // probabilities are forced to zero below (their d ctx rows are NOT zero, unlike the dense layout's padding); outputs
-  // are stored in 16-row boxes that stop at the slate's last packed row, and nothing is zero-filled.
+  // probabilities are forced to zero (their statistics are -inf); outputs are stored in 16-row boxes that stop at the
+  // slate's last packed row, and nothing is zero-filled.
   const int n_full = (S + 127) / 128;
   const float c_log2e = scale * 1.4426950408889634f;
   const bool packed = pack_off != nullptr;
-  const BwdWalk walk{n_items, int(gridDim.x), n_heads, S, extent, pack_off};
 
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmQk); ptx::prefetch_tmap(&tmQm); ptx::prefetch_tmap(&tmKk); ptx::prefetch_tmap(&tmKm);
-    ptx::prefetch_tmap(&tmVk); ptx::prefetch_tmap(&tmDOk); ptx::prefetch_tmap(&tmDOm);
-    ptx::mbar_init(kv_bar, 1);
-    ptx::mbar_init(q_bar, 1);
-    ptx::mbar_init(s_bar, 1);
-    ptx::mbar_init(s_bar + 1, 1);
-    ptx::mbar_init(p_bar, BWD_COMPUTE);
-    ptx::mbar_init(p_bar + 1, BWD_COMPUTE);
-    ptx::mbar_init(mma_bar, 1);
-    ptx::mbar_init(qm_bar, 1);
-    ptx::mbar_init(km_bar, 1);
+  if (threadIdx.x == 0) {
+    ptx::prefetch_tmap(&tmQ); ptx::prefetch_tmap(&tmK); ptx::prefetch_tmap(&tmV); ptx::prefetch_tmap(&tmDO);
+    ptx::mbar_init(load_bar, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
+  if (dbias_qkv != nullptr)
+    for (int i = threadIdx.x; i < 3 * d_model; i += BWD_THREADS) bias_acc[i] = 0.f;
   arb_pdl_wait();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t T_ST = tmem_base, T_DPT = tmem_base + 128, T_DV = tmem_base + 256, T_DK = tmem_base + 320;
-  const uint32_t T_DQ0 = tmem_base + 384;   // + 64 * qc
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      BwdIter c;
-      c.item = blockIdx.x;
-      bool ok = walk.seek(c);
-      for (uint32_t g = 0; ok; ++g, ok = walk.next(c)) {
-        const int bc = packed ? 0 : c.b;
-        // The K-major tiles are read only by the S^T / dP^T MMAs, so they can be refilled as soon as the previous
-        // iteration's second half of S^T / dP^T has completed -- i.e. while its compute phases and trailing MMAs run.
-        if (g > 0) ptx::mbar_wait(s_bar + 1, (g - 1) & 1);
-        ptx::mbar_expect_tx(q_bar, 2 * TILE_BYTES);
-        ptx::tma_load_4d(tile(BwdSmem::Q_KM), &tmQk, q_bar, 0, c.row_base + 128 * c.qc, c.head, bc);
-        ptx::tma_load_4d(tile(BwdSmem::DO_KM), &tmDOk, q_bar, 0, c.row_base + 128 * c.qc, c.head, bc);
-        if (c.qc == 0) {
-          ptx::mbar_expect_tx(kv_bar, 2 * TILE_BYTES);
-          ptx::tma_load_4d(tile(BwdSmem::K_KM), &tmKk, kv_bar, 0, c.row_base + 128 * c.jt, c.head, bc);
-          ptx::tma_load_4d(tile(BwdSmem::V_KM), &tmVk, kv_bar, 0, c.row_base + 128 * c.jt, c.head, bc);
-        }
-        // the MN-major tiles are still in use by the trailing MMAs (dV, dK, dQ) of the previous iteration
-        if (g > 0) ptx::mbar_wait(mma_bar, (g - 1) & 1);
-        ptx::mbar_expect_tx(qm_bar, 2 * TILE_BYTES);
-        ptx::tma_load_4d(tile(BwdSmem::Q_MN), &tmQm, qm_bar, 0, c.row_base + 128 * c.qc, c.head, bc);
-        ptx::tma_load_4d(tile(BwdSmem::DO_MN), &tmDOm, qm_bar, 0, c.row_base + 128 * c.qc, c.head, bc);
-        if (c.qc == 0) {
-          ptx::mbar_expect_tx(km_bar, TILE_BYTES);
-          ptx::tma_load_4d(tile(BwdSmem::K_MN), &tmKm, km_bar, 0, c.row_base + 128 * c.jt, c.head, bc);
-        }
+  // one operand word: element (r, e) of a [256][32] operand (two 128-row boxes)
+  auto op = [&](const uint8_t* base, int r, int e) -> uint32_t {
+    const float x = ptx::ld_f32(base + (r >> 7) * TILE_BYTES, r & 127, e);
+    return rnd ? ptx::cvt_tf32(x) : __float_as_uint(x);
+  };
+  auto key_live = [&](int key) { return (key_bits[key >> 5] >> (key & 31)) & 1u; };
+  // stage rows r, r + 8 (tile-relative) of an accumulator [KS][4] (x mul) into output tile `which`
+  auto stage_rows = [&](int which, int r, const float (&acc)[KS][4], float mul) {
+    uint8_t* ot = out_tile(which);
+#pragma unroll
+    for (int nt = 0; nt < KS; ++nt) {
+      const int e = 8 * nt + 2 * t;
+      if constexpr (OUT16) {
+        // bf16 mode: dQ / dK / dV only feed the QKV weight- and input-gradient products: dense bfloat16 rows of
+        // 32 columns (64 bytes), unswizzled tensor maps
+        *reinterpret_cast<uint32_t*>(ot + r * 64 + 2 * e) = ptx::pack_bf16(acc[nt][0] * mul, acc[nt][1] * mul);
+        *reinterpret_cast<uint32_t*>(ot + (r + 8) * 64 + 2 * e) = ptx::pack_bf16(acc[nt][2] * mul, acc[nt][3] * mul);
+      } else {
+        *reinterpret_cast<float2*>(ot + ptx::sw128(r, 4 * e)) = make_float2(acc[nt][0] * mul, acc[nt][1] * mul);
+        *reinterpret_cast<float2*>(ot + ptx::sw128(r + 8, 4 * e)) = make_float2(acc[nt][2] * mul, acc[nt][3] * mul);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr int KSTEPS = (DK + 7) / 8;                 // contraction steps over the head width
-      constexpr int DKN = DK < 16 ? 16 : DK;               // UMMA N of the dk-wide outputs
-      const uint32_t id_ts = ptx::idesc_tf32(128, DKN, 0, 1);     // A from TMEM, B MN-major
-      const uint32_t id_dq = ptx::idesc_tf32(128, DKN, 1, 1);     // A MN-major (staged dS^T), B MN-major
-      const uint32_t kk = ptx::smem_u32(tile(BwdSmem::K_KM)), km = ptx::smem_u32(tile(BwdSmem::K_MN));
-      const uint32_t vk = ptx::smem_u32(tile(BwdSmem::V_KM));
-      const uint32_t qk = ptx::smem_u32(tile(BwdSmem::Q_KM)), qm = ptx::smem_u32(tile(BwdSmem::Q_MN));
-      const uint32_t dok = ptx::smem_u32(tile(BwdSmem::DO_KM)), dom = ptx::smem_u32(tile(BwdSmem::DO_MN));
-      const uint32_t sg = ptx::smem_u32(stage);
-      const uint32_t id_sh = ptx::idesc_tf32(128, 64, 0, 0);      // one 64-query half of S^T / dP^T
-      // Descriptors are built once; the k-steps of a family differ only by the start-address field (units of 16 B):
-      // +2 per 32-byte k-step of a K-major tile, +64 per 1024-byte k-step of an MN-major tile, +512 for rows 64..127.
-      const uint64_t d_kk = ptx::smem_desc_sw128<2>(kk, 16, 1024), d_vk = ptx::smem_desc_sw128<2>(vk, 16, 1024);
-      const uint64_t d_qk = ptx::smem_desc_sw128<2>(qk, 16, 1024), d_dok = ptx::smem_desc_sw128<2>(dok, 16, 1024);
-      const uint64_t d_dom = ptx::smem_desc_sw128<1>(dom, TILE_BYTES, 512), d_qm = ptx::smem_desc_sw128<1>(qm, TILE_BYTES, 512);
-      const uint64_t d_sg = ptx::smem_desc_sw128<1>(sg, TILE_BYTES, 512), d_km = ptx::smem_desc_sw128<1>(km, TILE_BYTES, 512);
-      uint32_t kv_seen = 0, km_seen = 0;      // key tiles of the stream whose K-major / MN-major loads were awaited
-      // S^T / dP^T of half `hf` of stream iteration `t` (queries 64*hf.. of the chunk: rows 64*hf.. of the K-major Q /
-      // dO tiles); the two independent accumulators are interleaved so that consecutive MMAs never depend on each other
-      auto issue_scores = [&](const BwdIter& x, uint32_t t, int hf) {
-        if (hf == 0) {
-          if (x.qc == 0) { ptx::mbar_wait(kv_bar, kv_seen & 1); ++kv_seen; }
-          ptx::mbar_wait(q_bar, t & 1);
-          ptx::tc_fence_after();
+  };
+  // store output tiles [first, last] (staged by every warp) at tile row `tile` of item (b, head) and add their column
+  // sums to the QKV bias gradient; returns with the staging free again
+  auto flush = [&](int first, int last, int tile, int b, int head, int row_base, int ext16) {
+    ptx::fence_proxy_async_smem();
+    __syncthreads();
+    const CUtensorMap* maps[3] = {&tmDV, &tmDK, &tmDQ};
+    if (threadIdx.x == 0) {
+      for (int w = first; w <= last; ++w) {
+        if (packed) {      // 16-row boxes up to the slate's last packed row (staged rows are 128 / 64 bytes wide)
+          constexpr int BOX = OUT16 ? 1024 : 2048;
+          const int n16 = (min(128, ext16 - 128 * tile) + 15) >> 4;
+          for (int i = 0; i < n16; ++i) ptx::tma_store_4d(maps[w], out_tile(w) + i * BOX, 0, row_base + 128 * tile + 16 * i, head, 0);
+        } else {
+          ptx::tma_store_4d(maps[w], out_tile(w), 0, 128 * tile, head, b);
         }
-        const uint64_t hoff = uint64_t(hf) * 512;
-        if (hf == 0 || x.half_b_live()) {       // (a dead half b: no products, the barrier phase still advances)
-#pragma unroll
-          for (int k = 0; k < KSTEPS; ++k) {
-            ptx::mma_tf32_ss(T_ST + 64 * hf, d_kk + 2 * k, d_qk + hoff + 2 * k, id_sh, k > 0);
-            ptx::mma_tf32_ss(T_DPT + 64 * hf, d_vk + 2 * k, d_dok + hoff + 2 * k, id_sh, k > 0);
-          }
-        }
-        ptx::mma_commit(s_bar + hf);
-      };
-      BwdIter c, n;
-      c.item = blockIdx.x;
-      bool ok = walk.seek(c);
-      if (ok) {
-        issue_scores(c, 0, 0);
-        issue_scores(c, 0, 1);
       }
-      n = c;
-      bool has_n = ok && walk.next(n);
-      for (uint32_t g = 0; ok; ++g) {
-        const uint32_t acc_kv = c.qc > 0 ? 1u : 0u, acc_q = c.jt > 0 ? 1u : 0u;
-        // ---- half a: dV / dK over its 64 queries, then the next iteration's half-a scores into the freed columns
-        ptx::mbar_wait(p_bar, g & 1);
-        ptx::mbar_wait(qm_bar, g & 1);
-        ptx::tc_fence_after();
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          ptx::mma_tf32_ts(T_DV, T_ST + 8 * i, d_dom + 64 * i, id_ts, i > 0 ? 1u : acc_kv);
-          ptx::mma_tf32_ts(T_DK, T_DPT + 8 * i, d_qm + 64 * i, id_ts, i > 0 ? 1u : acc_kv);
+      ptx::tma_store_commit();
+    }
+    if (dbias_qkv != nullptr) {
+      // bias gradient of the QKV projection: column sums of the staged tiles (rows the slate does not have are 0), added
+      // to the CTA's accumulator -- one thread per (tile, column), flushes ordered by the barriers around them
+      const int which = first + int(threadIdx.x) / DK, cc = int(threadIdx.x) % DK;
+      if (which <= last) {
+        const uint8_t* tl = out_tile(which);
+        float s = 0.f;
+#pragma unroll 8
+        for (int r = 0; r < 128; ++r) {
+          if constexpr (OUT16) s += __uint_as_float(uint32_t(*reinterpret_cast<const uint16_t*>(tl + r * 64 + cc * 2)) << 16);
+          else s += *reinterpret_cast<const float*>(tl + ptx::sw128(r, 4 * cc));
         }
-        if (has_n) issue_scores(n, g + 1, 0);
-        // ---- half b: dV / dK, the next half-b scores, and dQ (contracts over all 128 keys: both halves staged)
-        ptx::mbar_wait(p_bar + 1, g & 1);
-        ptx::tc_fence_after();
-        if (c.half_b_live()) {
-#pragma unroll
-          for (int i = 8; i < 16; ++i) {
-            ptx::mma_tf32_ts(T_DV, T_ST + 8 * i, d_dom + 64 * i, id_ts, 1u);
-            ptx::mma_tf32_ts(T_DK, T_DPT + 8 * i, d_qm + 64 * i, id_ts, 1u);
-          }
-        }
-        if (has_n) issue_scores(n, g + 1, 1);
-        if (c.qc == 0) { ptx::mbar_wait(km_bar, km_seen & 1); ++km_seen; }
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          ptx::mma_tf32_ss(T_DQ0 + 64 * c.qc, d_sg + 64 * i, d_km + 64 * i, id_dq, i > 0 ? 1u : acc_q);
-        ptx::mma_commit(mma_bar);
-        c = n;
-        ok = has_n;
-        if (ok) has_n = walk.next(n);
+        bias_acc[(which == 0 ? 2 * d_model : (which == 1 ? d_model : 0)) + head * DK + cc] += s;
       }
     }
-  } else {
-    // ===================== compute + epilogue (512 threads) =====================
-    const int ct = threadIdx.x - 64;            // 0..511
-    const int quad = warp & 3;
-    const int row = 32 * quad + lane;           // key row inside the tile == TMEM lane
-    const int sub = (warp - 2) >> 2;            // which 16 of the 64 query columns of a half this warp handles
-    const uint32_t lane_addr = uint32_t(32 * quad) << 16;
+    if (threadIdx.x == 0) ptx::tma_store_wait_read();
+    __syncthreads();
+  };
 
-    // per-query statistics of an iteration's chunk -> smem buffer `buf` (nm = -max*c - log2(sum); -inf for queries the
-    // slate does not have)
-    auto load_stats = [&](const BwdIter& x, int buf, int slot) {
-      const int qi = 128 * x.qc + slot;
+  uint32_t phase = 0;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int b = item / n_heads, head = item - b * n_heads;
+    int e = extent ? __ldg(extent + b) : S;
+    if (packed && e <= 0) continue;               // packed rows: an empty slate holds no rows
+    e = max(1, min(S, e));
+    const int n_kt = (e + 127) / 128;             // active key tiles == active query tiles
+    const int ext16 = (e + 15) & ~15;
+    const int q_lim = packed ? min(S, ext16) : S; // queries at or beyond it do not exist in this slate
+    // queries at or beyond q_live contribute nothing (the dense layout's padding has zero d ctx rows; packed rows: the
+    // slate has no such queries)
+    const int q_live = packed ? q_lim : (extent ? e : S);
+    const int row_base = packed ? __ldg(pack_off + b) : 0;
+    const int bc = packed ? 0 : b;
+    if (threadIdx.x == 0) {
+      ptx::fence_proxy_async_smem();
+      ptx::mbar_expect_tx(load_bar, 4 * n_kt * TILE_BYTES);
+      for (int kt = 0; kt < n_kt; ++kt) {
+        const int r = row_base + 128 * kt;
+        ptx::tma_load_4d(q_s + kt * TILE_BYTES, &tmQ, load_bar, 0, r, head, bc);
+        ptx::tma_load_4d(k_s + kt * TILE_BYTES, &tmK, load_bar, 0, r, head, bc);
+        ptx::tma_load_4d(v_s + kt * TILE_BYTES, &tmV, load_bar, 0, r, head, bc);
+        ptx::tma_load_4d(do_s + kt * TILE_BYTES, &tmDO, load_bar, 0, r, head, bc);
+      }
+    }
+    {
+      // per-query statistics (nm = -max*c - log2(sum); -inf for queries the slate does not have) and the key mask
+      const int qi = threadIdx.x;
       float2 st = make_float2(-CUDART_INF_F, 0.f);
-      if (qi < x.q_lim) {
-        const size_t so = (size_t(x.b) * n_heads + x.head) * S + qi;
+      if (qi < q_lim) {
+        const size_t so = (size_t(b) * n_heads + head) * S + qi;
         st.x = -(stat_max[so] * c_log2e) - log2f(stat_sum[so]);
         st.y = delta[so];
       }
-      qstats[buf * 128 + slot] = st;
-    };
-    // dense layout: zero rows of the skipped tiles of item x -- one zero slab, TMA-stored over every skipped dQ / dK /
-    // dV tile (TMA clips at S).  The staging area must be idle (start of the stream, or right after an epilogue).
-    auto zero_fill = [&](const BwdIter& x) {
-      for (int i = ct; i < TILE_BYTES / 16; i += BWD_COMPUTE) reinterpret_cast<uint4*>(stage)[i] = make_uint4(0u, 0u, 0u, 0u);
+      qstats[qi] = st;
+      const uint32_t w = __ballot_sync(FULL, qi < S && mask[size_t(b) * S + qi] == 0);
+      if (lane == 0) key_bits[warp] = w;
+    }
+    if (!packed && n_kt < n_full) {
+      // dense layout: zero rows of the skipped tiles -- one zero tile, TMA-stored over every skipped dQ / dK / dV tile
+      // (TMA clips at S)
+      for (int i = threadIdx.x; i < TILE_BYTES / 16; i += BWD_THREADS) reinterpret_cast<uint4*>(out_tile(0))[i] = make_uint4(0u, 0u, 0u, 0u);
       ptx::fence_proxy_async_smem();
-      ptx::named_bar_sync(1, BWD_COMPUTE);
-      if (ct == 0) {
-        for (int jt = x.n_kt; jt < n_full; ++jt) {
-          ptx::tma_store_4d(&tmDQ, stage, 0, 128 * jt, x.head, x.b);
-          ptx::tma_store_4d(&tmDK, stage, 0, 128 * jt, x.head, x.b);
-          ptx::tma_store_4d(&tmDV, stage, 0, 128 * jt, x.head, x.b);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        for (int jt = n_kt; jt < n_full; ++jt) {
+          ptx::tma_store_4d(&tmDQ, out_tile(0), 0, 128 * jt, head, b);
+          ptx::tma_store_4d(&tmDK, out_tile(0), 0, 128 * jt, head, b);
+          ptx::tma_store_4d(&tmDV, out_tile(0), 0, 128 * jt, head, b);
         }
         ptx::tma_store_commit();
         ptx::tma_store_wait_read();
       }
-      ptx::named_bar_sync(1, BWD_COMPUTE);
-    };
-
-    bool outputs_pending = false;      // an epilogue's stores / column sums may still be reading the output tiles
-    auto out_tile = [&](int which) { return which < 2 ? stage + (2 + which) * TILE_BYTES : smem + BwdSmem::OUT_OFF; };
-    // Outputs of iteration `e` that became final with it: dV / dK of its key tile after the last query chunk, dQ of
-    // its query chunk after the last key tile.  TMEM -> swizzled staging -> TMA store (+ the QKV bias column sums).
-    auto epilogue = [&](const BwdIter& e) {
-      const int e_jt = e.jt, e_qc = e.qc;
-      const bool last_qc = (e_qc == e.n_kt - 1), last_jt = (e_jt == e.n_kt - 1);
-      if (!(last_qc || last_jt)) return;
-      // up to 3 output tiles of DK <= 32 columns, one per warp group: sub 0 -> dV, sub 1 -> dK, sub 2 -> dQ
-      if (sub < 3 && ((sub < 2) ? last_qc : last_jt)) {
-        const uint32_t src = sub == 0 ? T_DV : (sub == 1 ? T_DK : T_DQ0 + 64 * e_qc);
-        const float mul = sub == 0 ? 1.0f : scale;
-        uint32_t v[32];
-        ptx::tmem_ld_32x32(src + lane_addr, v);
-        ptx::tmem_ld_wait();
-        if constexpr (OUT16) {
-          // bf16 mode: dQ / dK / dV only feed the QKV weight- and input-gradient products: dense bfloat16 rows of
-          // 32 columns (64 bytes), unswizzled tensor maps
-          uint4* orow = reinterpret_cast<uint4*>(out_tile(sub) + row * 64);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            uint4 pk;
-            pk.x = ptx::pack_bf16(__uint_as_float(v[8 * k + 0]) * mul, __uint_as_float(v[8 * k + 1]) * mul);
-            pk.y = ptx::pack_bf16(__uint_as_float(v[8 * k + 2]) * mul, __uint_as_float(v[8 * k + 3]) * mul);
-            pk.z = ptx::pack_bf16(__uint_as_float(v[8 * k + 4]) * mul, __uint_as_float(v[8 * k + 5]) * mul);
-            pk.w = ptx::pack_bf16(__uint_as_float(v[8 * k + 6]) * mul, __uint_as_float(v[8 * k + 7]) * mul);
-            orow[k] = pk;
-          }
-        } else {
-          uint8_t* orow = out_tile(sub) + row * 128;
-#pragma unroll
-          for (int piece = 0; piece < 8; ++piece) {
-            float4 o;
-            o.x = __uint_as_float(v[piece * 4 + 0]) * mul;
-            o.y = __uint_as_float(v[piece * 4 + 1]) * mul;
-            o.z = __uint_as_float(v[piece * 4 + 2]) * mul;
-            o.w = __uint_as_float(v[piece * 4 + 3]) * mul;
-            *reinterpret_cast<float4*>(orow + ((piece ^ (row & 7)) << 4)) = o;
-          }
-        }
-      }
-      ptx::fence_proxy_async_smem();
-      ptx::tc_fence_before();
-      ptx::named_bar_sync(1, BWD_COMPUTE);
-      if (ct == 0) {
-        if (packed) {      // 16-row boxes up to the slate's last packed row (staged rows are 128 / 64 bytes wide)
-          constexpr int BOX = OUT16 ? 1024 : 2048;
-          if (last_qc) {
-            const int n16 = (min(128, e.ext16 - 128 * e_jt) + 15) >> 4;
-            for (int i = 0; i < n16; ++i) {
-              ptx::tma_store_4d(&tmDV, out_tile(0) + i * BOX, 0, e.row_base + 128 * e_jt + 16 * i, e.head, 0);
-              ptx::tma_store_4d(&tmDK, out_tile(1) + i * BOX, 0, e.row_base + 128 * e_jt + 16 * i, e.head, 0);
-            }
-          }
-          if (last_jt) {
-            const int n16 = (min(128, e.ext16 - 128 * e_qc) + 15) >> 4;
-            for (int i = 0; i < n16; ++i)
-              ptx::tma_store_4d(&tmDQ, out_tile(2) + i * BOX, 0, e.row_base + 128 * e_qc + 16 * i, e.head, 0);
-          }
-        } else {
-          if (last_qc) {
-            ptx::tma_store_4d(&tmDV, out_tile(0), 0, 128 * e_jt, e.head, e.b);
-            ptx::tma_store_4d(&tmDK, out_tile(1), 0, 128 * e_jt, e.head, e.b);
-          }
-          if (last_jt) ptx::tma_store_4d(&tmDQ, out_tile(2), 0, 128 * e_qc, e.head, e.b);
-        }
-        ptx::tma_store_commit();
-      }
-      if (dbias_qkv != nullptr && ct < 384) {
-        // bias gradient of the QKV projection: column sums of the staged dV / dK / dQ tiles (rows the slate does not
-        // have are 0); 96 columns x 4 row segments, the 4 partial sums sit in adjacent lanes
-        const int col = ct >> 2, seg = ct & 3;
-        const int which = col >> 5, cc = col & 31;
-        const bool live = ((which < 2) ? last_qc : last_jt) && cc < DK;
-        float t = 0.f;
-        if (live) {
-          const uint8_t* tl = out_tile(which);
-#pragma unroll 8
-          for (int r = 32 * seg; r < 32 * seg + 32; ++r) {
-            if constexpr (OUT16) t += __uint_as_float(uint32_t(*reinterpret_cast<const uint16_t*>(tl + r * 64 + cc * 2)) << 16);
-            else t += *reinterpret_cast<const float*>(tl + r * 128 + ((((cc >> 2) ^ (r & 7)) << 4) | ((cc & 3) << 2)));
-          }
-        }
-        t += __shfl_xor_sync(FULL, t, 1);
-        t += __shfl_xor_sync(FULL, t, 2);
-        if (live && seg == 0)
-          atomicAdd(dbias_qkv + (which == 0 ? 2 * d_model : (which == 1 ? d_model : 0)) + e.head * DK + cc, t);
-      }
-      // The stores drain behind the half-a staging (slabs 0 / 1) and arithmetic that follow; drain_outputs() is called
-      // before anything writes slabs 2 / 3 or the dQ tile again.
-      outputs_pending = true;
-    };
-    // the output tiles may be rewritten: the TMA stores have read them, every thread has finished its column sums
-    auto drain_outputs = [&]() {
-      if (!outputs_pending) return;
-      if (ct == 0) ptx::tma_store_wait_read();
-      ptx::named_bar_sync(1, BWD_COMPUTE);
-      outputs_pending = false;
-    };
-
-    BwdIter c, n, prev;
-    c.item = blockIdx.x;
-    bool ok = walk.seek(c);
-    if (ok) {
-      if (!packed && c.n_kt < n_full) zero_fill(c);
-      if (ct < 128) load_stats(c, 0, ct);
     }
-    n = c;
-    prev = c;
-    bool has_n = ok && walk.next(n);
-    // is this thread's key of x's key tile a real key?  (fetched one iteration ahead: the load would otherwise sit at
-    // the head of every item's first iteration)
-    auto key_live = [&](const BwdIter& x) {
-      const int key = 128 * x.jt + row;
-      return key < S && mask[size_t(x.b) * S + key] == 0;
-    };
-    bool key_ok = ok && key_live(c), key_ok_n = false;
-    uint32_t g = 0;
-    for (; ok; ++g) {
-      ptx::named_bar_sync(1, BWD_COMPUTE);     // this chunk's statistics are in place; iteration g-1 is fully read
-      if (has_n && ct >= 128 && ct < 256) load_stats(n, (g + 1) & 1, ct - 128);   // prefetch behind the arithmetic
-      if (has_n && n.qc == 0) key_ok_n = key_live(n);    // the next iteration opens a new key tile
-      const float2* qs = qstats + (g & 1) * 128;
-#pragma unroll 1
-      for (int hf = 0; hf < 2; ++hf) {
-        ptx::mbar_wait(s_bar + hf, g & 1);
-        ptx::tc_fence_after();
-        const int col0 = 64 * hf + 16 * sub;            // first query column of this warp's 16-wide piece
-        if (hf == 1 && !c.half_b_live()) {
-          // none of these 64 queries contributes: their dS^T columns are staged as zeros for the dQ product (its rows
-          // for them are then exactly zero) and the dV / dK products of the half are not issued
-          drain_outputs();
-          uint8_t* zrow = stage + (col0 >> 5) * TILE_BYTES + row * 128;
-          const int z0 = (col0 & 31) >> 2;
+    __syncthreads();
+    ptx::mbar_wait(load_bar, phase & 1);
+    ++phase;
+
+    const unsigned long long dbase = (unsigned long long)(b * n_heads + head) * S;
+    // ===== phase 1: dV, dK of each key tile (this warp: keys kA, kA + 8 of its 16)
+    const int nq8 = (min(q_live, 128 * n_kt) + 7) & ~7;
+    for (int jt = 0; jt < n_kt; ++jt) {
+      const int kA = 128 * jt + 16 * warp + g, kB = kA + 8;
+      const bool liveA = key_live(kA), liveB = key_live(kB);
+      uint32_t ka[KS][4], va[KS][4];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int piece = z0 + k;
-            const int phys = (((piece >> 1) ^ (row & 3)) << 5) + ((piece & 1) << 4);
-            *reinterpret_cast<uint4*>(zrow + phys) = make_uint4(0u, 0u, 0u, 0u);
-          }
-          ptx::fence_proxy_async_smem();
-          ptx::tc_fence_before();
-          ptx::mbar_arrive(p_bar + hf);
-          continue;
+      for (int ks = 0; ks < KS; ++ks) {
+        const int e0 = 8 * ks + t;
+        ka[ks][0] = op(k_s, kA, e0); ka[ks][1] = op(k_s, kB, e0); ka[ks][2] = op(k_s, kA, e0 + 4); ka[ks][3] = op(k_s, kB, e0 + 4);
+        va[ks][0] = op(v_s, kA, e0); va[ks][1] = op(v_s, kB, e0); va[ks][2] = op(v_s, kA, e0 + 4); va[ks][3] = op(v_s, kB, e0 + 4);
+      }
+      float dv[KS][4], dk[KS][4];
+#pragma unroll
+      for (int nt = 0; nt < KS; ++nt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dv[nt][i] = dk[nt][i] = 0.f;
+      for (int q0 = 0; q0 < nq8; q0 += 8) {
+        float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          const uint32_t qb[2] = {op(q_s, q0 + g, 8 * ks + t), op(q_s, q0 + g, 8 * ks + t + 4)};
+          const uint32_t ob[2] = {op(do_s, q0 + g, 8 * ks + t), op(do_s, q0 + g, 8 * ks + t + 4)};
+          ptx::mma_tf32(s, ka[ks], qb);
+          ptx::mma_tf32(dp, va[ks], ob);
         }
-        uint32_t sv[16], dv[16];
-        ptx::tmem_ld_32x16(T_ST + lane_addr + col0, sv);
-        ptx::tmem_ld_32x16(T_DPT + lane_addr + col0, dv);
-        ptx::tmem_ld_wait();
+        float pu[4], ds[4];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float2 st = qs[col0 + j];
-          const float p = key_ok ? ex2_approx_b(fmaf(__uint_as_float(sv[j]), c_log2e, st.x)) : 0.0f;
-          float p_used = p, dp = __uint_as_float(dv[j]);
+        for (int i = 0; i < 4; ++i) {
+          const int q = q0 + 2 * t + (i & 1);
+          const float2 st = qstats[q];
+          const float p = (i < 2 ? liveA : liveB) ? ex2_approx_b(fmaf(s[i], c_log2e, st.x)) : 0.0f;
+          float p_used = p, dpv = dp[i];
           if constexpr (DROP) {        // regenerate the forward's dropout mask on the probabilities
-            const unsigned long long idx =
-                ((unsigned long long)(c.b * n_heads + c.head) * S + (128 * c.qc + col0 + j)) * (unsigned long long)S +
-                (128 * c.jt + row);
+            const unsigned long long idx = (dbase + q) * (unsigned long long)S + (i < 2 ? kA : kB);
             const float m = drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
             p_used = p * m;
-            dp *= m;
+            dpv *= m;
           }
-          const float ds = p * (dp - st.y);
-          sv[j] = round_tf32_b(p_used);
-          dv[j] = round_tf32_b(ds);
+          pu[i] = round_tf32_b(p_used);
+          ds[i] = round_tf32_b(p * (dpv - st.y));
         }
-        ptx::tmem_st_32x16(T_ST + lane_addr + col0, sv);
-        ptx::tmem_st_32x16(T_DPT + lane_addr + col0, dv);
-        if (hf == 0 && g > 0) {
-          // The staging slabs still feed the previous iteration's dQ product (and hold its output tiles): wait for
-          // its trailing MMAs -- they ran behind this half's arithmetic -- and flush what became final.
-          ptx::mbar_wait(mma_bar, (g - 1) & 1);
-          ptx::tc_fence_after();
-          epilogue(prev);
-          if (!packed && c.jt == 0 && c.qc == 0 && c.n_kt < n_full) { drain_outputs(); zero_fill(c); }   // a new item's skipped tiles
-        }
-        if (hf == 1) drain_outputs();      // this half stages into slabs 2 / 3
-        // dS^T also goes to shared memory as the MN-major A operand of dQ: slab = 32-query group, row = key
-        uint8_t* srow = stage + (col0 >> 5) * TILE_BYTES + row * 128;
-        const int p0 = (col0 & 31) >> 2;                // first 16-byte piece of these 16 columns in the slab row
+        uint32_t pa[4], dsa[4];
+        ptx::acc_to_a_tf32(pu, pa, lane);
+        ptx::acc_to_a_tf32(ds, dsa, lane);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int piece = p0 + k;
-          const int phys = (((piece >> 1) ^ (row & 3)) << 5) + ((piece & 1) << 4);
-          *reinterpret_cast<uint4*>(srow + phys) = make_uint4(dv[k * 4], dv[k * 4 + 1], dv[k * 4 + 2], dv[k * 4 + 3]);
+        for (int nt = 0; nt < KS; ++nt) {
+          const uint32_t ob[2] = {op(do_s, q0 + t, 8 * nt + g), op(do_s, q0 + t + 4, 8 * nt + g)};
+          const uint32_t qb[2] = {op(q_s, q0 + t, 8 * nt + g), op(q_s, q0 + t + 4, 8 * nt + g)};
+          ptx::mma_tf32(dv[nt], pa, ob);
+          ptx::mma_tf32(dk[nt], dsa, qb);
         }
-        ptx::tmem_st_wait();
-        ptx::fence_proxy_async_smem();
-        ptx::tc_fence_before();
-        ptx::mbar_arrive(p_bar + hf);
       }
-      prev = c;
-      c = n;
-      ok = has_n;
-      if (ok && c.qc == 0) key_ok = key_ok_n;
-      if (ok) has_n = walk.next(n);
+      stage_rows(0, 16 * warp + g, dv, 1.0f);
+      stage_rows(1, 16 * warp + g, dk, scale);
+      flush(0, 1, jt, b, head, row_base, ext16);
     }
-    if (g > 0) {
-      ptx::mbar_wait(mma_bar, (g - 1) & 1);
-      ptx::tc_fence_after();
-      epilogue(prev);
-      ptx::tc_fence_before();
+    // ===== phase 2: dQ of each query tile (this warp: queries qA, qA + 8 of its 16)
+    const int nk8 = (e + 7) & ~7;          // keys at or beyond the extent are masked
+    for (int qc = 0; qc < n_kt; ++qc) {
+      const int qA = 128 * qc + 16 * warp + g, qB = qA + 8;
+      const float2 stA = qstats[qA], stB = qstats[qB];
+      uint32_t qa[KS][4], oa[KS][4];
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks) {
+        const int e0 = 8 * ks + t;
+        qa[ks][0] = op(q_s, qA, e0); qa[ks][1] = op(q_s, qB, e0); qa[ks][2] = op(q_s, qA, e0 + 4); qa[ks][3] = op(q_s, qB, e0 + 4);
+        oa[ks][0] = op(do_s, qA, e0); oa[ks][1] = op(do_s, qB, e0); oa[ks][2] = op(do_s, qA, e0 + 4); oa[ks][3] = op(do_s, qB, e0 + 4);
+      }
+      float dq[KS][4];
+#pragma unroll
+      for (int nt = 0; nt < KS; ++nt) dq[nt][0] = dq[nt][1] = dq[nt][2] = dq[nt][3] = 0.f;
+      if (128 * qc + 16 * warp < q_live) {
+        for (int k0 = 0; k0 < nk8; k0 += 8) {
+          float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int ks = 0; ks < KS; ++ks) {
+            const uint32_t kb2[2] = {op(k_s, k0 + g, 8 * ks + t), op(k_s, k0 + g, 8 * ks + t + 4)};
+            const uint32_t vb[2] = {op(v_s, k0 + g, 8 * ks + t), op(v_s, k0 + g, 8 * ks + t + 4)};
+            ptx::mma_tf32(s, qa[ks], kb2);
+            ptx::mma_tf32(dp, oa[ks], vb);
+          }
+          float ds[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int key = k0 + 2 * t + (i & 1);
+            const float2 st = i < 2 ? stA : stB;
+            const float p = key_live(key) ? ex2_approx_b(fmaf(s[i], c_log2e, st.x)) : 0.0f;
+            float dpv = dp[i];
+            if constexpr (DROP) {
+              const unsigned long long idx = (dbase + (i < 2 ? qA : qB)) * (unsigned long long)S + key;
+              dpv *= drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
+            }
+            ds[i] = round_tf32_b(p * (dpv - st.y));
+          }
+          uint32_t dsa[4];
+          ptx::acc_to_a_tf32(ds, dsa, lane);
+#pragma unroll
+          for (int nt = 0; nt < KS; ++nt) {
+            const uint32_t kb2[2] = {op(k_s, k0 + t, 8 * nt + g), op(k_s, k0 + t + 4, 8 * nt + g)};
+            ptx::mma_tf32(dq[nt], dsa, kb2);
+          }
+        }
+      }
+      stage_rows(2, 16 * warp + g, dq, scale);
+      flush(2, 2, qc, b, head, row_base, ext16);
     }
-    if (ct == 0) ptx::tma_store_wait_all();
   }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<512>(tmem_base);
+  if (dbias_qkv != nullptr) {
+    // this CTA's slot of the bias gradient (its items in a fixed order; the slots are summed in order by DetParts)
+    __syncthreads();
+    for (int i = threadIdx.x; i < 3 * d_model; i += BWD_THREADS) dbias_qkv[size_t(blockIdx.x) * 3 * d_model + i] = bias_acc[i];
   }
+  if (threadIdx.x == 0) ptx::tma_store_wait_all();
 }
 
 static int g_attn_bwd_persistent = ARB_DEFAULT_ATTN_BWD_PERSISTENT;
@@ -595,24 +387,21 @@ void set_attn_bwd_persistent(int on) { g_attn_bwd_persistent = on; }
 
 template <int DK>
 static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
-  alignas(64) CUtensorMap tQk, tQm, tKk, tKm, tVk, tDOk, tDOm, tDQ, tDK, tDV;
+  alignas(64) CUtensorMap tQ, tK, tV, tDO, tDQ, tDK, tDV;
   int rc;
   const TmapBox box{{32, 128, 1, 1}};
-  if ((rc = make_tmap_4d(&tQk, a.q, box, 0, 1))) return rc;
-  if ((rc = make_tmap_4d(&tQm, a.q, box, 1, 1))) return rc;
-  if ((rc = make_tmap_4d(&tKk, a.k, box, 0, 1))) return rc;
-  if ((rc = make_tmap_4d(&tKm, a.k, box, 1, 1))) return rc;
-  if ((rc = make_tmap_4d(&tVk, a.v, box, 0, 1))) return rc;
-  if ((rc = make_tmap_4d(&tDOk, a.d_o, box, 0, 1))) return rc;
-  if ((rc = make_tmap_4d(&tDOm, a.d_o, box, 1, 1))) return rc;
+  if ((rc = make_tmap_4d(&tQ, a.q, box, 0))) return rc;
+  if ((rc = make_tmap_4d(&tK, a.k, box, 0))) return rc;
+  if ((rc = make_tmap_4d(&tV, a.v, box, 0))) return rc;
+  if ((rc = make_tmap_4d(&tDO, a.d_o, box, 0))) return rc;
   const bool out16 = a.dq.bf16 != 0;
   if ((a.dk_.bf16 != 0) != out16 || (a.dv.bf16 != 0) != out16) { arb_set_error("attn_bwd: dQ, dK, dV must share an element type"); return ARB_E_INVALID_ARG; }
   const bool packed = a.pack_off != nullptr;
   if (packed && !(a.extent && a.rows_dev && a.rowmap)) { arb_set_error("attn_bwd: packed rows need the extents, the row count and the row map"); return ARB_E_INVALID_ARG; }
   const TmapBox obox{{32, packed ? 16u : 128u, 1, 1}};
-  if ((rc = make_tmap_4d(&tDQ, a.dq, obox, out16 ? 2 : 0, 0))) return rc;
-  if ((rc = make_tmap_4d(&tDK, a.dk_, obox, out16 ? 2 : 0, 0))) return rc;
-  if ((rc = make_tmap_4d(&tDV, a.dv, obox, out16 ? 2 : 0, 0))) return rc;
+  if ((rc = make_tmap_4d(&tDQ, a.dq, obox, out16 ? 1 : 0))) return rc;
+  if ((rc = make_tmap_4d(&tDK, a.dk_, obox, out16 ? 1 : 0))) return rc;
+  if ((rc = make_tmap_4d(&tDV, a.dv, obox, out16 ? 1 : 0))) return rc;
   const double rf = packed ? arb_row_frac() : 1.0;
   {
     ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
@@ -625,15 +414,16 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const bool drop = a.drop.thresh != 0;
   auto kern = out16 ? (drop ? attn_bwd_kernel<DK, true, true> : attn_bwd_kernel<DK, false, true>)
                     : (drop ? attn_bwd_kernel<DK, true> : attn_bwd_kernel<DK, false>);
-  static bool configured[ARB_MAX_DEVICES][4] = {};
+  static int configured[ARB_MAX_DEVICES][4] = {};      // dynamic shared memory limit set so far
   const int dev = arb_device_slot();
   const int cslot = (drop ? 1 : 0) + (out16 ? 2 : 0);
-  if (!configured[dev][cslot]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::total()) != cudaSuccess) {
+  const int smem = BwdSmem::total(a.dbias_qkv ? a.d_model : 0);
+  if (configured[dev][cslot] < smem) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       arb_set_error("attn_bwd: cannot raise the dynamic shared memory limit");
       return ARB_E_CUDA;
     }
-    configured[dev][cslot] = true;
+    configured[dev][cslot] = smem;
   }
   // one CTA per (slate, head), or -- persistent (default) -- one per SM walking the items head-fastest
   const int n_items = a.h * a.B;
@@ -641,7 +431,7 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   if (g_attn_bwd_persistent) {
     static int n_sm_of[ARB_MAX_DEVICES] = {};
     if (!n_sm_of[dev]) {
-      int id = 0, n = 148;
+      int id = 0, n = 132;
       cudaGetDevice(&id);
       cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, id);
       n_sm_of[dev] = n;
@@ -649,17 +439,22 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
     n_ctas = std::min(n_items, n_sm_of[dev]);
   }
   dim3 grid(n_ctas);
+  // the QKV bias gradient: one slot per CTA, summed in CTA order afterwards
+  float* dbias = a.dbias_qkv;
+  DetParts dp;
+  dp.add(dbias, n_ctas, 1, 3LL * a.d_model, 3LL * a.d_model);
+  if ((rc = dp.begin(st))) return rc;
   {
     ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 10.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                  rf * 4.0 * double(a.B) * a.h * a.S * (7.0 * a.dk + 3.0), "attn_bwd_kernel");
-    arb_launch(kern, grid, dim3(BWD_THREADS), size_t(BwdSmem::total()), st, tQk, tQm, tKk, tKm, tVk, tDOk, tDOm, tDQ, tDK, tDV, a.mask,
-                                                      a.stat_max, a.stat_sum, a.delta, a.S, a.h, a.scale, a.drop, a.dbias_qkv,
-                                                      a.d_model, a.extent, a.pack_off, n_items);
+    arb_launch(kern, grid, dim3(BWD_THREADS), size_t(smem), st, tQ, tK, tV, tDO, tDQ, tDK, tDV, a.mask,
+               a.stat_max, a.stat_sum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent, a.pack_off,
+               n_items, tf32_round_on_load());
   }
   arb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  return dp.finish(st);
 }
 
 bool attn_fused_bwd_supported(int S, int dk) { return S >= 1 && S <= 256 && (dk == 16 || dk == 32); }

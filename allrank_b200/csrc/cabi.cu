@@ -120,3 +120,113 @@ extern "C" int64_t arb_prof_report(char* buf, int64_t cap) {
   buf[n] = 0;
   return n;
 }
+
+// ------------------------------------------------------------------------------------------------ deterministic reductions
+// Two-level ordered sum over the slots: slot group g = slots 64 g .. 64 g + 63; warp w of a block sums slots
+// 64 g + w, + 8, ... in ascending order, the 8 warp sums are combined in warp order.  One block per (32 elements, group):
+//   n_groups > 1: out[g * elems + e] = group sum   (the next level sums the groups the same way)
+//   n_groups = 1: dst[r * ld + c] += group sum
+// The grouping is fixed by the slot count, so the result does not depend on the grid or on the order blocks run in.
+constexpr long long DET_GROUP = 64;
+__global__ void __launch_bounds__(256) det_reduce_kernel(const float* __restrict__ part, long long n, long long rows,
+                                                         long long cols, long long ld, float* __restrict__ out) {
+  arb_pdl_wait();
+  __shared__ float sh[8][33];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long e = (long long)blockIdx.x * 32 + lane, elems = rows * cols;
+  const long long s0 = (long long)blockIdx.y * DET_GROUP, s1 = min(n, s0 + DET_GROUP);
+  float t = 0.f;
+  if (e < elems)
+    for (long long s = s0 + w; s < s1; s += 8) t += part[s * elems + e];
+  sh[w][lane] = t;
+  __syncthreads();
+  if (w == 0 && e < elems) {
+    float v = sh[0][lane];
+#pragma unroll
+    for (int g = 1; g < 8; ++g) v += sh[g][lane];
+    if (gridDim.y > 1) {
+      out[(long long)blockIdx.y * elems + e] = v;
+    } else {
+      const long long r = e / cols, c = e - r * cols;
+      out[r * ld + c] += v;
+    }
+  }
+}
+
+static long long det_groups(long long n) { return (n + DET_GROUP - 1) / DET_GROUP; }
+
+int DetParts::begin(cudaStream_t st) {
+  if (k == 0) return ARB_OK;
+  stream = st;
+  // slots of every registered array, then two buffers for the intermediate levels of the largest one
+  size_t slots = 0, lvl1 = 0, lvl2 = 0;
+  for (int i = 0; i < k; ++i) {
+    const long long elems = reg[i].rows * reg[i].cols;
+    slots += size_t(reg[i].n * elems);
+    lvl1 = std::max(lvl1, size_t(det_groups(reg[i].n) * elems));
+    lvl2 = std::max(lvl2, size_t(det_groups(det_groups(reg[i].n)) * elems));
+  }
+  static bool pool_set[ARB_MAX_DEVICES] = {};
+  const int dev = arb_device_slot();
+  if (!pool_set[dev]) {
+    // the slots come from the device's stream-ordered pool: keep what it has reserved across synchronisations instead
+    // of returning it to the driver after every step (bounded; nothing stays allocated between calls)
+    int id = 0;
+    cudaGetDevice(&id);
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, id) == cudaSuccess) {
+      uint64_t keep = uint64_t(512) << 20;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+    pool_set[dev] = true;
+  }
+  const size_t total = slots + lvl1 + lvl2;
+  void* p = nullptr;
+  if (cudaMallocAsync(&p, total * sizeof(float), st) != cudaSuccess) {
+    cudaGetLastError();
+    arb_set_error("reduction slots: cudaMallocAsync failed");
+    return ARB_E_CUDA;
+  }
+  base = static_cast<float*>(p);
+  if (cudaMemsetAsync(base, 0, slots * sizeof(float), st) != cudaSuccess) {
+    arb_set_error("reduction slots: memset failed");
+    return ARB_E_CUDA;
+  }
+  float* q = base;
+  for (int i = 0; i < k; ++i) {
+    *reg[i].var = q;
+    q += reg[i].n * reg[i].rows * reg[i].cols;
+  }
+  tmp[0] = q;
+  tmp[1] = q + lvl1;
+  return ARB_OK;
+}
+
+int DetParts::finish(cudaStream_t st) {
+  for (int i = 0; i < k; ++i) {
+    const long long elems = reg[i].rows * reg[i].cols;
+    const float* src = *reg[i].var;
+    long long n = reg[i].n;
+    for (int level = 0;; ++level) {
+      const long long groups = det_groups(n);
+      float* out = groups > 1 ? tmp[level & 1] : reg[i].dst;
+      ProfScope ps(ARB_PROF_SCORER_SIMT, 4.0 * double(n) * double(elems), st, 0.0, "det_reduce_kernel");
+      arb_launch(det_reduce_kernel, dim3(unsigned((elems + 31) / 32), unsigned(groups)), dim3(256), 0, st, src, n,
+                 reg[i].rows, reg[i].cols, reg[i].ld, out);
+      arb_count_launch();
+      if (groups == 1) break;
+      src = out;
+      n = groups;
+    }
+    *reg[i].var = reg[i].dst;
+  }
+  release();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
+  return ARB_OK;
+}
+
+void DetParts::release() {
+  if (base) cudaFreeAsync(base, stream);     // stream-ordered: after every launch above has read the slots
+  base = nullptr;
+}

@@ -29,7 +29,7 @@ bool arb_prof_enabled();
 // The step is a chain of ~50 dependent kernels; at allRank's own batch size (64 slates) every one of them is
 // latency-bound, so the gap between a kernel's last wave and its successor's first instruction matters.  Kernels
 // launched through arb_launch carry cudaLaunchAttributeProgrammaticStreamSerialization (when enabled): the successor
-// may start its prologue (barrier init, TMEM allocation, tensor-map prefetch, smem carve-up) while the predecessor
+// may start its prologue (barrier init, tensor-map prefetch, smem carve-up) while the predecessor
 // drains, and blocks in arb_pdl_wait() -- griddepcontrol.wait -- until the predecessor has completed and flushed its
 // memory.  Every kernel launched this way executes arb_pdl_wait() on every thread before its first access to global
 // memory; without the launch attribute the instruction is a no-op.
@@ -50,6 +50,32 @@ inline cudaError_t arb_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 #endif
+
+// ---- deterministic reductions -------------------------------------------------------------------------------------
+// Gradient reductions across blocks do not use floating-point atomics (their order, and so their rounding, changes from
+// run to run; Adam turns the rounding noise of a mathematically zero gradient into full-size steps).  Instead every
+// block stores its partial result in a slot of its own and dst += sum of the slots in a fixed order afterwards:
+//   DetParts dp;  dp.add(grad, n_slots, rows, cols, ld);  ...;  dp.begin(st);   // grad now points at the zeroed slots
+//   <launch: slot s writes grad[s * rows * cols + r * cols + c]>;  dp.finish(st);
+// The slots are a stream-ordered allocation of this call (cudaMallocAsync / cudaFreeAsync on `st`): calls on different
+// streams or host threads never share them, nothing is synchronised, and under stream capture they become memory
+// nodes owned by the graph.
+struct DetParts {
+  struct Reg { float** var; float* dst; long long n, rows, cols, ld; };
+  Reg reg[6];
+  int k = 0;
+  float* base = nullptr;         // the allocation: slots, then two buffers for the intermediate levels of the sum
+  float* tmp[2] = {nullptr, nullptr};
+  cudaStream_t stream = nullptr;
+  // registers the pointer variable `p` (ignored when null) for n slots of a rows x cols block (dst row pitch ld)
+  void add(float*& p, long long n, long long rows, long long cols, long long ld) {
+    if (p) reg[k++] = Reg{&p, p, n, rows, cols, ld};
+  }
+  int begin(cudaStream_t st);    // 0 or ARB_E_*: slots allocated and zeroed, registered pointers redirected to them
+  int finish(cudaStream_t st);   // 0 or ARB_E_*: dst += slot sums, slots released
+  void release();
+  ~DetParts() { release(); }
+};
 
 // loss = sum(val)/sum(cnt), grad *= 1/sum(cnt); an all-zero count gives loss 0 and zero grad (slate_kernels.cu)
 int arb_finalize_mean_over_count(const float* val, const float* cnt, int B, float* loss, float* grad, size_t n_grad,

@@ -1,16 +1,20 @@
-// Batched TF32 GEMM on the 5th-generation tensor cores:  C[M,N] = epilogue(alpha * A * B^T)
+// Batched TF32 GEMM on the Hopper tensor cores:  C[M,N] = epilogue(alpha * A * B^T)
 //
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a STAGES-deep shared-memory ring,
-//   * tcgen05.mma.kind::tf32 issued by one elected thread, fp32 accumulator tile [128 x BLOCK_N] in TMEM,
-//   * epilogue warps read TMEM (tcgen05.ld 32x32b), apply bias / ReLU / residual / ReLU-mask, stage the tile in
-//     swizzled shared memory and write it with one TMA store per 32-column slab (TMA clips ragged edges, so a
-//     240-row slate or a 136-wide feature matrix needs no masking code),
+//   * four consumer warps, each owning 32 rows of the 128-row tile, run warp-level mma.sync (m16n8k8 tf32 / m16n8k16
+//     bf16) straight out of the swizzled ring and keep the fp32 accumulator in registers,
+//   * the epilogue turns each 32-column chunk of a warp's accumulator into one row per thread (through a small
+//     per-warp transpose buffer), applies bias / ReLU / residual / ReLU-mask, stages the tile in swizzled shared
+//     memory and writes it with one TMA store per 32-column slab (TMA clips ragged edges, so a 240-row slate or a
+//     136-wide feature matrix needs no masking code),
 //   * either operand may be "K-major" (rows of K contiguous, e.g. nn.Linear weights [out,in]) or "MN-major"
-//     (the transpose), which is what the backward GEMMs dX = dY W and dW = dY^T X need,
-//   * split-K with red.global.add for the weight gradients (K = all rows of the batch).
+//     (the transpose), which is what the backward GEMMs dX = dY W and dW = dY^T X need; the fragment loads address
+//     either layout directly, so no transposition pass is needed,
+//   * split-K for the weight gradients (K = all rows of the batch): every split stores its tile into a slot of its own
+//     and the slots are summed in split order (DetParts), so results do not depend on the order splits finish in.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2-5 = epilogue
-// (warp w owns TMEM lanes 32*(w%4) .. +31, i.e. 32 rows of the tile).
+// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = idle, warps 2-5 = MMA + epilogue (warp w owns rows
+// 32*(w%4) .. +31 of the tile).
 //
 // This one kernel is the tensor-core workhorse of the scorer: every nn.Linear forward/backward and the
 // generic (unfused) attention contractions go through it.  Reference ops replaced: aten::addmm / aten::bmm
@@ -23,22 +27,21 @@
 #include "common.h"
 #include "defaults.h"
 #include "gemm_tf32.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace arb {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 32;                    // 32 fp32 = one 128-byte swizzle row
-constexpr int UMMA_K = 8;                      // kind::tf32: 8 elements (32 bytes) per instruction
-// bf16 operands (kind::f16) keep the BYTE geometry: a k-block is still one 128-byte swizzle row (64 bf16), an
-// instruction still consumes 32 bytes of K (16 bf16), so ring stages, K-major descriptors and k-step advances are
-// shared; only MN-major tiles differ (plain SWIZZLE_128B slabs of 64 MN-elements x 64 k-rows instead of tf32's
-// 32-byte-atom slabs of 32 x 32).
+// bf16 operands keep the BYTE geometry: a k-block is still one 128-byte swizzle row (64 bf16), so ring stages and
+// K-major tiles are shared; only MN-major tiles differ (SWIZZLE_128B slabs of 64 MN-elements x 64 k-rows instead of
+// 32 x 32).
 constexpr int BLOCK_K_BF16 = 64;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 4;   // 16 KB
-constexpr int GEMM_EPI_GROUPS = 1;            // epilogue warps per TMEM lane quadrant (2 measured slower: fewer CTAs per SM)
+constexpr int GEMM_EPI_GROUPS = 1;            // consumer warps per 32-row quarter of the tile
 constexpr int GEMM_EPI_THREADS = 128 * GEMM_EPI_GROUPS;
 constexpr int GEMM_THREADS = 64 + GEMM_EPI_THREADS;
+constexpr int XPOSE_BYTES = 32 * 33 * 4;      // per-warp accumulator transpose buffer (32 rows x 32 columns, padded)
 
 struct GemmParams {
   int M, N, K;
@@ -46,9 +49,10 @@ struct GemmParams {
   int a_b2, a_b3, b_b2, b_b3, c_b2, c_b3;
   int flags;
   int kb_per_split;   // k-blocks per split (split-K), or total k-blocks
+  int rnd;            // round fp32 operands to tf32 (nearest) before the MMA; else the tensor core truncates them
   float alpha;
   const float* bias;
-  float* atomic_out;
+  float* atomic_out;     // split-K: the splits' slots [split][M][atomic_ld] (DetParts), summed in order afterwards
   long long atomic_ld;
   DropSite drop;
   float* colsum_out;
@@ -56,12 +60,90 @@ struct GemmParams {
   uint32_t* bits;        // EPI_RELU_BITS / EPI_MASK_BITS: [M, N / 32] words
 };
 
+// ---- MMA main loop ------------------------------------------------------------------------------------------------
+// One 32-bit operand word of a ring stage: an fp32 element (tf32 mode) or the bf16 pair (k, k+1) (k even) of row /
+// column `rc`.  K-major tiles are [rows][128 B]; MN-major tiles are slabs of [k-rows][128 B] (32 fp32 / 64 bf16
+// MN-elements per slab row).
+template <bool MN, bool IN16>
+__device__ __forceinline__ uint32_t op_word(const uint8_t* s, int rc, int k, int rnd) {
+  if constexpr (IN16) {
+    if constexpr (MN) {
+      const uint8_t* slab = s + (rc >> 6) * 8192;
+      const uint32_t lo = *reinterpret_cast<const uint16_t*>(slab + ptx::sw128(k, 2 * (rc & 63)));
+      const uint32_t hi = *reinterpret_cast<const uint16_t*>(slab + ptx::sw128(k + 1, 2 * (rc & 63)));
+      return lo | (hi << 16);
+    } else {
+      return *reinterpret_cast<const uint32_t*>(s + ptx::sw128(rc, 2 * k));
+    }
+  } else {
+    const float x = MN ? ptx::ld_f32(s + (rc >> 5) * 4096, k, rc & 31) : ptx::ld_f32(s, rc, k);
+    return rnd ? ptx::cvt_tf32(x) : __float_as_uint(x);
+  }
+}
+
+// acc[mt][nt] += rows row0 + 16 mt .. of A  x  columns col(nt) .. +7 of B over one k-block of the ring.
+// col(nt) = 32 * (slab0 + slab_step * (nt / 4)) + 8 * (nt % 4): the warp's 32-column slabs of the tile.
+template <int NT, bool A_MN, bool B_MN, bool IN16>
+__device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], const uint8_t* a_s, const uint8_t* b_s, int row0,
+                                                int slab0, int slab_step, int rnd) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    // tf32: k8 steps (k = 8 ks + t, +4); bf16: k16 steps (pairs at k = 16 ks + 2t, +8)
+    const int k0 = IN16 ? 16 * ks + 2 * t : 8 * ks + t;
+    const int kh = IN16 ? 8 : 4;
+    uint32_t a[2][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      const int r = row0 + 16 * mt + g;
+      a[mt][0] = op_word<A_MN, IN16>(a_s, r, k0, rnd);
+      a[mt][1] = op_word<A_MN, IN16>(a_s, r + 8, k0, rnd);
+      a[mt][2] = op_word<A_MN, IN16>(a_s, r, k0 + kh, rnd);
+      a[mt][3] = op_word<A_MN, IN16>(a_s, r + 8, k0 + kh, rnd);
+    }
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      const int n = 32 * (slab0 + slab_step * (nt >> 2)) + 8 * (nt & 3) + g;
+      const uint32_t b[2] = {op_word<B_MN, IN16>(b_s, n, k0, rnd), op_word<B_MN, IN16>(b_s, n, k0 + kh, rnd)};
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        if constexpr (IN16) ptx::mma_bf16(acc[mt][nt], a[mt], b);
+        else ptx::mma_tf32(acc[mt][nt], a[mt], b);
+      }
+    }
+  }
+}
+
+// The 32 accumulator values of chunk `c` (n-tiles 4c .. 4c+3) of row (row0 + lane) of the warp, one row per thread:
+// the fragments go through the warp's transpose buffer `xp`.
+template <int NT>
+__device__ __forceinline__ void acc_chunk_row(const float (&acc)[2][NT][4], int c, float* xp, uint32_t (&v)[32]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  __syncwarp();
+#pragma unroll
+  for (int cc = 0; cc < NT / 4; ++cc) {
+    if (cc != c) continue;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float* r0 = xp + (16 * mt + g) * 33 + 8 * j + 2 * t;
+        r0[0] = acc[mt][4 * cc + j][0];
+        r0[1] = acc[mt][4 * cc + j][1];
+        r0[8 * 33] = acc[mt][4 * cc + j][2];
+        r0[8 * 33 + 1] = acc[mt][4 * cc + j][3];
+      }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(xp[lane * 33 + j]);
+}
+
 // ---- epilogue element transform -----------------------------------------------------------------------------------
 // One thread turns its 32 accumulator values of a 32-column chunk into the staged fp32 output row piece by piece.
 // The flags are COMPILE-TIME here: with run-time flags the unrolled loop carries a test per element and flag (about
-// 20 instructions per element), and the epilogue -- not HBM -- bounds the short-K linears (ncu, round 2: the eight
-// epilogue warps of the persistent kernel issue 37 % of all cycles at 31 % DRAM utilisation).  epi_chunk_dispatch
-// picks the instantiation once per chunk; unusual flag combinations take the generic run-time path.
+// 20 instructions per element), and the epilogue bounds the short-K linears.  epi_chunk_dispatch picks the
+// instantiation once per chunk; unusual flag combinations take the generic run-time path.
 // `word`: the chunk's 32 mask bits of this row (EPI_MASK_BITS); returns the chunk's ReLU bits (EPI_RELU_BITS, else 0).
 template <int F>
 __device__ __forceinline__ uint32_t epi_chunk_f32(const uint32_t (&v)[32], uint8_t* slab_row, int row, const float* bias_c,
@@ -127,17 +209,15 @@ struct SmemLayout {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 4;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGING_BYTES = BLOCK_M * BLOCK_N * 4;
-  // Two stages: the contraction is short (K = 32..512) and latency is hidden by co-resident CTAs instead
-  // (~80 KB per CTA with an epilogue tile -> 2 per SM; ~50 KB without -> 4 per SM).
+  // Two stages: the contraction is short (K = 32..512) and latency is hidden by co-resident CTAs instead.
   // weight-gradient GEMMs (both operands MN-major, K = all rows of the batch) run a long K loop per CTA: 4 stages
   static constexpr int stages() { return NST; }
   static constexpr int pipe_bytes() { return stages() * STAGE_BYTES; }
-  // without an aux (residual / mask) tile the output staging aliases the operand ring: it is only written after
-  // the last MMA has consumed the ring
   // The output staging tile (and the residual / mask tile, fetched only after the last MMA) aliases the operand
-  // ring: both are touched only once every MMA of the CTA has completed.
+  // ring: both are touched only once every consumer warp has finished reading it.
   static constexpr int body_bytes() { return pipe_bytes() > STAGING_BYTES ? pipe_bytes() : STAGING_BYTES; }
-  static constexpr int total() { return body_bytes() + 256 + BLOCK_N * 4 + 1024; }
+  static constexpr int XPOSE_OFF = 256 + BLOCK_N * 4;     // after the barriers and the bias row, in the tail
+  static constexpr int total() { return body_bytes() + XPOSE_OFF + (GEMM_EPI_THREADS / 32) * XPOSE_BYTES + 1024; }
 };
 
 template <int BLOCK_N, int A_MN, int B_MN, bool DROP, int NST, bool IN16 = false, bool OUT16 = false>
@@ -148,8 +228,9 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
                                                                  const GemmParams p) {
   using L = SmemLayout<BLOCK_N, NST>;
   constexpr int STAGES = L::stages();
-  constexpr int TMEM_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
   constexpr int N_SLABS = BLOCK_N / 32;                       // 32-column accumulator chunks
+  constexpr int NT = BLOCK_N / 8;                             // 8-column MMA tiles per warp
+  constexpr int N_CONSUMERS = GEMM_EPI_THREADS / 32;
   constexpr int OUT_COLS = OUT16 ? 64 : 32;                   // output columns per 128-byte staging slab row
   constexpr int OUT_SLABS = (BLOCK_N + OUT_COLS - 1) / OUT_COLS;
   static_assert(!OUT16 || BLOCK_N >= 64, "bf16 outputs need at least one full 128-byte slab row");
@@ -161,9 +242,8 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
   uint8_t* tail = smem + L::body_bytes();
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint64_t* aux_bar = tmem_full_bar + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aux_bar + 1);
+  uint64_t* ring_done_bar = empty_bar + STAGES;   // every consumer warp has read its last k-block
+  uint64_t* aux_bar = ring_done_bar + 1;
   float* bias_s = reinterpret_cast<float*>(tail + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -190,17 +270,13 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
     ptx::prefetch_tmap(&tmB);
     if (!split) ptx::prefetch_tmap(&tmC);
     if (has_aux) ptx::prefetch_tmap(&tmAux);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    ptx::mbar_init(tmem_full_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], N_CONSUMERS); }
+    ptx::mbar_init(ring_done_bar, N_CONSUMERS);
     ptx::mbar_init(aux_bar, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(tmem_slot);
   arb_pdl_wait();          // everything above overlaps the previous kernel's tail; global memory is touched below
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -226,85 +302,56 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
         }
       }
       if (has_aux) {
-        // the residual / ReLU-mask tile goes into the staging area, i.e. over the operand ring: wait until the
-        // tensor core has finished reading it.  It has the output's element type: 128-byte slab rows hold 32 fp32 or
-        // 64 bf16 columns.
-        if (nkb > 0) ptx::mbar_wait(tmem_full_bar, 0);
+        // the residual / ReLU-mask tile goes into the staging area, i.e. over the operand ring: wait until every
+        // consumer warp has finished reading it.  It has the output's element type: 128-byte slab rows hold 32 fp32
+        // or 64 bf16 columns.
+        if (nkb > 0) ptx::mbar_wait(ring_done_bar, 0);
         ptx::mbar_expect_tx(aux_bar, OUT16 ? L::STAGING_BYTES / 2 : L::STAGING_BYTES);
         for (int c = 0; c < OUT_SLABS; ++c)
           ptx::tma_load_4d(staging + c * (BLOCK_M * 128), &tmAux, aux_bar, n0 + OUT_COLS * c, m0, b2 * p.c_b2, b3 * p.c_b3);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = IN16 ? ptx::idesc_bf16(BLOCK_M, BLOCK_N, A_MN, B_MN)
-                                      : ptx::idesc_tf32(BLOCK_M, BLOCK_N, A_MN, B_MN);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % STAGES, round = i / STAGES;
-        ptx::mbar_wait(&full_bar[s], round & 1);
-        ptx::tc_fence_after();
-        const uint32_t a_addr = ptx::smem_u32(smem + s * L::STAGE_BYTES);
-        const uint32_t b_addr = a_addr + A_STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {      // 4 instructions per k-block for both element types
-          // K-major : rows of 128 B, 8-row groups 1024 B apart (SBO); advance 32 B per K step inside the swizzle row
-          // MN-major tf32: 32-wide slabs of [32 k-rows x 128 B] 4096 B apart (LBO); swizzle atom = 4 k-rows (512 B,
-          //           SBO); 8 k-rows (1024 B) per K step
-          // MN-major bf16: 64-wide slabs of [64 k-rows x 128 B] 8192 B apart (LBO); 8-k-row groups 1024 B apart (SBO);
-          //           16 k-rows (2048 B) per K step; plain SWIZZLE_128B
-          uint64_t da, db;
-          if constexpr (IN16) {
-            da = A_MN ? ptx::smem_desc_sw128<2>(a_addr + k * 2048, 8192, 1024) : ptx::smem_desc_sw128<2>(a_addr + k * 32, 16, 1024);
-            db = B_MN ? ptx::smem_desc_sw128<2>(b_addr + k * 2048, 8192, 1024) : ptx::smem_desc_sw128<2>(b_addr + k * 32, 16, 1024);
-            ptx::mma_bf16_ss(tmem_base, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-          } else {
-            da = A_MN ? ptx::smem_desc_sw128<1>(a_addr + k * 1024, 4096, 512) : ptx::smem_desc_sw128<2>(a_addr + k * 32, 16, 1024);
-            db = B_MN ? ptx::smem_desc_sw128<1>(b_addr + k * 1024, 4096, 512) : ptx::smem_desc_sw128<2>(b_addr + k * 32, 16, 1024);
-            ptx::mma_tf32_ss(tmem_base, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-          }
-        }
-        ptx::mma_commit(&empty_bar[s]);     // frees the stage when these MMAs have read it
-      }
-      ptx::mma_commit(tmem_full_bar);       // accumulator complete
-    }
-  } else {
-    // ===================== epilogue (warps 2..) =====================
-    // One warp per TMEM lane quadrant walks the 32-column chunks of the accumulator.  (GEMM_EPI_GROUPS = 2 -- two
-    // warps per quadrant on alternate chunks -- shortens a CTA's epilogue but costs a resident CTA per SM: the
-    // short-K products with an aux tile went from 0.73 / 0.90 to 0.59 / 0.77 of the HBM roof; profiles/r2/call18.)
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int row = 32 * q + lane;          // row of the tile owned by this thread
+  } else if (warp >= 2) {
+    // ===================== MMA + epilogue (warps 2..) =====================
+    const int q = warp & 3;                 // 32-row quarter of the tile this warp computes
+    const int row = 32 * q + lane;          // row of the tile owned by this thread in the epilogue
     const int et = threadIdx.x - 64;        // 0..GEMM_EPI_THREADS-1
     const int grp = (warp - 2) >> 2;        // which chunks: grp, grp + GEMM_EPI_GROUPS, ...
+    float* xp = reinterpret_cast<float*>(tail + L::XPOSE_OFF) + (warp - 2) * (XPOSE_BYTES / 4);
     if (p.flags & EPI_BIAS) {
       for (int j = et; j < BLOCK_N; j += GEMM_EPI_THREADS) bias_s[j] = (n0 + j < p.N) ? p.bias[n0 + j] : 0.0f;
     }
-    ptx::named_bar_sync(1, GEMM_EPI_THREADS);
     // EPI_MASK_BITS: this row's mask word of a chunk is fetched one chunk ahead (a global load per row and chunk); the
-    // first one goes out before the wait for the accumulator
+    // first one goes out before the main loop
     auto mask_word = [&](int c) -> uint32_t {
       return ((p.flags & EPI_MASK_BITS) && c < N_SLABS && m0 + row < p.M && n0 + 32 * c < p.N)
                  ? p.bits[(long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c)] : 0u;
     };
     uint32_t word_next = mask_word(grp);
-    if (nkb > 0) {
-      ptx::mbar_wait(tmem_full_bar, 0);
-      ptx::tc_fence_after();
+    float acc[2][NT][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % STAGES, round = i / STAGES;
+      ptx::mbar_wait(&full_bar[s], round & 1);
+      const uint8_t* a_s = smem + s * L::STAGE_BYTES;
+      warp_mma_kblock<NT, A_MN, B_MN, IN16>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, 0, 1, p.rnd);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);      // this warp is done with the stage
     }
+    if (lane == 0) ptx::mbar_arrive(ring_done_bar);
+    // the staging tile aliases the ring: no warp writes it before every warp has finished its MMAs (this barrier also
+    // publishes the bias row)
+    ptx::named_bar_sync(1, GEMM_EPI_THREADS);
     if (has_aux) ptx::mbar_wait(aux_bar, 0);
 #pragma unroll 1
     for (int c = grp; c < N_SLABS; c += GEMM_EPI_GROUPS) {
       const uint32_t word_in = word_next;
       word_next = mask_word(c + GEMM_EPI_GROUPS);
       uint32_t v[32];
-      if (nkb > 0) {
-        ptx::tmem_ld_32x32(tmem_base + (uint32_t(32 * q) << 16) + uint32_t(32 * c), v);
-        ptx::tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0u;
-      }
+      acc_chunk_row<NT>(acc, c, xp, v);
       if constexpr (OUT16) {
         // bf16 output: a 128-byte staging row holds 64 columns; this 32-column chunk fills 16-byte pieces
         // 4*(c&1) .. +3 of slab c/2.  The aux (ReLU-mask) tile has the same layout and type.
@@ -374,18 +421,16 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
           }
         }
         if (split) {
-          // one 128-bit reduction per 4 columns: the weight-gradient GEMMs are bound by the number of L2 atomic
-          // operations (measured: 4.8 M scalar atomics = ~120 us regardless of the bytes streamed)
+          // this split's slot of the weight gradient (summed over the splits in order by DetParts::finish)
           const int gm = m0 + row, gn = n0 + 32 * c + piece * 4;
           if (gm < p.M && gn < p.N) {
-            float* dstg = p.atomic_out + (long long)gm * p.atomic_ld + gn;
+            float* dstg = p.atomic_out + (long long)blockIdx.z * p.M * p.atomic_ld + (long long)gm * p.atomic_ld + gn;
             if (gn + 3 < p.N && (p.atomic_ld & 3) == 0) {
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dstg), "f"(o[0]), "f"(o[1]), "f"(o[2]),
-                           "f"(o[3]) : "memory");
+              *reinterpret_cast<float4*>(dstg) = make_float4(o[0], o[1], o[2], o[3]);
             } else {
 #pragma unroll
               for (int e = 0; e < 4; ++e)
-                if (gn + e < p.N) atomicAdd(dstg + e, o[e]);
+                if (gn + e < p.N) dstg[e] = o[e];
             }
           }
         } else {
@@ -421,39 +466,35 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
           for (int r = 0; r < BLOCK_M; ++r)
             t += *reinterpret_cast<const float*>(slab + r * 128 + ((((cc >> 2) ^ (r & 7)) << 4) | ((cc & 3) << 2)));
         }
-        atomicAdd(p.colsum_out + n0 + et, t);
+        p.colsum_out[((long long)blockIdx.z * gridDim.y + blockIdx.y) * p.N + n0 + et] = t;   // this tile's slot
       }
       if (et == 0) ptx::tma_store_wait_read();   // smem may be released once the TMA engine has read it
     }
-    ptx::tc_fence_before();
   }
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ persistent variant
-// Same maths and epilogues as gemm_tf32_kernel, restructured as a persistent, fully decoupled pipeline: one CTA per
-// SM walks a static round-robin list of output tiles; the TMA producer keeps a 4-stage operand ring (128 KB) full
-// ACROSS tile boundaries, the MMA issuer alternates between two TMEM accumulators, and the epilogue warps drain one
-// accumulator while the next tile's loads and MMAs are already in flight.  This keeps ~128 KB of loads in flight
-// per SM at all times, which is what an HBM-bound GEMM with K = 128..512 needs (the non-persistent kernel has no
-// loads in flight during its epilogue).
+// Same maths and epilogues as gemm_tf32_kernel, restructured as a persistent pipeline: one CTA per SM walks a static
+// round-robin list of output tiles; the TMA producer keeps a deep operand ring full ACROSS tile boundaries, so the
+// next tile's loads are in flight while the consumer warps run the current tile's epilogue (the non-persistent kernel
+// has no loads in flight during its epilogue).
 template <int BLOCK_N>
 struct PersistLayout {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 4;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = BLOCK_N <= 64 ? 6 : 4;
+  static constexpr int STAGES = BLOCK_N <= 64 ? 6 : 3;
   static constexpr int STAGING_BYTES = BLOCK_M * BLOCK_N * 4;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int total() { return RING_BYTES + STAGING_BYTES + 512 + BLOCK_N * 4 + 1024; }
+  static constexpr int XPOSE_OFF = RING_BYTES + STAGING_BYTES + 512 + BLOCK_N * 4;
+  static constexpr int total();
 };
 
-constexpr int EPI_GROUPS = 2;                 // epilogue groups of four warps (one warp per TMEM lane quadrant)
+constexpr int EPI_GROUPS = 2;                 // consumer groups of four warps (one warp per 32-row quarter)
 constexpr int EPI_THREADS = 128 * EPI_GROUPS;
 constexpr int PERSIST_THREADS = 64 + EPI_THREADS;
+template <int BLOCK_N>
+constexpr int PersistLayout<BLOCK_N>::total() { return XPOSE_OFF + (EPI_THREADS / 32) * XPOSE_BYTES + 1024; }
 
 template <int BLOCK_N, int A_MN, int B_MN>
 __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const __grid_constant__ CUtensorMap tmA,
@@ -464,20 +505,18 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
                                                                         int n_tiles_m, int n_z) {
   using L = PersistLayout<BLOCK_N>;
   constexpr int STAGES = L::STAGES;
-  constexpr int ACC_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
-  constexpr int TMEM_COLS = 2 * ACC_COLS;
   constexpr int N_SLABS = BLOCK_N / 32;
+  constexpr int NGA = N_SLABS < EPI_GROUPS ? N_SLABS : EPI_GROUPS;   // active consumer groups
+  constexpr int SLABS_PER_GROUP = N_SLABS / NGA;
+  constexpr int NT = 4 * SLABS_PER_GROUP;                            // 8-column MMA tiles per warp
 
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint8_t* staging = smem + L::RING_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + L::STAGING_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full = empty_bar + STAGES;        // [2] accumulator complete
-  uint64_t* acc_empty = acc_full + 2;             // [2] accumulator drained by the epilogue (128 arrivals)
-  uint64_t* aux_full = acc_empty + 2;             // aux tile landed in staging
-  uint64_t* stage_free = aux_full + 1;            // staging free again (store has read it), 1 arrival
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stage_free + 1);
+  uint64_t* empty_bar = full_bar + STAGES;        // 4 * NGA consumer-warp arrivals
+  uint64_t* aux_full = empty_bar + STAGES;        // aux tile landed in staging
+  uint64_t* stage_free = aux_full + 1;            // staging free again (store has read it), one arrival per group
   float* bias_s = reinterpret_cast<float*>(staging + L::STAGING_BYTES + 512);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -494,18 +533,13 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
     ptx::prefetch_tmap(&tmB);
     if (!split) ptx::prefetch_tmap(&tmC);
     if (has_aux) ptx::prefetch_tmap(&tmAux);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { ptx::mbar_init(&acc_full[a], 1); ptx::mbar_init(&acc_empty[a], EPI_THREADS); }
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 4 * NGA); }
     ptx::mbar_init(aux_full, 1);
-    ptx::mbar_init(stage_free, N_SLABS < EPI_GROUPS ? N_SLABS : EPI_GROUPS);   // one arrival per epilogue group that stores
+    ptx::mbar_init(stage_free, NGA);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(tmem_slot);
   arb_pdl_wait();          // everything above overlaps the previous kernel's tail; global memory is touched below
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto decode = [&](int t, int& n0, int& m0, int& z) {
     const int nt = t % n_tiles_n;
@@ -567,85 +601,57 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::idesc_tf32(BLOCK_M, BLOCK_N, A_MN, B_MN);
+  } else if (warp >= 2) {
+    // ===================== MMA + epilogue (warps 2..9) =====================
+    // NGA = min(EPI_GROUPS, slabs) groups of four warps are active, group g owning the 32-column slabs g, g + NGA, ...
+    // of the tile (each warp: 32 rows of them).  A group turns a slab registers -> swizzled staging and its leader
+    // immediately issues that slab's TMA store; the staging slab is reclaimed lazily (cp.async.bulk.wait_group.read)
+    // right before the group writes it again one tile later.  No barrier spans more than the 128 threads of a group.
+    const int q = warp & 3;
+    const int row = 32 * q + lane;
+    const int grp = (warp - 2) >> 2;                    // 0 .. EPI_GROUPS-1
+    const int gt = threadIdx.x - 64 - 128 * grp;        // 0..127 inside the group
+    const bool leader = gt == 0;
+    float* xp = reinterpret_cast<float*>(smem + L::XPOSE_OFF) + (warp - 2) * (XPOSE_BYTES / 4);
+    if (grp < NGA) {
       uint32_t it = 0;
       int local = 0;
       for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++local) {
         int n0, m0, z, kb0, nkb;
         decode(t, n0, m0, z);
         k_range(z, kb0, nkb);
-        const int acc = local & 1;
-        const uint32_t use = local >> 1;      // how many times this accumulator has been used before
-        if (use > 0) ptx::mbar_wait(&acc_empty[acc], (use - 1) & 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
+        const int b2 = split ? 0 : z % p.nb2, b3 = split ? 0 : z / p.nb2;
+        ptx::named_bar_sync(1 + grp, 128);            // the group's previous epilogue is done with the bias row
+        if (p.flags & EPI_BIAS) {                     // this group's columns only (ordered by the group barriers)
+          for (int j = gt; j < 32 * SLABS_PER_GROUP; j += 128) {
+            const int col = 32 * (grp + NGA * (j >> 5)) + (j & 31);
+            bias_s[col] = (n0 + col < p.N) ? p.bias[n0 + col] : 0.0f;
+          }
+        }
+        // EPI_MASK_BITS: this row's mask words of the group's slabs, fetched before the main loop
+        uint32_t mword[2] = {0u, 0u};
+        if ((p.flags & EPI_MASK_BITS) && m0 + row < p.M) {
+#pragma unroll
+          for (int ci = 0; ci < (SLABS_PER_GROUP < 2 ? SLABS_PER_GROUP : 2); ++ci) {
+            const int c = grp + NGA * ci;
+            if (n0 + 32 * c < p.N) mword[ci] = p.bits[(long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c)];
+          }
+        }
+        float acc[2][NT][4];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.f;
         for (int i = 0; i < nkb; ++i, ++it) {
           const int s = it % STAGES;
           const uint32_t round = it / STAGES;
           ptx::mbar_wait(&full_bar[s], round & 1);
-          ptx::tc_fence_after();
-          const uint32_t a_addr = ptx::smem_u32(smem + s * L::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + A_STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint64_t da = A_MN ? ptx::smem_desc_sw128<1>(a_addr + k * 1024, 4096, 512)
-                                     : ptx::smem_desc_sw128<2>(a_addr + k * 32, 16, 1024);
-            const uint64_t db = B_MN ? ptx::smem_desc_sw128<1>(b_addr + k * 1024, 4096, 512)
-                                     : ptx::smem_desc_sw128<2>(b_addr + k * 32, 16, 1024);
-            ptx::mma_tf32_ss(d_tmem, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-          }
-          ptx::mma_commit(&empty_bar[s]);
+          const uint8_t* a_s = smem + s * L::STAGE_BYTES;
+          warp_mma_kblock<NT, A_MN, B_MN, false>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, grp, NGA, p.rnd);
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);
         }
-        ptx::mma_commit(&acc_full[acc]);     // (with nkb == 0 this still arrives: nothing outstanding)
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // GROUPS of four warps (one warp per TMEM lane quadrant each): NGA = min(EPI_GROUPS, slabs) of them are active,
-    // group g owning the 32-column slabs g, g + NGA, ... of the tile (EPI_GROUPS = 2; four groups -- one slab per group
-    // on 128-wide tiles -- measured 1-3 % slower on every shape: profiles/r2/call17).  A group turns a slab TMEM -> registers -> swizzled staging and its leader
-    // immediately issues that slab's TMA store; the staging slab is reclaimed lazily (cp.async.bulk.wait_group.read)
-    // right before the group writes it again one tile later.  Stores, staging writes and the other groups' work
-    // therefore overlap, and no barrier spans more than the 128 threads of a group.
-    const int q = warp & 3;
-    const int row = 32 * q + lane;
-    const int grp = (warp - 2) >> 2;                    // 0 .. EPI_GROUPS-1
-    const int gt = threadIdx.x - 64 - 128 * grp;        // 0..127 inside the group
-    const bool leader = gt == 0;
-    constexpr int NGA = N_SLABS < EPI_GROUPS ? N_SLABS : EPI_GROUPS;   // active groups
-    constexpr int SLABS_PER_GROUP = N_SLABS / NGA;
-    const bool active = grp < NGA;                      // the other groups only drain the accumulator barriers
-    int local = 0;
-    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++local) {
-      int n0, m0, z, kb0, nkb;
-      decode(t, n0, m0, z);
-      k_range(z, kb0, nkb);
-      const int b2 = split ? 0 : z % p.nb2, b3 = split ? 0 : z / p.nb2;
-      const int acc = local & 1;
-      const uint32_t use = local >> 1;
-      if (active && (p.flags & EPI_BIAS)) {             // this group's columns only (ordered by the group barriers)
-        for (int j = gt; j < 32 * SLABS_PER_GROUP; j += 128) {
-          const int col = 32 * (grp + NGA * (j >> 5)) + (j & 31);
-          bias_s[col] = (n0 + col < p.N) ? p.bias[n0 + col] : 0.0f;
-        }
-      }
-      // EPI_MASK_BITS: this row's mask words of the group's slabs, fetched before the wait for the accumulator
-      uint32_t mword[2] = {0u, 0u};
-      if (active && (p.flags & EPI_MASK_BITS) && m0 + row < p.M) {
-#pragma unroll
-        for (int ci = 0; ci < (SLABS_PER_GROUP < 2 ? SLABS_PER_GROUP : 2); ++ci) {
-          const int c = grp + NGA * ci;
-          if (n0 + 32 * c < p.N) mword[ci] = p.bits[(long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c)];
-        }
-      }
-      ptx::mbar_wait(&acc_full[acc], use & 1);
-      ptx::tc_fence_after();
-      if (has_aux) ptx::mbar_wait(aux_full, local & 1);
-      const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-      if (active) {
+        if (has_aux) ptx::mbar_wait(aux_full, local & 1);
 #pragma unroll 1
         for (int ci = 0; ci < SLABS_PER_GROUP; ++ci) {
           const int c = grp + NGA * ci;
@@ -658,13 +664,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
           }
           ptx::named_bar_sync(1 + grp, 128);
           uint32_t v[32];
-          if (nkb > 0) {
-            ptx::tmem_ld_32x32(d_tmem + (uint32_t(32 * q) << 16) + uint32_t(32 * c), v);
-            ptx::tmem_ld_wait();
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = 0u;
-          }
+          acc_chunk_row<NT>(acc, ci, xp, v);
           uint8_t* slab_row = staging + c * (BLOCK_M * 128) + row * 128;
           uint32_t* bits_at = (p.bits && m0 + row < p.M && n0 + 32 * c < p.N)
                                   ? p.bits + (long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c) : nullptr;
@@ -697,14 +697,13 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
             if (split) {
               const int gm = m0 + row, gn = n0 + 32 * c + piece * 4;
               if (gm < p.M && gn < p.N) {
-                float* dstg = p.atomic_out + (long long)gm * p.atomic_ld + gn;
+                float* dstg = p.atomic_out + (long long)z * p.M * p.atomic_ld + (long long)gm * p.atomic_ld + gn;
                 if (gn + 3 < p.N && (p.atomic_ld & 3) == 0) {
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dstg), "f"(o[0]), "f"(o[1]), "f"(o[2]),
-                               "f"(o[3]) : "memory");
+                  *reinterpret_cast<float4*>(dstg) = make_float4(o[0], o[1], o[2], o[3]);
                 } else {
 #pragma unroll
                   for (int e = 0; e < 4; ++e)
-                    if (gn + e < p.N) atomicAdd(dstg + e, o[e]);
+                    if (gn + e < p.N) dstg[e] = o[e];
                 }
               }
             } else {
@@ -731,26 +730,20 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
                 tsum += *reinterpret_cast<const float*>(slab + r * 128 + ((((cc >> 2) ^ (r & 7)) << 4) | ((cc & 3) << 2)));
               tsum += __shfl_xor_sync(0xffffffffu, tsum, 1);
               tsum += __shfl_xor_sync(0xffffffffu, tsum, 2);
-              if (seg == 0 && n0 + 32 * c + cc < p.N) atomicAdd(p.colsum_out + n0 + 32 * c + cc, tsum);
+              if (seg == 0 && n0 + 32 * c + cc < p.N)      // this tile's slot
+                p.colsum_out[((long long)z * ((p.M + BLOCK_M - 1) / BLOCK_M) + m0 / BLOCK_M) * p.N + n0 + 32 * c + cc] = tsum;
             }
           }
         }
+        if (!split && has_aux && leader) {     // the producer refills the staging area with the next aux tile
+          ptx::tma_store_wait_read();
+          ptx::mbar_arrive(stage_free);
+        }
       }
-      // this accumulator may be overwritten by the MMA warp from now on
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&acc_empty[acc]);
-      if (!split && has_aux && active && leader) {     // the producer refills the staging area with the next aux tile
-        ptx::tma_store_wait_read();
-        ptx::mbar_arrive(stage_free);
-      }
+      if (!split && leader) ptx::tma_store_wait_read();
     }
-    if (!split && active && leader) ptx::tma_store_wait_read();
   }
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -770,12 +763,13 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// MMA operands are loaded through TFLOAT32 tensor maps: the TMA unit rounds fp32 -> tf32 (instead of the tensor
-// core truncating the mantissa), which removes the systematic bias truncation puts on gradients (DESIGN.md 5).
+// MMA operands are rounded fp32 -> tf32 (nearest even) as the kernels load them from shared memory, instead of letting the
+// tensor core truncate the mantissa: this removes the systematic bias truncation puts on gradients (DESIGN.md 5).
 static int g_round_on_load = 1;
 void set_tf32_round_on_load(int enable) { g_round_on_load = enable; }
+int tf32_round_on_load() { return g_round_on_load; }
 
-int make_tmap_4d(void* out, const TRef& t, TmapBox box, int atom32, int as_tf32) {
+int make_tmap_4d(void* out, const TRef& t, TmapBox box, int unswizzled) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { arb_set_error("cuTensorMapEncodeTiled is not available from this driver"); return ARB_E_CUDA; }
   const int64_t esz = t.bf16 ? 2 : 4;
@@ -792,14 +786,10 @@ int make_tmap_4d(void* out, const TRef& t, TmapBox box, int atom32, int as_tf32)
     if (gstride[i - 1] % 16 != 0) { arb_set_error("tensor map: strides must be multiples of 16 bytes"); return ARB_E_INVALID_ARG; }
   }
   if ((reinterpret_cast<uintptr_t>(t.ptr) & 15) != 0) { arb_set_error("tensor map: base must be 16-byte aligned"); return ARB_E_INVALID_ARG; }
-  if (t.bf16 && atom32 == 1) { arb_set_error("tensor map: the 32-byte-atom swizzle is a tf32 layout"); return ARB_E_INVALID_ARG; }
-  const CUtensorMapDataType dt = t.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                        : ((as_tf32 && g_round_on_load) ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32
-                                                                        : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+  const CUtensorMapDataType dt = t.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = enc(reinterpret_cast<CUtensorMap*>(out), dt, 4, const_cast<void*>(t.ptr),
                    gdim, gstride, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   atom32 == 2 ? CU_TENSOR_MAP_SWIZZLE_NONE
-                               : (atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B),
+                   unswizzled ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char msg[256];
@@ -839,7 +829,7 @@ static int launch_persistent_t(const GemmDesc& d, const CUtensorMap& tA, const C
       arb_set_error("gemm_tf32 (persistent): cannot raise the dynamic shared memory limit");
       return ARB_E_CUDA;
     }
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     n_sm_of[dev_slot] = n;
@@ -864,7 +854,7 @@ static int launch_persistent_t(const GemmDesc& d, const CUtensorMap& tA, const C
   return ARB_OK;
 }
 
-// bf16 operands (kind::f16): the one-tile-per-CTA kernel; 4-stage ring for the split-K weight gradients, else 3 stages
+// bf16 operands (mma m16n8k16): the one-tile-per-CTA kernel; 4-stage ring for the split-K weight gradients, else 3 stages
 // (a k-block is 64 elements, so K = 256 is four blocks); fp32 or bf16 output.
 template <int BLOCK_N, int A_MN, int B_MN>
 static int launch_bf16_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
@@ -918,12 +908,8 @@ template <int BLOCK_N, int A_MN, int B_MN>
 static int launch_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
                     const CUtensorMap& tX, const GemmParams& p, dim3 grid, cudaStream_t st) {
   if (d.A.bf16) return launch_bf16_t<BLOCK_N, A_MN, B_MN>(d, tA, tB, tC, tX, p, grid, st);
-  // Mode 2 (default), measured per launch in round 2 after the epilogue was specialised (profiles/r2): the persistent
-  // pipeline wins on every unbatched, non-split shape (short-K wide-N forward linears 0.76-0.86 of the HBM roof against
-  // 0.58-0.62 for one-tile CTAs; K >= 256: 0.93-0.98) EXCEPT short-K products with a residual / mask tile, whose aux
-  // load it can only issue once the previous tile's stores have left the staging area (dgrad N512 K128 mask: 0.70
-  // against 0.85; the K128 +res projection ties).  (Giving the aux tile a shared-memory buffer of its own, at the price
-  // of one ring stage, measured slower on every shape: 19.17 against 18.63 ms per cfg2 step -- not kept.)
+  // Mode 2 (default): the persistent pipeline for every unbatched, non-split shape EXCEPT short-K products with a
+  // residual / mask tile, whose aux load it can only issue once the previous tile's stores have left the staging area.
   const bool has_aux_tile = (p.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) != 0;
   // Mode 3 (measurement): as 2, but the short-K products with an aux tile go to the persistent kernel too (under packed
   // rows half of a one-tile grid are CTAs of dead tiles that only exit; the persistent kernel has none).
@@ -991,15 +977,15 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   const uint32_t ocol = out16 ? 64u : 32u;        // output columns per 128-byte staging row
   alignas(64) CUtensorMap tA, tB, tC, tX;
   int rc;
-  if ((rc = make_tmap_4d(&tA, d.A, d.a_mn ? TmapBox{{kel, kel, 1, 1}} : TmapBox{{kel, 128, 1, 1}}, d.a_mn && !in16, 1))) return rc;
-  if ((rc = make_tmap_4d(&tB, d.B, d.b_mn ? TmapBox{{kel, kel, 1, 1}} : TmapBox{{kel, uint32_t(d.block_n), 1, 1}}, d.b_mn && !in16, 1))) return rc;
+  if ((rc = make_tmap_4d(&tA, d.A, d.a_mn ? TmapBox{{kel, kel, 1, 1}} : TmapBox{{kel, 128, 1, 1}}, 0))) return rc;
+  if ((rc = make_tmap_4d(&tB, d.B, d.b_mn ? TmapBox{{kel, kel, 1, 1}} : TmapBox{{kel, uint32_t(d.block_n), 1, 1}}, 0))) return rc;
   if (!split) {
-    if ((rc = make_tmap_4d(&tC, d.C, TmapBox{{ocol, 128, 1, 1}}, 0, 0))) return rc;
+    if ((rc = make_tmap_4d(&tC, d.C, TmapBox{{ocol, 128, 1, 1}}, 0))) return rc;
   } else {
     tC = tA;
   }
   if (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) {
-    if ((rc = make_tmap_4d(&tX, d.Aux, TmapBox{{ocol, 128, 1, 1}}, 0, 0))) return rc;
+    if ((rc = make_tmap_4d(&tX, d.Aux, TmapBox{{ocol, 128, 1, 1}}, 0))) return rc;
   } else {
     tX = tA;
   }
@@ -1013,6 +999,7 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   p.colsum_out = d.colsum_out;
   p.rows_dev = d.rows_dev;
   p.bits = d.bits;
+  p.rnd = g_round_on_load;
   if (d.flags & (EPI_RELU_BITS | EPI_MASK_BITS)) {
     if (!d.bits || d.N % 32 || out16 || split || d.nb2 != 1 || d.nb3 != 1 || (d.flags & (EPI_DROPOUT | EPI_ADD_AUX | EPI_MASK_AUX)) ||
         ((d.flags & EPI_RELU_BITS) && !(d.flags & EPI_RELU))) {
@@ -1031,14 +1018,23 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   p.kb_per_split = (total_kb + splits - 1) / splits;
   const int eff_splits = split ? (total_kb + p.kb_per_split - 1) / std::max(1, p.kb_per_split) : 1;
   dim3 grid((d.N + d.block_n - 1) / d.block_n, (d.M + BLOCK_M - 1) / BLOCK_M, split ? std::max(1, eff_splits) : d.nb2 * d.nb3);
+  int (*launch)(const GemmDesc&, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,
+                const GemmParams&, dim3, cudaStream_t) = nullptr;
 #define ARB_GEMM_CASE(BN, AM, BM) \
-  if (d.block_n == BN && d.a_mn == AM && d.b_mn == BM) return launch_t<BN, AM, BM>(d, tA, tB, tC, tX, p, grid, st);
+  if (d.block_n == BN && d.a_mn == AM && d.b_mn == BM) launch = launch_t<BN, AM, BM>;
   ARB_GEMM_CASE(32, 0, 0) ARB_GEMM_CASE(32, 0, 1) ARB_GEMM_CASE(32, 1, 0) ARB_GEMM_CASE(32, 1, 1)
   ARB_GEMM_CASE(64, 0, 0) ARB_GEMM_CASE(64, 0, 1) ARB_GEMM_CASE(64, 1, 0) ARB_GEMM_CASE(64, 1, 1)
   ARB_GEMM_CASE(128, 0, 0) ARB_GEMM_CASE(128, 0, 1) ARB_GEMM_CASE(128, 1, 0) ARB_GEMM_CASE(128, 1, 1)
 #undef ARB_GEMM_CASE
-  arb_set_error("gemm_tf32: unsupported configuration");
-  return ARB_E_UNSUPPORTED;
+  if (!launch) { arb_set_error("gemm_tf32: unsupported configuration"); return ARB_E_UNSUPPORTED; }
+  // split-K partial tiles and the per-tile bias-gradient column sums go to slots that are summed in order afterwards
+  DetParts dp;
+  if (p.flags & EPI_COLSUM) dp.add(p.colsum_out, (long long)grid.z * grid.y, 1, d.N, d.N);
+  if (split) dp.add(p.atomic_out, grid.z, d.M, d.N, d.atomic_ld);
+  if ((rc = dp.begin(st))) return rc;
+  if (split) p.atomic_ld = d.N;       // slot row pitch
+  if ((rc = launch(d, tA, tB, tC, tX, p, grid, st))) return rc;
+  return dp.finish(st);
 }
 
 }  // namespace arb
@@ -1073,7 +1069,7 @@ extern "C" int32_t arb_gemm_tf32(const float* A, const float* B, float* C, const
   return launch_gemm_tf32(d, static_cast<cudaStream_t>(stream));
 }
 
-// The same building block with bf16 operands (tcgen05 kind::f16, fp32 accumulation): A, B are bfloat16 matrices in the
+// The same building block with bf16 operands (tensor-core m16n8k16, fp32 accumulation): A, B are bfloat16 matrices in the
 // layouts described above; C (and aux, if given) is bfloat16 when out_bf16 != 0, else fp32.  With EPI_ATOMIC
 // (split-K) C must be fp32 and is accumulated into.
 extern "C" int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const void* aux, const float* bias, int32_t M,

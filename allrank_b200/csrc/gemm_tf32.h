@@ -21,7 +21,7 @@ enum : int {
   EPI_RELU = 2,       // max(., 0)
   EPI_ADD_AUX = 4,    // + Aux[m,n]          (residual; Aux may alias C)
   EPI_MASK_AUX = 8,   // . * (Aux[m,n] > 0)  (ReLU backward)
-  EPI_ATOMIC = 16,    // red.add into atomic_out instead of storing C (split-K weight gradients)
+  EPI_ATOMIC = 16,    // atomic_out += C instead of storing C (split-K weight gradients; splits summed in order)
   EPI_DROPOUT = 32,   // inverted dropout on (alpha*acc + bias [relu]) before the aux tile is added
   EPI_COLSUM = 64,    // colsum_out[n] += sum_m C[m,n]  (bias gradient of the layer that produced C's input)
   EPI_RELU_BITS = 128,  // with EPI_RELU (fp32 output): also write bits[m, n/32] -- bit j = (C[m, 32*(n/32) + j] > 0)
@@ -44,13 +44,13 @@ struct GemmDesc {
   float* atomic_out = nullptr;  // row-major [M, atomic_ld]
   int64_t atomic_ld = 0;
   DropSite drop{0u, 0u, 1.0f};  // EPI_DROPOUT: element index = m * N + n (unbatched problems only)
-  float* colsum_out = nullptr;  // EPI_COLSUM: [N], accumulated with atomics
+  float* colsum_out = nullptr;  // EPI_COLSUM: [N], += column sums (per-tile slots summed in order)
   uint32_t* bits = nullptr;     // EPI_RELU_BITS (written) / EPI_MASK_BITS (read): [M, N / 32] words, row-major
   const int* rows_dev = nullptr;   // packed rows (unbatched launches): device pointer to the live row count, a
                                    // multiple of 128.  It bounds M (tiles beyond it are not computed) or, with
                                    // EPI_ATOMIC, K (the weight gradients reduce over the live rows only); the host-side
                                    // M / K stay the upper bound the tensor maps and the grid are built from.
-  // Element types come from the views: A and B must agree (both fp32 -> kind::tf32, both bf16 -> kind::f16, fp32
+  // Element types come from the views: A and B must agree (both fp32 -> tf32 MMA, both bf16 -> bf16 MMA, fp32
   // accumulation either way); C may be fp32 or bf16; an Aux tile has C's type (fp32 residual into an fp32 stream,
   // bf16 ReLU-mask tile into a bf16 gradient).  bf16 outputs need block_n >= 64.
 };
@@ -59,12 +59,12 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t stream);   // 0 or ARB_E_*
 
 // 4-D tiled tensor map with 128-byte swizzle; box[0] must span 128 bytes (32 fp32 / 64 bf16 elements).
 struct TmapBox { uint32_t b[4]; };
-// atom32 = 0: SWIZZLE_128B (16-byte chunks); 1: SWIZZLE_128B_ATOM_32B (MN-major tf32 operands); 2: no swizzle (dense
-// rows narrower than 128 bytes: the bf16 outputs of the attention kernels)
-// as_tf32 = 1: MMA operand (TFLOAT32 map, rounded on load when enabled); 0: plain fp32 (stores, epilogue tiles)
-int make_tmap_4d(void* out_CUtensorMap, const TRef& t, TmapBox box, int atom32, int as_tf32);
+// unswizzled = 0: SWIZZLE_128B (16-byte chunks); 1: no swizzle (dense rows narrower than 128 bytes: the bf16 outputs
+// of the attention kernels)
+int make_tmap_4d(void* out_CUtensorMap, const TRef& t, TmapBox box, int unswizzled);
 
 void set_tf32_round_on_load(int enable);
+int tf32_round_on_load();   // 1: MMA kernels round fp32 operands to tf32 (nearest even) after loading them
 void set_gemm_persistent(int on);
 
 }  // namespace arb

@@ -5,10 +5,11 @@
 //   backward: the exact reverse, parameter gradients accumulated into a flat buffer.
 //
 // Reference: allrank/models/model.py:62-92 (LTRModel), allrank/models/transformer.py:43-56,126-134,178-203,227.
-// Every contraction is a launch of the tcgen05 TF32 GEMM (gemm_tf32.cu) -- per-head attention products are
+// Every contraction is a launch of the tensor-core TF32 GEMM (gemm_tf32.cu) -- per-head attention products are
 // batched launches over 4-D tensor maps (head and slate are TMA coordinates, so no transposes/copies exist:
 // the reference's `transpose(1,2).contiguous()` at transformer.py:201 vanishes).  The host sequence contains no
-// synchronisation and no allocation, so a training step can be captured into a CUDA graph by the host layer.
+// synchronisation and only stream-ordered allocations (the reduction slots, common.h: DetParts), so a training step can
+// be captured into a CUDA graph by the host layer.
 #include <cstdint>
 #include <vector>
 #include <cuda_runtime.h>
@@ -291,8 +292,8 @@ static int linear_bwd_weight(const Ctx& k, V dY, int64_t dy_pitch, int out, V X,
   const int tiles = ((out + 127) / 128) * ((in + g.block_n - 1) / g.block_n);
   const int kel = dY.bf16 ? 64 : 32;          // rows of the batch per k-block
   const int kb = int((k.R + kel - 1) / kel);
-  // 4-stage ring => 1 CTA per SM: one wave of ~148 CTAs (fewer splits = fewer L2 reductions of the dW tile)
-  g.split_k = std::max(1, std::min(kb / 8 + 1, std::max(1, 148 / tiles)));
+  // 4-stage ring => 1 CTA per SM: one wave of ~132 CTAs (H100 SXM) (fewer splits = fewer L2 reductions of the dW tile)
+  g.split_k = std::max(1, std::min(kb / 8 + 1, std::max(1, 132 / tiles)));
   g.rows_dev = k.rows_dev;
   return launch_gemm_tf32(g, k.st);
 }
@@ -449,7 +450,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
                        bf ? xn1 : nullptr, plan));
     ARB_TRY(linear_fwd(k, act(xn1), d, d, wt(pl.wqkv), P + pl.bqkv, 3 * d, qkv, 3 * d, 0, nullptr, 0));
     if (W.fused) {
-      AttnFwdArgs a;   // QK^T, key mask, softmax, PV in one kernel; the S x S tile never leaves TMEM
+      AttnFwdArgs a;   // QK^T, key mask, softmax, PV in one kernel; the S x S tile never leaves registers
       a.q = hview(qkv, 3 * d);
       a.k = hview(qkv + d, 3 * d);
       a.v = hview(qkv + 2 * d, 3 * d);
@@ -656,7 +657,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), d, d, G + pl.wo));   // (bo gradient: fused into the LayerNorm backward above)
     ARB_TRY(linear_bwd_input(k, dyo, d, d, wt(pl.wo), d, dctx, d, 0, nullptr, 0));
     if (use_fused_bwd(c, S)) {
-      AttnBwdArgs a;   // dQ, dK, dV from d ctx in one kernel; P is recomputed in TMEM from the saved row statistics
+      AttnBwdArgs a;   // dQ, dK, dV from d ctx in one kernel; P is recomputed from the saved row statistics
       a.q = hview(qkv, 3 * d);
       a.k = hview(qkv + d, 3 * d);
       a.v = hview(qkv + 2 * d, 3 * d);

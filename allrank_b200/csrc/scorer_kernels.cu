@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
 
 // ------------------------------------------------------------------------------------------------ LayerNorm bwd
 // dx = [dres +] r (dxh - mean(dxh)) - r^2 (sum_k dxh_k c_k) / ((d-1) std) * c,   dxh = dy * a, c = x - mean,
-// r = 1/(std+eps).   grad_a += sum_rows dy * xhat,  grad_b += sum_rows dy  (block partials -> atomicAdd).
+// r = 1/(std+eps).   grad_a += sum_rows dy * xhat,  grad_b += sum_rows dy  (block partials -> DetParts slots).
 template <int NV>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_kernel(const float* __restrict__ dy,
                                                                     const float* __restrict__ x,
@@ -318,7 +318,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
       float t = 0.f;
 #pragma unroll
       for (int w = 0; w < ROWS_PER_BLOCK; ++w) t += sh[w][c];
-      atomicAdd(dst + c, t);
+      dst[size_t(blockIdx.x) * width + c] = t;      // this block's slot (DetParts)
     }
     __syncthreads();
   }
@@ -450,7 +450,7 @@ __global__ void __launch_bounds__(256) slate_extent_kernel(const uint8_t* __rest
 // ------------------------------------------------------------------------------------------------ column sums
 // out[c] += sum_rows in[row, c]   (bias gradients).  A warp reads whole rows with 128-bit loads (4 rows in
 // flight per lane), 8 warps per block stride over the block's rows, then one shared-memory reduction and one
-// atomicAdd per column per block.
+// store per column per block into the block's DetParts slot.
 template <int NV>
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ in, long long rows, int width,
                                                      long long ld, int rows_per_block, float* __restrict__ out) {
@@ -491,7 +491,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ i
     float t = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) t += sh[w][c];
-    atomicAdd(out + c, t);
+    out[size_t(blockIdx.x) * width + c] = t;        // this block's slot (DetParts)
   }
 }
 
@@ -783,7 +783,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
       float t = 0.f;
 #pragma unroll
       for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += sh[ww][c];
-      atomicAdd(dst + c, t);
+      dst[size_t(blockIdx.x) * width + c] = t;      // this block's slot (DetParts)
     }
     __syncthreads();
   }
@@ -793,7 +793,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
-    atomicAdd(grad_wb, t);
+    grad_wb[blockIdx.x] = t;                        // this block's slot (DetParts)
   }
 }
 
@@ -885,17 +885,18 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
     for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = acc.v[k];
     if (lane == 0) shb[wid] = acc_b;
     __syncthreads();
-    float* dst = j < 0 ? colsum_out : grad_w + (long long)j * width;
+    // this block's slots (DetParts): colsum_out [block][width], grad_w [block][n][width], grad_wb [block][n]
+    float* dst = j < 0 ? colsum_out + (long long)blockIdx.x * width : grad_w + ((long long)blockIdx.x * n + j) * width;
     for (int c = threadIdx.x; c < width; c += blockDim.x) {
       float t = 0.f;
 #pragma unroll
       for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += sh[ww][c];
-      atomicAdd(dst + c, t);
+      dst[c] = t;
     }
     if (j >= 0 && threadIdx.x == 0) {
       float t = 0.f;
       for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
-      atomicAdd(grad_wb + j, t);
+      grad_wb[(long long)blockIdx.x * n + j] = t;
     }
     __syncthreads();
   }
@@ -961,11 +962,13 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
                                                       long long rows, int width, int act, DropSite site, float mul,
                                                       int tx_n, int rows_per_block, float* __restrict__ colsum_out,
                                                       const int* __restrict__ rows_dev) {
-  extern __shared__ float sh_cols[];
-  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
-  for (int c = threadIdx.x; c < width; c += blockDim.x) sh_cols[c] = 0.f;
-  __syncthreads();
+  extern __shared__ float sh_cols[];     // [ty_n][width]: one row of column partials per row group
   const int tx = threadIdx.x % tx_n, ty = threadIdx.x / tx_n, ty_n = blockDim.x / tx_n;
+  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
+  if (colsum_out) {
+    for (int c = threadIdx.x; c < ty_n * width; c += blockDim.x) sh_cols[c] = 0.f;
+    __syncthreads();
+  }
   const int groups = width / 4;
   const long long r0 = (long long)blockIdx.x * rows_per_block;
   const long long r1 = min(rows, r0 + rows_per_block);
@@ -987,14 +990,15 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
       *reinterpret_cast<float4*>(dz + at) = gv;
       acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
     }
-    if (colsum_out) {
-      atomicAdd(&sh_cols[g * 4 + 0], acc.x); atomicAdd(&sh_cols[g * 4 + 1], acc.y);
-      atomicAdd(&sh_cols[g * 4 + 2], acc.z); atomicAdd(&sh_cols[g * 4 + 3], acc.w);
-    }
+    if (colsum_out) *reinterpret_cast<float4*>(&sh_cols[ty * width + g * 4]) = acc;
   }
   if (colsum_out) {
     __syncthreads();
-    for (int c = threadIdx.x; c < width; c += blockDim.x) atomicAdd(colsum_out + c, sh_cols[c]);
+    for (int c = threadIdx.x; c < width; c += blockDim.x) {
+      float t = 0.f;
+      for (int y = 0; y < ty_n; ++y) t += sh_cols[y * width + c];
+      colsum_out[size_t(blockIdx.x) * width + c] = t;   // this block's slot (DetParts)
+    }
   }
 }
 
@@ -1011,7 +1015,7 @@ static int nv_for(int width) { return (width + 127) / 128; }
   }
 
 // rows per warp of the backward row kernels (LayerNorm, head): more rows per warp = fewer block-level reductions and
-// atomics of the gain / bias gradients per byte moved.  ARB_ROWS_PER_WARP overrides (measurement knob).
+// block slots of the gain / bias gradients per byte moved.  ARB_ROWS_PER_WARP overrides (measurement knob).
 static int bwd_rows_per_warp() {
   static int v = 0;
   if (!v) {
@@ -1086,7 +1090,8 @@ __device__ __forceinline__ void r_drop(float4 (&v)[4], long long row, int lane, 
     }
   }
 }
-// sum the per-column accumulators of the warp's row groups, then over the block's warps, then into `dst` (atomics)
+// sum the per-column accumulators of the warp's row groups, then over the block's warps, then into the block's slot of
+// `dst` (DetParts)
 template <int LPR>
 __device__ __forceinline__ void r_reduce_columns(float4 (&acc)[4], float (*sh)[16 * LPR + 4], int lane, int wid,
                                                  float* __restrict__ dst) {
@@ -1109,7 +1114,7 @@ __device__ __forceinline__ void r_reduce_columns(float4 (&acc)[4], float (*sh)[1
     float t = 0.f;
 #pragma unroll
     for (int w = 0; w < ROWS_PER_BLOCK; ++w) t += sh[w][c];
-    atomicAdd(dst + c, t);
+    dst[size_t(blockIdx.x) * W + c] = t;            // this block's slot (DetParts)
   }
   __syncthreads();
 }
@@ -1444,7 +1449,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) head_bwd_r_kernel(
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
-    atomicAdd(grad_wb, t);
+    grad_wb[blockIdx.x] = t;                        // this block's slot (DetParts)
   }
 }
 
@@ -1613,15 +1618,20 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
   const int rpw = bwd_rows_per_warp();
   const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * ((dres ? 16.0 : 12.0) * width + 8), st);
-  if (const int lpr = r_lpr(width, R_LN_BWD)) {
-    const int steps = r_bwd_rows_per_warp(rows) / (32 / lpr), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
-    const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
+  const int lpr = r_lpr(width, R_LN_BWD);
+  const int steps = lpr ? r_bwd_rows_per_warp(rows) / (32 / lpr) : 0;
+  const unsigned nblk = lpr ? unsigned((rows + ROWS_PER_BLOCK * (32 / lpr) * steps - 1) / (ROWS_PER_BLOCK * (32 / lpr) * steps)) : blocks;
+  DetParts dp;
+  dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width);
+  if (int rc = dp.begin(st)) return rc;
+  if (lpr) {
     if (lpr == 8) arb_launch(ln_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
     else arb_launch(ln_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
-    return check_launch();
+  } else {
+    ARB_DISPATCH_NV(width, (arb_launch(ln_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev)));
   }
-  ARB_DISPATCH_NV(width, (arb_launch(ln_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev)));
-  return check_launch();
+  if (int rc = check_launch()) return rc;
+  return dp.finish(st);
 }
 
 int pos_forward(float* x, const long long* indices, const uint8_t* mask, const float* pe, int pe_rows, float scale,
@@ -1643,7 +1653,7 @@ int act_forward(float* h, long long rows, int width, int act, DropSite site, cud
   if (width % 4) { arb_set_error("activation: width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   const long long n4 = rows * width / 4;
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * 8.0 * width, st);
-  const unsigned blocks = unsigned(std::min<long long>((n4 + 255) / 256, 148 * 16));
+  const unsigned blocks = unsigned(std::min<long long>((n4 + 255) / 256, 132 * 16));
   act_fwd_kernel<<<blocks, 256, 0, st>>>(h, n4, act, site, rows_dev, width / 4);
   return check_launch();
 }
@@ -1655,9 +1665,14 @@ int act_backward(const float* dh, const float* h, float* dz, long long rows, int
   while (tx_n < width / 4 && tx_n < 256) tx_n *= 2;
   const int rpb = 64 * (256 / tx_n);
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * 12.0 * width, st);
-  act_bwd_kernel<<<unsigned((rows + rpb - 1) / rpb), 256, size_t(width) * 4, st>>>(dh, h, dz, rows, width, act, site, mul,
-                                                                                  tx_n, rpb, colsum_out, rows_dev);
-  return check_launch();
+  const unsigned blocks = unsigned((rows + rpb - 1) / rpb);
+  DetParts dp;
+  dp.add(colsum_out, blocks, 1, width, width);
+  if (int rc = dp.begin(st)) return rc;
+  act_bwd_kernel<<<blocks, 256, size_t(256 / tx_n) * width * 4, st>>>(dh, h, dz, rows, width, act, site, mul, tx_n, rpb,
+                                                                     colsum_out, rows_dev);
+  if (int rc = check_launch()) return rc;
+  return dp.finish(st);
 }
 
 int softmax_forward(float* sc, const uint8_t* mask, int B, int h, int S, int pitch, cudaStream_t st, DropSite site) {
@@ -1686,7 +1701,7 @@ int slate_extents(const uint8_t* mask, const float* dscores, int n_out, int B, i
 int convert_to_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
   const long long n4 = (n + 3) / 4;
   ProfScope ps(ARB_PROF_SCORER_SIMT, 6.0 * double(n), st);
-  arb_launch(to_bf16_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n4 + 255) / 256, 148 * 8)))), dim3(256), 0, st,
+  arb_launch(to_bf16_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n4 + 255) / 256, 132 * 8)))), dim3(256), 0, st,
              reinterpret_cast<const float4*>(src), static_cast<uint2*>(dst), n);
   return check_launch();
 }
@@ -1696,8 +1711,12 @@ int colsum_accumulate(const float* in, long long rows, int width, long long ld, 
   const int rpb = 256;
   const unsigned blocks = unsigned((rows + rpb - 1) / rpb);
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * 4.0 * width, st);
+  DetParts dp;
+  dp.add(out, blocks, 1, width, width);
+  if (int rc = dp.begin(st)) return rc;
   ARB_DISPATCH_NV(width, (colsum_kernel<NV><<<blocks, 256, 0, st>>>(in, rows, width, ld, rpb, out)));
-  return check_launch();
+  if (int rc = check_launch()) return rc;
+  return dp.finish(st);
 }
 
 int head_forward(const float* x, const float* a, const float* b, float eps, const float* w, const float* wb,
@@ -1728,15 +1747,21 @@ int head_backward(const float* dscore, const float* score, const float* x, const
   const int rpw = bwd_rows_per_warp();
   const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * (8.0 * width + 16), st);
-  if (const int lpr = r_lpr(width, R_HEAD_BWD)) {
-    const int steps = r_bwd_rows_per_warp(rows) / (32 / lpr), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
-    const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
+  const int lpr = r_lpr(width, R_HEAD_BWD);
+  const int steps = lpr ? r_bwd_rows_per_warp(rows) / (32 / lpr) : 0;
+  const unsigned nblk = lpr ? unsigned((rows + ROWS_PER_BLOCK * (32 / lpr) * steps - 1) / (ROWS_PER_BLOCK * (32 / lpr) * steps)) : blocks;
+  DetParts dp;
+  if (has_norm) { dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); }
+  dp.add(grad_w, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width); dp.add(grad_wb, nblk, 1, 1, 1);
+  if (int rc = dp.begin(st)) return rc;
+  if (lpr) {
     if (lpr == 8) arb_launch(head_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
     else arb_launch(head_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
-    return check_launch();
+  } else {
+    ARB_DISPATCH_NV(width, (arb_launch(head_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, wb, has_norm, act, rows, width, rpw, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap)));
   }
-  ARB_DISPATCH_NV(width, (arb_launch(head_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, wb, has_norm, act, rows, width, rpw, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap)));
-  return check_launch();
+  if (int rc = check_launch()) return rc;
+  return dp.finish(st);
 }
 
 int head_multi_forward(const float* xf, const float* w, const float* wb, int act, long long rows, int width, int n,
@@ -1755,8 +1780,13 @@ int head_multi_backward(const float* dscore, const float* score, const float* xf
   const int rpw = bwd_rows_per_warp();
   const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * (8.0 * width + 8.0 * n), st);
+  DetParts dp;
+  dp.add(grad_w, blocks, 1, (long long)n * width, (long long)n * width); dp.add(grad_wb, blocks, 1, n, n);
+  dp.add(colsum_out, blocks, 1, width, width);
+  if (int rc = dp.begin(st)) return rc;
   ARB_DISPATCH_NV(width, (head_multi_bwd_kernel<NV><<<blocks, ROWS_PER_BLOCK * 32, 0, st>>>(dscore, score, xf, w, act, rows, width, n, rpw, dxf, grad_w, grad_wb, dx_masked, site, colsum_out)));
-  return check_launch();
+  if (int rc = check_launch()) return rc;
+  return dp.finish(st);
 }
 
 }  // namespace arb

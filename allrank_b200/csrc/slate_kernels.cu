@@ -941,7 +941,7 @@ extern "C" int32_t arb_rank_metrics(const float* y_pred, const float* y_true, in
 static int finalize(const float* val, const float* cnt, int B, int mode, float* loss, float* grad, size_t n_grad,
                     cudaStream_t st) {
   int blocks = 1;
-  if (mode != 0 && grad) blocks = int(std::min<size_t>((n_grad + 1023) / 1024, 148 * 4));
+  if (mode != 0 && grad) blocks = int(std::min<size_t>((n_grad + 1023) / 1024, 132 * 4));
   if (blocks < 1) blocks = 1;
   finalize_kernel<<<blocks, 256, 0, st>>>(val, cnt, B, mode, loss, grad, n_grad);
   arb_count_launch();

@@ -1,8 +1,8 @@
 """Data-parallel training over slates: one process per GPU, ONE NCCL all-reduce of the flat gradient buffer.
 
 The reference's only multi-GPU mechanism is single-process nn.DataParallel (allrank/main.py:76-78,
-allrank/models/model_utils.py:40-53).  Slates are independent (SURVEY.md 8e), so the B200-native equivalent
-shards the batch axis across ranks and sums gradients with a single `all_reduce` over NVLink 5 / NVSwitch:
+allrank/models/model_utils.py:40-53).  Slates are independent (SURVEY.md 8e), so the native equivalent
+shards the batch axis across ranks and sums gradients with a single `all_reduce` over NVLink / NVSwitch:
 the model's parameters are views of one flat buffer, so there is exactly one bucket (1.66 MB for the
 N=2,d=128 model, 12.8 MB for N=4,d=256) -- latency-bound, no bucketing logic needed.
 

@@ -1,8 +1,9 @@
 """One training step -- scorer forward, loss, backward, optimiser -- captured into a CUDA graph and replayed.
 
 At allRank's own batch size (64 slates) a step is some fifty kernels of 5-10 us each and the host, not the GPU, sets the
-pace: the Python / ctypes launch path costs more than the kernels run.  The C side of allrank_b200 neither allocates nor
-synchronises (DESIGN.md section 2), so the whole step captures into one graph; replaying it costs one launch.
+pace: the Python / ctypes launch path costs more than the kernels run.  The C side of allrank_b200 never synchronises
+and its only allocations are stream-ordered (DESIGN.md section 2: they become memory nodes owned by the graph), so the
+whole step captures into one graph; replaying it costs one launch.
 
     step = GraphedTrainStep(model, loss_fn, optimizer, x, y)     # x [B,S,F], y [B,S] on the device: shapes are fixed
     for xb, yb in loader:

@@ -5,7 +5,7 @@ allRank resolves its hot-path callables by NAME at run time:
     metric : getattr(allrank.models.metrics, name)                   allrank/training/train_utils.py:50
     model  : allrank.models.model.make_model(...)                    allrank/main.py:75
 so `patch_allrank()` only has to rebind those attributes; `allrank/main.py` and `train_utils.fit` then run
-unchanged on the B200 kernels.  (allRank must be importable; nothing here imports it otherwise.)
+unchanged on the CUDA kernels.  (allRank must be importable; nothing here imports it otherwise.)
 
 The callers either side of the path (SURVEY.md 8(f) ranks 3-4) are rebound the same way:
     epoch metrics : allrank.training.train_utils.{metric_on_epoch, compute_metrics}    train_utils.py:37-56
@@ -33,7 +33,7 @@ _MODULES = {"losses": "allrank.models.losses", "metrics": "allrank.models.metric
 
 def single_process_model(model):
     """Stands in for allrank.models.model_utils.CustomDataParallel when allrank/main.py:76-78 runs on a box with
-    several visible GPUs.  The B200 path scales as ONE PROCESS PER GPU (torchrun + allrank_b200.ddp.FlatDDP, a single
+    several visible GPUs.  The CUDA path scales as ONE PROCESS PER GPU (torchrun + allrank_b200.ddp.FlatDDP, a single
     NCCL all-reduce of the flat gradient); single-process nn.DataParallel would replicate a model whose parameters
     are views of one flat device buffer, which cannot work.  The model is returned unwrapped and trains on the device
     allRank selects (cuda:0 of the visible devices): launch one process per GPU with CUDA_VISIBLE_DEVICES / torchrun."""
@@ -49,7 +49,7 @@ def _rebind(saved, mod_key, name, fn):
 
 def patch_allrank(patch_model=True, patch_eval=True, patch_data=False):
     """Rebind allrank.models.{losses,metrics}.<name> (and make_model, the epoch-metric helpers, rank_slates and --
-    opt-in -- the slate loaders) to the B200 implementations.
+    opt-in -- the slate loaders) to the CUDA implementations.
     Returns the dict of original callables so the caller can restore them."""
     import allrank.models.losses as ref_losses
     import allrank.models.metrics as ref_metrics

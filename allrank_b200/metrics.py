@@ -1,6 +1,6 @@
 """Drop-in replacements for allrank.models.metrics -- same names, arguments and defaults
 (/root/reference/allrank/models/metrics.py: ndcg :7-28, dcg :41-77, mrr :80-113), computed by one
-sm_100a kernel launch per call (csrc/slate_kernels.cu: metrics_kernel) through the C ABI.
+sm_90a kernel launch per call (csrc/slate_kernels.cu: metrics_kernel) through the C ABI.
 
 `metric(y_pred, y_true, ats=...) -> [B, len(ats)]` fp32 on the input device, as consumed by
 allrank/training/train_utils.py:32-56.

@@ -1,4 +1,4 @@
-"""Drop-in replacement for allrank.models.model.make_model / LTRModel on B200.
+"""Drop-in replacement for allrank.models.model.make_model / LTRModel on the GPU.
 
 Same call surface as the reference (/root/reference/allrank/models/model.py):
 
@@ -13,7 +13,7 @@ and the same state_dict keys and shapes as the reference's module tree (so a ref
 `encoder.norm.{a_2,b_2}`, `output_layer.w_1.{weight,bias}`; same initialisation order (nn.Linear defaults,
 clones share the prototype's bias, xavier_uniform_ on every parameter with dim > 1: model.py:148-150).
 
-The forward and backward passes are fixed launch sequences inside liballrank_b200.so (csrc/scorer.cu): tcgen05
+The forward and backward passes are fixed launch sequences inside liballrank_b200.so (csrc/scorer.cu): tensor-core
 TF32 GEMMs + fp32 SIMT kernels.  The nn.Parameters are views of ONE flat fp32 buffer and their .grad are views of
 one flat gradient buffer -- which is what makes the single-bucket NCCL all-reduce (allrank_b200/ddp.py) and
 flat optimisers possible.  There is no eager fallback: CPU tensors raise.
@@ -174,7 +174,7 @@ class _ScorerFn(torch.autograd.Function):
 
 
 class LTRModel(nn.Module):
-    """B200 scorer with the reference LTRModel's surface (model.py:47-92)."""
+    """CUDA scorer with the reference LTRModel's surface (model.py:47-92)."""
 
     def __init__(self, n_features, d_model, n_layers, n_heads, d_ff, dropout, output_activation, fc_dropout=0.0,
                  positional=None, d_output=1, fc_sizes=None, fc_activation=None, input_norm=False,
@@ -241,7 +241,7 @@ class LTRModel(nn.Module):
     # ---- arithmetic of the encoder's matrix products ------------------------------------------------
     @property
     def compute_dtype(self):
-        """"tf32" (default): tcgen05 kind::tf32 products on fp32 data.  "bf16": every encoder linear is a kind::f16
+        """"tf32" (default): tensor-core tf32 products on fp32 data.  "bf16": every encoder linear is a tensor-core
         product of bfloat16 operands with fp32 accumulation -- bfloat16 shadow of the fp32 master weights, bfloat16
         LayerNorm outputs / attention context / FFN hidden layer and product-only gradients; residual stream,
         normalisation statistics, softmax, attention scores, head, loss and parameter gradients stay fp32

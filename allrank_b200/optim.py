@@ -2,7 +2,7 @@
 
 The reference builds its optimiser by name from the config (allrank/main.py:82, `getattr(optim, name)`); any
 torch optimiser works unchanged on allrank_b200 models because their parameters are ordinary nn.Parameters.
-FlatAdam is the B200-native alternative for the flat storage: it steps every parameter of the model with one
+FlatAdam is the native alternative for the flat storage: it steps every parameter of the model with one
 128-bit-vectorised launch (csrc/optim.cu), and optionally folds the 1/world_size of a sum all-reduce in.
 """
 import ctypes

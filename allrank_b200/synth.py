@@ -4,7 +4,7 @@ Shapes and conventions follow the reference's data pipeline
 (/root/reference/allrank/data/dataset_loading.py:15-16,29,88-93): features fp32 `[B,S,F]` zeroed on
 padded rows, labels fp32 `[B,S]` holding small integers with -1 = padding, indices int64 `[B,S]`
 with -1 = padding.  Label marginals approximate MSLR-WEB30K; true slate lengths ~ N(120, 60)
-clipped to [1, S].  No dataset is read: there is no network on the build or GPU boxes.
+clipped to [1, S].  No dataset is read: the benchmark and the tests need no download.
 """
 import torch
 

@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""Benchmark of the allRank hot path on B200: slates/sec of a full training step
+"""Benchmark of the allRank hot path on H100: slates/sec of a full training step
 (scorer forward + listwise loss + backward + Adam) on synthetic MSLR-WEB30K-shaped slates.
 
     python bench.py --gpus 1 --steps 20 --warmup 5                  # this repo's CUDA path
     python bench.py --impl reference --steps 5 --warmup 3           # the reference's eager CPU path (oracle port)
+    python bench.py --steps 20 --dump-outputs DIR                   # + the last timed step's outputs as DIR/*.npy
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 Prints ONE JSON line (rank 0).  Contract: see the task statement; fields are documented in DESIGN.md section 6.
-Workloads (BASELINE.json configs):
+Workloads (BASELINE.json configs; default batches sized for one 80 GB H100):
     cfg2  Transformer(N=2,h=4,d=128,d_ff=512) + approxNDCGLoss, S=240, F=136      <- the metric's configuration
     cfg3  Transformer(N=4,h=8,d=256,d_ff=1024) + lambdaLoss(ndcgLoss2PP), S=240
     cfg4  Transformer(N=2,h=4,d=128,d_ff=512) + neuralNDCG, S=120
@@ -30,11 +31,11 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     "cfg2": dict(N=2, h=4, d=128, dff=512, S=240, loss="approxNDCGLoss", loss_args={"alpha": 1.0}),
-    "cfg3": dict(N=4, h=8, d=256, dff=1024, S=240, loss="lambdaLoss",
+    "cfg3": dict(N=4, h=8, d=256, dff=1024, S=240, batch=1024, loss="lambdaLoss",
                  loss_args={"weighing_scheme": "ndcgLoss2PP_scheme", "k": None, "mu": 10.0, "sigma": 1.0}),
     "cfg4": dict(N=2, h=4, d=128, dff=512, S=120, loss="neuralNDCG",
                  loss_args={"temperature": 1.0, "k": None, "powered_relevancies": True}),
-    "cfg5": dict(N=4, h=8, d=256, dff=1024, S=240, loss="listMLE", loss_args={}),
+    "cfg5": dict(N=4, h=8, d=256, dff=1024, S=240, batch=1024, loss="listMLE", loss_args={}),
 }
 F = 136
 PAD = -1
@@ -54,11 +55,12 @@ def measured_peaks():
             p = json.load(fh)
         return dict(hbm_gbs=p["hbm_gbs"], bf16_tflops=p["bf16_tflops"],
                     bf16_tflops_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s -- not measured values
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -114,14 +116,14 @@ def dist_env():
 
 # ------------------------------------------------------------------------------------------------ CPU arm
 def reference_available():
-    return os.path.isfile(os.path.join(ROOT, "baseline", "_ref", "allrank", "main.py"))
+    return os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "allrank", "main.py"))
 
 
 def cpu_reference_steps(w, batch, steps, warmup, threads):
     """The reference's own eager PyTorch path on the host cores, one step = train_utils.loss_batch
     (allrank/training/train_utils.py:18-29: forward, loss, backward, Adam step, loss.item()).
-    kind "reference": the UNMODIFIED package installed in baseline/_ref (oracle/install_reference.py) -- its make_model,
-    its loss function, its loss_batch; kind "port": the oracle restatement (only when baseline/_ref is absent).
+    kind "reference": the UNMODIFIED package installed in oracle/_ref (oracle/install_reference.py) -- its make_model,
+    its loss function, its loss_batch; kind "port": the oracle restatement (only when oracle/_ref is absent).
     Must run in a process where CUDA is hidden: the reference hard-wires cuda:0 whenever a GPU is visible
     (allrank/models/model_utils.py:13-18)."""
     from allrank_b200.synth import make_slates
@@ -187,8 +189,8 @@ def run_reference(args, w):
     threads = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     batch = args.ref_batch
     sps, ms, used, kind = cpu_reference_steps(w, batch, args.steps, args.warmup, threads)
-    what = "the unmodified allRank package (baseline/_ref): make_model + loss + train_utils.loss_batch" \
-        if kind == "reference" else "oracle port of the reference (baseline/_ref absent)"
+    what = "the unmodified allRank package (oracle/_ref): make_model + loss + train_utils.loss_batch" \
+        if kind == "reference" else "oracle port of the reference (oracle/_ref absent)"
     sample = (f"{batch} slates/step x {args.steps} steps (S={w['S']}, F={F}), {what}, eager PyTorch fp32 on the host, "
               f"{used} intra-op threads (fastest of 8..{threads} on a {threads}-thread host)")
     out = {
@@ -204,14 +206,14 @@ def run_reference(args, w):
 
 
 def run_reference_gpu(args, w):
-    """Optional, stricter bar (SURVEY.md 8d): the UNMODIFIED reference (baseline/_ref) in eager PyTorch on the same
-    B200 -- its make_model, its loss, train_utils.loss_batch, torch.optim.Adam, fp32 (torch's default matmul precision),
+    """Optional, stricter bar (SURVEY.md 8d): the UNMODIFIED reference (oracle/_ref) in eager PyTorch on the same
+    GPU -- its make_model, its loss, train_utils.loss_batch, torch.optim.Adam, fp32 (torch's default matmul precision),
     inputs resident on the device.  One JSON line with impl "reference-gpu"."""
     rank, local_rank, world = dist_env()
     if rank != 0:
         return
     if not reference_available():
-        print(json.dumps({"impl": "reference-gpu", "unavailable": "baseline/_ref is not installed"}), flush=True)
+        print(json.dumps({"impl": "reference-gpu", "unavailable": "oracle/_ref is not installed"}), flush=True)
         return
     from oracle.install_reference import import_path
     sys.path[:0] = import_path()
@@ -246,7 +248,7 @@ def run_reference_gpu(args, w):
                       "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms,
                       "higher_is_better": True, "dtype": "f32", "data": "synthetic",
                       "config": workload_config(args, w, B),
-                      "note": "unmodified allRank (baseline/_ref) in eager PyTorch on cuda:0; loss.item() every step "
+                      "note": "unmodified allRank (oracle/_ref) in eager PyTorch on cuda:0; loss.item() every step "
                               "(train_utils.loss_batch)"}), flush=True)
 
 
@@ -268,7 +270,7 @@ def cpu_baseline_subprocess(args, w, steps=3, warmup=1):
 
 
 def workload_config(args, w, batch, live_frac=1.0):
-    # bytes one step touches: ~20 MB of activations per slate for cfg2 (profiles/README.md), inputs batch*S*F*4;
+    # bytes one step touches: the activations estimated below, inputs batch*S*F*4;
     # live_frac: the share of the B * S rows the encoder runs over (packed rows, include/allrank_b200.h)
     act_mb = live_frac * batch * w["S"] * (w["N"] * (10 * w["d"] + 2 * w["dff"]) + w["d"]) * 4 * 2 / 1e6
     return {"workload": f"{args.workload}: Transformer(N={w['N']},h={w['h']},d_model={w['d']},d_ff={w['dff']}) + "
@@ -303,7 +305,7 @@ def kernel_table(lib, psteps, peaks, dtype):
             continue
         flops = work if cls == 0 else 0.0
         nbytes = nbytes if cls == 0 else work          # non-GEMM classes state their algorithmic bytes as `work`
-        tensor_peak = bf16_peak if "_bf16" in name else tf32_peak     # kind::f16 products vs kind::tf32 products
+        tensor_peak = bf16_peak if "_bf16" in name else tf32_peak     # bf16 products vs tf32 products
         t_tensor = flops / (tensor_peak * 1e12) * 1e3
         t_hbm = nbytes / (peaks["hbm_gbs"] * 1e9) * 1e3
         bound = "tensor" if t_tensor >= t_hbm else "hbm"
@@ -367,9 +369,14 @@ def run_b200(args, w):
     if ddp:
         ddp.average = mode != "sum"              # lambdaLoss(reduction="sum") gradients are summed across ranks
 
+    last = {}                                          # --dump-outputs: the scores of the latest step
+
     def step(x, y):
         mask = y == PAD                                    # train_utils.py:19
-        loss = loss_fn(model(x, mask, None), y, **w["loss_args"])
+        scores = model(x, mask, None)
+        if args.dump_outputs:
+            last["scores"] = scores
+        loss = loss_fn(scores, y, **w["loss_args"])
         loss.backward()
         scale = 1.0
         if ddp:
@@ -425,6 +432,8 @@ def run_b200(args, w):
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     launches = launches_per_replay * args.steps if gstep else _lib.launch_count() - l0
     final_loss = loss.item()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, None if gstep else last["scores"], model)
 
     # ---- (2) end to end: every step's inputs come from pinned host memory (H2D inside the timed region, issued on
     #      a copy stream one step ahead, the way a training loop with a prefetching loader runs) and the loss is
@@ -533,11 +542,10 @@ def run_b200(args, w):
             "bound": top["bound"], "kernel": top["kernel"],
             "achieved": top["tflops"] if top["bound"] == "tensor" else top["gbs"],
             "peak": top["tensor_peak"] if top["bound"] == "tensor" else peaks["hbm_gbs"], "unit": unit, "frac": top["frac"],
-            "traffic": measured_traffic(args, B, top["kernel"]),
             "us_per_step": top["us_per_step"], "launches_per_step": top["launches_per_step"],
             "share_of_step": round(top["us_per_step"] / 1e3 / step_ms_profiled, 4) if step_ms_profiled else None,
             "peak_source": f"{peaks['source']} (MEASURED_PEAKS.json): tensor = bf16_tflops_sustained "
-                           f"{peaks['bf16_tflops_sustained']} for kind::f16 (bf16) products, half of it for kind::tf32 "
+                           f"{peaks['bf16_tflops_sustained']} for bf16 products, half of it for tf32 "
                            "products (tf32 issues at half the bf16 rate)" +
                            f", HBM = copy {peaks['hbm_gbs']} GB/s",
             "definition": "dominant kernel = largest device time per step; achieved = algorithmic flops (or bytes) of its "
@@ -561,20 +569,18 @@ def run_b200(args, w):
         dist.destroy_process_group()
 
 
-def measured_traffic(args, batch, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed ncu capture of
-    this exact workload / batch (profiles/r2_dram_traffic.json: {workload: {batch: {kernel: bytes}}}), else null."""
-    path = os.path.join(ROOT, "profiles", "r2_dram_traffic.json")
-    try:
-        with open(path) as f:
-            cap = json.load(f)
-        per_kernel = cap[args.workload][str(int(batch))]
-        for name, val in per_kernel.items():
-            if kernel.startswith(name):
-                return val
-    except (OSError, ValueError, TypeError, KeyError):
-        pass
-    return None
+def dump_outputs(out_dir, loss, scores, model):
+    """What the timed path hands its caller after its last step, as float32 .npy files: the loss, the scores (absent
+    when the step is replayed as a CUDA graph) and every parameter after the optimiser step."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().reshape(1)}
+    if scores is not None:
+        arrays["scores"] = scores.detach()
+    for name, p in model.named_parameters():
+        arrays["param." + name] = p.detach()
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
 
 
 def main():
@@ -586,8 +592,9 @@ def main():
     ap.add_argument("--workload", default="cfg2", choices=sorted(WORKLOADS))
     ap.add_argument("--dtype", default="tf32", choices=["tf32", "bf16"],
                     help="arithmetic of the encoder's tensor-core products (LTRModel.compute_dtype); fp32 elsewhere")
-    ap.add_argument("--batch", type=int, default=4096,
-                    help="slates per step per GPU (saturating batch; 64 = allRank's default batch_size, see profiles/)")
+    ap.add_argument("--batch", type=int, default=None,
+                    help="slates per step per GPU (default: the workload's saturating batch that fits 80 GB -- 4096, "
+                         "1024 for cfg3 / cfg5; 64 = allRank's default batch_size)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="weak: --batch slates per GPU; strong: --global-batch slates split over the GPUs")
     ap.add_argument("--global-batch", type=int, default=512, help="global batch of --scaling strong (SURVEY.md 8e)")
@@ -599,10 +606,15 @@ def main():
                     help="replay the training step as one CUDA graph (allrank_b200.graph.GraphedTrainStep; one GPU, "
                          "flat optimiser): for small batches, where the host's launch path sets the pace")
     ap.add_argument("--allow-short-warmup", action="store_true", help="(internal: the bounded CPU leg)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss, scores and updated parameters as DIR/*.npy "
+                         "(float32; the inputs and the initialisation are seeded, so runs with the same arguments compare)")
     args = ap.parse_args()
     if args.warmup < 3 and not args.allow_short_warmup:
         args.warmup = 3
     w = WORKLOADS[args.workload]
+    if args.batch is None:
+        args.batch = w.get("batch", 4096)
     if args.impl == "reference":
         os.environ["CUDA_VISIBLE_DEVICES"] = ""      # the reference hard-wires cuda:0 when it sees a GPU
         run_reference(args, w)

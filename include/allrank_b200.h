@@ -1,4 +1,4 @@
-/* allrank_b200 -- C ABI of the B200 (sm_100a) scoring + listwise-loss + metric path.
+/* allrank_b200 -- C ABI of the H100 (sm_90a) scoring + listwise-loss + metric path.
  *
  * This is the drop-in boundary (DESIGN.md section 2).  allRank is pure Python, so there is no
  * existing FFI to mirror; each entry point below replaces one *Python call surface* of the
@@ -9,8 +9,12 @@
  * Conventions
  *   - plain pointers + sizes only; no torch types.  All pointers are DEVICE pointers unless the
  *     parameter name ends in `_host`.  Tensors are row-major, contiguous, fp32 unless stated.
- *   - the library never allocates or frees device memory: outputs and workspaces are caller-owned
- *     (the host layer allocates them with PyTorch's caching allocator).
+ *   - outputs and workspaces are caller-owned (the host layer allocates them with PyTorch's caching allocator).
+ *     The one allocation the library makes is stream-ordered scratch for its gradient reductions: a call that sums
+ *     partial results across blocks takes per-block slots with cudaMallocAsync on `stream`, adds them in a fixed
+ *     order (so gradients are bitwise reproducible) and releases them with cudaFreeAsync on the same stream before it
+ *     returns.  Calls on different streams never share slots; under stream capture the slots become memory nodes
+ *     owned by the graph.  No device memory is held between calls.
  *   - every call enqueues work on `stream` (a cudaStream_t passed as void*; NULL = legacy default
  *     stream) of the CURRENT device and returns without synchronising; calls are re-entrant.
  *   - return value: 0 = ok, <0 = ARB_E_* below; arb_last_error() gives a thread-local message.
@@ -152,7 +156,7 @@ int32_t arb_neural_sort_debug(const float* y_pred, const float* y_true, int32_t 
  * mask, PositionwiseFeedForward, residuals) -> final LayerNorm -> Linear(d_model -> 1) head (model.py:95-128).
  * Called from allrank/training/train_utils.py:20 (`model(xb, mask, indices)`) and :34 (`model.score`).
  *
- * Every matrix product runs on the tcgen05 tensor cores in TF32 with fp32 accumulation (csrc/gemm_tf32.cu);
+ * Every matrix product runs on the tensor cores in TF32 with fp32 accumulation (csrc/gemm_tf32.cu);
  * LayerNorm / softmax / head are fp32 SIMT kernels (csrc/scorer_kernels.cu).  Dropout masks are a counter-based
  * hash of (seed, layer, site, element index) fused into the producing kernels and regenerated in backward
  * (csrc/dropout.cuh); `seed` must be the same in the forward and the backward call of a step.
@@ -190,8 +194,8 @@ typedef struct arb_scorer_config {
   int32_t fc_act;       /* ARB_ACT_*: fc_model.activation applied after every FC linear, before its dropout          */
   int32_t fc_input_norm;/* fc_model.input_norm: nn.LayerNorm(n_features) (eps 1e-5, biased variance) on x first;
                            needs n_features % 4 == 0 (no feature padding)                                             */
-  int32_t bf16;         /* 1: bf16 mode of the encoder (BASELINE config 3): every encoder linear runs as a tcgen05
-                           kind::f16 product of bfloat16 operands with fp32 accumulation -- weights from a bfloat16
+  int32_t bf16;         /* 1: bf16 mode of the encoder (BASELINE config 3): every encoder linear runs as a tensor-core
+                           product of bfloat16 operands with fp32 accumulation -- weights from a bfloat16
                            shadow of the fp32 master parameters (refreshed by every forward call), activations that only
                            feed products (LayerNorm outputs, attention context, FFN hidden layer) and the gradients that
                            only feed products stored as bfloat16; residual stream, LayerNorm statistics, softmax,
@@ -221,7 +225,7 @@ int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float* params, c
                             float* workspace, int64_t workspace_floats, float* scratch, int64_t scratch_floats,
                             uint64_t seed, void* stream);
 
-/* 0: unfused attention (materialised logits + generic GEMMs); 1: fused tcgen05 attention forward kernel, unfused
+/* 0: unfused attention (materialised logits + generic GEMMs); 1: fused tensor-core attention forward kernel, unfused
  * backward; 2 (default): fused forward and backward kernels.  Fused kernels serve slates of <= 256 items (backward:
  * head width <= 32); other shapes use the unfused path automatically.  Process-wide; exists for A/B tests. */
 void arb_set_attention_mode(int32_t mode);
@@ -249,21 +253,20 @@ void arb_set_attention_bwd_persistent(int32_t on);
 int32_t arb_get_pack_rows(void);
 
 /* 1 (default): the kernels of a step are chained with programmatic dependent launch -- a kernel's prologue (barrier
- * init, TMEM allocation, tensor-map prefetch) overlaps its predecessor's last wave, and it blocks in griddepcontrol.wait
+ * init, tensor-map prefetch) overlaps its predecessor's last wave, and it blocks in griddepcontrol.wait
  * before its first global-memory access; 0: every launch fully serialised.  For A/B measurements. */
 void arb_set_pdl(int32_t on);
 
-/* 1 (default): the fused attention forward runs as the two-pass / two-CTAs-per-SM kernel (head width <= 32);
- * 0: the single-pass kernel that keeps the whole S x S tile in TMEM (one CTA per SM). For A/B measurements. */
+/* Accepted for compatibility: every setting runs the same fused attention forward kernel. */
 void arb_set_attention_fwd_two_pass(int32_t on);
 
 /* GEMM kernel choice.  0: one CTA per output tile everywhere; 1: the persistent, decoupled-pipeline kernel (one CTA per
  * SM walking all tiles) wherever it is supported; 2 (default): persistent for every unbatched, non-split product except
- * short-K ones (K < 256) with a residual / mask tile -- the per-launch measurements of profiles/r2.  Process-wide; exists
+ * short-K ones (K < 256) with a residual / mask tile.  Process-wide; exists
  * for A/B measurements. */
 void arb_set_gemm_persistent(int32_t on);
 
-/* 1 (default): MMA operands are rounded fp32 -> tf32 by the TMA unit (TFLOAT32 tensor maps); 0: the tensor core
+/* 1 (default): MMA operands are rounded fp32 -> tf32 (nearest even) as the kernels load them; 0: the tensor core
  * truncates.  Process-wide; exists for the precision tests. */
 void arb_set_tf32_round_on_load(int32_t enable);
 
@@ -273,7 +276,7 @@ int32_t arb_gemm_tf32(const float* A, const float* B, float* C, const float* aux
                       int64_t b_bstride, int64_t c_bstride, int32_t block_n, int32_t flags, float alpha,
                       int32_t split_k, void* stream);
 
-/* The same building block with bf16 operands (tcgen05 kind::f16, fp32 accumulation) -- the matrix products of the
+/* The same building block with bf16 operands (tensor-core bf16 MMA, fp32 accumulation) -- the matrix products of the
  * scorer's bf16 mode (BASELINE config 3).  A and B are bfloat16; C (and aux) bfloat16 when out_bf16 != 0, else fp32;
  * flags as for arb_gemm_tf32 (the ARB_GEMM_* values below); colsum_out: optional [N] bias-gradient accumulator. */
 int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const void* aux, const float* bias, int32_t M, int32_t N,
@@ -315,7 +318,7 @@ int32_t arb_gather_slates(const float* x, const float* y, const int32_t* order, 
                           float* x_out, float* y_out, void* stream);
 
 /* Per-launch device timing for bench.py's roofline: enable, run steps, collect per kernel class
- * (0 = tcgen05 GEMM [work = flops], 1 = scorer SIMT, 2 = losses, 3 = metrics, 4 = optimiser, 5 = slate assembly /
+ * (0 = tensor-core GEMM [work = flops], 1 = scorer SIMT, 2 = losses, 3 = metrics, 4 = optimiser, 5 = slate assembly /
  * gather [work = bytes]). */
 void arb_prof_enable(int32_t on);
 int32_t arb_prof_collect(int32_t cls, double* total_ms, double* total_work, int64_t* launches);

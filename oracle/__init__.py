@@ -21,7 +21,7 @@ function cites the reference file:line it follows.
 
 Pinning
 -------
-The reference is pure Python and importable in the build container (behind the
+The reference is pure Python and importable wherever an allRank source tree is available (behind the
 three stub modules in ``oracle/_stubs``).  ``oracle/make_golden.py`` imports the
 *unmodified* reference from ``/root/reference``, runs it on seeded inputs and
 commits the input/output vectors under ``tests/golden/``; ``tests/test_oracle_*``

@@ -1,5 +1,5 @@
-"""Stub so the read-only allRank reference can be imported in the build container
-(only used by oracle/make_golden.py; never on the GPU box, never by the product)."""
+"""Stub so the read-only allRank reference can be imported without its optional cloud / logging dependencies
+(only used by the oracle and the tests; never by the product)."""
 
 
 class GCSFileSystem:

@@ -1,13 +1,12 @@
-"""Install the UNMODIFIED reference package into baseline/_ref (git-ignored, travels to the GPU box with the gpurun
-snapshot) -- TEST / BENCH INFRASTRUCTURE, run in the build container only (needs /root/reference).
+"""Install the UNMODIFIED reference package into oracle/_ref (git-ignored) -- TEST / BENCH INFRASTRUCTURE, run where
+an allRank source tree is available ($ALLRANK_REFERENCE, default /root/reference).
 
     python oracle/install_reference.py
 
-Recipe (the task's reference-arm rule): pip install --no-index --no-build-isolation --no-deps --find-links
-/opt/wheelhouse --target baseline/_ref <copy of /root/reference under /tmp>   (the tree itself is read-only and the
-pinned dependency versions -- torch 1.13, numpy <= 1.21 ... -- do not exist here, hence --no-deps; the three
-missing pure-Python dependencies are the stubs in oracle/_stubs).  Nothing of the reference enters the repository:
-baseline/_ref is listed in .gitignore.
+Recipe: pip install --no-index --no-build-isolation --no-deps --target oracle/_ref <copy of the source tree in a
+temporary directory>  (the source tree may be read-only; its pinned dependency versions -- torch 1.13, numpy <= 1.21
+... -- are not what this project runs on, hence --no-deps; the three missing pure-Python dependencies are the stubs in
+oracle/_stubs).  Nothing of the reference enters the repository: oracle/_ref is listed in .gitignore.
 """
 import os
 import shutil
@@ -16,8 +15,8 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SRC = "/root/reference"
-TARGET = os.path.join(ROOT, "baseline", "_ref")
+REF_SRC = os.environ.get("ALLRANK_REFERENCE", "/root/reference")
+TARGET = os.path.join(ROOT, "oracle", "_ref")
 
 
 def installed():
@@ -28,7 +27,7 @@ def install(force=False):
     if installed() and not force:
         return TARGET
     if not os.path.isdir(os.path.join(REF_SRC, "allrank")):
-        raise RuntimeError("the reference tree is not present on this box; baseline/_ref must come with the snapshot")
+        raise RuntimeError(f"no allRank source tree at {REF_SRC} (set ALLRANK_REFERENCE)")
     shutil.rmtree(TARGET, ignore_errors=True)
     os.makedirs(TARGET, exist_ok=True)
     tmp = tempfile.mkdtemp(prefix="allrank_src_")
@@ -36,7 +35,7 @@ def install(force=False):
         src = os.path.join(tmp, "reference")
         shutil.copytree(REF_SRC, src, ignore=shutil.ignore_patterns(".git", "__pycache__"))
         cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps",
-               "--find-links", "/opt/wheelhouse", "--target", TARGET, src]
+               "--target", TARGET, src]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0 or not installed():
             # last resort: the package is pure Python -- copy the package directory as it is
@@ -47,7 +46,7 @@ def install(force=False):
 
 
 def import_path():
-    """sys.path entries that make `import allrank` resolve to baseline/_ref behind the three stub modules."""
+    """sys.path entries that make `import allrank` resolve to oracle/_ref behind the three stub modules."""
     return [os.path.join(ROOT, "oracle", "_stubs"), TARGET]
 
 

@@ -1,11 +1,11 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference (run in the build container only).
+"""Generate tests/golden/*.npz from the UNMODIFIED reference (run where an allRank source tree is available).
 
     PYTHONDONTWRITEBYTECODE=1 python oracle/make_golden.py
 
-Imports /root/reference/allrank behind oracle/_stubs (gcsfs / tensorboardX / flatten_dict are the
-only missing deps) with CUDA hidden (model_utils.get_torch_device() hard-wires cuda:0), runs the
-reference on seeded inputs and stores inputs + outputs.  /root/reference does not exist on the GPU
-box, so tests only ever read the committed .npz files.
+Imports the allRank source tree ($ALLRANK_REFERENCE, default /root/reference) behind oracle/_stubs (gcsfs /
+tensorboardX / flatten_dict are the only missing deps) with CUDA hidden (model_utils.get_torch_device() hard-wires
+cuda:0), runs the reference on seeded inputs and stores inputs + outputs.  The tests only ever read the committed
+files in tests/golden.
 """
 import os
 import sys
@@ -13,7 +13,7 @@ import sys
 os.environ["CUDA_VISIBLE_DEVICES"] = ""
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-sys.path[:0] = [os.path.join(HERE, "_stubs"), "/root/reference", ROOT]
+sys.path[:0] = [os.path.join(HERE, "_stubs"), os.environ.get("ALLRANK_REFERENCE", "/root/reference"), ROOT]
 sys.dont_write_bytecode = True
 
 import numpy as np  # noqa: E402
@@ -467,9 +467,34 @@ def gen_init():
     print("init:", len(blob), "tensors")
 
 
+def gen_signatures():
+    """Parameter names of every reference callable the integration patch replaces, in order
+    (tests/test_integration_patch.py compares the package's call surfaces with them)."""
+    import inspect
+    import json
+    import allrank.data.dataset_loading as ref_dl
+    import allrank.inference.inference_utils as ref_iu
+    import allrank.models.model as ref_model
+    import allrank.training.train_utils as ref_tu
+    from allrank_b200 import integration
+    sig = lambda f: list(inspect.signature(f).parameters)
+    out = {"losses": {n: sig(getattr(ref_losses, n)) for n in integration.LOSS_NAMES},
+           "metrics": {n: sig(getattr(ref_metrics, n)) for n in integration.METRIC_NAMES},
+           "model": {"make_model": sig(ref_model.make_model)},
+           "train_utils": {n: sig(getattr(ref_tu, n)) for n in ("metric_on_batch", "metric_on_epoch", "compute_metrics")},
+           "inference_utils": {"rank_slates": sig(ref_iu.rank_slates)},
+           "dataset_loading": {n: sig(getattr(ref_dl, n)) for n in ("load_libsvm_dataset", "load_libsvm_dataset_role",
+                                                                    "load_libsvm_role", "create_data_loaders")},
+           "constants": {"PADDED_Y_VALUE": ref_dl.PADDED_Y_VALUE, "PADDED_INDEX_VALUE": ref_dl.PADDED_INDEX_VALUE}}
+    with open(os.path.join(OUT, "reference_signatures.json"), "w") as fh:
+        json.dump(out, fh, indent=1, sort_keys=True)
+    print("signatures:", sum(len(v) for v in out.values()), "entries")
+
+
 if __name__ == "__main__":
     torch.set_num_threads(4)
     gens = {"losses": gen_losses, "listmle": gen_listmle, "bce": gen_bce, "ordinal": gen_ordinal, "metrics": gen_metrics,
-            "scorer": gen_scorer, "scorer_pe": gen_scorer_pe, "scorer_multi": gen_scorer_multi, "scorer_shipped": gen_scorer_shipped, "neural_sort": gen_neural_sort, "slates": gen_slates, "init": gen_init}
+            "scorer": gen_scorer, "scorer_pe": gen_scorer_pe, "scorer_multi": gen_scorer_multi, "scorer_shipped": gen_scorer_shipped, "neural_sort": gen_neural_sort, "slates": gen_slates, "init": gen_init,
+            "signatures": gen_signatures}
     for name in (sys.argv[1:] or list(gens)):      # optionally: only the named generators
         gens[name]()

@@ -1,4 +1,4 @@
-"""Run the UNMODIFIED `allrank.main.run()` (baseline/_ref) on `generate_dummy_data.py` data -- TEST INFRASTRUCTURE for
+"""Run the UNMODIFIED `allrank.main.run()` (oracle/_ref) on `generate_dummy_data.py` data -- TEST INFRASTRUCTURE for
 the L3 parity layer (SURVEY.md 8c): once as the pure reference on the CPU, once with `patch_allrank()` on cuda:0.
 
     python oracle/run_reference_main.py --workdir DIR --config CONFIG.json [--patched] [--run-id NAME]
@@ -27,7 +27,7 @@ def main():
     sys.path.insert(0, ROOT)
     from oracle.install_reference import import_path, installed
     if not installed():
-        raise SystemExit("baseline/_ref is missing: run oracle/install_reference.py in the build container")
+        raise SystemExit("oracle/_ref is missing: run oracle/install_reference.py (needs an allRank source tree, $ALLRANK_REFERENCE)")
     sys.path[:0] = import_path()
     os.makedirs(a.workdir, exist_ok=True)
     os.chdir(a.workdir)

@@ -2,7 +2,7 @@
 
 Same maths as oracle/scorer_ref.py (reference: allrank/models/{model,transformer}.py), but every matrix
 product -- forward and backward -- sees its operands with the mantissa cut to 10 bits, which is what the
-tcgen05 kind::tf32 datapath does to fp32 operands; accumulation stays fp32/fp64.  It separates "TF32 rounding"
+tensor-core tf32 datapath does to fp32 operands; accumulation stays fp32/fp64.  It separates "TF32 rounding"
 from "kernel bug" when the CUDA scorer is compared with the fp32 reference: the CUDA path must agree with this
 emulation much more tightly than with the fp32 oracle.
 """

@@ -1,5 +1,5 @@
 """bench.py contract on the CPU side: the reference arm (`--impl reference`) runs without a GPU -- the unmodified
-allRank package from baseline/_ref when it is installed (oracle/install_reference.py), else the oracle port -- and
+allRank package from oracle/_ref when it is installed (oracle/install_reference.py), else the oracle port -- and
 prints ONE JSON line with the keys the driver reads."""
 import json
 import os

@@ -1,5 +1,5 @@
 """bf16 mode of the scorer (BASELINE config 3: Transformer(N=4, h=8, d=256) + lambdaLoss ndcgLoss2++, bf16):
-every encoder linear is a tcgen05 kind::f16 product of bfloat16 operands with fp32 accumulation; residual stream,
+every encoder linear is a tensor-core product of bfloat16 operands with fp32 accumulation; residual stream,
 LayerNorm statistics, softmax, head, loss and parameter gradients stay fp32.
 Bounds: SURVEY.md 8(c) L2 for bf16 -- score abs error <= 6e-2 at unit-scale scores, NDCG@10 within 5e-3, loss within
 1e-2 relative of the fp32 oracle -- and an order tighter against the bf16-operand emulation of the same maths

@@ -113,8 +113,8 @@ def test_fc_block_train_mode_uses_the_same_masks_forward_and_backward(case):
         # forward (the fused attention rounds the un-normalised probabilities, the eager maths the normalised ones: scores
         # agree to 1e-3).  A hidden unit whose pre-activation lies within that noise of zero then has ReLU derivative 1 on
         # one side and 0 on the other; a fraction f of such units moves the gradients BELOW the first ReLU by ~sqrt(f)
-        # (measured: 2-8 % on these small models, 0.03 % with the unfused attention path whose rounding matches the
-        # eager maths exactly -- profiles/r2/call4_debug_case2.log, call5_debug_attn_dropout.log), while gradients above
+        # (2-8 % on these small models, 0.03 % with the unfused attention path whose rounding matches the eager maths
+        # exactly), while gradients above
         # it (w_2, final norm, head) agree to 1e-3.  Mask mismatches would show as O(1) errors everywhere.
         tight = N == 0 or any(t in k for t in above_relu)
         assert v <= (3e-2 if tight else 1e-1), (k, v)

@@ -1,4 +1,4 @@
-"""The tcgen05/TMA TF32 GEMM building block against a plain PyTorch fp32 reference of the same op.
+"""The TMA + tensor-core TF32 GEMM building block against a plain PyTorch fp32 reference of the same op.
 
 TF32 keeps 10 mantissa bits of each operand (truncation by the tensor core datapath), fp32 accumulate:
 tolerance = 2^-10 relative per operand -> |err| <= ~2e-3 * sqrt(K)-ish of the operand scale; we bound by

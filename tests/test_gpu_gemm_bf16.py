@@ -1,4 +1,4 @@
-"""The bf16 variant of the tcgen05/TMA GEMM building block (kind::f16 operands, fp32 accumulation; BASELINE config 3's
+"""The bf16 variant of the TMA + tensor-core GEMM building block (bf16 operands, fp32 accumulation; BASELINE config 3's
 arithmetic) against a plain PyTorch reference of the same op.  bf16 x bf16 products are exact in fp32, so with fp32
 outputs only the summation order differs (tolerance 1e-5 of sum |a||b|); bf16 outputs add one rounding (2^-8 relative)."""
 import ctypes

@@ -251,7 +251,7 @@ def _set_attention_mode(mode):
                                    dict(F=136, d=128, N=1, h=2, dff=256, B=5, S=256),      # dk = 64, S = 256
                                    dict(F=136, d=64, N=1, h=2, dff=128, B=3, S=129)])
 def test_fused_attention_matches_unfused_path(shape):
-    """The fused tcgen05 attention kernel (S x S tile only in TMEM) against the materialised generic-GEMM path."""
+    """The fused tensor-core attention kernels (S x S tile only in registers) against the materialised generic-GEMM path."""
     from allrank_b200.model import make_model
     from allrank_b200.synth import make_slates
     F, d, N, h, dff, B, S = (shape[k] for k in ("F", "d", "N", "h", "dff", "B", "S"))
@@ -453,6 +453,42 @@ def test_skipping_padding_tiles_is_bit_identical_to_dense_tiles():
             finally:
                 lib.arb_set_attention_skip_padding(1)
         assert torch.equal(out[1][0], out[0][0]), p
-        # (the weight-gradient GEMMs reduce with red.add in a run-dependent order: equal up to fp32 summation order)
+        # (skipping changes how many tiles and splits the gradient reductions add up: equal up to fp32 summation order)
         gap = (out[1][1] - out[0][1]).abs().max().item()
         assert gap <= 2e-6 * out[0][1].abs().max().item(), (p, gap)
+
+
+@pytest.mark.parametrize("rows", ["dense", "packed"])
+@pytest.mark.parametrize("gemm_mode", [0, 2])
+def test_backward_is_bitwise_reproducible(rows, gemm_mode):
+    """No gradient reduction depends on the order in which blocks finish (include/allrank_b200.h: every cross-block
+    sum goes through per-block slots added in a fixed order): the same forward + backward from the same state gives
+    bit-identical scores and gradients -- including the gradients that are mathematically zero under a listwise loss
+    (output bias, final LayerNorm bias, key-projection biases), which are pure rounding noise that Adam would otherwise
+    turn into run-dependent steps."""
+    from allrank_b200 import _lib, losses
+    from allrank_b200.model import make_model
+    from allrank_b200.synth import make_slates
+    lib = _lib.lib()
+    lib.arb_set_pack_rows(1 if rows == "packed" else 0)
+    lib.arb_set_gemm_persistent(gemm_mode)
+    try:
+        torch.manual_seed(5)
+        model = make_model(fc_model={"sizes": [128], "input_norm": False, "activation": None, "dropout": 0.0},
+                           transformer={"N": 2, "d_ff": 512, "h": 4, "positional_encoding": None, "dropout": 0.0},
+                           post_model={"d_output": 1, "output_activation": None}, n_features=136).cuda().train()
+        x, y, _ = make_slates(512, 240, 136, seed=23)
+        x, y = x.cuda(), y.cuda()
+        runs = []
+        for _ in range(3):
+            model.zero_grad(set_to_none=True)
+            s = model(x, y == -1, None)
+            losses.approxNDCGLoss(s, y).backward()
+            runs.append((s.detach().clone(), {k: p.grad.detach().clone() for k, p in model.named_parameters()}))
+        for s, g in runs[1:]:
+            assert torch.equal(s, runs[0][0])
+            for k, v in g.items():
+                assert torch.equal(v, runs[0][1][k]), k
+    finally:
+        lib.arb_set_pack_rows(_lib.default_pack_rows())
+        lib.arb_set_gemm_persistent(2)

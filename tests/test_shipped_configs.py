@@ -131,8 +131,8 @@ def test_shipped_config_trains_with_its_dropout_like_the_reference_maths(golden,
         # forward (the fused attention rounds the un-normalised probabilities, the eager maths the normalised ones: scores
         # agree to 1e-3).  A hidden unit whose pre-activation lies within that noise of zero then has ReLU derivative 1 on
         # one side and 0 on the other; a fraction f of such units moves the gradients BELOW the first ReLU by ~sqrt(f)
-        # (measured: 2-8 % on these small models, 0.03 % with the unfused attention path whose rounding matches the
-        # eager maths exactly -- profiles/r2/call4_debug_case2.log, call5_debug_attn_dropout.log), while gradients above
+        # (2-8 % on these small models, 0.03 % with the unfused attention path whose rounding matches the eager maths
+        # exactly), while gradients above
         # it (w_2, final norm, head) agree to 1e-3.  Mask mismatches would show as O(1) errors everywhere.
         last = f"encoder.layers.{N - 1}.feed_forward.w_2" if N else "output_layer"
         tight = N == 0 or k.startswith(last) or k.startswith("encoder.norm") or k.startswith("output_layer")
