@@ -16,8 +16,8 @@
 
 namespace arb {
 
-constexpr int BWD_THREADS = 256;          // 8 warps x 16 rows of a 128-row tile
-constexpr int TILE_BYTES = 128 * 128;     // one [128 rows][128 B] operand tile
+constexpr int BWD_WARPS = 8;              // each computes one 16-row strip at a time
+constexpr int BWD_THREADS = 32 * BWD_WARPS;
 
 __device__ __forceinline__ float ex2_approx_b(float x) {
   float y;
@@ -81,28 +81,108 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
   }
 }
 
+// Shared-memory accesses of the backward's inner loops, by 32-bit shared-window address (ld.shared / ldmatrix /
+// st.shared).
+__device__ __forceinline__ uint4 lds128(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ uint2 lds64(uint32_t a) {
+  uint2 v;
+  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a));
+  return v;
+}
+// four 8 x 4 fp32 matrices (8 x 8 b16): lane l gives the address of row l % 8 of matrix l / 8, and receives word
+// lane % 4 of row lane / 4 of each matrix
+__device__ __forceinline__ void ldsm_x4(uint32_t a, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+}
+__device__ __forceinline__ void sts128(uint32_t a, uint4 v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void sts64(uint32_t a, uint2 v) {
+  asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(v.x), "r"(v.y) : "memory");
+}
+
+// Operand rows in shared memory are 128 bytes (32 fp32; for dk = 16 TMA zero-fills columns 16..31), 128B-swizzled.
+// Every product keeps the standard assignment of its contraction index to the MMA k-slots (head dimension: slot t of
+// k-step ks is column 8 ks + t; queries / keys of an 8-row block: slot t is row t), so each output element is computed
+// by the same sequence of tensor-core operations as a straightforward fragment layout would use.  Only the positions
+// of output rows / columns inside an MMA are permuted, which changes where an element lands, not its value:
+//  * the second operand of S^T = K Q^T (S = Q K^T) takes row sigma(n) of its 8-row block as column n,
+//    sigma = {0, 4, 1, 5, 2, 6, 3, 7}: accumulator columns 2t, 2t + 1 are rows t, t + 4, which are exactly the k-slots
+//    of the lane's A fragment for the next product -- P / dS feed it without shuffles;
+//  * output column g of n-tile nt is head column 4 sigma(g) + nt (dk 32) or 2g + nt (dk 16): the B operand is one
+//    conflict-free 128-bit (64-bit) load per row, and a lane's accumulator holds 16-byte runs of its two rows.
+__device__ __forceinline__ int sigma8(int n) { return (n >> 1) + 4 * (n & 1); }
+// A fragments over the head dimension of the 16 rows r0 ... r0 + 15:
+// a[ks] = {X[r0 + g][8ks + t], X[r0 + g + 8][8ks + t], X[r0 + g][8ks + t + 4], X[r0 + g + 8][8ks + t + 4]}
+template <int KS>
+__device__ __forceinline__ void ld_a_head(uint32_t op, int r0, int lane, uint32_t (&a)[KS][4]) {
+  const int m = lane >> 3, r = r0 + (lane & 7) + 8 * (m & 1);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) ldsm_x4(op + uint32_t(r) * 128u + (uint32_t((2 * ks + (m >> 1)) ^ (r & 7)) << 4), a[ks]);
+}
+// B fragments over the head dimension of the 8 rows r0 + sigma(n): b[ks] = {X[r0 + sigma(g)][8ks + t], ...[8ks + t + 4]}
+template <int KS>
+__device__ __forceinline__ void ld_b_head(uint32_t op, int r0, int lane, uint32_t (&b)[KS][2]) {
+  const int r = r0 + sigma8(lane & 7);
+#pragma unroll
+  for (int p = 0; p < KS / 2; ++p) {
+    uint32_t x[4];
+    ldsm_x4(op + uint32_t(r) * 128u + (uint32_t((4 * p + (lane >> 3)) ^ (r & 7)) << 4), x);
+    b[2 * p][0] = x[0]; b[2 * p][1] = x[1]; b[2 * p + 1][0] = x[2]; b[2 * p + 1][1] = x[3];
+  }
+}
+// the B operand of an output product from row r: v[nt] = X[r][column of output column g in n-tile nt]
+template <int KS>
+__device__ __forceinline__ void ld_b_out(uint32_t op, int r, int g, uint32_t (&v)[KS]) {
+  if constexpr (KS == 4) {
+    const uint4 x = lds128(op + uint32_t(r) * 128u + (uint32_t(sigma8(g) ^ (r & 7)) << 4));
+    v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+  } else {
+    const uint2 x = lds64(op + ptx::sw128(r, 8 * g));
+    v[0] = x.x; v[1] = x.y;
+  }
+}
+
+constexpr int BOX_BYTES = 16 * 128;       // one 16-row box of 128-byte rows
+constexpr int PART_BYTES = 128 * 128;     // one 128-row output tile of 128-byte rows
+constexpr int ITEM_ROW_BYTES = 4 * 128;   // Q, K, V, dO of one item row
+constexpr int POOL_ROWS_MAX = 352;        // item rows of the operand pool: two items of MSLR-shaped slates fit
+
 struct BwdSmem {
-  // operand tiles: Q, K, V, dO of the whole slate (up to 256 rows = two 128-row boxes each, DK <= 32 -> one 128-byte
-  // row per item), then the output staging tiles dV | dK | dQ
-  static constexpr int OPS = 4 * 2 * TILE_BYTES;
-  static constexpr int OUT_OFF = OPS;
-  static constexpr int STATS_OFF = OUT_OFF + 3 * TILE_BYTES;    // float2 {nm_q, delta_q} x 256
-  static constexpr int BITS_OFF = STATS_OFF + 256 * 8;          // 8 words: key is a real item
-  static constexpr int BARS_OFF = BITS_OFF + 64;
-  static constexpr int BIAS_OFF = BARS_OFF + 64;                // float [3 * d_model]: this CTA's QKV bias gradient
-  static int total(int d_model) { return BIAS_OFF + 12 * d_model + 1024; }
+  // [operand pool: pool_rows x (Q | K | V | dO) rows] [output tile staging: dV | dK | dQ, 128 rows each] [zero box]
+  // [float2 stats x 256] [key bits: 8 words] [2 mbarriers] [QKV bias gradient: 3 * d_model floats]
+  __host__ __device__ static int stage_off(int pool_rows) { return pool_rows * ITEM_ROW_BYTES; }
+  __host__ __device__ static int zero_off(int pool_rows) { return stage_off(pool_rows) + 3 * PART_BYTES; }
+  __host__ __device__ static int stats_off(int pool_rows) { return zero_off(pool_rows) + BOX_BYTES; }
+  __host__ __device__ static int bits_off(int pool_rows) { return stats_off(pool_rows) + 256 * 8; }
+  __host__ __device__ static int bars_off(int pool_rows) { return bits_off(pool_rows) + 64; }
+  __host__ __device__ static int bias_off(int pool_rows) { return bars_off(pool_rows) + 64; }
+  __host__ __device__ static int total(int pool_rows, int d_model) { return bias_off(pool_rows) + 12 * d_model + 1024; }
 };
 
-// One CTA walks the (slate, head) items item0, item0 + gridDim.x, ...  (one CTA per item, or -- persistent -- one per
-// SM).  Per item, eight warps run two phases on the tensor cores (mma.sync m16n8k8 tf32), each keeping its products
-// in registers:
-//   phase 1, per 128-key tile (warp = 16 keys):  S^T = K Q^T, dP^T = V dO^T over 8-query blocks,
-//            P^T = exp2(S^T c + nm_q) (key mask, dropout), dS^T = P^T * (dP^T - delta_q),
-//            dV += P^T dO,  dK += dS^T Q   (P^T / dS^T go straight from the accumulators into the next product)
-//   phase 2, per 128-query tile (warp = 16 queries):  S = Q K^T, dP = dO V^T over 8-key blocks, dS as above,
-//            dQ += dS K
-// with nm_q = -max_q c - log2 l_q from the forward's row statistics and c = log2(e) / sqrt(dk).  Outputs are staged in
-// shared memory and TMA-stored (+ the QKV bias column sums).
+// One CTA walks the (slate, head) items blockIdx.x, blockIdx.x + gridDim.x, ... (one CTA per item, or -- persistent --
+// one per SM).  An item's Q, K, V, dO rows below round_up(extent, 16) are TMA-loaded in 16-row boxes into an operand
+// pool that holds two items: even items of the CTA from its bottom, odd ones from its top.  The next item's loads are
+// issued before the current item's products when both fit, else as soon as the current item is done.  Once an item's
+// operands land they are rounded to tf32 in place.  Per 128-row tile of the item, its key strips (dK, dV) and query
+// strips (dQ) of 16 rows below round_up(extent, 16) are spread over the eight warps; a warp runs a strip on the tensor
+// cores (mma.sync m16n8k8 tf32) with its products in registers:
+//   key strip (16 keys):      S^T = K Q^T, dP^T = V dO^T over 8-query blocks, P^T = exp2(S^T c + nm_q) (key mask,
+//                             dropout), dS^T = P^T * (dP^T - delta_q), dV += P^T dO, dK += dS^T Q
+//   query strip (16 queries): S = Q K^T, dP = dO V^T over 8-key blocks, dS as above, dQ += dS K
+// with nm_q = -max_q c - log2 l_q from the forward's row statistics and c = log2(e) / sqrt(dk).  The warp stages its
+// finished strip in the tile staging and TMA-stores it as a 16-row box.  Once the tile is complete, the QKV bias
+// gradient takes its column sums, one thread per column adding the rows in order.
 template <int DK, bool DROP, bool OUT16 = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -111,275 +191,329 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
     const __grid_constant__ CUtensorMap tmDV, const uint8_t* __restrict__ mask, const float* __restrict__ stat_max,
     const float* __restrict__ stat_sum, const float* __restrict__ delta, int S, int n_heads, float scale, DropSite drop,
     float* __restrict__ dbias_qkv, int d_model, const int* __restrict__ extent, const int* __restrict__ pack_off,
-    int n_items, int rnd) {
+    int n_items, int rnd, int pool_rows) {
   constexpr int KS = DK / 8;
-  extern __shared__ uint8_t smem_dyn[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_s = smem;
-  uint8_t* k_s = smem + 2 * TILE_BYTES;
-  uint8_t* v_s = smem + 4 * TILE_BYTES;
-  uint8_t* do_s = smem + 6 * TILE_BYTES;
-  auto out_tile = [&](int which) { return smem + BwdSmem::OUT_OFF + which * TILE_BYTES; };   // 0 dV, 1 dK, 2 dQ
-  float2* qstats = reinterpret_cast<float2*>(smem + BwdSmem::STATS_OFF);
-  uint32_t* key_bits = reinterpret_cast<uint32_t*>(smem + BwdSmem::BITS_OFF);
-  uint64_t* load_bar = reinterpret_cast<uint64_t*>(smem + BwdSmem::BARS_OFF);
-  float* bias_acc = reinterpret_cast<float*>(smem + BwdSmem::BIAS_OFF);
+  constexpr int ROWB = OUT16 ? 64 : 128;    // bytes of a staged output row
+  extern __shared__ __align__(1024) uint8_t smem_dyn[];
+  const uint32_t sbase = (ptx::smem_u32(smem_dyn) + 1023u) & ~1023u;
+  uint8_t* smem = smem_dyn + (sbase - ptx::smem_u32(smem_dyn));
+  const uint32_t stats_s = sbase + BwdSmem::stats_off(pool_rows), bits_s = sbase + BwdSmem::bits_off(pool_rows);
+  float2* qstats = reinterpret_cast<float2*>(smem + BwdSmem::stats_off(pool_rows));
+  uint32_t* key_bits = reinterpret_cast<uint32_t*>(smem + BwdSmem::bits_off(pool_rows));
+  uint64_t* load_bar = reinterpret_cast<uint64_t*>(smem + BwdSmem::bars_off(pool_rows));
+  uint8_t* zero_box = smem + BwdSmem::zero_off(pool_rows);
+  float* bias_acc = reinterpret_cast<float*>(smem + BwdSmem::bias_off(pool_rows));
+  uint8_t* stage = smem + BwdSmem::stage_off(pool_rows);                       // part 0 dV, 1 dK, 2 dQ
+  const uint32_t stage_s = sbase + BwdSmem::stage_off(pool_rows);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  // Rows at or beyond a slate's extent are masked keys (probability exactly 0) whose d ctx rows are exactly zero:
-  // neither their key tiles nor their query tiles contribute anything, and their dQ / dK / dV rows are zero.  Only
-  // the tiles below the extent are processed; in the dense layout the rest is written as zeros.
-  // Packed rows (see attn_fwd_kernel): slate b holds its first ext16 = round_up(extent, 16) rows at row pack_off[b] of
-  // one long tensor.  Tiles that overrun the slate read other slates' rows: as keys they are masked, as queries their
-  // probabilities are forced to zero (their statistics are -inf); outputs are stored in 16-row boxes that stop at the
-  // slate's last packed row, and nothing is zero-filled.
-  const int n_full = (S + 127) / 128;
   const float c_log2e = scale * 1.4426950408889634f;
   const bool packed = pack_off != nullptr;
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmQ); ptx::prefetch_tmap(&tmK); ptx::prefetch_tmap(&tmV); ptx::prefetch_tmap(&tmDO);
     ptx::mbar_init(load_bar, 1);
+    ptx::mbar_init(load_bar + 1, 1);
     ptx::fence_barrier_init();
   }
+  for (int i = threadIdx.x; i < BOX_BYTES / 16; i += BWD_THREADS) reinterpret_cast<uint4*>(zero_box)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (dbias_qkv != nullptr)
     for (int i = threadIdx.x; i < 3 * d_model; i += BWD_THREADS) bias_acc[i] = 0.f;
+  ptx::fence_proxy_async_smem();
   arb_pdl_wait();
   __syncthreads();
 
-  // one operand word: element (r, e) of a [256][32] operand (two 128-row boxes)
-  auto op = [&](const uint8_t* base, int r, int e) -> uint32_t {
-    const float x = ptx::ld_f32(base + (r >> 7) * TILE_BYTES, r & 127, e);
-    return rnd ? ptx::cvt_tf32(x) : __float_as_uint(x);
-  };
-  auto key_live = [&](int key) { return (key_bits[key >> 5] >> (key & 31)) & 1u; };
-  // stage rows r, r + 8 (tile-relative) of an accumulator [KS][4] (x mul) into output tile `which`
-  auto stage_rows = [&](int which, int r, const float (&acc)[KS][4], float mul) {
-    uint8_t* ot = out_tile(which);
-#pragma unroll
-    for (int nt = 0; nt < KS; ++nt) {
-      const int e = 8 * nt + 2 * t;
-      if constexpr (OUT16) {
-        // bf16 mode: dQ / dK / dV only feed the QKV weight- and input-gradient products: dense bfloat16 rows of
-        // 32 columns (64 bytes), unswizzled tensor maps
-        *reinterpret_cast<uint32_t*>(ot + r * 64 + 2 * e) = ptx::pack_bf16(acc[nt][0] * mul, acc[nt][1] * mul);
-        *reinterpret_cast<uint32_t*>(ot + (r + 8) * 64 + 2 * e) = ptx::pack_bf16(acc[nt][2] * mul, acc[nt][3] * mul);
-      } else {
-        *reinterpret_cast<float2*>(ot + ptx::sw128(r, 4 * e)) = make_float2(acc[nt][0] * mul, acc[nt][1] * mul);
-        *reinterpret_cast<float2*>(ot + ptx::sw128(r + 8, 4 * e)) = make_float2(acc[nt][2] * mul, acc[nt][3] * mul);
-      }
-    }
-  };
-  // store output tiles [first, last] (staged by every warp) at tile row `tile` of item (b, head) and add their column
-  // sums to the QKV bias gradient; returns with the staging free again
-  auto flush = [&](int first, int last, int tile, int b, int head, int row_base, int ext16) {
-    ptx::fence_proxy_async_smem();
-    __syncthreads();
-    const CUtensorMap* maps[3] = {&tmDV, &tmDK, &tmDQ};
-    if (threadIdx.x == 0) {
-      for (int w = first; w <= last; ++w) {
-        if (packed) {      // 16-row boxes up to the slate's last packed row (staged rows are 128 / 64 bytes wide)
-          constexpr int BOX = OUT16 ? 1024 : 2048;
-          const int n16 = (min(128, ext16 - 128 * tile) + 15) >> 4;
-          for (int i = 0; i < n16; ++i) ptx::tma_store_4d(maps[w], out_tile(w) + i * BOX, 0, row_base + 128 * tile + 16 * i, head, 0);
-        } else {
-          ptx::tma_store_4d(maps[w], out_tile(w), 0, 128 * tile, head, b);
-        }
-      }
-      ptx::tma_store_commit();
-    }
-    if (dbias_qkv != nullptr) {
-      // bias gradient of the QKV projection: column sums of the staged tiles (rows the slate does not have are 0), added
-      // to the CTA's accumulator -- one thread per (tile, column), flushes ordered by the barriers around them
-      const int which = first + int(threadIdx.x) / DK, cc = int(threadIdx.x) % DK;
-      if (which <= last) {
-        const uint8_t* tl = out_tile(which);
-        float s = 0.f;
-#pragma unroll 8
-        for (int r = 0; r < 128; ++r) {
-          if constexpr (OUT16) s += __uint_as_float(uint32_t(*reinterpret_cast<const uint16_t*>(tl + r * 64 + cc * 2)) << 16);
-          else s += *reinterpret_cast<const float*>(tl + ptx::sw128(r, 4 * cc));
-        }
-        bias_acc[(which == 0 ? 2 * d_model : (which == 1 ? d_model : 0)) + head * DK + cc] += s;
-      }
-    }
-    if (threadIdx.x == 0) ptx::tma_store_wait_read();
-    __syncthreads();
-  };
-
-  uint32_t phase = 0;
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    const int b = item / n_heads, head = item - b * n_heads;
-    int e = extent ? __ldg(extent + b) : S;
-    if (packed && e <= 0) continue;               // packed rows: an empty slate holds no rows
+  // Rows at or beyond a slate's extent are masked keys (probability exactly 0) whose d ctx rows are exactly zero:
+  // neither their key strips nor their query strips contribute anything, and their dQ / dK / dV rows are zero.  Only
+  // the strips below round_up(extent, 16) are processed; in the dense layout the rows beyond are written as zeros.
+  // Packed rows (see attn_fwd_kernel): slate b holds its first ext16 = round_up(extent, 16) rows at row pack_off[b] of
+  // one long tensor -- exactly the rows loaded and stored here.  Its queries at or beyond S get probability zero
+  // through their statistics (-inf).
+  struct Item { int b, head, e, rows, q_lim, q_live, row_base, bc; };
+  auto item_info = [&](int item) {
+    Item it{};
+    it.b = item / n_heads;
+    it.head = item - it.b * n_heads;
+    int e = extent ? __ldg(extent + it.b) : S;
+    if (packed && e <= 0) return it;            // packed rows: an empty slate holds no rows (rows = 0: skipped)
     e = max(1, min(S, e));
-    const int n_kt = (e + 127) / 128;             // active key tiles == active query tiles
-    const int ext16 = (e + 15) & ~15;
-    const int q_lim = packed ? min(S, ext16) : S; // queries at or beyond it do not exist in this slate
+    it.e = e;
+    it.rows = (e + 15) & ~15;
+    it.q_lim = packed ? min(S, it.rows) : S;    // queries at or beyond it do not exist in this slate
     // queries at or beyond q_live contribute nothing (the dense layout's padding has zero d ctx rows; packed rows: the
     // slate has no such queries)
-    const int q_live = packed ? q_lim : (extent ? e : S);
-    const int row_base = packed ? __ldg(pack_off + b) : 0;
-    const int bc = packed ? 0 : b;
-    if (threadIdx.x == 0) {
-      ptx::fence_proxy_async_smem();
-      ptx::mbar_expect_tx(load_bar, 4 * n_kt * TILE_BYTES);
-      for (int kt = 0; kt < n_kt; ++kt) {
-        const int r = row_base + 128 * kt;
-        ptx::tma_load_4d(q_s + kt * TILE_BYTES, &tmQ, load_bar, 0, r, head, bc);
-        ptx::tma_load_4d(k_s + kt * TILE_BYTES, &tmK, load_bar, 0, r, head, bc);
-        ptx::tma_load_4d(v_s + kt * TILE_BYTES, &tmV, load_bar, 0, r, head, bc);
-        ptx::tma_load_4d(do_s + kt * TILE_BYTES, &tmDO, load_bar, 0, r, head, bc);
+    it.q_live = packed ? it.q_lim : (extent ? e : S);
+    it.row_base = packed ? __ldg(pack_off + it.b) : 0;
+    it.bc = packed ? 0 : it.b;
+    return it;
+  };
+  // pool offset of an item's rows: slot 0 from the bottom, slot 1 from the top
+  auto region_off = [&](int slot, int rows) { return slot ? (pool_rows - rows) * ITEM_ROW_BYTES : 0; };
+  // warp 0: an item's Q, K, V, dO rows in 16-row boxes (operand o at region + o * rows * 128), completing on load_bar[slot]
+  auto issue_loads = [&](const Item& it, int slot) {
+    const int nb = it.rows >> 4;
+    uint8_t* region = smem + region_off(slot, it.rows);
+    ptx::fence_proxy_async_smem();
+    if (lane == 0) ptx::mbar_expect_tx(load_bar + slot, uint32_t(it.rows) * ITEM_ROW_BYTES);
+    __syncwarp();
+    for (int j = lane; j < 4 * nb; j += 32) {
+      const int o = j / nb, i = j - o * nb;
+      const CUtensorMap* m = o == 0 ? &tmQ : (o == 1 ? &tmK : (o == 2 ? &tmV : &tmDO));
+      ptx::tma_load_4d(region + (o * it.rows + 16 * i) * 128, m, load_bar + slot, 0, it.row_base + 16 * i, it.head, it.bc);
+    }
+  };
+  // this thread's query row statistics of an item, fetched one item ahead
+  float r_max = 0.f, r_sum = 1.f, r_delta = 0.f;
+  bool r_key = false;
+  auto fetch_stats = [&](const Item& it) {
+    const int qi = threadIdx.x;
+    if (qi < it.q_lim) {
+      const size_t so = (size_t(it.b) * n_heads + it.head) * S + qi;
+      r_max = stat_max[so];
+      r_sum = stat_sum[so];
+      r_delta = delta[so];
+    }
+    r_key = qi < S && mask[size_t(it.b) * S + qi] == 0;
+  };
+  // a warp's finished strip of one output (rows g, g + 8 of its accumulator, x mul) into rows rt ... rt + 15 of
+  // staging part p
+  auto stage_strip = [&](int p, int rt, const float (&acc)[KS][4], float mul) {
+    const uint32_t part = stage_s + p * PART_BYTES;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rt + g + 8 * h;
+      float v[2][KS];      // v[0]: head columns of output column 2t, v[1]: of 2t + 1 (n-tile order)
+#pragma unroll
+      for (int nt = 0; nt < KS; ++nt) { v[0][nt] = acc[nt][2 * h] * mul; v[1][nt] = acc[nt][2 * h + 1] * mul; }
+      if constexpr (OUT16) {
+        // bf16 mode: dQ / dK / dV only feed the QKV weight- and input-gradient products: dense bfloat16 rows of 32
+        // columns (64 bytes), unswizzled tensor maps
+        if constexpr (KS == 4) {
+          sts64(part + r * 64 + 8 * t, make_uint2(ptx::pack_bf16(v[0][0], v[0][1]), ptx::pack_bf16(v[0][2], v[0][3])));
+          sts64(part + r * 64 + 32 + 8 * t, make_uint2(ptx::pack_bf16(v[1][0], v[1][1]), ptx::pack_bf16(v[1][2], v[1][3])));
+        } else {
+          sts64(part + r * 64 + 8 * t, make_uint2(ptx::pack_bf16(v[0][0], v[0][1]), ptx::pack_bf16(v[1][0], v[1][1])));
+        }
+      } else {
+        if constexpr (KS == 4) {
+          sts128(part + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[0][2]), __float_as_uint(v[0][3])));
+          sts128(part + ptx::sw128(r, 64 + 16 * t), make_uint4(__float_as_uint(v[1][0]), __float_as_uint(v[1][1]), __float_as_uint(v[1][2]), __float_as_uint(v[1][3])));
+        } else {
+          sts128(part + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[1][0]), __float_as_uint(v[1][1])));
+        }
       }
     }
-    {
-      // per-query statistics (nm = -max*c - log2(sum); -inf for queries the slate does not have) and the key mask
-      const int qi = threadIdx.x;
-      float2 st = make_float2(-CUDART_INF_F, 0.f);
-      if (qi < q_lim) {
-        const size_t so = (size_t(b) * n_heads + head) * S + qi;
-        st.x = -(stat_max[so] * c_log2e) - log2f(stat_sum[so]);
-        st.y = delta[so];
-      }
-      qstats[qi] = st;
-      const uint32_t w = __ballot_sync(FULL, qi < S && mask[size_t(b) * S + qi] == 0);
-      if (lane == 0) key_bits[warp] = w;
+  };
+  // lane 0: TMA-store rows rt ... rt + 15 of staging parts p0 (and p1 when >= 0) at rows row0 ... row0 + 15 of item it
+  auto store_strip = [&](const Item& it, int p0, const CUtensorMap* m0, int p1, const CUtensorMap* m1, int rt, int row0) {
+    ptx::fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      const int r = it.row_base + row0;
+      ptx::tma_store_4d(m0, stage + p0 * PART_BYTES + rt * ROWB, 0, r, it.head, it.bc);
+      if (p1 >= 0) ptx::tma_store_4d(m1, stage + p1 * PART_BYTES + rt * ROWB, 0, r, it.head, it.bc);
+      ptx::tma_store_commit();
     }
-    if (!packed && n_kt < n_full) {
-      // dense layout: zero rows of the skipped tiles -- one zero tile, TMA-stored over every skipped dQ / dK / dV tile
-      // (TMA clips at S)
-      for (int i = threadIdx.x; i < TILE_BYTES / 16; i += BWD_THREADS) reinterpret_cast<uint4*>(out_tile(0))[i] = make_uint4(0u, 0u, 0u, 0u);
-      ptx::fence_proxy_async_smem();
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        for (int jt = n_kt; jt < n_full; ++jt) {
-          ptx::tma_store_4d(&tmDQ, out_tile(0), 0, 128 * jt, head, b);
-          ptx::tma_store_4d(&tmDK, out_tile(0), 0, 128 * jt, head, b);
-          ptx::tma_store_4d(&tmDV, out_tile(0), 0, 128 * jt, head, b);
+  };
+
+  uint32_t phases = 0;
+  Item cur = item_info(blockIdx.x);
+  if (warp == 0 && cur.rows > 0) issue_loads(cur, 0);
+  fetch_stats(cur);
+  int k = 0;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k) {
+    const int slot = k & 1;
+    Item nxt{};
+    if (item + int(gridDim.x) < n_items) nxt = item_info(item + gridDim.x);
+    // prefetch: the next item's loads go out now when both items fit in the pool
+    const bool early = nxt.rows > 0 && cur.rows + nxt.rows <= pool_rows;
+    if (warp == 0 && early) issue_loads(nxt, slot ^ 1);
+    if (cur.rows > 0) {
+      {
+        // per-query statistics (nm = -max*c - log2(sum); -inf for queries the slate does not have) and the key mask
+        const int qi = threadIdx.x;
+        float2 st = make_float2(-CUDART_INF_F, 0.f);
+        if (qi < cur.q_lim) st = make_float2(-(r_max * c_log2e) - log2f(r_sum), r_delta);
+        qstats[qi] = st;
+        const uint32_t w = __ballot_sync(FULL, r_key);
+        if (lane == 0) key_bits[warp] = w;
+      }
+      if (!packed && warp == 1 && cur.rows < S) {
+        // dense layout: rows at or beyond round_up(extent, 16) are zero -- one zero box, TMA-stored over every such
+        // 16-row box of dQ, dK and dV (TMA clips at S)
+        const int z0 = cur.rows >> 4, nz = (S + 15) / 16 - z0;
+        for (int j = lane; j < 3 * nz; j += 32) {
+          const int o = j / nz, i = z0 + j - o * nz;
+          ptx::tma_store_4d(o == 0 ? &tmDQ : (o == 1 ? &tmDK : &tmDV), zero_box, 0, 16 * i, cur.head, cur.b);
         }
         ptx::tma_store_commit();
-        ptx::tma_store_wait_read();
       }
     }
-    __syncthreads();
-    ptx::mbar_wait(load_bar, phase & 1);
-    ++phase;
+    if (nxt.rows > 0) fetch_stats(nxt);
+    if (cur.rows > 0) {
+      ptx::mbar_wait(load_bar + slot, (phases >> slot) & 1u);
+      phases ^= 1u << slot;
+      const int off = region_off(slot, cur.rows);
+      if (rnd) {
+        // round every operand to tf32 once (nearest even, as the products would on each use)
+        uint4* p = reinterpret_cast<uint4*>(smem + off);
+        for (int i = threadIdx.x; i < cur.rows * (ITEM_ROW_BYTES / 16); i += BWD_THREADS) {
+          uint4 v = p[i];
+          v.x = ptx::cvt_tf32(__uint_as_float(v.x)); v.y = ptx::cvt_tf32(__uint_as_float(v.y));
+          v.z = ptx::cvt_tf32(__uint_as_float(v.z)); v.w = ptx::cvt_tf32(__uint_as_float(v.w));
+          p[i] = v;
+        }
+      }
+      __syncthreads();
 
-    const unsigned long long dbase = (unsigned long long)(b * n_heads + head) * S;
-    // ===== phase 1: dV, dK of each key tile (this warp: keys kA, kA + 8 of its 16)
-    const int nq8 = (min(q_live, 128 * n_kt) + 7) & ~7;
-    for (int jt = 0; jt < n_kt; ++jt) {
-      const int kA = 128 * jt + 16 * warp + g, kB = kA + 8;
-      const bool liveA = key_live(kA), liveB = key_live(kB);
-      uint32_t ka[KS][4], va[KS][4];
+      const uint32_t q_s = sbase + off, k_s = q_s + cur.rows * 128, v_s = k_s + cur.rows * 128, do_s = v_s + cur.rows * 128;
+      const int n = cur.rows >> 4;
+      const unsigned long long dbase = (unsigned long long)(cur.b * n_heads + cur.head) * S;
+      for (int tile = 0; 8 * tile < n; ++tile) {
+        const int ns = min(8, n - 8 * tile);     // strips of this 128-row tile
+        for (int l = warp; l < 2 * ns; l += BWD_WARPS) {
+          if (l < ns) {
+            // ===== key strip: dV, dK of keys kA = 16 strip + g, kB = kA + 8
+            const int strip = 8 * tile + l, kA = 16 * strip + g, kB = kA + 8;
+            const uint32_t kw = lds32(bits_s + 4 * (strip >> 1));
+            const bool liveA = (kw >> (kA & 31)) & 1u, liveB = (kw >> (kB & 31)) & 1u;
+            uint32_t ka[KS][4], va[KS][4];
+            ld_a_head<KS>(k_s, 16 * strip, lane, ka);
+            ld_a_head<KS>(v_s, 16 * strip, lane, va);
+            float dv[KS][4], dk[KS][4];
 #pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        const int e0 = 8 * ks + t;
-        ka[ks][0] = op(k_s, kA, e0); ka[ks][1] = op(k_s, kB, e0); ka[ks][2] = op(k_s, kA, e0 + 4); ka[ks][3] = op(k_s, kB, e0 + 4);
-        va[ks][0] = op(v_s, kA, e0); va[ks][1] = op(v_s, kB, e0); va[ks][2] = op(v_s, kA, e0 + 4); va[ks][3] = op(v_s, kB, e0 + 4);
-      }
-      float dv[KS][4], dk[KS][4];
+            for (int nt = 0; nt < KS; ++nt)
 #pragma unroll
-      for (int nt = 0; nt < KS; ++nt)
+              for (int i = 0; i < 4; ++i) dv[nt][i] = dk[nt][i] = 0.f;
+            const int nq8 = (cur.q_live + 7) & ~7;
+            for (int q0 = 0; q0 < nq8; q0 += 8) {
+              float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+              {
+                uint32_t qb[KS][2], ob[KS][2];
+                ld_b_head<KS>(q_s, q0, lane, qb);
+                ld_b_head<KS>(do_s, q0, lane, ob);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) dv[nt][i] = dk[nt][i] = 0.f;
-      for (int q0 = 0; q0 < nq8; q0 += 8) {
-        float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+                for (int ks = 0; ks < KS; ++ks) {
+                  ptx::mma_tf32(s, ka[ks], qb[ks]);
+                  ptx::mma_tf32(dp, va[ks], ob[ks]);
+                }
+              }
+              // accumulator columns 2t, 2t + 1 are queries q0 + t, q0 + t + 4: their {nm, delta}
+              const uint2 st0 = lds64(stats_s + 8 * (q0 + t)), st1 = lds64(stats_s + 8 * (q0 + t + 4));
+              float pu[4], ds[4];
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          const uint32_t qb[2] = {op(q_s, q0 + g, 8 * ks + t), op(q_s, q0 + g, 8 * ks + t + 4)};
-          const uint32_t ob[2] = {op(do_s, q0 + g, 8 * ks + t), op(do_s, q0 + g, 8 * ks + t + 4)};
-          ptx::mma_tf32(s, ka[ks], qb);
-          ptx::mma_tf32(dp, va[ks], ob);
-        }
-        float pu[4], ds[4];
+              for (int i = 0; i < 4; ++i) {
+                const int q = q0 + t + 4 * (i & 1);
+                const float nm = __uint_as_float((i & 1) ? st1.x : st0.x), dl = __uint_as_float((i & 1) ? st1.y : st0.y);
+                const float p = (i < 2 ? liveA : liveB) ? ex2_approx_b(fmaf(s[i], c_log2e, nm)) : 0.0f;
+                float p_used = p, dpv = dp[i];
+                if constexpr (DROP) {        // regenerate the forward's dropout mask on the probabilities
+                  const unsigned long long idx = (dbase + q) * (unsigned long long)S + (i < 2 ? kA : kB);
+                  const float m = drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
+                  p_used = p * m;
+                  dpv *= m;
+                }
+                pu[i] = round_tf32_b(p_used);
+                ds[i] = round_tf32_b(p * (dpv - dl));
+              }
+              // the accumulators {rows g, g+8} x {queries t, t+4} are the A fragments over k-slots {t, t+4}
+              const uint32_t pa[4] = {__float_as_uint(pu[0]), __float_as_uint(pu[2]), __float_as_uint(pu[1]), __float_as_uint(pu[3])};
+              const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
+              uint32_t o0[KS], o1[KS], q0v[KS], q1v[KS];
+              ld_b_out<KS>(do_s, q0 + t, g, o0); ld_b_out<KS>(do_s, q0 + t + 4, g, o1);
+              ld_b_out<KS>(q_s, q0 + t, g, q0v); ld_b_out<KS>(q_s, q0 + t + 4, g, q1v);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int q = q0 + 2 * t + (i & 1);
-          const float2 st = qstats[q];
-          const float p = (i < 2 ? liveA : liveB) ? ex2_approx_b(fmaf(s[i], c_log2e, st.x)) : 0.0f;
-          float p_used = p, dpv = dp[i];
-          if constexpr (DROP) {        // regenerate the forward's dropout mask on the probabilities
-            const unsigned long long idx = (dbase + q) * (unsigned long long)S + (i < 2 ? kA : kB);
-            const float m = drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
-            p_used = p * m;
-            dpv *= m;
-          }
-          pu[i] = round_tf32_b(p_used);
-          ds[i] = round_tf32_b(p * (dpv - st.y));
-        }
-        uint32_t pa[4], dsa[4];
-        ptx::acc_to_a_tf32(pu, pa, lane);
-        ptx::acc_to_a_tf32(ds, dsa, lane);
-#pragma unroll
-        for (int nt = 0; nt < KS; ++nt) {
-          const uint32_t ob[2] = {op(do_s, q0 + t, 8 * nt + g), op(do_s, q0 + t + 4, 8 * nt + g)};
-          const uint32_t qb[2] = {op(q_s, q0 + t, 8 * nt + g), op(q_s, q0 + t + 4, 8 * nt + g)};
-          ptx::mma_tf32(dv[nt], pa, ob);
-          ptx::mma_tf32(dk[nt], dsa, qb);
-        }
-      }
-      stage_rows(0, 16 * warp + g, dv, 1.0f);
-      stage_rows(1, 16 * warp + g, dk, scale);
-      flush(0, 1, jt, b, head, row_base, ext16);
-    }
-    // ===== phase 2: dQ of each query tile (this warp: queries qA, qA + 8 of its 16)
-    const int nk8 = (e + 7) & ~7;          // keys at or beyond the extent are masked
-    for (int qc = 0; qc < n_kt; ++qc) {
-      const int qA = 128 * qc + 16 * warp + g, qB = qA + 8;
-      const float2 stA = qstats[qA], stB = qstats[qB];
-      uint32_t qa[KS][4], oa[KS][4];
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        const int e0 = 8 * ks + t;
-        qa[ks][0] = op(q_s, qA, e0); qa[ks][1] = op(q_s, qB, e0); qa[ks][2] = op(q_s, qA, e0 + 4); qa[ks][3] = op(q_s, qB, e0 + 4);
-        oa[ks][0] = op(do_s, qA, e0); oa[ks][1] = op(do_s, qB, e0); oa[ks][2] = op(do_s, qA, e0 + 4); oa[ks][3] = op(do_s, qB, e0 + 4);
-      }
-      float dq[KS][4];
-#pragma unroll
-      for (int nt = 0; nt < KS; ++nt) dq[nt][0] = dq[nt][1] = dq[nt][2] = dq[nt][3] = 0.f;
-      if (128 * qc + 16 * warp < q_live) {
-        for (int k0 = 0; k0 < nk8; k0 += 8) {
-          float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-            const uint32_t kb2[2] = {op(k_s, k0 + g, 8 * ks + t), op(k_s, k0 + g, 8 * ks + t + 4)};
-            const uint32_t vb[2] = {op(v_s, k0 + g, 8 * ks + t), op(v_s, k0 + g, 8 * ks + t + 4)};
-            ptx::mma_tf32(s, qa[ks], kb2);
-            ptx::mma_tf32(dp, oa[ks], vb);
-          }
-          float ds[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int key = k0 + 2 * t + (i & 1);
-            const float2 st = i < 2 ? stA : stB;
-            const float p = key_live(key) ? ex2_approx_b(fmaf(s[i], c_log2e, st.x)) : 0.0f;
-            float dpv = dp[i];
-            if constexpr (DROP) {
-              const unsigned long long idx = (dbase + (i < 2 ? qA : qB)) * (unsigned long long)S + key;
-              dpv *= drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
+              for (int nt = 0; nt < KS; ++nt) {
+                const uint32_t ob[2] = {o0[nt], o1[nt]}, qb[2] = {q0v[nt], q1v[nt]};
+                ptx::mma_tf32(dv[nt], pa, ob);
+                ptx::mma_tf32(dk[nt], dsa, qb);
+              }
             }
-            ds[i] = round_tf32_b(p * (dpv - st.y));
-          }
-          uint32_t dsa[4];
-          ptx::acc_to_a_tf32(ds, dsa, lane);
+            stage_strip(0, 16 * l, dv, 1.0f);
+            stage_strip(1, 16 * l, dk, scale);
+            store_strip(cur, 0, &tmDV, 1, &tmDK, 16 * l, 16 * strip);
+          } else {
+            // ===== query strip: dQ of queries qA = 16 strip + g, qB = qA + 8
+            const int strip = 8 * tile + l - ns, qA = 16 * strip + g, qB = qA + 8;
+            float dq[KS][4];
 #pragma unroll
-          for (int nt = 0; nt < KS; ++nt) {
-            const uint32_t kb2[2] = {op(k_s, k0 + t, 8 * nt + g), op(k_s, k0 + t + 4, 8 * nt + g)};
-            ptx::mma_tf32(dq[nt], dsa, kb2);
+            for (int nt = 0; nt < KS; ++nt) dq[nt][0] = dq[nt][1] = dq[nt][2] = dq[nt][3] = 0.f;
+            if (16 * strip < cur.q_live) {
+              const float2 stA = qstats[qA], stB = qstats[qB];
+              uint32_t qa[KS][4], oa[KS][4];
+              ld_a_head<KS>(q_s, 16 * strip, lane, qa);
+              ld_a_head<KS>(do_s, 16 * strip, lane, oa);
+              const int nk8 = (cur.e + 7) & ~7;          // keys at or beyond the extent are masked
+              for (int k0 = 0; k0 < nk8; k0 += 8) {
+                float s[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+                {
+                  uint32_t kb[KS][2], vb[KS][2];
+                  ld_b_head<KS>(k_s, k0, lane, kb);
+                  ld_b_head<KS>(v_s, k0, lane, vb);
+#pragma unroll
+                  for (int ks = 0; ks < KS; ++ks) {
+                    ptx::mma_tf32(s, qa[ks], kb[ks]);
+                    ptx::mma_tf32(dp, oa[ks], vb[ks]);
+                  }
+                }
+                // accumulator columns 2t, 2t + 1 are keys k0 + t, k0 + t + 4
+                const uint32_t kw = lds32(bits_s + 4 * (k0 >> 5)) >> ((k0 & 31) + t);
+                float ds[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                  const int key = k0 + t + 4 * (i & 1);
+                  const float2 st = i < 2 ? stA : stB;
+                  const float p = ((kw >> (4 * (i & 1))) & 1u) ? ex2_approx_b(fmaf(s[i], c_log2e, st.x)) : 0.0f;
+                  float dpv = dp[i];
+                  if constexpr (DROP) {
+                    const unsigned long long idx = (dbase + (i < 2 ? qA : qB)) * (unsigned long long)S + key;
+                    dpv *= drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
+                  }
+                  ds[i] = round_tf32_b(p * (dpv - st.y));
+                }
+                const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
+                uint32_t k0v[KS], k1v[KS];
+                ld_b_out<KS>(k_s, k0 + t, g, k0v); ld_b_out<KS>(k_s, k0 + t + 4, g, k1v);
+#pragma unroll
+                for (int nt = 0; nt < KS; ++nt) {
+                  const uint32_t kb[2] = {k0v[nt], k1v[nt]};
+                  ptx::mma_tf32(dq[nt], dsa, kb);
+                }
+              }
+            }
+            stage_strip(2, 16 * (l - ns), dq, scale);
+            store_strip(cur, 2, &tmDQ, -1, nullptr, 16 * (l - ns), 16 * strip);
           }
         }
+        __syncthreads();
+        if (dbias_qkv != nullptr && threadIdx.x < 3 * DK) {
+          // bias gradient of the QKV projection: column sums of the tile's staged rows (dQ / dK / dV values as
+          // stored), each column added row by row in order, then added to the CTA's accumulator tile by tile
+          const int p = int(threadIdx.x) / DK, cc = int(threadIdx.x) % DK, nr = min(128, cur.rows - 128 * tile);
+          const uint8_t* pt = stage + p * PART_BYTES;
+          float s = 0.f;
+#pragma unroll 8
+          for (int r = 0; r < nr; ++r) {
+            if constexpr (OUT16) s += __uint_as_float(uint32_t(*reinterpret_cast<const uint16_t*>(pt + r * 64 + cc * 2)) << 16);
+            else s += *reinterpret_cast<const float*>(pt + ptx::sw128(r, 4 * cc));
+          }
+          bias_acc[(p == 0 ? 2 * d_model : (p == 1 ? d_model : 0)) + cur.head * DK + cc] += s;
+        }
+        // the staging is free again once every warp's stores have read it
+        if (lane == 0) ptx::tma_store_wait_read();
+        __syncthreads();
       }
-      stage_rows(2, 16 * warp + g, dq, scale);
-      flush(2, 2, qc, b, head, row_base, ext16);
     }
+    // every warp is done with this item's operands, statistics and key bits
+    __syncthreads();
+    if (warp == 0 && !early && nxt.rows > 0) issue_loads(nxt, slot ^ 1);
+    cur = nxt;
   }
   if (dbias_qkv != nullptr) {
     // this CTA's slot of the bias gradient (its items in a fixed order; the slots are summed in order by DetParts)
-    __syncthreads();
     for (int i = threadIdx.x; i < 3 * d_model; i += BWD_THREADS) dbias_qkv[size_t(blockIdx.x) * 3 * d_model + i] = bias_acc[i];
   }
-  if (threadIdx.x == 0) ptx::tma_store_wait_all();
+  ptx::tma_store_wait_all();
 }
 
 static int g_attn_bwd_persistent = ARB_DEFAULT_ATTN_BWD_PERSISTENT;
@@ -389,7 +523,7 @@ template <int DK>
 static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   alignas(64) CUtensorMap tQ, tK, tV, tDO, tDQ, tDK, tDV;
   int rc;
-  const TmapBox box{{32, 128, 1, 1}};
+  const TmapBox box{{32, 16, 1, 1}};
   if ((rc = make_tmap_4d(&tQ, a.q, box, 0))) return rc;
   if ((rc = make_tmap_4d(&tK, a.k, box, 0))) return rc;
   if ((rc = make_tmap_4d(&tV, a.v, box, 0))) return rc;
@@ -398,10 +532,9 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   if ((a.dk_.bf16 != 0) != out16 || (a.dv.bf16 != 0) != out16) { arb_set_error("attn_bwd: dQ, dK, dV must share an element type"); return ARB_E_INVALID_ARG; }
   const bool packed = a.pack_off != nullptr;
   if (packed && !(a.extent && a.rows_dev && a.rowmap)) { arb_set_error("attn_bwd: packed rows need the extents, the row count and the row map"); return ARB_E_INVALID_ARG; }
-  const TmapBox obox{{32, packed ? 16u : 128u, 1, 1}};
-  if ((rc = make_tmap_4d(&tDQ, a.dq, obox, out16 ? 1 : 0))) return rc;
-  if ((rc = make_tmap_4d(&tDK, a.dk_, obox, out16 ? 1 : 0))) return rc;
-  if ((rc = make_tmap_4d(&tDV, a.dv, obox, out16 ? 1 : 0))) return rc;
+  if ((rc = make_tmap_4d(&tDQ, a.dq, box, out16 ? 1 : 0))) return rc;
+  if ((rc = make_tmap_4d(&tDK, a.dk_, box, out16 ? 1 : 0))) return rc;
+  if ((rc = make_tmap_4d(&tDV, a.dv, box, out16 ? 1 : 0))) return rc;
   const double rf = packed ? arb_row_frac() : 1.0;
   {
     ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
@@ -414,10 +547,14 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const bool drop = a.drop.thresh != 0;
   auto kern = out16 ? (drop ? attn_bwd_kernel<DK, true, true> : attn_bwd_kernel<DK, false, true>)
                     : (drop ? attn_bwd_kernel<DK, true> : attn_bwd_kernel<DK, false>);
+  // the operand pool takes what the 227 KB of shared memory leave, up to POOL_ROWS_MAX; it must hold one whole slate
+  const int d_bias = a.dbias_qkv ? a.d_model : 0;
+  const int pool_rows = std::min(POOL_ROWS_MAX, ((227 * 1024 - BwdSmem::total(0, d_bias)) / ITEM_ROW_BYTES) & ~15);
+  if (pool_rows < ((a.S + 15) & ~15)) { arb_set_error("attn_bwd: d_model too large for the shared-memory operand pool"); return ARB_E_UNSUPPORTED; }
   static int configured[ARB_MAX_DEVICES][4] = {};      // dynamic shared memory limit set so far
   const int dev = arb_device_slot();
   const int cslot = (drop ? 1 : 0) + (out16 ? 2 : 0);
-  const int smem = BwdSmem::total(a.dbias_qkv ? a.d_model : 0);
+  const int smem = BwdSmem::total(pool_rows, d_bias);
   if (configured[dev][cslot] < smem) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       arb_set_error("attn_bwd: cannot raise the dynamic shared memory limit");
@@ -425,7 +562,8 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
     }
     configured[dev][cslot] = smem;
   }
-  // one CTA per (slate, head), or -- persistent (default) -- one per SM walking the items head-fastest
+  // one CTA per (slate, head), or -- persistent (default) -- one per SM walking the items head-fastest and loading
+  // the next item while it computes the current one
   const int n_items = a.h * a.B;
   int n_ctas = n_items;
   if (g_attn_bwd_persistent) {
@@ -449,13 +587,14 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
                  rf * 4.0 * double(a.B) * a.h * a.S * (7.0 * a.dk + 3.0), "attn_bwd_kernel");
     arb_launch(kern, grid, dim3(BWD_THREADS), size_t(smem), st, tQ, tK, tV, tDO, tDQ, tDK, tDV, a.mask,
                a.stat_max, a.stat_sum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent, a.pack_off,
-               n_items, tf32_round_on_load());
+               n_items, tf32_round_on_load(), pool_rows);
   }
   arb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
   return dp.finish(st);
 }
+
 
 bool attn_fused_bwd_supported(int S, int dk) { return S >= 1 && S <= 256 && (dk == 16 || dk == 32); }
 

@@ -246,9 +246,9 @@ void arb_set_attention_skip_padding(int32_t on);
  * the reference does.  Process-wide. */
 void arb_set_pack_rows(int32_t on);
 
-/* Fused attention backward: 1: one CTA per SM walks the (slate, head) items as one stream of tile iterations (an
- * item's first loads and products run behind the previous item's last iteration); 0: one CTA per item.  Same results.
- * Process-wide; exists for A/B measurements. */
+/* Fused attention backward: 1: one CTA per SM walks the (slate, head) items and loads the next item's operands while it
+ * computes the current one (when both fit its shared-memory pool, else as soon as the current one is done); 0: one CTA
+ * per item, no prefetch.  Same results.  Process-wide; exists for A/B measurements. */
 void arb_set_attention_bwd_persistent(int32_t on);
 int32_t arb_get_pack_rows(void);
 
