@@ -255,28 +255,12 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   } else {
     kern = drop ? attn_fwd_kernel<DK, true> : attn_fwd_kernel<DK, false>;
   }
-  static bool configured[ARB_MAX_DEVICES][4] = {};
-  const int slot = (drop ? 1 : 0) + (out16 ? 2 : 0);
-  const int dev = arb_device_slot();
-  if (!configured[dev][slot]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total()) != cudaSuccess) {
-      arb_set_error("attn_fwd: cannot raise the dynamic shared memory limit");
-      return ARB_E_CUDA;
-    }
-    configured[dev][slot] = true;
-  }
   dim3 grid((a.S + 127) / 128, a.h, a.B);
-  {
-    ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 4.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
-                 (packed ? arb_row_frac() : 1.0) * 4.0 * double(a.B) * a.h * a.S * ((out16 ? 3.5 : 4.0) * a.dk + 2.0),
-                 "attn_fwd_kernel");
-    arb_launch(kern, grid, dim3(ATT_THREADS), size_t(L::total()), st, tQ, tK, tV, tO, a.mask, a.stat_max, a.stat_sum, a.S,
-               a.h, a.scale * 1.4426950408889634f, a.drop, a.extent, a.pack_off, tf32_round_on_load());
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 4.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
+               (packed ? arb_row_frac() : 1.0) * 4.0 * double(a.B) * a.h * a.S * ((out16 ? 3.5 : 4.0) * a.dk + 2.0),
+               "attn_fwd_kernel");
+  return launch(kern, grid, dim3(ATT_THREADS), size_t(L::total()), st, /*pdl=*/true, tQ, tK, tV, tO, a.mask, a.stat_max,
+                a.stat_sum, a.S, a.h, a.scale * 1.4426950408889634f, a.drop, a.extent, a.pack_off, tf32_round_on_load());
 }
 
 bool attn_fused_supported(int S, int dk) { return S >= 1 && S <= 256 && (dk == 16 || dk == 32 || dk == 64); }

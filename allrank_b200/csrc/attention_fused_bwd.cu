@@ -539,11 +539,11 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   {
     ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
     const long long rows = packed ? (long long)a.q.dim[1] : (long long)a.B * a.S;   // packed: the buffers' row count
-    arb_launch(attn_delta_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0, st, a.do_ptr,
-               static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.B, a.S, a.h, a.dk, a.delta, a.o_bf16, a.rows_dev,
-               a.rowmap, rows);
+    if ((rc = launch(attn_delta_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0, st,
+                     /*pdl=*/true, a.do_ptr, static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.B, a.S, a.h,
+                     a.dk, a.delta, a.o_bf16, a.rows_dev, a.rowmap, rows)))
+      return rc;
   }
-  arb_count_launch();
   const bool drop = a.drop.thresh != 0;
   auto kern = out16 ? (drop ? attn_bwd_kernel<DK, true, true> : attn_bwd_kernel<DK, false, true>)
                     : (drop ? attn_bwd_kernel<DK, true> : attn_bwd_kernel<DK, false>);
@@ -551,31 +551,11 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const int d_bias = a.dbias_qkv ? a.d_model : 0;
   const int pool_rows = std::min(POOL_ROWS_MAX, ((227 * 1024 - BwdSmem::total(0, d_bias)) / ITEM_ROW_BYTES) & ~15);
   if (pool_rows < ((a.S + 15) & ~15)) { arb_set_error("attn_bwd: d_model too large for the shared-memory operand pool"); return ARB_E_UNSUPPORTED; }
-  static int configured[ARB_MAX_DEVICES][4] = {};      // dynamic shared memory limit set so far
-  const int dev = arb_device_slot();
-  const int cslot = (drop ? 1 : 0) + (out16 ? 2 : 0);
   const int smem = BwdSmem::total(pool_rows, d_bias);
-  if (configured[dev][cslot] < smem) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      arb_set_error("attn_bwd: cannot raise the dynamic shared memory limit");
-      return ARB_E_CUDA;
-    }
-    configured[dev][cslot] = smem;
-  }
   // one CTA per (slate, head), or -- persistent (default) -- one per SM walking the items head-fastest and loading
   // the next item while it computes the current one
   const int n_items = a.h * a.B;
-  int n_ctas = n_items;
-  if (g_attn_bwd_persistent) {
-    static int n_sm_of[ARB_MAX_DEVICES] = {};
-    if (!n_sm_of[dev]) {
-      int id = 0, n = 132;
-      cudaGetDevice(&id);
-      cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, id);
-      n_sm_of[dev] = n;
-    }
-    n_ctas = std::min(n_items, n_sm_of[dev]);
-  }
+  const int n_ctas = g_attn_bwd_persistent ? std::min(n_items, sm_count()) : n_items;
   dim3 grid(n_ctas);
   // the QKV bias gradient: one slot per CTA, summed in CTA order afterwards
   float* dbias = a.dbias_qkv;
@@ -585,13 +565,11 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   {
     ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 10.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                  rf * 4.0 * double(a.B) * a.h * a.S * (7.0 * a.dk + 3.0), "attn_bwd_kernel");
-    arb_launch(kern, grid, dim3(BWD_THREADS), size_t(smem), st, tQ, tK, tV, tDO, tDQ, tDK, tDV, a.mask,
-               a.stat_max, a.stat_sum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent, a.pack_off,
-               n_items, tf32_round_on_load(), pool_rows);
+    if ((rc = launch(kern, grid, dim3(BWD_THREADS), size_t(smem), st, /*pdl=*/true, tQ, tK, tV, tDO, tDQ, tDK, tDV,
+                     a.mask, a.stat_max, a.stat_sum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent,
+                     a.pack_off, n_items, tf32_round_on_load(), pool_rows)))
+      return rc;
   }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
   return dp.finish(st);
 }
 

@@ -1,6 +1,11 @@
-// C-ABI bookkeeping: thread-local error string, ABI version, launch counter.
+// C-ABI bookkeeping: thread-local error string, ABI version, launch counter, launch checks.
 #include <atomic>
+#include <cstdio>
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <set>
+#include <utility>
 
 #include "common.h"
 #include "defaults.h"
@@ -23,8 +28,60 @@ static std::atomic<int> g_pdl{ARB_DEFAULT_PDL};
 bool arb_pdl_enabled() { return g_pdl.load(std::memory_order_relaxed) != 0; }
 extern "C" void arb_set_pdl(int32_t on) { g_pdl.store(on ? 1 : 0, std::memory_order_relaxed); }
 
+// ---------------------------------------------------------------- per-device state (common.h: launch)
+// Kernel attributes and pool settings belong to a device, not to the process; the library may be called from several
+// host threads, so the caches below are guarded by one mutex.
+namespace {
+std::mutex g_dev_mu;
+std::map<std::pair<int, const void*>, size_t> g_smem_limit;   // dynamic shared memory limit set so far
+std::map<int, int> g_sm_count;
+std::set<int> g_pool_set;                                       // devices whose pool DetParts has configured
+int current_device() {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  return dev;
+}
+}  // namespace
+
+int arb_smem_opt_in(const void* kern, size_t smem) {
+  const int dev = current_device();
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  size_t& limit = g_smem_limit[{dev, kern}];
+  if (limit >= smem) return ARB_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    char msg[160];
+    std::snprintf(msg, sizeof msg, "cannot raise the dynamic shared memory limit to %zu bytes: %s", smem,
+                  cudaGetErrorString(e));
+    arb_set_error(msg);
+    return ARB_E_CUDA;
+  }
+  limit = smem;
+  return ARB_OK;
+}
+
+int arb_launch_done(cudaError_t e) {
+  arb_count_launch();
+  cudaGetLastError();
+  if (e == cudaSuccess) return ARB_OK;
+  arb_set_error(cudaGetErrorString(e));
+  return ARB_E_CUDA;
+}
+
+int sm_count() {
+  const int dev = current_device();
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  auto it = g_sm_count.find(dev);
+  if (it == g_sm_count.end()) {
+    int n = 132;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    it = g_sm_count.emplace(dev, n).first;
+  }
+  return it->second;
+}
+
 // ---------------------------------------------------------------- per-launch timing
-#include <mutex>
 #include <vector>
 namespace {
 struct ProfRec { int cls; double work; double bytes; cudaEvent_t e0, e1; char name[56]; };
@@ -166,19 +223,18 @@ int DetParts::begin(cudaStream_t st) {
     lvl1 = std::max(lvl1, size_t(det_groups(reg[i].n) * elems));
     lvl2 = std::max(lvl2, size_t(det_groups(det_groups(reg[i].n)) * elems));
   }
-  static bool pool_set[ARB_MAX_DEVICES] = {};
-  const int dev = arb_device_slot();
-  if (!pool_set[dev]) {
-    // the slots come from the device's stream-ordered pool: keep what it has reserved across synchronisations instead
-    // of returning it to the driver after every step (bounded; nothing stays allocated between calls)
-    int id = 0;
-    cudaGetDevice(&id);
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, id) == cudaSuccess) {
-      uint64_t keep = uint64_t(512) << 20;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+  const int dev = current_device();
+  {
+    std::lock_guard<std::mutex> lk(g_dev_mu);
+    if (g_pool_set.insert(dev).second) {
+      // the slots come from the device's stream-ordered pool: keep what it has reserved across synchronisations
+      // instead of returning it to the driver after every step (bounded; nothing stays allocated between calls)
+      cudaMemPool_t pool;
+      if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+        uint64_t keep = uint64_t(512) << 20;
+        cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+      }
     }
-    pool_set[dev] = true;
   }
   const size_t total = slots + lvl1 + lvl2;
   void* p = nullptr;
@@ -211,9 +267,9 @@ int DetParts::finish(cudaStream_t st) {
       const long long groups = det_groups(n);
       float* out = groups > 1 ? tmp[level & 1] : reg[i].dst;
       ProfScope ps(ARB_PROF_SCORER_SIMT, 4.0 * double(n) * double(elems), st, 0.0, "det_reduce_kernel");
-      arb_launch(det_reduce_kernel, dim3(unsigned((elems + 31) / 32), unsigned(groups)), dim3(256), 0, st, src, n,
-                 reg[i].rows, reg[i].cols, reg[i].ld, out);
-      arb_count_launch();
+      if (int rc = launch(det_reduce_kernel, dim3(unsigned((elems + 31) / 32), unsigned(groups)), dim3(256), 0, st,
+                          /*pdl=*/true, src, n, reg[i].rows, reg[i].cols, reg[i].ld, out))
+        return rc;
       if (groups == 1) break;
       src = out;
       n = groups;
@@ -221,8 +277,6 @@ int DetParts::finish(cudaStream_t st) {
     *reg[i].var = reg[i].dst;
   }
   release();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
   return ARB_OK;
 }
 

@@ -7,13 +7,6 @@
 #include "../../include/allrank_b200.h"
 
 void arb_set_error(const char* msg);
-// cudaFuncSetAttribute is per DEVICE: "already configured" flags are kept per device ordinal, not per process
-constexpr int ARB_MAX_DEVICES = 64;
-inline int arb_device_slot() {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return (dev >= 0 && dev < ARB_MAX_DEVICES) ? dev : 0;
-}
 void arb_count_launch(int n = 1);
 // Accounting only: the fraction of the nominal B * S rows that launches over packed rows actually process (set by the
 // scorer when per-launch profiling is on; 1.0 otherwise).  Never steers a kernel.
@@ -28,7 +21,7 @@ bool arb_prof_enabled();
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------------------------------
 // The step is a chain of ~50 dependent kernels; at allRank's own batch size (64 slates) every one of them is
 // latency-bound, so the gap between a kernel's last wave and its successor's first instruction matters.  Kernels
-// launched through arb_launch carry cudaLaunchAttributeProgrammaticStreamSerialization (when enabled): the successor
+// launched with pdl = true carry cudaLaunchAttributeProgrammaticStreamSerialization (when enabled): the successor
 // may start its prologue (barrier init, tensor-map prefetch, smem carve-up) while the predecessor
 // drains, and blocks in arb_pdl_wait() -- griddepcontrol.wait -- until the predecessor has completed and flushed its
 // memory.  Every kernel launched this way executes arb_pdl_wait() on every thread before its first access to global
@@ -39,17 +32,31 @@ __device__ __forceinline__ void arb_pdl_wait() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
+#endif
+
+// ---- kernel launches -----------------------------------------------------------------------------------------------
+// 0 or ARB_E_CUDA: raises `kern`'s dynamic shared-memory limit on the current device to at least `smem` bytes
+int arb_smem_opt_in(const void* kern, size_t smem);
+// 0 or ARB_E_CUDA: counts the launch (arb_launch_count), clears the CUDA last-error slot, reports a failed launch
+int arb_launch_done(cudaError_t e);
+// SMs of the current device (cached per device)
+int sm_count();
+
+// Launch `kern`; returns ARB_OK or ARB_E_* with arb_last_error() set.  A launch above 48 KB of dynamic shared memory
+// raises the kernel's limit first.
+// pdl = true only for kernels that execute arb_pdl_wait() before their first global-memory access.
 template <typename... KArgs, typename... Args>
-inline cudaError_t arb_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+int launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
+  if (smem > 48 * 1024)
+    if (int rc = arb_smem_opt_in(reinterpret_cast<const void*>(kern), smem)) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = arb_pdl_enabled() ? 1 : 0;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  if (pdl && arb_pdl_enabled()) { cfg.attrs = &at; cfg.numAttrs = 1; }
+  return arb_launch_done(cudaLaunchKernelEx(&cfg, kern, args...));
 }
-#endif
 
 // ---- deterministic reductions -------------------------------------------------------------------------------------
 // Gradient reductions across blocks do not use floating-point atomics (their order, and so their rounding, changes from

@@ -819,39 +819,18 @@ void set_gemm_persistent(int on) { g_persistent = on; }
 template <int BLOCK_N, int A_MN, int B_MN>
 static int launch_persistent_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
                                const CUtensorMap& tX, const GemmParams& p, dim3 tiles, cudaStream_t st) {
-  auto kern = gemm_tf32_persistent<BLOCK_N, A_MN, B_MN>;
-  constexpr int smem = PersistLayout<BLOCK_N>::total();
-  static bool configured[ARB_MAX_DEVICES] = {};
-  static int n_sm_of[ARB_MAX_DEVICES] = {};
-  const int dev_slot = arb_device_slot();
-  if (!configured[dev_slot]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      arb_set_error("gemm_tf32 (persistent): cannot raise the dynamic shared memory limit");
-      return ARB_E_CUDA;
-    }
-    int dev = 0, n = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    n_sm_of[dev_slot] = n;
-    configured[dev_slot] = true;
-  }
-  const int n_sm = n_sm_of[dev_slot];
   const long long n_tiles = (long long)tiles.x * tiles.y * tiles.z;
-  const int grid = int(std::min<long long>(n_tiles, n_sm));
-  {
-    const double nb = double(d.nb2) * double(d.nb3);
-    const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-    char pname[56];
-    gemm_prof_name(pname, d, "persist");
-    const double dM = live_m(d), dK = live_k(d);
-    ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-                 4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
-    arb_launch(kern, dim3(grid), dim3(PERSIST_THREADS), smem, st, tA, tB, tC, tX, p, int(tiles.x), int(tiles.y), int(tiles.z));
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  const int grid = int(std::min<long long>(n_tiles, sm_count()));
+  const double nb = double(d.nb2) * double(d.nb3);
+  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
+  char pname[56];
+  gemm_prof_name(pname, d, "persist");
+  const double dM = live_m(d), dK = live_k(d);
+  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
+               4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
+  return launch(gemm_tf32_persistent<BLOCK_N, A_MN, B_MN>, dim3(grid), dim3(PERSIST_THREADS),
+                PersistLayout<BLOCK_N>::total(), st, /*pdl=*/true, tA, tB, tC, tX, p, int(tiles.x), int(tiles.y),
+                int(tiles.z));
 }
 
 // bf16 operands (mma m16n8k16): the one-tile-per-CTA kernel; 4-stage ring for the split-K weight gradients, else 3 stages
@@ -863,45 +842,30 @@ static int launch_bf16_t(const GemmDesc& d, const CUtensorMap& tA, const CUtenso
   const bool drop = (p.flags & EPI_DROPOUT) != 0;
   if (drop && (A_MN || B_MN)) { arb_set_error("gemm_bf16: dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams) = nullptr;
-  int smem = 0, slot = 0;
+  int smem = 0;
   if constexpr (WGRAD) {
-    kern = gemm_tf32_kernel<BLOCK_N, 1, 1, false, 4, true, false>; smem = SmemLayout<BLOCK_N, 4>::total(); slot = 0;
+    kern = gemm_tf32_kernel<BLOCK_N, 1, 1, false, 4, true, false>; smem = SmemLayout<BLOCK_N, 4>::total();
   } else if constexpr (BLOCK_N >= 64) {
     constexpr bool CAN_DROP = (A_MN == 0 && B_MN == 0);
     if (d.C.bf16) {
-      if (drop) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3, true, true>; slot = 1; }
-      else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3, true, true>; slot = 2; }
+      if (drop) kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3, true, true>;
+      else      kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3, true, true>;
     } else {
-      if (drop) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3, true, false>; slot = 3; }
-      else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3, true, false>; slot = 4; }
+      if (drop) kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3, true, false>;
+      else      kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3, true, false>;
     }
     smem = SmemLayout<BLOCK_N, 3>::total();
   }
   if (!kern) { arb_set_error("gemm_bf16: block_n must be 64 or 128"); return ARB_E_UNSUPPORTED; }
-  static bool configured[ARB_MAX_DEVICES][5] = {};
-  const int dev_slot = arb_device_slot();
-  if (!configured[dev_slot][slot]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      arb_set_error("gemm_bf16: cannot raise the dynamic shared memory limit");
-      return ARB_E_CUDA;
-    }
-    configured[dev_slot][slot] = true;
-  }
-  {
-    const double nb = double(d.nb2) * double(d.nb3);
-    const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-    const double osz = d.C.bf16 ? 2.0 : 4.0;
-    char pname[56];
-    gemm_prof_name(pname, d, "tile");
-    const double dM = live_m(d), dK = live_k(d);
-    ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-                 nb * (2.0 * (dM * dK + double(d.N) * dK) + osz * (1.0 + has_x) * dM * d.N), pname);
-    arb_launch(kern, grid, dim3(GEMM_THREADS), smem, st, tA, tB, tC, tX, p);
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  const double nb = double(d.nb2) * double(d.nb3);
+  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
+  const double osz = d.C.bf16 ? 2.0 : 4.0;
+  char pname[56];
+  gemm_prof_name(pname, d, "tile");
+  const double dM = live_m(d), dK = live_k(d);
+  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
+               nb * (2.0 * (dM * dK + double(d.N) * dK) + osz * (1.0 + has_x) * dM * d.N), pname);
+  return launch(kern, grid, dim3(GEMM_THREADS), smem, st, /*pdl=*/true, tA, tB, tC, tX, p);
 }
 
 template <int BLOCK_N, int A_MN, int B_MN>
@@ -926,39 +890,24 @@ static int launch_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap&
   if (drop && !CAN_DROP) { arb_set_error("gemm_tf32: dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
   const bool deep = !WGRAD && d.K >= 256;
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
-  int smem, slot;
+  int smem;
   if (WGRAD) {
-    kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 4>; smem = SmemLayout<BLOCK_N, 4>::total(); slot = 0;
+    kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 4>; smem = SmemLayout<BLOCK_N, 4>::total();
   } else if (drop) {
-    if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); slot = 1; }
-    else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); slot = 2; }
+    if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); }
+    else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); }
   } else {
-    if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); slot = 3; }
-    else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); slot = 4; }
+    if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); }
+    else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); }
   }
-  static bool configured[ARB_MAX_DEVICES][5] = {};
-  const int dev_slot = arb_device_slot();
-  if (!configured[dev_slot][slot]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      arb_set_error("gemm_tf32: cannot raise the dynamic shared memory limit");
-      return ARB_E_CUDA;
-    }
-    configured[dev_slot][slot] = true;
-  }
-  {
-    const double nb = double(d.nb2) * double(d.nb3);
-    const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-    char pname[56];
-    gemm_prof_name(pname, d, "tile");
-    const double dM = live_m(d), dK = live_k(d);
-    ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-                 4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
-    arb_launch(kern, grid, dim3(GEMM_THREADS), smem, st, tA, tB, tC, tX, p);
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  const double nb = double(d.nb2) * double(d.nb3);
+  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
+  char pname[56];
+  gemm_prof_name(pname, d, "tile");
+  const double dM = live_m(d), dK = live_k(d);
+  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
+               4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
+  return launch(kern, grid, dim3(GEMM_THREADS), smem, st, /*pdl=*/true, tA, tB, tC, tX, p);
 }
 
 int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {

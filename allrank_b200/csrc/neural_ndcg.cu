@@ -709,21 +709,13 @@ extern "C" int32_t arb_neural_ndcg(const float* y_pred, const float* y_true, int
   if (S <= RG_N && rg_smem_bytes(max_iter) <= nn_smem_budget()) {
     // register-tiled kernel: the whole matrix and its adjoint stay in the registers of a 1024-thread CTA
     const size_t smem_rg = rg_smem_bytes(max_iter);
-    if (smem_rg > 48 * 1024 &&
-        cudaFuncSetAttribute((const void*)neural_ndcg_reg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             int(smem_rg)) != cudaSuccess) {
-      arb_set_error("arb_neural_ndcg: cannot raise the shared-memory limit");
-      return ARB_E_CUDA;
-    }
     NeuralCfg cfg_rg{pad_value, temperature, tol, powered_relevancies, k, max_iter};
     {
       ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-      neural_ndcg_reg_kernel<<<B, RG_THREADS, smem_rg, st>>>(y_pred, y_true, B, S, discounts, cfg_rg, scratch,
-                                                          scratch + B, grad, nullptr, nullptr);
+      if (int rc = launch(neural_ndcg_reg_kernel, dim3(B), dim3(RG_THREADS), smem_rg, st, /*pdl=*/false, y_pred, y_true,
+                          B, S, discounts, cfg_rg, scratch, scratch + B, grad, nullptr, nullptr))
+        return rc;
     }
-    arb_count_launch();
-    cudaError_t e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) { arb_set_error(cudaGetErrorString(e2)); return ARB_E_CUDA; }
     return arb_finalize_mean_over_count(scratch, scratch + B, B, loss, grad, size_t(B) * S, st);
   }
   const size_t small = nn_small_floats(S) * 4;
@@ -738,20 +730,13 @@ extern "C" int32_t arb_neural_ndcg(const float* y_pred, const float* y_true, int
       return ARB_E_WORKSPACE;
     }
   }
-  if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute((const void*)neural_ndcg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) !=
-          cudaSuccess) {
-    arb_set_error("arb_neural_ndcg: cannot raise the shared-memory limit");
-    return ARB_E_CUDA;
-  }
   NeuralCfg cfg{pad_value, temperature, tol, powered_relevancies, k, max_iter};
   const size_t ws_stride = nn_big_floats(S, max_iter, true);
   ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-  neural_ndcg_kernel<<<B, NN_THREADS, smem, st>>>(y_pred, y_true, B, S, discounts, cfg, scratch, scratch + B, grad,
-                                                  static_cast<float*>(workspace), ws_stride, smem_big_floats);
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
+  if (int rc = launch(neural_ndcg_kernel, dim3(B), dim3(NN_THREADS), smem, st, /*pdl=*/false, y_pred, y_true, B, S,
+                      discounts, cfg, scratch, scratch + B, grad, static_cast<float*>(workspace), ws_stride,
+                      smem_big_floats))
+    return rc;
   // mean over the slates with idcg != 0 (neuralNDCG.py:69); all-dead batch -> 0 (:66-67)
   return arb_finalize_mean_over_count(scratch, scratch + B, B, loss, grad, size_t(B) * S, st);
 }
@@ -772,18 +757,7 @@ extern "C" int32_t arb_neural_sort_debug(const float* y_pred, const float* y_tru
     return ARB_E_UNSUPPORTED;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t smem_rg = rg_smem_bytes(max_iter);
-  if (smem_rg > 48 * 1024 &&
-      cudaFuncSetAttribute((const void*)neural_ndcg_reg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           int(smem_rg)) != cudaSuccess) {
-    arb_set_error("arb_neural_sort_debug: cannot raise the shared-memory limit");
-    return ARB_E_CUDA;
-  }
   NeuralCfg cfg{pad_value, temperature, tol, 1, 0, max_iter};
-  neural_ndcg_reg_kernel<<<B, RG_THREADS, smem_rg, st>>>(y_pred, y_true, B, S, discounts, cfg, scratch, scratch + B,
-                                                        nullptr, p0_out, p_out);
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  return launch(neural_ndcg_reg_kernel, dim3(B), dim3(RG_THREADS), rg_smem_bytes(max_iter), st, /*pdl=*/false, y_pred,
+                y_true, B, S, discounts, cfg, scratch, scratch + B, nullptr, p0_out, p_out);
 }

@@ -75,16 +75,10 @@ extern "C" int32_t arb_adam_step_dev(float* params, const float* grads, float* e
   if (!state) { arb_set_error("arb_adam_step_dev: null state"); return ARB_E_INVALID_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long threads = (n + 3) / 4;
-  {
-    ProfScope ps(ARB_PROF_OPTIM, 28.0 * double(n), st);
-    arb::adam_prep_kernel<<<1, 1, 0, st>>>(state, lr, beta1, beta2);
-    arb::adam_kernel<<<unsigned((threads + 255) / 256), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n, 0.f, beta1,
-                                                                      beta2, eps, 0.f, weight_decay, grad_scale, state);
-  }
-  arb_count_launch(2);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  ProfScope ps(ARB_PROF_OPTIM, 28.0 * double(n), st);
+  if (int rc = launch(arb::adam_prep_kernel, dim3(1), dim3(1), 0, st, /*pdl=*/false, state, lr, beta1, beta2)) return rc;
+  return launch(arb::adam_kernel, dim3(unsigned((threads + 255) / 256)), dim3(256), 0, st, /*pdl=*/false, params, grads,
+                exp_avg, exp_avg_sq, n, 0.f, beta1, beta2, eps, 0.f, weight_decay, grad_scale, state);
 }
 
 extern "C" int32_t arb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
@@ -103,15 +97,8 @@ extern "C" int32_t arb_adam_step(float* params, const float* grads, float* exp_a
   const double bc2 = 1.0 - std::pow(double(beta2), double(step));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long threads = (n + 3) / 4;
-  {
-    ProfScope ps(ARB_PROF_OPTIM, 28.0 * double(n), st);
-    arb::adam_kernel<<<unsigned((threads + 255) / 256), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n,
-                                                                      float(lr / bc1), beta1, beta2, eps,
-                                                                      float(1.0 / std::sqrt(bc2)), weight_decay,
-                                                                      grad_scale, nullptr);
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  ProfScope ps(ARB_PROF_OPTIM, 28.0 * double(n), st);
+  return launch(arb::adam_kernel, dim3(unsigned((threads + 255) / 256)), dim3(256), 0, st, /*pdl=*/false, params, grads,
+                exp_avg, exp_avg_sq, n, float(lr / bc1), beta1, beta2, eps, float(1.0 / std::sqrt(bc2)), weight_decay,
+                grad_scale, nullptr);
 }

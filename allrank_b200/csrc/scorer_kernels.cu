@@ -1025,13 +1025,6 @@ static int bwd_rows_per_warp() {
   return v;
 }
 
-static int check_launch() {
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
-}
-
 
 // ------------------------------------------------------------------------------------------------ rows of 128 / 256
 // "R" layout of the row kernels for the common model widths W = 128 (LPR = 8 lanes per row, 4 rows per warp step)
@@ -1567,13 +1560,11 @@ int pack_plan(const float* x, const int* ext, int B, int S, int F, int* off, int
   if (F % 4) { arb_set_error("packed rows: the feature count must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   {
     ProfScope ps(ARB_PROF_SCORER_SIMT, 8.0 * B, st, 0.0, "pack_scan");
-    arb_launch(pack_scan_kernel, dim3(1), dim3(1024), 0, st, ext, B, off, plan);
-    arb_count_launch();
+    if (int rc = launch(pack_scan_kernel, dim3(1), dim3(1024), 0, st, /*pdl=*/true, ext, B, off, plan)) return rc;
   }
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(B) * S * arb_row_frac() * (8.0 * F + 4.0), st, 0.0, "pack_rows");
-  arb_launch(pack_rows_kernel, dim3(unsigned(B + 1)), dim3(256), 0, st, x, ext, static_cast<const int*>(off),
-             static_cast<const int*>(plan), B, S, F, xc, rowmap, int(cap_rows));
-  return check_launch();
+  return launch(pack_rows_kernel, dim3(unsigned(B + 1)), dim3(256), 0, st, /*pdl=*/true, x, ext,
+                static_cast<const int*>(off), static_cast<const int*>(plan), B, S, F, xc, rowmap, int(cap_rows));
 }
 
 int zero_rows(const ZeroRegions& z, const int* plan, long long cap_rows, cudaStream_t st) {
@@ -1585,8 +1576,7 @@ int zero_rows(const ZeroRegions& z, const int* plan, long long cap_rows, cudaStr
     bytes += 4.0 * (z.r[i].from == 0 ? z.r[i].n : 64) * z.r[i].width;
   }
   ProfScope ps(ARB_PROF_SCORER_SIMT, bytes, st, 0.0, "zero_rows");
-  arb_launch(zero_rows_kernel, dim3(unsigned((n + 7) / 8)), dim3(256), 0, st, z, plan, cap_rows);
-  return check_launch();
+  return launch(zero_rows_kernel, dim3(unsigned((n + 7) / 8)), dim3(256), 0, st, /*pdl=*/true, z, plan, cap_rows);
 }
 
 int ln_forward(const float* x, const float* a, const float* b, float eps, long long rows, int width, float* y,
@@ -1596,15 +1586,15 @@ int ln_forward(const float* x, const float* a, const float* b, float eps, long l
   if (const int lpr = r_lpr(width, R_LN_FWD)) {      // W = 128 / 256: several rows per warp step (see ln_fwd_r_kernel)
     const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    if (lpr == 8) arb_launch(ln_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
-    else arb_launch(ln_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
-    return check_launch();
+    if (lpr == 8) return launch(ln_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
+    return launch(ln_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
   }
   const int nb = fwd_batches_for(width, rows);
   const int per_block = ROWS_PER_BLOCK * FWD_RPW * nb;
   const unsigned blocks = unsigned((rows + per_block - 1) / per_block);
-  ARB_DISPATCH_NV(width, (arb_launch(ln_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, rows, width, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, nb)));
-  return check_launch();
+  int rc;
+  ARB_DISPATCH_NV(width, (rc = launch(ln_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, nb)));
+  return rc;
 }
 
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
@@ -1623,14 +1613,15 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
   const unsigned nblk = lpr ? unsigned((rows + ROWS_PER_BLOCK * (32 / lpr) * steps - 1) / (ROWS_PER_BLOCK * (32 / lpr) * steps)) : blocks;
   DetParts dp;
   dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width);
-  if (int rc = dp.begin(st)) return rc;
+  int rc = dp.begin(st);
+  if (rc) return rc;
   if (lpr) {
-    if (lpr == 8) arb_launch(ln_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
-    else arb_launch(ln_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
+    if (lpr == 8) rc = launch(ln_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
+    else rc = launch(ln_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
   } else {
-    ARB_DISPATCH_NV(width, (arb_launch(ln_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev)));
+    ARB_DISPATCH_NV(width, (rc = launch(ln_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev)));
   }
-  if (int rc = check_launch()) return rc;
+  if (rc) return rc;
   return dp.finish(st);
 }
 
@@ -1638,15 +1629,15 @@ int pos_forward(float* x, const long long* indices, const uint8_t* mask, const f
                 long long rows, int width, cudaStream_t st) {
   if (width % 4) { arb_set_error("positional encoding: width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * 12.0 * width, st);
-  pos_fwd_kernel<<<unsigned((rows + 7) / 8), 256, 0, st>>>(x, indices, mask, pe, pe_rows, scale, rows, width);
-  return check_launch();
+  return launch(pos_fwd_kernel, dim3(unsigned((rows + 7) / 8)), dim3(256), 0, st, /*pdl=*/false, x, indices, mask, pe,
+                pe_rows, scale, rows, width);
 }
 
 int pos_backward(const float* dx, const long long* indices, const uint8_t* mask, float* dpe, int pe_rows, long long rows,
                  int width, cudaStream_t st) {
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * 8.0 * width, st);
-  pos_bwd_kernel<<<unsigned((rows + 7) / 8), 256, 0, st>>>(dx, indices, mask, dpe, pe_rows, rows, width);
-  return check_launch();
+  return launch(pos_bwd_kernel, dim3(unsigned((rows + 7) / 8)), dim3(256), 0, st, /*pdl=*/false, dx, indices, mask, dpe,
+                pe_rows, rows, width);
 }
 
 int act_forward(float* h, long long rows, int width, int act, DropSite site, cudaStream_t st, const int* rows_dev) {
@@ -1654,8 +1645,7 @@ int act_forward(float* h, long long rows, int width, int act, DropSite site, cud
   const long long n4 = rows * width / 4;
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * 8.0 * width, st);
   const unsigned blocks = unsigned(std::min<long long>((n4 + 255) / 256, 132 * 16));
-  act_fwd_kernel<<<blocks, 256, 0, st>>>(h, n4, act, site, rows_dev, width / 4);
-  return check_launch();
+  return launch(act_fwd_kernel, dim3(blocks), dim3(256), 0, st, /*pdl=*/false, h, n4, act, site, rows_dev, width / 4);
 }
 
 int act_backward(const float* dh, const float* h, float* dz, long long rows, int width, int act, DropSite site, float mul,
@@ -1669,9 +1659,9 @@ int act_backward(const float* dh, const float* h, float* dz, long long rows, int
   DetParts dp;
   dp.add(colsum_out, blocks, 1, width, width);
   if (int rc = dp.begin(st)) return rc;
-  act_bwd_kernel<<<blocks, 256, size_t(256 / tx_n) * width * 4, st>>>(dh, h, dz, rows, width, act, site, mul, tx_n, rpb,
-                                                                     colsum_out, rows_dev);
-  if (int rc = check_launch()) return rc;
+  if (int rc = launch(act_bwd_kernel, dim3(blocks), dim3(256), size_t(256 / tx_n) * width * 4, st, /*pdl=*/false, dh, h,
+                      dz, rows, width, act, site, mul, tx_n, rpb, colsum_out, rows_dev))
+    return rc;
   return dp.finish(st);
 }
 
@@ -1679,31 +1669,28 @@ int softmax_forward(float* sc, const uint8_t* mask, int B, int h, int S, int pit
   if (S > 32 * 48) { arb_set_error("attention softmax supports slate_length <= 1536"); return ARB_E_UNSUPPORTED; }
   const long long rows = (long long)B * h * S;
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * 8.0 * S, st);
-  if (site.thresh) softmax_fwd_kernel<true><<<unsigned((rows + 7) / 8), 256, 0, st>>>(sc, mask, B, h, S, pitch, site);
-  else softmax_fwd_kernel<false><<<unsigned((rows + 7) / 8), 256, 0, st>>>(sc, mask, B, h, S, pitch, site);
-  return check_launch();
+  return launch(site.thresh ? softmax_fwd_kernel<true> : softmax_fwd_kernel<false>, dim3(unsigned((rows + 7) / 8)),
+                dim3(256), 0, st, /*pdl=*/false, sc, mask, B, h, S, pitch, site);
 }
 
 int softmax_backward(float* dp, float* prob, long long rows, int S, int pitch, cudaStream_t st, DropSite site) {
   if (S > 32 * 48) { arb_set_error("attention softmax supports slate_length <= 1536"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * (site.thresh ? 16.0 : 12.0) * S, st);
-  if (site.thresh) softmax_bwd_kernel<true><<<unsigned((rows + 7) / 8), 256, 0, st>>>(dp, prob, rows, S, pitch, site);
-  else softmax_bwd_kernel<false><<<unsigned((rows + 7) / 8), 256, 0, st>>>(dp, prob, rows, S, pitch, site);
-  return check_launch();
+  return launch(site.thresh ? softmax_bwd_kernel<true> : softmax_bwd_kernel<false>, dim3(unsigned((rows + 7) / 8)),
+                dim3(256), 0, st, /*pdl=*/false, dp, prob, rows, S, pitch, site);
 }
 
 int slate_extents(const uint8_t* mask, const float* dscores, int n_out, int B, int S, int* extent, cudaStream_t st) {
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(B) * S * (dscores ? 1.0 + 4.0 * n_out : 1.0), st);
-  arb_launch(slate_extent_kernel, dim3(unsigned((B + 7) / 8)), dim3(256), 0, st, mask, dscores, n_out, B, S, extent);
-  return check_launch();
+  return launch(slate_extent_kernel, dim3(unsigned((B + 7) / 8)), dim3(256), 0, st, /*pdl=*/true, mask, dscores, n_out, B,
+                S, extent);
 }
 
 int convert_to_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
   const long long n4 = (n + 3) / 4;
   ProfScope ps(ARB_PROF_SCORER_SIMT, 6.0 * double(n), st);
-  arb_launch(to_bf16_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n4 + 255) / 256, 132 * 8)))), dim3(256), 0, st,
-             reinterpret_cast<const float4*>(src), static_cast<uint2*>(dst), n);
-  return check_launch();
+  return launch(to_bf16_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n4 + 255) / 256, 132 * 8)))), dim3(256), 0, st,
+                /*pdl=*/true, reinterpret_cast<const float4*>(src), static_cast<uint2*>(dst), n);
 }
 
 int colsum_accumulate(const float* in, long long rows, int width, long long ld, float* out, cudaStream_t st) {
@@ -1713,9 +1700,10 @@ int colsum_accumulate(const float* in, long long rows, int width, long long ld, 
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * 4.0 * width, st);
   DetParts dp;
   dp.add(out, blocks, 1, width, width);
-  if (int rc = dp.begin(st)) return rc;
-  ARB_DISPATCH_NV(width, (colsum_kernel<NV><<<blocks, 256, 0, st>>>(in, rows, width, ld, rpb, out)));
-  if (int rc = check_launch()) return rc;
+  int rc = dp.begin(st);
+  if (rc) return rc;
+  ARB_DISPATCH_NV(width, (rc = launch(colsum_kernel<NV>, dim3(blocks), dim3(256), 0, st, /*pdl=*/false, in, rows, width, ld, rpb, out)));
+  if (rc) return rc;
   return dp.finish(st);
 }
 
@@ -1727,15 +1715,15 @@ int head_forward(const float* x, const float* a, const float* b, float eps, cons
   if (const int lpr = r_lpr(width, R_HEAD_FWD)) {
     const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    if (lpr == 8) arb_launch(head_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
-    else arb_launch(head_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
-    return check_launch();
+    if (lpr == 8) return launch(head_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
+    return launch(head_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
   }
   const int nb = fwd_batches_for(width, rows);
   const int per_block = ROWS_PER_BLOCK * FWD_RPW * nb;
   const unsigned blocks = unsigned((rows + per_block - 1) / per_block);
-  ARB_DISPATCH_NV(width, (arb_launch(head_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, x, a, b, eps, w, wb, has_norm, act, rows, width, score, mean, sd, rows_dev, rowmap, nb)));
-  return check_launch();
+  int rc;
+  ARB_DISPATCH_NV(width, (rc = launch(head_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, width, score, mean, sd, rows_dev, rowmap, nb)));
+  return rc;
 }
 
 int head_backward(const float* dscore, const float* score, const float* x, const float* a, const float* b,
@@ -1753,14 +1741,15 @@ int head_backward(const float* dscore, const float* score, const float* x, const
   DetParts dp;
   if (has_norm) { dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); }
   dp.add(grad_w, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width); dp.add(grad_wb, nblk, 1, 1, 1);
-  if (int rc = dp.begin(st)) return rc;
+  int rc = dp.begin(st);
+  if (rc) return rc;
   if (lpr) {
-    if (lpr == 8) arb_launch(head_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
-    else arb_launch(head_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
+    if (lpr == 8) rc = launch(head_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
+    else rc = launch(head_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
   } else {
-    ARB_DISPATCH_NV(width, (arb_launch(head_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, dscore, score, x, a, b, mean, sd, eps, w, wb, has_norm, act, rows, width, rpw, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap)));
+    ARB_DISPATCH_NV(width, (rc = launch(head_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, wb, has_norm, act, rows, width, rpw, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap)));
   }
-  if (int rc = check_launch()) return rc;
+  if (rc) return rc;
   return dp.finish(st);
 }
 
@@ -1769,8 +1758,9 @@ int head_multi_forward(const float* xf, const float* w, const float* wb, int act
   if (width % 4) { arb_set_error("model width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK - 1) / ROWS_PER_BLOCK);
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * (4.0 * width + 4.0 * n), st);
-  ARB_DISPATCH_NV(width, (head_multi_fwd_kernel<NV><<<blocks, ROWS_PER_BLOCK * 32, 0, st>>>(xf, w, wb, act, rows, width, n, score)));
-  return check_launch();
+  int rc;
+  ARB_DISPATCH_NV(width, (rc = launch(head_multi_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/false, xf, w, wb, act, rows, width, n, score)));
+  return rc;
 }
 
 int head_multi_backward(const float* dscore, const float* score, const float* xf, const float* w, int act,
@@ -1783,9 +1773,10 @@ int head_multi_backward(const float* dscore, const float* score, const float* xf
   DetParts dp;
   dp.add(grad_w, blocks, 1, (long long)n * width, (long long)n * width); dp.add(grad_wb, blocks, 1, n, n);
   dp.add(colsum_out, blocks, 1, width, width);
-  if (int rc = dp.begin(st)) return rc;
-  ARB_DISPATCH_NV(width, (head_multi_bwd_kernel<NV><<<blocks, ROWS_PER_BLOCK * 32, 0, st>>>(dscore, score, xf, w, act, rows, width, n, rpw, dxf, grad_w, grad_wb, dx_masked, site, colsum_out)));
-  if (int rc = check_launch()) return rc;
+  int rc = dp.begin(st);
+  if (rc) return rc;
+  ARB_DISPATCH_NV(width, (rc = launch(head_multi_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/false, dscore, score, xf, w, act, rows, width, n, rpw, dxf, grad_w, grad_wb, dx_masked, site, colsum_out)));
+  if (rc) return rc;
   return dp.finish(st);
 }
 

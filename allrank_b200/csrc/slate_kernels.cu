@@ -875,14 +875,8 @@ __global__ void __launch_bounds__(128) ordinal_warp_kernel(const float* __restri
 // ================================================================================================
 using namespace arb;
 
-static int set_smem(const void* fn, size_t bytes) {
-  if (bytes > 48 * 1024) {
-    if (bytes > 227 * 1024) return ARB_E_UNSUPPORTED;
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)) != cudaSuccess)
-      return ARB_E_CUDA;
-  }
-  return ARB_OK;
-}
+// the largest dynamic shared memory a block may use on sm_90
+constexpr size_t MAX_SMEM = 227 * 1024;
 
 #define ARB_CHECK_ARGS(cond, msg)            \
   do {                                       \
@@ -890,15 +884,6 @@ static int set_smem(const void* fn, size_t bytes) {
       arb_set_error(msg);                    \
       return ARB_E_INVALID_ARG;              \
     }                                        \
-  } while (0)
-
-#define ARB_LAUNCH_OK()                                         \
-  do {                                                          \
-    cudaError_t e__ = cudaGetLastError();                       \
-    if (e__ != cudaSuccess) {                                   \
-      arb_set_error(cudaGetErrorString(e__));                   \
-      return ARB_E_CUDA;                                        \
-    }                                                           \
   } while (0)
 
 extern "C" int32_t arb_rank_metrics(const float* y_pred, const float* y_true, int32_t B, int32_t S,
@@ -922,20 +907,15 @@ extern "C" int32_t arb_rank_metrics(const float* y_pred, const float* y_true, in
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t smem = slate_smem_bytes(S);
-  int rc = set_smem((const void*)metrics_kernel, smem);
-  if (rc) { arb_set_error("arb_rank_metrics: slate too long for shared memory"); return rc; }
+  if (smem > MAX_SMEM) { arb_set_error("arb_rank_metrics: slate too long for shared memory"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_METRICS, double(B) * (8.0 * S + 4.0 * n_ats), st);
-  metrics_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, discounts, ats, gain_mode, pad_value, filler, out_dcg,
-                                      out_idcg, out_ndcg, out_mrr ? mrr_scratch : nullptr,
-                                      out_mrr ? mrr_scratch + B : nullptr, out_order);
-  arb_count_launch();
-  ARB_LAUNCH_OK();
-  if (out_mrr) {
-    mrr_finalize_kernel<<<1, 256, 0, st>>>(mrr_scratch, mrr_scratch + B, B, ats, out_mrr);
-    arb_count_launch();
-    ARB_LAUNCH_OK();
-  }
-  return ARB_OK;
+  if (int rc = launch(metrics_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, discounts, ats,
+                      gain_mode, pad_value, filler, out_dcg, out_idcg, out_ndcg, out_mrr ? mrr_scratch : nullptr,
+                      out_mrr ? mrr_scratch + B : nullptr, out_order))
+    return rc;
+  if (!out_mrr) return ARB_OK;
+  return launch(mrr_finalize_kernel, dim3(1), dim3(256), 0, st, /*pdl=*/false, mrr_scratch, mrr_scratch + B, B, ats,
+                out_mrr);
 }
 
 static int finalize(const float* val, const float* cnt, int B, int mode, float* loss, float* grad, size_t n_grad,
@@ -943,10 +923,7 @@ static int finalize(const float* val, const float* cnt, int B, int mode, float* 
   int blocks = 1;
   if (mode != 0 && grad) blocks = int(std::min<size_t>((n_grad + 1023) / 1024, 132 * 4));
   if (blocks < 1) blocks = 1;
-  finalize_kernel<<<blocks, 256, 0, st>>>(val, cnt, B, mode, loss, grad, n_grad);
-  arb_count_launch();
-  ARB_LAUNCH_OK();
-  return ARB_OK;
+  return launch(finalize_kernel, dim3(blocks), dim3(256), 0, st, /*pdl=*/false, val, cnt, B, mode, loss, grad, n_grad);
 }
 
 int arb_finalize_mean_over_count(const float* val, const float* cnt, int B, float* loss, float* grad, size_t n_grad,
@@ -959,19 +936,19 @@ extern "C" int32_t arb_listnet(const float* y_pred, const float* y_true, int32_t
   ARB_CHECK_ARGS(y_pred && y_true && loss && scratch && B > 0 && S > 0, "arb_listnet: null pointer or bad shape");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const float inv_B = 1.0f / float(B);
+  int rc;
   if (S <= 32 * LISTNET_MAX_PER_LANE) {
     const int wpb = 4;
     ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-  listnet_warp_kernel<<<(B + wpb - 1) / wpb, wpb * 32, 0, st>>>(y_pred, y_true, B, S, eps, pad_value, inv_B,
-                                                                 scratch, grad);
+    rc = launch(listnet_warp_kernel, dim3((B + wpb - 1) / wpb), dim3(wpb * 32), 0, st, /*pdl=*/false, y_pred, y_true, B,
+                S, eps, pad_value, inv_B, scratch, grad);
   } else {
     const size_t smem = size_t(S) * 8 + 128;
-    int rc = set_smem((const void*)listnet_block_kernel, smem);
-    if (rc) { arb_set_error("arb_listnet: slate too long"); return rc; }
-    listnet_block_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, eps, pad_value, inv_B, scratch, grad);
+    if (smem > MAX_SMEM) { arb_set_error("arb_listnet: slate too long"); return ARB_E_UNSUPPORTED; }
+    rc = launch(listnet_block_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, eps, pad_value,
+                inv_B, scratch, grad);
   }
-  arb_count_launch();
-  ARB_LAUNCH_OK();
+  if (rc) return rc;
   return finalize(scratch, nullptr, B, 0, loss, nullptr, 0, st);
 }
 
@@ -982,13 +959,11 @@ extern "C" int32_t arb_listmle(const float* y_pred, const float* y_true, int32_t
                  "arb_listmle: null pointer or bad shape");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t smem = size_t(next_pow2(S)) * 8 + size_t(S) * 16 + 256 * 4 + 64;
-  int rc = set_smem((const void*)listmle_kernel, smem);
-  if (rc) { arb_set_error("arb_listmle: slate too long"); return rc; }
+  if (smem > MAX_SMEM) { arb_set_error("arb_listmle: slate too long"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-  listmle_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, eps, pad_value, perm, order, 1.0f / float(B), scratch,
-                                      grad);
-  arb_count_launch();
-  ARB_LAUNCH_OK();
+  if (int rc = launch(listmle_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, eps, pad_value,
+                      perm, order, 1.0f / float(B), scratch, grad))
+    return rc;
   return finalize(scratch, nullptr, B, 0, loss, nullptr, 0, st);
 }
 
@@ -999,13 +974,11 @@ extern "C" int32_t arb_approx_ndcg(const float* y_pred, const float* y_true, int
                  "arb_approx_ndcg: null pointer or bad shape");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t smem = slate_smem_bytes(S);
-  int rc = set_smem((const void*)approx_ndcg_kernel, smem);
-  if (rc) { arb_set_error("arb_approx_ndcg: slate too long"); return rc; }
+  if (smem > MAX_SMEM) { arb_set_error("arb_approx_ndcg: slate too long"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-  approx_ndcg_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, eps, pad_value, alpha, 1.0f / float(B), scratch,
-                                          grad);
-  arb_count_launch();
-  ARB_LAUNCH_OK();
+  if (int rc = launch(approx_ndcg_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, eps,
+                      pad_value, alpha, 1.0f / float(B), scratch, grad))
+    return rc;
   return finalize(scratch, nullptr, B, 0, loss, nullptr, 0, st);
 }
 
@@ -1022,13 +995,12 @@ extern "C" int32_t arb_lambda_loss(const float* y_pred, const float* y_true, int
                  "Reduction logarithm base can be either natural or binary");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t smem = slate_smem_bytes(S) + size_t(S) * 4;
-  int rc = set_smem((const void*)lambda_loss_kernel, smem);
-  if (rc) { arb_set_error("arb_lambda_loss: slate too long"); return rc; }
+  if (smem > MAX_SMEM) { arb_set_error("arb_lambda_loss: slate too long"); return ARB_E_UNSUPPORTED; }
   LambdaCfg cfg{scheme, k, log_base, sigma, mu, eps};
   ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-  lambda_loss_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, pad_value, cfg, scratch, scratch + B, grad);
-  arb_count_launch();
-  ARB_LAUNCH_OK();
+  if (int rc = launch(lambda_loss_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, pad_value,
+                      cfg, scratch, scratch + B, grad))
+    return rc;
   return finalize(scratch, scratch + B, B, reduction == ARB_REDUCTION_MEAN ? 1 : 0, loss, grad, size_t(B) * S, st);
 }
 
@@ -1038,14 +1010,13 @@ extern "C" int32_t arb_ranknet(const float* y_pred, const float* y_true, int32_t
   ARB_CHECK_ARGS(weight_mode >= 0 && weight_mode <= 2, "arb_ranknet: weight_mode must be 0, 1 or 2");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t smem = size_t(S) * 8 + 256;
-  int rc = set_smem((const void*)ranknet_kernel, smem);
-  if (rc) { arb_set_error("arb_ranknet: slate too long"); return rc; }
+  if (smem > MAX_SMEM) { arb_set_error("arb_ranknet: slate too long"); return ARB_E_UNSUPPORTED; }
   {
     ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-    ranknet_kernel<<<B, 256, smem, st>>>(y_pred, y_true, B, S, pad_value, weight_mode, scratch, scratch + B, grad);
+    if (int rc = launch(ranknet_kernel, dim3(B), dim3(256), smem, st, /*pdl=*/false, y_pred, y_true, B, S, pad_value,
+                        weight_mode, scratch, scratch + B, grad))
+      return rc;
   }
-  arb_count_launch();
-  ARB_LAUNCH_OK();
   return finalize(scratch, scratch + B, B, 1, loss, grad, size_t(B) * S, st);   // mean over selected pairs
 }
 
@@ -1059,11 +1030,10 @@ extern "C" int32_t arb_pointwise_loss(const float* y_pred, const float* y_true, 
   const int wpb = 4;
   {
     ProfScope ps(ARB_PROF_LOSS, double(B) * ((grad ? 12.0 : 8.0) * S + 4.0), st);
-    pointwise_warp_kernel<<<(B + wpb - 1) / wpb, wpb * 32, 0, st>>>(y_pred, y_true, B, S, pad_value, mode, param, eps,
-                                                                   1.0f / float(B), scratch, scratch + B, grad);
+    if (int rc = launch(pointwise_warp_kernel, dim3((B + wpb - 1) / wpb), dim3(wpb * 32), 0, st, /*pdl=*/false, y_pred,
+                        y_true, B, S, pad_value, mode, param, eps, 1.0f / float(B), scratch, scratch + B, grad))
+      return rc;
   }
-  arb_count_launch();
-  ARB_LAUNCH_OK();
   // binary_listNet / rmse: mean over the batch is already folded in; bce: divide by the number of non-empty slates
   return finalize(scratch, scratch + B, B, mode == 2 ? 1 : 0, loss, grad, size_t(B) * S, st);
 }
@@ -1075,10 +1045,9 @@ extern "C" int32_t arb_ordinal(const float* y_pred, const float* y_true, int32_t
   const int wpb = 4;
   {
     ProfScope ps(ARB_PROF_LOSS, double(B) * S * ((grad ? 8.0 : 4.0) * n + 4.0) + 4.0, st);
-    ordinal_warp_kernel<<<(B + wpb - 1) / wpb, wpb * 32, 0, st>>>(y_pred, y_true, B, S, n, pad_value, scratch,
-                                                                 scratch + B, grad);
+    if (int rc = launch(ordinal_warp_kernel, dim3((B + wpb - 1) / wpb), dim3(wpb * 32), 0, st, /*pdl=*/false, y_pred,
+                        y_true, B, S, n, pad_value, scratch, scratch + B, grad))
+      return rc;
   }
-  arb_count_launch();
-  ARB_LAUNCH_OK();
   return finalize(scratch, scratch + B, B, 1, loss, grad, size_t(B) * S * n, st);   // / total number of valid items
 }

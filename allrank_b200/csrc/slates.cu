@@ -144,25 +144,13 @@ extern "C" int32_t arb_assemble_slates(const float* docs_x, const float* docs_y,
     arb_set_error("arb_assemble_slates: queries above 16384 items (or slate_length above ~50k) are not supported");
     return ARB_E_UNSUPPORTED;
   }
-  if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute(assemble_slates_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-    arb_set_error("arb_assemble_slates: cannot reserve shared memory");
-    return ARB_E_CUDA;
-  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int vec = (F % 4 == 0) && aligned16(docs_x) && aligned16(x_out);
   const int key_slots = max_query_len >= S ? next_pow2(max_query_len) : 0;
-  {
-    ProfScope ps(ARB_PROF_SLATES, double(B) * S * (8.0 * F + 16.0), st);
-    assemble_slates_kernel<<<B, ASM_THREADS, smem, st>>>(docs_x, docs_y, reinterpret_cast<const long long*>(offsets),
-                                                         reinterpret_cast<const long long*>(queries), n_queries, S, F,
-                                                         key_slots, seed, vec, x_out, y_out,
-                                                         reinterpret_cast<long long*>(idx_out));
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  ProfScope ps(ARB_PROF_SLATES, double(B) * S * (8.0 * F + 16.0), st);
+  return launch(assemble_slates_kernel, dim3(B), dim3(ASM_THREADS), smem, st, /*pdl=*/false, docs_x, docs_y,
+                reinterpret_cast<const long long*>(offsets), reinterpret_cast<const long long*>(queries), n_queries, S,
+                F, key_slots, seed, vec, x_out, y_out, reinterpret_cast<long long*>(idx_out));
 }
 
 extern "C" int32_t arb_gather_slates(const float* x, const float* y, const int32_t* order, int32_t B, int32_t S,
@@ -174,12 +162,7 @@ extern "C" int32_t arb_gather_slates(const float* x, const float* y, const int32
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long rows = (long long)B * S;
   const int vec = (F % 4 == 0) && aligned16(x) && aligned16(x_out);
-  {
-    ProfScope ps(ARB_PROF_SLATES, double(rows) * (8.0 * F + 12.0), st);
-    gather_slates_kernel<<<unsigned((rows + 7) / 8), 256, 0, st>>>(x, y, order, rows, S, F, vec, x_out, y_out);
-  }
-  arb_count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { arb_set_error(cudaGetErrorString(e)); return ARB_E_CUDA; }
-  return ARB_OK;
+  ProfScope ps(ARB_PROF_SLATES, double(rows) * (8.0 * F + 12.0), st);
+  return launch(gather_slates_kernel, dim3(unsigned((rows + 7) / 8)), dim3(256), 0, st, /*pdl=*/false, x, y, order, rows,
+                S, F, vec, x_out, y_out);
 }
