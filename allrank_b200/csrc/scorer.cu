@@ -3,6 +3,8 @@
 //   forward : x -> FC -> N x [ LN -> QKV -> (Q K^T / sqrt(dk), key mask, softmax, P V) -> O + residual
 //                               -> LN -> W1 + ReLU -> W2 + residual ] -> LN -> head
 //   backward: the exact reverse, parameter gradients accumulated into a flat buffer.
+//   encode  : the forward without the head: the final LayerNorm's output [B, S, d] (LTRModel.prepare_for_output);
+//             backward_ex starts from its gradient instead of the score's and can also emit d loss / d x.
 //
 // Reference: allrank/models/model.py:62-92 (LTRModel), allrank/models/transformer.py:43-56,126-134,178-203,227.
 // Every contraction is a launch of the tensor-core TF32 GEMM (gemm_tf32.cu) -- per-head attention products are
@@ -268,6 +270,7 @@ static int linear_bwd_input(const Ctx& k, V dY, int64_t dy_pitch, int out, V Wt,
   GemmDesc g;
   g.alpha = alpha;
   g.colsum_out = colsum_out;
+  if (!colsum_out) flags &= ~EPI_COLSUM;     // (no parameter gradients requested)
   g.M = int(k.R); g.N = in; g.K = out; g.b_mn = 1;
   g.A = rows_view(dY, out, k.R, dy_pitch);
   g.B = rows_view(Wt, in, out, in);          // dim0 = in (N, contiguous), dim1 = out (K)
@@ -319,9 +322,12 @@ static void batch_all(GemmDesc& g, int h, int B) {
 
 #define ARB_TRY(expr) do { int rc__ = (expr); if (rc__ != ARB_OK) return rc__; } while (0)
 
+// Exactly one of `scores` (the model's output) and `hidden` (the encoder's output, [B, S, d]; the head is not run) is
+// non-null.
 static int forward_impl(const arb_scorer_config& c, const float* P, const float* x, const uint8_t* mask,
                         const int64_t* indices, const float* pe_table, int B, int S,
-                        float* scores, float* ws, int64_t ws_floats, int training, uint64_t seed, cudaStream_t st) {
+                        float* scores, float* hidden, float* ws, int64_t ws_floats, int training, uint64_t seed,
+                        cudaStream_t st) {
   ParamLayout L;
   ARB_TRY(make_param_layout(c, L));
   WsLayout W;
@@ -375,8 +381,10 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     poff = reinterpret_cast<const int*>(ws + W.poff);
     ARB_TRY(pack_plan(x, kext, B, S, F, reinterpret_cast<int*>(ws + W.poff), reinterpret_cast<int*>(ws + W.plan),
                       reinterpret_cast<int*>(ws + W.rowmap), ws + W.xc, buffer_rows(c, B, S), st));
-    // items beyond their slate's extent get the score 0
-    if (cudaMemsetAsync(scores, 0, size_t(B) * S * sizeof(float), st) != cudaSuccess) { arb_set_error("scorer: memset failed"); return ARB_E_CUDA; }
+    // items beyond their slate's extent get the score 0 (encoder output: a zero row)
+    float* const out = hidden ? hidden : scores;
+    const size_t out_floats = size_t(B) * S * (hidden ? d : 1);
+    if (cudaMemsetAsync(out, 0, out_floats * sizeof(float), st) != cudaSuccess) { arb_set_error("scorer: memset failed"); return ARB_E_CUDA; }
     k.R = buffer_rows(c, B, S);       // upper bound of the packed row count (grids, tensor maps)
     if (arb_prof_enabled()) {     // per-launch accounting (bench.py) needs the live row count on the host
       int live = 0;
@@ -497,6 +505,16 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     xcur = xout;
   }
   const int has_norm = c.n_layers > 0;
+  if (hidden) {   // encoder output (model.py:62-70): the final norm's output, written at the items' places
+    if (has_norm)
+      return ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, d, hidden, ws + W.meanf, ws + W.stdf, st, 0,
+                        nullptr, plan, rowmap);
+    // no encoder: the reference's encoder is the identity (model.py:59), so this is the activated FC output
+    if (cudaMemcpyAsync(hidden, xcur, size_t(k.R) * d * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+      arb_set_error("scorer: device copy failed"); return ARB_E_CUDA;
+    }
+    return ARB_OK;
+  }
   if (n_outputs(c) > 1) {   // d_output > 1: final norm as its own kernel, then one dot product per output (model.py:116)
     const float* xf = xcur;
     if (has_norm) {
@@ -510,8 +528,10 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   return ARB_OK;
 }
 
-struct ScratchLayout { int64_t dxa, dxb, dxn, dxm, dqkv, dctx, dprob, prob, delta, dfa, dfb, ext, dy16, total; };
-static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, ScratchLayout& Z) {
+struct ScratchLayout { int64_t dxa, dxb, dxn, dxm, dqkv, dctx, dprob, prob, delta, dfa, dfb, ext, dy16, dxin, total; };
+// want_dx: room for d loss / d x over packed rows (backward_ex), after everything the plain backward uses
+static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, ScratchLayout& Z,
+                                bool want_dx = false) {
   const int64_t R = buffer_rows(c, B, S), d = c.d_model;
   const int Sp = int(align_up(S, 4));
   int64_t o = 0;
@@ -535,25 +555,31 @@ static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L
   Z.dfb = widest ? take(R * widest) : 0;
   Z.ext = take(B);      // [B] ints: gradient extent of every slate
   Z.dy16 = (c.bf16 && c.n_layers > 0) ? take(R * d / 2) : 0;   // bf16 copy of the residual-stream gradient
+  Z.dxin = (want_dx && pack_eligible(c, S)) ? take(R * c.n_features) : 0;
   Z.total = o;
 }
 
+// The gradient arrives as d loss / d scores (after a forward call) or as d loss / d hidden (after an encode call):
+// exactly one of dscores / dhidden is non-null.  G == null: no parameter gradient is computed (no weight-gradient
+// product, no gain / bias / column-sum output); dX != null: d loss / d x [B, S, F] is written there.
 static int backward_impl(const arb_scorer_config& c, const float* P, const float* x, const uint8_t* mask,
                          const int64_t* indices, int B, int S,
-                         const float* scores, const float* dscores, float* G, float* ws, int64_t ws_floats,
-                         float* scratch, int64_t scratch_floats, uint64_t seed, cudaStream_t st) {
+                         const float* scores, const float* dscores, const float* dhidden, float* G, float* dX,
+                         float* ws, int64_t ws_floats, float* scratch, int64_t scratch_floats, uint64_t seed,
+                         cudaStream_t st) {
   ParamLayout L;
   ARB_TRY(make_param_layout(c, L));
   WsLayout W;
   make_ws_layout(c, L, B, S, 1, W);
   ScratchLayout Z;
-  make_scratch_layout(c, L, B, S, Z);
+  make_scratch_layout(c, L, B, S, Z, dX != nullptr);
   if (ws_floats < W.total) { arb_set_error("arb_scorer_backward: workspace too small"); return ARB_E_WORKSPACE; }
   if (scratch_floats < Z.total) { arb_set_error("arb_scorer_backward: scratch too small"); return ARB_E_WORKSPACE; }
   Ctx k{c, B, S, int64_t(B) * S, st};
   const int d = c.d_model, F = c.n_features, f = c.d_ff, h = c.n_heads;
   const int dk = c.n_layers > 0 ? d / h : 0;
   const float alpha = c.n_layers > 0 ? 1.0f / sqrtf(float(dk)) : 1.0f;
+  auto g = [&](int64_t off) { return G ? G + off : nullptr; };   // a parameter's gradient, or null
   float* dx = scratch + Z.dxa;      // gradient w.r.t. the residual stream at the current depth
   float* dx_alt = scratch + Z.dxb;
   float* dxn = scratch + Z.dxn;
@@ -581,7 +607,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   const bool fc_act = c.fc_act != ARB_ACT_NONE;
   const DropSite none_site{0u, 0u, 1.0f};
   const DropSite fc_site = make_drop_site(seed, L.n_fc - 1, SITE_FC, p_fc);
-  float* const fc_bias_grad = fc_act ? nullptr : G + L.fc_b[L.n_fc - 1];
+  float* const fc_bias_grad = fc_act ? nullptr : g(L.fc_b[L.n_fc - 1]);
   const DropSite top_site = c.n_layers > 0 ? make_drop_site(seed, c.n_layers - 1, SITE_FFN_OUT, p_drop)
                                            : (fc_act ? none_site : fc_site);
 
@@ -596,7 +622,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   const int* rowmap = pack ? reinterpret_cast<const int*>(ws + W.rowmap) : nullptr;
   const int* poff = pack ? reinterpret_cast<const int*>(ws + W.poff) : nullptr;
   if (pack) { k.rows_dev = plan; k.R = buffer_rows(c, B, S); x = ws + W.xc; gext = reinterpret_cast<int*>(ws + W.kext); }
-  else if (skip) ARB_TRY(slate_extents(mask, dscores, n_outputs(c), B, S, gext, st));
+  else if (skip) ARB_TRY(slate_extents(mask, dhidden ? dhidden : dscores, dhidden ? d : n_outputs(c), B, S, gext, st));
   auto hview = [&](V v, int64_t pitch) { return pack ? head_view(v, dk, int(k.R), h, 1, pitch) : head_view(v, dk, S, h, B, pitch); };
   if (pack) {
     // 256 finite rows of d ctx behind the packed rows (the attention backward's boxes overrun the last slates), and
@@ -609,24 +635,33 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   }
   const int has_norm = c.n_layers > 0;
   const float* xlast = c.n_layers > 0 ? ws + W.layer[c.n_layers - 1].xout : ws + W.x0;
-  float* top_bias_grad = c.n_layers > 0 ? G + L.layer[c.n_layers - 1].b2 : fc_bias_grad;
-  if (n_outputs(c) > 1) {
+  float* top_bias_grad = c.n_layers > 0 ? g(L.layer[c.n_layers - 1].b2) : fc_bias_grad;
+  const float* dy = top_site.thresh ? dxm : dx;   // gradient w.r.t. the output of the linear below the dropout
+  if (dhidden) {
+    if (has_norm) {   // the final norm's backward from the given gradient (packed rows: read at the items' places)
+      ARB_TRY(ln_backward(dhidden, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, d, dx,
+                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16, plan, rowmap));
+    } else if (!fc_act) {   // FC-only model: d hidden through the FC dropout; the FC bias gradient is its column sums
+      if (fc_site.thresh || fc_bias_grad)
+        ARB_TRY(act_backward(dhidden, ws + W.x0, dx, k.R, d, ARB_ACT_NONE, fc_site, 1.0f, fc_bias_grad, st));
+      dy = (fc_site.thresh || fc_bias_grad) ? dx : dhidden;
+    }   // (FC-only with an activation: act_backward below reads dhidden)
+  } else if (n_outputs(c) > 1) {
     if (has_norm) {   // d xf into dxn, then the final norm's backward emits dx (+ its masked copy and the b2 gradient)
       ARB_TRY(head_multi_backward(dscores, scores, ws + W.xf, P + L.head_w, c.out_act, k.R, d, n_outputs(c), dxn,
-                                  G + L.head_w, G + L.head_b, st));
+                                  g(L.head_w), g(L.head_b), st));
       ARB_TRY(ln_backward(dxn, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, d, dx,
-                          G + L.lnf_a, G + L.lnf_b, st, dxm, top_site, top_bias_grad, 0, nullptr, dy16));
+                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16));
     } else {
       ARB_TRY(head_multi_backward(dscores, scores, xlast, P + L.head_w, c.out_act, k.R, d, n_outputs(c), dx,
-                                  G + L.head_w, G + L.head_b, st, dxm, top_site, top_bias_grad));
+                                  g(L.head_w), g(L.head_b), st, dxm, top_site, top_bias_grad));
     }
   } else {
     ARB_TRY(head_backward(dscores, scores, xlast, has_norm ? P + L.lnf_a : nullptr, has_norm ? P + L.lnf_b : nullptr,
                           ws + W.meanf, ws + W.stdf, c.ln_eps, P + L.head_w, P + L.head_b, has_norm, c.out_act, k.R, d,
-                          dx, has_norm ? G + L.lnf_a : nullptr, has_norm ? G + L.lnf_b : nullptr, G + L.head_w,
-                          G + L.head_b, st, dxm, top_site, top_bias_grad, dy16, plan, rowmap));
+                          dx, has_norm ? g(L.lnf_a) : nullptr, has_norm ? g(L.lnf_b) : nullptr, g(L.head_w),
+                          g(L.head_b), st, dxm, top_site, top_bias_grad, dy16, plan, rowmap));
   }
-  const float* dy = top_site.thresh ? dxm : dx;   // gradient w.r.t. the output of the linear below the dropout
   for (int l = c.n_layers - 1; l >= 0; --l) {
     const auto& pl = L.layer[l];
     const auto& wl = W.layer[l];
@@ -636,25 +671,25 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     float* xmid = ws + wl.xmid; float* xn2 = ws + wl.xn2; float* hdn = ws + wl.hdn;
     // ---- feed-forward sublayer backward:  xout = xmid + W2 relu(W1 xn2 + b1) + b2
     const V dyv = bf ? b16(dy16) : V(dy);      // what the sublayer's products read as the incoming gradient
-    ARB_TRY(linear_bwd_weight(k, dyv, d, d, act(hdn), f, f, G + pl.w2));   // (b2 gradient: fused into the kernel that emitted dy)
+    if (G) ARB_TRY(linear_bwd_weight(k, dyv, d, d, act(hdn), f, f, G + pl.w2));   // (b2 gradient: fused into the kernel that emitted dy)
     // hdn <- d hdn in place; hdn > 0 <=> ReLU active AND kept by the hidden dropout, so the mask tile also carries
     // the dropout mask and only the 1/(1-p) scale is needed
     if (wl.hbits)    // ReLU mask from the forward's bit mask (1 bit per unit) instead of the fp32 activation tile
-      ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_COLSUM, nullptr, 0, 1.0f, G + pl.b1,
+      ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_COLSUM, nullptr, 0, 1.0f, g(pl.b1),
                                reinterpret_cast<const uint32_t*>(ws + wl.hbits)));
     else
     ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_MASK_AUX | EPI_COLSUM, act(hdn), f,
-                             drop_on ? 1.0f / (1.0f - p_drop) : 1.0f, G + pl.b1));   // b1 gradient in the epilogue
-    ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
+                             drop_on ? 1.0f / (1.0f - p_drop) : 1.0f, g(pl.b1)));   // b1 gradient in the epilogue
+    if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
     ARB_TRY(linear_bwd_input(k, act(hdn), f, f, wt(pl.w1), d, act(dxn), d, 0, nullptr, 0));
     const DropSite site_ao = make_drop_site(seed, l, SITE_ATTN_OUT, p_drop);
     ARB_TRY(ln_backward(dxn, xmid, P + pl.ln2_a, ws + wl.mean2, ws + wl.std2, c.ln_eps, dx, k.R, d, dx_alt,
-                        G + pl.ln2_a, G + pl.ln2_b, st, dxm, site_ao, G + pl.bo, 0, bf ? dxn : nullptr, dy16, plan));
+                        g(pl.ln2_a), g(pl.ln2_b), st, dxm, site_ao, g(pl.bo), 0, bf ? dxn : nullptr, dy16, plan));
     // dx_alt = d loss / d xmid ; dy = the same through the dropout on the attention sublayer output
     dy = site_ao.thresh ? dxm : dx_alt;
     // ---- attention sublayer backward:  xmid = xin + Wo ctx + bo
     const V dyo = bf ? b16(dy16) : V(dy);
-    ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), d, d, G + pl.wo));   // (bo gradient: fused into the LayerNorm backward above)
+    if (G) ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), d, d, G + pl.wo));   // (bo gradient: fused into the LayerNorm backward above)
     ARB_TRY(linear_bwd_input(k, dyo, d, d, wt(pl.wo), d, dctx, d, 0, nullptr, 0));
     if (use_fused_bwd(c, S)) {
       AttnBwdArgs a;   // dQ, dK, dV from d ctx in one kernel; P is recomputed from the saved row statistics
@@ -677,7 +712,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
       a.mask = mask; a.stat_max = ws + wl.smax; a.stat_sum = ws + wl.ssum; a.delta = scratch + Z.delta;
       a.B = B; a.h = h; a.S = S; a.dk = dk; a.scale = alpha;
       a.drop = make_drop_site(seed, l, SITE_ATTN_P, p_drop);
-      a.dbias_qkv = G + pl.bqkv; a.d_model = d;          // bias gradient of the QKV projection, fused
+      a.dbias_qkv = g(pl.bqkv); a.d_model = d;           // bias gradient of the QKV projection, fused
       a.extent = (skip || pack) ? gext : nullptr;
       ARB_TRY(launch_attn_bwd(a, st));
     } else {
@@ -733,20 +768,20 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         ARB_TRY(launch_gemm_tf32(g, st));
       }
     }
-    ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * d, 3 * d, act(xn1), d, d, G + pl.wqkv));
-    if (!use_fused_bwd(c, S)) ARB_TRY(colsum_accumulate(dqkv, k.R, 3 * d, 3 * d, G + pl.bqkv, st));
+    if (G) ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * d, 3 * d, act(xn1), d, d, G + pl.wqkv));
+    if (G && !use_fused_bwd(c, S)) ARB_TRY(colsum_accumulate(dqkv, k.R, 3 * d, 3 * d, G + pl.bqkv, st));
     ARB_TRY(linear_bwd_input(k, act(dqkv), 3 * d, 3 * d, wt(pl.wqkv), d, act(dxn), d, 0, nullptr, 0));
     DropSite site_below = l > 0 ? make_drop_site(seed, l - 1, SITE_FFN_OUT, p_drop) : (fc_act ? none_site : fc_site);
     // with a positional encoding the encoder input is sqrt(d) * fc_out + pe: the gradient that reaches the FC
     // (through its dropout mask, if any) carries the extra sqrt(d)
     if (l == 0 && c.pe_mode != 0 && !fc_act) site_below.scale *= sqrtf(float(d));
     ARB_TRY(ln_backward(dxn, xin, P + pl.ln1_a, ws + wl.mean1, ws + wl.std1, c.ln_eps, dx_alt, k.R, d, dx,
-                        G + pl.ln1_a, G + pl.ln1_b, st, dxm, site_below, l > 0 ? G + L.layer[l - 1].b2 : fc_bias_grad,
+                        g(pl.ln1_a), g(pl.ln1_b), st, dxm, site_below, l > 0 ? g(L.layer[l - 1].b2) : fc_bias_grad,
                         0, bf ? dxn : nullptr, l > 0 ? dy16 : nullptr, plan));   // (the FC block below layer 0 stays TF32)
     // dx = d loss / d xin ; dy = the same through the dropout that produced xin's last summand
     dy = (site_below.thresh || site_below.scale != 1.0f) ? dxm : dx;
   }
-  if (c.pe_mode == 2) {   // learned table: d pe[idx] += d x0
+  if (c.pe_mode == 2 && G) {   // learned table: d pe[idx] += d x0
     if (!indices) { arb_set_error("scorer: positional encoding needs indices"); return ARB_E_INVALID_ARG; }
     ARB_TRY(pos_backward(dx, reinterpret_cast<const long long*>(indices), mask, G + L.pe, c.pe_rows, k.R, d, st));
   }
@@ -756,32 +791,43 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   float* dfb = scratch + Z.dfb;
   if (fc_act) {
     const float* h_last = W.fc_last ? ws + W.fc_last : ws + W.x0;
-    ARB_TRY(act_backward(dx, h_last, dfa, k.R, d, c.fc_act, fc_site, c.pe_mode != 0 ? sqrtf(float(d)) : 1.0f,
-                         G + L.fc_b[L.n_fc - 1], st, plan));
+    const float* dh = (dhidden && c.n_layers == 0) ? dhidden : dx;   // d loss / d (activated FC output)
+    ARB_TRY(act_backward(dh, h_last, dfa, k.R, d, c.fc_act, fc_site, c.pe_mode != 0 ? sqrtf(float(d)) : 1.0f,
+                         g(L.fc_b[L.n_fc - 1]), st, plan));
     dz = dfa; std::swap(dfa, dfb);
   }
   for (int i = L.n_fc - 1; i >= 0; --i) {
     const int out = L.fc_size[i];
     const int in = i > 0 ? L.fc_size[i - 1] : F;
     const float* hin = i > 0 ? ws + W.fch[i - 1] : (c.fc_input_norm ? ws + W.xnorm : x);
-    ARB_TRY(linear_bwd_weight(k, dz, out, out, hin, in, in, G + L.fc_w[i]));
+    if (G) ARB_TRY(linear_bwd_weight(k, dz, out, out, hin, in, in, G + L.fc_w[i]));
     if (i > 0) {
       const DropSite site = make_drop_site(seed, i - 1, SITE_FC, p_fc);
       if (c.fc_act == ARB_ACT_RELU) {        // h > 0 <=> ReLU active and kept by the dropout: mask tile + 1/(1-p)
         ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, EPI_MASK_AUX | EPI_COLSUM, hin, in,
-                                 site.scale, G + L.fc_b[i - 1]));
+                                 site.scale, g(L.fc_b[i - 1])));
       } else if (c.fc_act == ARB_ACT_NONE && site.thresh == 0) {
-        ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, EPI_COLSUM, nullptr, 0, 1.0f, G + L.fc_b[i - 1]));
+        ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, EPI_COLSUM, nullptr, 0, 1.0f, g(L.fc_b[i - 1])));
       } else {
         ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, 0, nullptr, 0));
-        ARB_TRY(act_backward(dfa, hin, dfa, k.R, in, c.fc_act, site, 1.0f, G + L.fc_b[i - 1], st, plan));
+        ARB_TRY(act_backward(dfa, hin, dfa, k.R, in, c.fc_act, site, 1.0f, g(L.fc_b[i - 1]), st, plan));
       }
       dz = dfa; std::swap(dfa, dfb);
-    } else if (c.fc_input_norm) {            // x is data: only the LayerNorm's weight / bias gradients are needed
-      ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[0], in, dfa, in, 0, nullptr, 0));
-      ARB_TRY(ln_backward(dfa, x, P + L.in_a, ws + W.in_mean, ws + W.in_std, 0.0f, nullptr, k.R, F, dfb,
-                          G + L.in_a, G + L.in_b, st, nullptr, none_site, nullptr, 1, nullptr, nullptr, plan));
+      continue;
     }
+    // the first layer's input: d loss / d x goes to dX (dense rows) or to a packed buffer scattered into dX below
+    float* const dxin = dX ? (pack ? scratch + Z.dxin : dX) : nullptr;
+    if (c.fc_input_norm && (G || dX)) {      // the LayerNorm's backward emits d x (kept only when asked for)
+      ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[0], in, dfa, in, 0, nullptr, 0));
+      ARB_TRY(ln_backward(dfa, x, P + L.in_a, ws + W.in_mean, ws + W.in_std, 0.0f, nullptr, k.R, F, dxin ? dxin : dfb,
+                          g(L.in_a), g(L.in_b), st, nullptr, none_site, nullptr, 1, nullptr, nullptr, plan));
+    } else if (dX) {                         // dX = dZ0 W0
+      ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[0], in, dxin, in, 0, nullptr, 0));
+    }
+  }
+  if (dX && pack) {   // items beyond their slate's packed rows get 0, like their score
+    if (cudaMemsetAsync(dX, 0, size_t(B) * S * F * sizeof(float), st) != cudaSuccess) { arb_set_error("scorer: memset failed"); return ARB_E_CUDA; }
+    ARB_TRY(scatter_rows(scratch + Z.dxin, plan, rowmap, k.R, F, dX, st));
   }
   return ARB_OK;
 }
@@ -818,6 +864,14 @@ extern "C" int64_t arb_scorer_backward_scratch_floats(const arb_scorer_config* c
   make_scratch_layout(*cfg, L, B, S, Z);
   return Z.total;
 }
+extern "C" int64_t arb_scorer_backward_ex_scratch_floats(const arb_scorer_config* cfg, int32_t B, int32_t S,
+                                                         int32_t want_dx) {
+  ParamLayout L;
+  if (!cfg || B <= 0 || S <= 0 || make_param_layout(*cfg, L) != ARB_OK) return -1;
+  ScratchLayout Z;
+  make_scratch_layout(*cfg, L, B, S, Z, want_dx != 0);
+  return Z.total;
+}
 extern "C" int32_t arb_scorer_forward(const arb_scorer_config* cfg, const float* params, const float* x,
                                       const uint8_t* mask, const int64_t* indices, const float* pe_table, int32_t B,
                                       int32_t S, float* scores, float* workspace, int64_t workspace_floats,
@@ -826,8 +880,19 @@ extern "C" int32_t arb_scorer_forward(const arb_scorer_config* cfg, const float*
     arb_set_error("arb_scorer_forward: null pointer or bad shape");
     return ARB_E_INVALID_ARG;
   }
-  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, scores, workspace, workspace_floats, training, seed,
-                      static_cast<cudaStream_t>(stream));
+  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, scores, nullptr, workspace, workspace_floats,
+                      training, seed, static_cast<cudaStream_t>(stream));
+}
+extern "C" int32_t arb_scorer_encode(const arb_scorer_config* cfg, const float* params, const float* x,
+                                     const uint8_t* mask, const int64_t* indices, const float* pe_table, int32_t B,
+                                     int32_t S, float* hidden, float* workspace, int64_t workspace_floats,
+                                     int32_t training, uint64_t seed, void* stream) {
+  if (!cfg || !params || !x || !mask || !hidden || !workspace || B <= 0 || S <= 0) {
+    arb_set_error("arb_scorer_encode: null pointer or bad shape");
+    return ARB_E_INVALID_ARG;
+  }
+  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, nullptr, hidden, workspace, workspace_floats,
+                      training, seed, static_cast<cudaStream_t>(stream));
 }
 extern "C" int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float* params, const float* x,
                                        const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
@@ -838,6 +903,19 @@ extern "C" int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float
     arb_set_error("arb_scorer_backward: null pointer or bad shape");
     return ARB_E_INVALID_ARG;
   }
-  return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, grads, workspace, workspace_floats, scratch,
-                       scratch_floats, seed, static_cast<cudaStream_t>(stream));
+  return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, nullptr, grads, nullptr, workspace,
+                       workspace_floats, scratch, scratch_floats, seed, static_cast<cudaStream_t>(stream));
+}
+extern "C" int32_t arb_scorer_backward_ex(const arb_scorer_config* cfg, const float* params, const float* x,
+                                          const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
+                                          const float* scores, const float* d_scores, const float* d_hidden,
+                                          float* grads, float* d_x, float* workspace, int64_t workspace_floats,
+                                          float* scratch, int64_t scratch_floats, uint64_t seed, void* stream) {
+  if (!cfg || !params || !x || !mask || !workspace || !scratch || B <= 0 || S <= 0 || (!d_scores == !d_hidden) ||
+      (d_scores && !scores)) {
+    arb_set_error("arb_scorer_backward_ex: null pointer, bad shape, or not exactly one of d_scores / d_hidden");
+    return ARB_E_INVALID_ARG;
+  }
+  return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, d_hidden, grads, d_x, workspace,
+                       workspace_floats, scratch, scratch_floats, seed, static_cast<cudaStream_t>(stream));
 }

@@ -100,7 +100,8 @@ struct FwdBatches { static constexpr int value = NV <= 2 ? 4 : 1; };
 // (small launches keep one batch per warp: more batches would leave SMs without a block -- B = 64 has 8 k live rows)
 static inline int fwd_batches_for(int width, long long rows) { return (width <= 256 && rows >= (1 << 17)) ? 4 : 1; }
 
-template <int NV>
+// MAP: packed rows with a row-mapped output (rowmap_out); a template flag so that the plain kernels compile unchanged
+template <int NV, bool MAP>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float* __restrict__ x,
                                                                     const float* __restrict__ a,
                                                                     const float* __restrict__ b, float eps,
@@ -108,7 +109,8 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
                                                                     float* __restrict__ y, float* __restrict__ mean_o,
                                                                     float* __restrict__ std_o, int torch_mode,
                                                                     uint16_t* __restrict__ y16,
-                                                                    const int* __restrict__ rows_dev, int n_batches) {
+                                                                    const int* __restrict__ rows_dev, int n_batches,
+                                                                    const int* __restrict__ rowmap_out) {
   arb_pdl_wait();
   constexpr int NBMAX = FwdBatches<NV>::value;
   const int NB = NBMAX > 1 ? n_batches : 1;
@@ -186,7 +188,10 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
         r[q].v[k].w = ga.v[k].w * (r[q].v[k].w - m) * rinv + gb.v[k].w;
       }
       if (y16) store_row_bf16<NV>(y16 + (row0 + q) * width, width, lane, r[q]);   // bf16 mode: the GEMM operand copy only
-      else store_row<NV>(y + (row0 + q) * width, width, lane, r[q]);
+      else {   // packed rows with rowmap_out: row r goes to y[rowmap_out[r]] (alignment rows: nowhere)
+        const long long yr = MAP ? (long long)rowmap_out[row0 + q] : row0 + q;
+        if (!MAP || yr >= 0) store_row<NV>(y + yr * width, width, lane, r[q]);
+      }
       if (lane == 0) { mean_o[row0 + q] = m; std_o[row0 + q] = sdq; }
     }
     if (NBMAX > 1) {
@@ -202,7 +207,8 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
 // ------------------------------------------------------------------------------------------------ LayerNorm bwd
 // dx = [dres +] r (dxh - mean(dxh)) - r^2 (sum_k dxh_k c_k) / ((d-1) std) * c,   dxh = dy * a, c = x - mean,
 // r = 1/(std+eps).   grad_a += sum_rows dy * xhat,  grad_b += sum_rows dy  (block partials -> DetParts slots).
-template <int NV>
+// MAP: packed rows reading a row-mapped gradient (rowmap_in); a template flag as in ln_fwd_kernel
+template <int NV, bool MAP>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_kernel(const float* __restrict__ dy,
                                                                     const float* __restrict__ x,
                                                                     const float* __restrict__ a,
@@ -216,7 +222,8 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
                                                                     float* __restrict__ colsum_out, int torch_mode,
                                                                     const uint16_t* __restrict__ dy16_in,
                                                                     uint16_t* __restrict__ dy16_out,
-                                                                    const int* __restrict__ rows_dev) {
+                                                                    const int* __restrict__ rows_dev,
+                                                                    const int* __restrict__ rowmap_in) {
   arb_pdl_wait();
   if (rows_dev) {
     rows = min(rows, (long long)__ldg(rows_dev));
@@ -235,7 +242,14 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
   float mean = 0.f, sd = 1.f, mean_n = 0.f, sd_n = 1.f;
   auto fetch = [&](long long row, RowRegs<NV>& gg, RowRegs<NV>& xx, RowRegs<NV>& rr, float& mm, float& ss) {
     if (dy16_in) load_row_bf16<NV>(dy16_in + row * width, width, lane, gg);
-    else load_row<NV>(dy + row * width, width, lane, gg);
+    else if (MAP) {   // packed rows: dy of row r is dy[rowmap_in[r]]; alignment rows have a zero gradient
+      const long long src = rowmap_in[row];
+      if (src >= 0) load_row<NV>(dy + src * width, width, lane, gg);
+      else {
+#pragma unroll
+        for (int k = 0; k < NV; ++k) gg.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    } else load_row<NV>(dy + row * width, width, lane, gg);
     load_row<NV>(x + row * width, width, lane, xx);
     if (dres) load_row<NV>(dres + row * width, width, lane, rr);
     mm = mean_i[row]; ss = std_i[row];
@@ -308,12 +322,12 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
   // block-level reduction of the gain/bias gradients
 #pragma unroll
   for (int pass = 0; pass < 3; ++pass) {
-    if (pass == 2 && !colsum_out) continue;
+    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : colsum_out);
+    if (!dst) continue;      // (no parameter gradients requested: grad_a / grad_b are null)
     const RowRegs<NV>& src = pass == 0 ? acc_a : (pass == 1 ? acc_b : acc_c);
 #pragma unroll
     for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = src.v[k];
     __syncthreads();
-    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : colsum_out);
     for (int c = threadIdx.x; c < width; c += blockDim.x) {
       float t = 0.f;
 #pragma unroll
@@ -773,12 +787,12 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
 #pragma unroll
   for (int pass = 0; pass < 4; ++pass) {
     if (!has_norm && pass < 2) continue;
-    if (pass == 3 && !colsum_out) continue;
+    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : (pass == 2 ? grad_w : colsum_out));
+    if (!dst) continue;      // (no parameter gradients requested: the gradient outputs are null)
     const RowRegs<NV>& src = pass == 0 ? acc_a : (pass == 1 ? acc_b : (pass == 2 ? acc_w : acc_c));
 #pragma unroll
     for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = src.v[k];
     __syncthreads();
-    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : (pass == 2 ? grad_w : colsum_out));
     for (int c = threadIdx.x; c < width; c += blockDim.x) {
       float t = 0.f;
 #pragma unroll
@@ -790,7 +804,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
   acc_wb = warp_sum(acc_wb);
   if (lane == 0) shb[wid] = acc_wb;
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && grad_wb) {
     float t = 0.f;
     for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
     grad_wb[blockIdx.x] = t;                        // this block's slot (DetParts)
@@ -863,7 +877,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
     }
   }
   // block-level column reductions: pass -1 = colsum_out, pass j = grad_w row j
-  for (int j = colsum_out ? -1 : 0; j < n; ++j) {
+  for (int j = colsum_out ? -1 : 0; j < (grad_w ? n : 0); ++j) {
     float acc_b = 0.f;
     if (j >= 0) {
 #pragma unroll
@@ -1112,7 +1126,7 @@ __device__ __forceinline__ void r_reduce_columns(float4 (&acc)[4], float (*sh)[1
   __syncthreads();
 }
 
-template <int LPR>
+template <int LPR, bool MAP>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_r_kernel(const float* __restrict__ x,
                                                                       const float* __restrict__ a,
                                                                       const float* __restrict__ b, float eps,
@@ -1120,7 +1134,8 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_r_kernel(const flo
                                                                       float* __restrict__ mean_o,
                                                                       float* __restrict__ std_o, int torch_mode,
                                                                       uint16_t* __restrict__ y16,
-                                                                      const int* __restrict__ rows_dev, int steps) {
+                                                                      const int* __restrict__ rows_dev, int steps,
+                                                                      const int* __restrict__ rowmap_out) {
   arb_pdl_wait();
   constexpr int RW = 32 / LPR, W = 16 * LPR;
   const int lane = threadIdx.x & 31, rg = lane / LPR;
@@ -1159,7 +1174,10 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_r_kernel(const flo
     }
     if (row < rows) {
       if (y16) r_store_bf16<LPR>(y16 + row * W, lane, cur);
-      else r_store<LPR>(y + row * W, lane, cur);
+      else {   // (rowmap_out: see ln_fwd_kernel)
+        const long long yr = MAP ? (long long)rowmap_out[row] : row;
+        if (!MAP || yr >= 0) r_store<LPR>(y + yr * W, lane, cur);
+      }
       if (lane % LPR == 0) { mean_o[row] = m; std_o[row] = sdq; }
     }
 #pragma unroll
@@ -1167,13 +1185,14 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_r_kernel(const flo
   }
 }
 
-template <int LPR>
+template <int LPR, bool MAP>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) ln_bwd_r_kernel(
     const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ a,
     const float* __restrict__ mean_i, const float* __restrict__ std_i, float eps, const float* __restrict__ dres,
     long long rows, int steps, float* __restrict__ dx, float* __restrict__ grad_a, float* __restrict__ grad_b,
     float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out, int torch_mode,
-    const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev) {
+    const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
+    const int* __restrict__ rowmap_in) {
   arb_pdl_wait();
   constexpr int RW = 32 / LPR, W = 16 * LPR;
   if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
@@ -1193,7 +1212,9 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) ln_bwd_r_kernel(
     float mean = 0.f, sd = 1.f;
     r_zero(g); r_zero(xr); r_zero(res);
     if (ok) {
-      if (dy16_in) r_load_bf16<LPR>(dy16_in + row * W, lane, g); else r_load<LPR>(dy + row * W, lane, g);
+      if (dy16_in) r_load_bf16<LPR>(dy16_in + row * W, lane, g);
+      else if (MAP) { const long long src = rowmap_in[row]; if (src >= 0) r_load<LPR>(dy + src * W, lane, g); }
+      else r_load<LPR>(dy + row * W, lane, g);
       r_load<LPR>(x + row * W, lane, xr);
       if (dres) r_load<LPR>(dres + row * W, lane, res);
       mean = mean_i[row]; sd = std_i[row];
@@ -1249,8 +1270,8 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) ln_bwd_r_kernel(
       }
     }
   }
-  r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
-  r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
+  if (grad_a) r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
+  if (grad_b) r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
   if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, lane, wid, colsum_out);
 }
 
@@ -1430,16 +1451,14 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) head_bwd_r_kernel(
       }
     }
   }
-  if (has_norm) {
-    r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
-    r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
-  }
-  r_reduce_columns<LPR>(acc_w, sh, lane, wid, grad_w);
+  if (has_norm && grad_a) r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
+  if (has_norm && grad_b) r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
+  if (grad_w) r_reduce_columns<LPR>(acc_w, sh, lane, wid, grad_w);
   if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, lane, wid, colsum_out);
   acc_wb = warp_sum(acc_wb);
   if (lane == 0) shb[wid] = acc_wb;
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && grad_wb) {
     float t = 0.f;
     for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
     grad_wb[blockIdx.x] = t;                        // this block's slot (DetParts)
@@ -1555,6 +1574,30 @@ __global__ void __launch_bounds__(256) zero_rows_kernel(ZeroRegions z, const int
   }
 }
 
+// The inverse of the feature packing: packed row r of src [rows, width] goes to dst[rowmap[r]] of the dense [B * S, width]
+// tensor, which the caller has zero-filled (items beyond their slate's packed rows keep 0).  A warp per row, 128-bit
+// accesses.
+__global__ void __launch_bounds__(256) scatter_rows_kernel(const float* __restrict__ src, const int* __restrict__ plan,
+                                                           const int* __restrict__ rowmap, long long cap_rows, int width,
+                                                           float* __restrict__ dst) {
+  arb_pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= min(cap_rows, (long long)plan[1])) return;      // (rows from plan[1] on are alignment rows)
+  const long long to = rowmap[row];
+  if (to < 0) return;
+  for (int c = lane * 4; c < width; c += 128)
+    *reinterpret_cast<float4*>(dst + to * width + c) = *reinterpret_cast<const float4*>(src + row * width + c);
+}
+
+int scatter_rows(const float* src, const int* plan, const int* rowmap, long long cap_rows, int width, float* dst,
+                 cudaStream_t st) {
+  if (width % 4) { arb_set_error("scatter_rows: the width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
+  ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(cap_rows, plan) * 8.0 * width, st);
+  return launch(scatter_rows_kernel, dim3(unsigned((cap_rows + 7) / 8)), dim3(256), 0, st, /*pdl=*/true, src, plan,
+                rowmap, cap_rows, width, dst);
+}
+
 int pack_plan(const float* x, const int* ext, int B, int S, int F, int* off, int* plan, int* rowmap, float* xc,
               long long cap_rows, cudaStream_t st) {
   if (F % 4) { arb_set_error("packed rows: the feature count must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
@@ -1580,27 +1623,30 @@ int zero_rows(const ZeroRegions& z, const int* plan, long long cap_rows, cudaStr
 }
 
 int ln_forward(const float* x, const float* a, const float* b, float eps, long long rows, int width, float* y,
-               float* mean, float* sd, cudaStream_t st, int torch_mode, void* y16, const int* rows_dev) {
+               float* mean, float* sd, cudaStream_t st, int torch_mode, void* y16, const int* rows_dev,
+               const int* rowmap_out) {
+  if (rowmap_out && y16) { arb_set_error("ln_forward: a row-mapped output is fp32 only"); return ARB_E_INVALID_ARG; }
   if (width % 4) { arb_set_error("LayerNorm width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * ((y16 ? 6.0 : 8.0) * width + 8), st);
   if (const int lpr = r_lpr(width, R_LN_FWD)) {      // W = 128 / 256: several rows per warp step (see ln_fwd_r_kernel)
     const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    if (lpr == 8) return launch(ln_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
-    return launch(ln_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps);
+    if (lpr == 8) return launch(rowmap_out ? ln_fwd_r_kernel<8, true> : ln_fwd_r_kernel<8, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
+    return launch(rowmap_out ? ln_fwd_r_kernel<16, true> : ln_fwd_r_kernel<16, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
   }
   const int nb = fwd_batches_for(width, rows);
   const int per_block = ROWS_PER_BLOCK * FWD_RPW * nb;
   const unsigned blocks = unsigned((rows + per_block - 1) / per_block);
   int rc;
-  ARB_DISPATCH_NV(width, (rc = launch(ln_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, nb)));
+  ARB_DISPATCH_NV(width, (rc = launch(rowmap_out ? ln_fwd_kernel<NV, true> : ln_fwd_kernel<NV, false>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, nb, rowmap_out)));
   return rc;
 }
 
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
                 const float* dres, long long rows, int width, float* dx, float* grad_a, float* grad_b,
                 cudaStream_t st, float* dx_masked, DropSite site, float* colsum_out, int torch_mode,
-                const void* dy16_in, void* dy16_out, const int* rows_dev) {
+                const void* dy16_in, void* dy16_out, const int* rows_dev, const int* rowmap_in) {
+  if (rowmap_in && dy16_in) { arb_set_error("ln_backward: a row-mapped gradient is fp32 only"); return ARB_E_INVALID_ARG; }
   if (site.thresh == 0 && site.scale == 1.0f) dx_masked = nullptr;
   if (dy16_out && dx_masked == nullptr && (site.thresh != 0 || site.scale != 1.0f)) {
     arb_set_error("ln_backward: a masked bf16 copy needs the masked fp32 buffer too"); return ARB_E_INVALID_ARG;
@@ -1616,10 +1662,10 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
   int rc = dp.begin(st);
   if (rc) return rc;
   if (lpr) {
-    if (lpr == 8) rc = launch(ln_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
-    else rc = launch(ln_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev);
+    if (lpr == 8) rc = launch(rowmap_in ? ln_bwd_r_kernel<8, true> : ln_bwd_r_kernel<8, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in);
+    else rc = launch(rowmap_in ? ln_bwd_r_kernel<16, true> : ln_bwd_r_kernel<16, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in);
   } else {
-    ARB_DISPATCH_NV(width, (rc = launch(ln_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev)));
+    ARB_DISPATCH_NV(width, (rc = launch(rowmap_in ? ln_bwd_kernel<NV, true> : ln_bwd_kernel<NV, false>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in)));
   }
   if (rc) return rc;
   return dp.finish(st);

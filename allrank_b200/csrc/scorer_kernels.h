@@ -13,8 +13,9 @@ namespace arb {
 int ln_forward(const float* x, const float* a, const float* b, float eps, long long rows, int width, float* y,
                float* mean, float* sd, cudaStream_t st, int torch_mode = 0,
                void* y16 = nullptr,    // y16 != nullptr: write the output as bfloat16 there INSTEAD of y (bf16 mode)
-               const int* rows_dev = nullptr);   // packed rows: device pointer to the live row count (<= rows)
-// dx = (dres ? dres : 0) + LayerNormBackward(dy); grad_a / grad_b are accumulated (atomicAdd)
+               const int* rows_dev = nullptr,    // packed rows: device pointer to the live row count (<= rows)
+               const int* rowmap_out = nullptr); // packed rows: write row r to y[rowmap_out[r]] (< 0: not at all); fp32
+// dx = (dres ? dres : 0) + LayerNormBackward(dy); grad_a / grad_b (null: not computed) are accumulated
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
                 const float* dres, long long rows, int width, float* dx, float* grad_a, float* grad_b,
                 cudaStream_t st, float* dx_masked = nullptr, DropSite site = DropSite{0u, 0u, 1.0f},
@@ -22,7 +23,8 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
                 int torch_mode = 0,
                 const void* dy16_in = nullptr,  // bf16 mode: dy is read from this bfloat16 buffer instead
                 void* dy16_out = nullptr,       // bf16 mode: bfloat16 copy of the emitted (masked) gradient
-                const int* rows_dev = nullptr);
+                const int* rows_dev = nullptr,
+                const int* rowmap_in = nullptr);  // packed rows: dy of row r is dy[rowmap_in[r]] (< 0: zero); fp32
 int pos_forward(float* x, const long long* indices, const uint8_t* mask, const float* pe, int pe_rows, float scale,
                 long long rows, int width, cudaStream_t st);
 int pos_backward(const float* dx, const long long* indices, const uint8_t* mask, float* dpe, int pe_rows, long long rows,
@@ -52,7 +54,8 @@ int head_forward(const float* x, const float* a, const float* b, float eps, cons
                  const int* rowmap = nullptr);   // packed rows: score[rowmap[row]] (rows with rowmap < 0 have no score)
 int head_backward(const float* dscore, const float* score, const float* x, const float* a, const float* b,
                   const float* mean, const float* sd, float eps, const float* w, const float* wb, int has_norm,
-                  int act, long long rows, int width, float* dx, float* grad_a, float* grad_b, float* grad_w,
+                  int act, long long rows, int width, float* dx,
+                  float* grad_a, float* grad_b, float* grad_w,   // (gradient outputs: null = not computed)
                   float* grad_wb, cudaStream_t st, float* dx_masked = nullptr,
                   DropSite site = DropSite{0u, 0u, 1.0f}, float* colsum_out = nullptr, void* dy16_out = nullptr,
                   const int* rows_dev = nullptr, const int* rowmap = nullptr);
@@ -76,6 +79,10 @@ struct ZeroRegions {
   }
 };
 int zero_rows(const ZeroRegions& z, const int* plan, long long cap_rows, cudaStream_t st);
+// dst[rowmap[r]] = src[r] for the packed rows r below plan[1] (and cap_rows); dst is dense [B * S, width], zero-filled
+// by the caller
+int scatter_rows(const float* src, const int* plan, const int* rowmap, long long cap_rows, int width, float* dst,
+                 cudaStream_t st);
 // d_output = n > 1: scores [rows, n] from the (already normalised) rows xf; see scorer_kernels.cu
 int head_multi_forward(const float* xf, const float* w, const float* wb, int act, long long rows, int width, int n,
                        float* score, cudaStream_t st);

@@ -5,6 +5,7 @@ Same call surface as the reference (/root/reference/allrank/models/model.py):
     model = make_model(fc_model=..., transformer=..., post_model=..., n_features=...)      # model.py:131
     scores = model(x, mask, indices)            # [B,S] ([B,S,d_output] when d_output > 1; model.py:72-80)
     scores = model.score(x, mask, indices)      # [B,S]   (model.py:82-92,  train_utils.py:34)
+    hidden = model.prepare_for_output(x, mask, indices)   # [B,S,d_model], the encoder output (model.py:62-70)
     model.parameters() / .state_dict() / .load_state_dict() / .train() / .eval() / .to(device)
 
 and the same state_dict keys and shapes as the reference's module tree (so a reference `model.pkl` loads):
@@ -29,6 +30,11 @@ parameter buffer.
 The input block is the reference's general FCModel (model.py:16-44): optional nn.LayerNorm on the features, then any
 number of Linear layers each followed by the activation (None / ReLU / Tanh / Sigmoid) and dropout.  With
 `transformer=None` the model is that MLP plus the output head (the `*_mlp.json` configurations of the paper).
+Autograd reaches `x` as well as the parameters: x.grad (in x's dtype and shape) comes from the CUDA backward, which
+then also runs the first FC layer's input-gradient product; with every parameter frozen it computes no parameter
+gradient at all.  In the default packed-row layout (include/allrank_b200.h: arb_set_pack_rows) items at or beyond their
+slate's packed rows get 0 in `prepare_for_output` and in x.grad, and a gradient sent to their hidden rows is ignored --
+the same contract as their score.  Double backward is not supported (it raises).
 Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes.
 """
 import copy
@@ -59,6 +65,11 @@ _lib.register("arb_scorer_forward", c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i
                                           c_p])
 _lib.register("arb_scorer_backward", c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64,
                                            ctypes.c_uint64, c_p])
+_lib.register("arb_scorer_encode", c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i64, c_i, ctypes.c_uint64,
+                                         c_p])
+_lib.register("arb_scorer_backward_ex_scratch_floats", c_i64, [c_p, c_i, c_i, c_i])
+_lib.register("arb_scorer_backward_ex", c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p,
+                                              c_i64, ctypes.c_uint64, c_p])
 
 
 # ------------------------------------------------------------------------------------------------ module tree
@@ -151,26 +162,58 @@ def _clone_linear(proto):
 
 
 # ------------------------------------------------------------------------------------------------ autograd glue
+# `anchor` requires grad exactly when some parameter does (it stands for all of them: they are views of one flat buffer
+# that the C backward fills); `x` is the caller's tensor, padded to the C layout inside the Function.
 class _ScorerFn(torch.autograd.Function):
+    """x -> scores (arb_scorer_forward / arb_scorer_backward_ex from d_scores)."""
+
     @staticmethod
     def forward(ctx, anchor, x, mask, model, indices):
-        keep = ctx.needs_input_grad[0]
+        keep = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        xin = model._pad_features(x)
         seed = model._draw_seed()
-        scores, ws = model._launch_forward(x, mask, keep, seed, indices)
+        scores, ws = model._launch_forward(xin, mask, keep, seed, indices)
         if keep:
-            ctx.model = model
-            ctx.ws = ws
-            ctx.seed = seed
-            ctx.indices = indices
-            ctx.save_for_backward(x, mask, scores)
+            ctx.model, ctx.ws, ctx.seed, ctx.indices = model, ws, seed, indices
+            ctx.x_meta = (x.shape, x.dtype)
+            ctx.save_for_backward(xin, mask, scores)
         return scores
 
     @staticmethod
+    @torch.autograd.function.once_differentiable
     def backward(ctx, d_scores):
-        x, mask, scores = ctx.saved_tensors
-        ctx.model._launch_backward(x, mask, scores, d_scores.contiguous().float(), ctx.ws, ctx.seed, ctx.indices)
+        xin, mask, scores = ctx.saved_tensors
+        dx = ctx.model._launch_backward(xin, mask, scores, d_scores.contiguous().float(), ctx.ws, ctx.seed,
+                                        ctx.indices, want_params=ctx.needs_input_grad[0],
+                                        want_dx=ctx.needs_input_grad[1])
         ctx.ws = None
-        return None, None, None, None, None
+        return None, ctx.model._input_grad(dx, ctx.x_meta), None, None, None
+
+
+class _EncodeFn(torch.autograd.Function):
+    """x -> hidden [B,S,d_model] (arb_scorer_encode / arb_scorer_backward_ex from d_hidden)."""
+
+    @staticmethod
+    def forward(ctx, anchor, x, mask, model, indices):
+        keep = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        xin = model._pad_features(x)
+        seed = model._draw_seed()
+        hidden, ws = model._launch_forward(xin, mask, keep, seed, indices, encode=True)
+        if keep:
+            ctx.model, ctx.ws, ctx.seed, ctx.indices = model, ws, seed, indices
+            ctx.x_meta = (x.shape, x.dtype)
+            ctx.save_for_backward(xin, mask)
+        return hidden
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_hidden):
+        xin, mask = ctx.saved_tensors
+        dx = ctx.model._launch_backward(xin, mask, None, d_hidden.contiguous().float(), ctx.ws, ctx.seed, ctx.indices,
+                                        want_params=ctx.needs_input_grad[0], want_dx=ctx.needs_input_grad[1],
+                                        from_hidden=True)
+        ctx.ws = None
+        return None, ctx.model._input_grad(dx, ctx.x_meta), None, None, None
 
 
 class LTRModel(nn.Module):
@@ -367,10 +410,21 @@ class LTRModel(nn.Module):
             raise ValueError(f"x must be [batch, slate, {self.n_features}]")
         if mask.shape != x.shape[:2]:
             raise ValueError("mask must be [batch, slate]")
+        return mask.detach().to(torch.uint8).contiguous()
+
+    def _pad_features(self, x):
+        """The C layout of x: contiguous fp32 [B, S, _Fp] (features zero-padded to a multiple of 4)."""
         x = x.detach().float()
         if self._Fp != self.n_features:
             x = torch.nn.functional.pad(x, (0, self._Fp - self.n_features))
-        return x.contiguous(), mask.detach().to(torch.uint8).contiguous()
+        return x.contiguous()
+
+    def _input_grad(self, dx, x_meta):
+        """d loss / d x in the caller's shape and dtype (the padded feature columns dropped), or None."""
+        if dx is None:
+            return None
+        shape, dtype = x_meta
+        return dx[..., :self.n_features].to(dtype).reshape(shape)
 
     def _draw_seed(self):
         """Per-call dropout seed from torch's global CPU generator (so torch.manual_seed makes runs repeatable)."""
@@ -378,7 +432,8 @@ class LTRModel(nn.Module):
             return int(torch.randint(0, 2 ** 62, (1,)).item())
         return 0
 
-    def _launch_forward(self, x, mask, keep_for_backward, seed=0, indices=None):
+    def _launch_forward(self, x, mask, keep_for_backward, seed=0, indices=None, encode=False):
+        """scores (encode: the encoder output [B,S,d_model]) and the workspace kept for backward (or None)."""
         training = keep_for_backward
         B, S = x.shape[0], x.shape[1]
         dev = x.device
@@ -390,39 +445,50 @@ class LTRModel(nn.Module):
         self._cfg.fc_dropout = self.fc_dropout_p if self.training else 0.0
         n_ws = int(_lib.lib().arb_scorer_workspace_floats(cfg, B, S, 1 if training else 0))
         ws = torch.empty(n_ws, dtype=torch.float32, device=dev)
-        shape = (B, S) if self.d_output == 1 else (B, S, self.d_output)   # squeeze(dim=2) is a no-op for n > 1 (model.py:117)
+        if encode:
+            shape = (B, S, self.d_model)
+        else:
+            shape = (B, S) if self.d_output == 1 else (B, S, self.d_output)   # squeeze(dim=2) is a no-op for n > 1 (model.py:117)
         scores = torch.empty(shape, dtype=torch.float32, device=dev)
+        name = "arb_scorer_encode" if encode else "arb_scorer_forward"
         with torch.cuda.device(dev):
             table = self._pe_table(dev)
-            rc = _lib.lib().arb_scorer_forward(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
-                                               _lib.ptr(indices), _lib.ptr(table), B, S,
-                                               _lib.ptr(scores), _lib.ptr(ws), n_ws, 1 if training else 0,
-                                               ctypes.c_uint64(seed), _lib.stream_ptr(dev))
-        _lib.check(rc, "arb_scorer_forward")
+            rc = getattr(_lib.lib(), name)(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
+                                           _lib.ptr(indices), _lib.ptr(table), B, S,
+                                           _lib.ptr(scores), _lib.ptr(ws), n_ws, 1 if training else 0,
+                                           ctypes.c_uint64(seed), _lib.stream_ptr(dev))
+        _lib.check(rc, name)
         return scores, (ws if training else None)
 
-    def _launch_backward(self, x, mask, scores, d_scores, ws, seed=0, indices=None):
+    def _launch_backward(self, x, mask, scores, d_out, ws, seed=0, indices=None, want_params=True, want_dx=False,
+                         from_hidden=False):
+        """Accumulates the parameter gradients (want_params) and returns d loss / d x [B,S,_Fp] (want_dx, else None).
+        d_out is d loss / d scores, or d loss / d hidden (from_hidden)."""
         B, S = x.shape[0], x.shape[1]
         dev = x.device
         cfg = ctypes.byref(self._cfg)
-        fresh = any(p.grad is None or p.grad.data_ptr() != gv.data_ptr() for p, _, gv in self._views)
+        fresh = want_params and any(p.grad is None or p.grad.data_ptr() != gv.data_ptr() for p, _, gv in self._views)
         if fresh:                      # after optimizer.zero_grad(set_to_none=True): start from zero
             self._flat_grad.zero_()
         self._cfg.dropout = self.dropout_p if seed else 0.0          # same mask configuration as the forward call
         self._cfg.fc_dropout = self.fc_dropout_p if seed else 0.0
-        n_sc = int(_lib.lib().arb_scorer_backward_scratch_floats(cfg, B, S))
+        n_sc = int(_lib.lib().arb_scorer_backward_ex_scratch_floats(cfg, B, S, 1 if want_dx else 0))
         scratch = torch.empty(n_sc, dtype=torch.float32, device=dev)
+        dx = torch.empty((B, S, self._Fp), dtype=torch.float32, device=dev) if want_dx else None
         with torch.cuda.device(dev):
-            rc = _lib.lib().arb_scorer_backward(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
-                                                _lib.ptr(indices), B, S,
-                                                _lib.ptr(scores), _lib.ptr(d_scores), _lib.ptr(self._flat_grad),
-                                                _lib.ptr(ws), ws.numel(), _lib.ptr(scratch), n_sc,
-                                                ctypes.c_uint64(seed), _lib.stream_ptr(dev))
-        _lib.check(rc, "arb_scorer_backward")
+            rc = _lib.lib().arb_scorer_backward_ex(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
+                                                   _lib.ptr(indices), B, S, _lib.ptr(scores),
+                                                   None if from_hidden else _lib.ptr(d_out),
+                                                   _lib.ptr(d_out) if from_hidden else None,
+                                                   _lib.ptr(self._flat_grad) if want_params else None, _lib.ptr(dx),
+                                                   _lib.ptr(ws), ws.numel(), _lib.ptr(scratch), n_sc,
+                                                   ctypes.c_uint64(seed), _lib.stream_ptr(dev))
+        _lib.check(rc, "arb_scorer_backward_ex")
         if fresh:
             for p, _, gv in self._views:
                 if p.requires_grad:
                     p.grad = gv
+        return dx
 
     def _replicate_for_data_parallel(self):
         raise RuntimeError(
@@ -432,18 +498,26 @@ class LTRModel(nn.Module):
             "CustomDataParallel wrap of allrank/main.py:76-78")
 
     # ---- public surface (model.py:62-92) ---------------------------------------------------------------
-    def prepare_for_output(self, x, mask, indices):
-        raise NotImplementedError("the fused scorer does not expose the encoder output; use forward()/score()")
+    def _call(self, fn_cls, x, mask, indices):
+        """fn_cls (_ScorerFn / _EncodeFn) through autograd when a gradient may be wanted, else a plain launch."""
+        m = self._prep_inputs(x, mask)
+        idx = self._prep_indices(indices, x.device)
+        self._ensure_packed(x.device)
+        params = any(p.requires_grad for p in self.parameters())
+        if torch.is_grad_enabled() and (params or x.requires_grad):
+            anchor = self._anchor if params else self._anchor.detach()
+            return fn_cls.apply(anchor, x, m, self, idx)
+        out, _ = self._launch_forward(self._pad_features(x), m, False, self._draw_seed(), idx,
+                                      encode=fn_cls is _EncodeFn)
+        return out
+
+    def prepare_for_output(self, x, mask, indices=None):
+        """The encoder output [B, S, d_model] (model.py:62-70): the final LayerNorm's output, or with
+        `transformer=None` the FC block's output.  Dropout follows train() / eval() as in forward()."""
+        return self._call(_EncodeFn, x, mask, indices)
 
     def forward(self, x, mask, indices=None):
-        xin, m = self._prep_inputs(x, mask)
-        idx = self._prep_indices(indices, xin.device)
-        self._ensure_packed(xin.device)
-        needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
-        if needs_grad:
-            return _ScorerFn.apply(self._anchor, xin, m, self, idx)
-        scores, _ = self._launch_forward(xin, m, False, self._draw_seed(), idx)
-        return scores
+        return self._call(_ScorerFn, x, mask, indices)
 
     def score(self, x, mask, indices=None):
         out = self.forward(x, mask, indices)

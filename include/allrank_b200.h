@@ -225,6 +225,30 @@ int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float* params, c
                             float* workspace, int64_t workspace_floats, float* scratch, int64_t scratch_floats,
                             uint64_t seed, void* stream);
 
+/* The encoder output (LTRModel.prepare_for_output, model.py:62-70): the arguments of arb_scorer_forward, but instead
+ * of scores it writes hidden [B,S,d_model] fp32 -- the final LayerNorm's output, or with n_layers == 0 the FC block's
+ * output after its activation and dropout (the reference's encoder is then the identity).  The head is not run.
+ * training != 0 keeps the workspace for arb_scorer_backward_ex(d_hidden = ...), as the forward does.
+ * Packed rows (arb_set_pack_rows): items at or beyond their slate's packed rows get a zero row, as they get the score 0. */
+int32_t arb_scorer_encode(const arb_scorer_config* cfg, const float* params, const float* x, const uint8_t* mask,
+                          const int64_t* indices, const float* pe_table,
+                          int32_t B, int32_t S, float* hidden, float* workspace, int64_t workspace_floats,
+                          int32_t training, uint64_t seed, void* stream);
+/* The backward with a choice of starting point and outputs.  Exactly one of
+ *   d_scores [B,S] (or [B,S,d_output]; after arb_scorer_forward, `scores` its output) and
+ *   d_hidden [B,S,d_model] (after arb_scorer_encode; `scores` may be NULL)
+ * is non-null.  grads: accumulated as by arb_scorer_backward; NULL computes and writes no parameter gradient (no
+ * weight-gradient product, no gain / bias / column-sum output).  d_x: NULL, or [B,S,cfg->n_features] fp32, overwritten
+ * with d loss / d x (packed rows: items at or beyond their slate's packed rows get 0, and d_hidden sent to them is
+ * ignored).  `scratch`: arb_scorer_backward_ex_scratch_floats(cfg, B, S, d_x != NULL) floats.
+ * arb_scorer_backward(..., d_scores, grads, ...) is arb_scorer_backward_ex(..., d_scores, NULL, grads, NULL, ...). */
+int64_t arb_scorer_backward_ex_scratch_floats(const arb_scorer_config* cfg, int32_t B, int32_t S, int32_t want_dx);
+int32_t arb_scorer_backward_ex(const arb_scorer_config* cfg, const float* params, const float* x, const uint8_t* mask,
+                               const int64_t* indices, int32_t B, int32_t S, const float* scores,
+                               const float* d_scores, const float* d_hidden, float* grads, float* d_x,
+                               float* workspace, int64_t workspace_floats, float* scratch, int64_t scratch_floats,
+                               uint64_t seed, void* stream);
+
 /* 0: unfused attention (materialised logits + generic GEMMs); 1: fused tensor-core attention forward kernel, unfused
  * backward; 2 (default): fused forward and backward kernels.  Fused kernels serve slates of <= 256 items (backward:
  * head width <= 32); other shapes use the unfused path automatically.  Process-wide; exists for A/B tests. */
