@@ -7,6 +7,7 @@ sequence dcg/ndcg/mrr see) and one gather kernel (`arb_gather_slates`, csrc/slat
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -82,4 +83,29 @@ def rank_slates(datasets, model, config):
     return {role: rank_dataloader(_as_loader(ds, config), model) for role, ds in datasets.items()}
 
 
-__all__ = ["rank_slates", "rank_dataloader", "rank_batch", "reorder_slates"]
+def metrics_on_clicked_slates(clicked_slates, chunk=8192):
+    """inference_utils.metrics_on_clicked_slates (:63-82): per clicked slate {"slate_length", "no_of_clicks", "dcg",
+    "ndcg"}, the metrics of the clicks (-1 = padding) under the order the slate is in (scores S..1).  One
+    arb_rank_metrics launch per chunk of equal-length slates computes dcg and ndcg (bit-identical to the reference's
+    ndcg / dcg); no_of_clicks is sum(y > 0) of the caller's row, numpy's integer for an array."""
+    Xs, ys = clicked_slates
+    ys = list(ys)
+    lengths = np.array([len(y) for y in ys], dtype=np.int64)
+    dcgs, ndcgs = [0.0] * len(ys), [0.0] * len(ys)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    for S in np.unique(lengths):
+        idx = np.flatnonzero(lengths == S)
+        y_pred = torch.arange(int(S), 0, -1, dtype=torch.float32, device=dev)
+        for c0 in range(0, len(idx), chunk):
+            part = idx[c0:c0 + chunk]
+            labels = torch.as_tensor(np.stack([np.asarray(ys[k], dtype=np.float32) for k in part])).to(dev)
+            out = _metrics._launch(y_pred.expand(len(part), int(S)).contiguous(), labels, [int(S)], [int(S)],
+                                   _metrics.GAIN_POW2, PADDED_Y_VALUE, 1.0, ("dcg", "ndcg"))
+            for k, d, n in zip(part, out["dcg"][:, 0].tolist(), out["ndcg"][:, 0].tolist()):
+                dcgs[k], ndcgs[k] = d, n
+    for y, d, n in zip(ys, dcgs, ndcgs):
+        clicked = y > 0
+        yield {"slate_length": len(y), "no_of_clicks": clicked.sum(), "dcg": d, "ndcg": n}
+
+
+__all__ = ["rank_slates", "rank_dataloader", "rank_batch", "reorder_slates", "metrics_on_clicked_slates"]

@@ -12,7 +12,13 @@ The callers either side of the path (SURVEY.md 8(f) ranks 3-4) are rebound the s
     rank_slates   : allrank.inference.inference_utils.rank_slates                      inference_utils.py:12-30
     slate loading : allrank.data.dataset_loading.{load_libsvm_dataset, create_data_loaders} (+ the names main.py
                     imported from it, main.py:8) -- opt-in (`patch_data=True`): the corpus then lives in HBM.
+    click metrics : allrank.inference.inference_utils.metrics_on_clicked_slates                inference_utils.py:63-82
+    clicks        : allrank.click_models.click_utils.click_on_slates -- opt-in (`patch_clicks=True`): random
+                    click models then draw from a counter hash instead of numpy's stream.
+allrank/rank_and_click.py imports make_model, CustomDataParallel, rank_slates, metrics_on_clicked_slates and
+click_on_slates by name (rank_and_click.py:11-18); those bindings are rebound too.
 """
+from . import click_models as _click_models
 from . import data as _data
 from . import inference as _inference
 from . import losses as _losses
@@ -28,7 +34,8 @@ METRIC_NAMES = ("ndcg", "dcg", "mrr")
 
 _MODULES = {"losses": "allrank.models.losses", "metrics": "allrank.models.metrics", "model": "allrank.models.model",
             "main": "allrank.main", "train_utils": "allrank.training.train_utils",
-            "inference_utils": "allrank.inference.inference_utils", "dataset_loading": "allrank.data.dataset_loading"}
+            "inference_utils": "allrank.inference.inference_utils", "dataset_loading": "allrank.data.dataset_loading",
+            "rank_and_click": "allrank.rank_and_click", "click_utils": "allrank.click_models.click_utils"}
 
 
 def single_process_model(model):
@@ -47,9 +54,17 @@ def _rebind(saved, mod_key, name, fn):
     setattr(target, name, fn)
 
 
-def patch_allrank(patch_model=True, patch_eval=True, patch_data=False):
-    """Rebind allrank.models.{losses,metrics}.<name> (and make_model, the epoch-metric helpers, rank_slates and --
-    opt-in -- the slate loaders) to the CUDA implementations.
+def _import_rank_and_click():
+    try:
+        import allrank.rank_and_click  # noqa: F401
+        return True
+    except Exception:
+        return False
+
+
+def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_clicks=False):
+    """Rebind allrank.models.{losses,metrics}.<name> (and make_model, the epoch-metric helpers, rank_slates,
+    metrics_on_clicked_slates and -- opt-in -- the slate loaders and click_on_slates) to the CUDA implementations.
     Returns the dict of original callables so the caller can restore them."""
     import allrank.models.losses as ref_losses
     import allrank.models.metrics as ref_metrics
@@ -73,10 +88,24 @@ def patch_allrank(patch_model=True, patch_eval=True, patch_data=False):
             ref_main.CustomDataParallel = single_process_model
         except Exception:
             pass
+    have_rac = _import_rank_and_click()
+    if patch_model and have_rac:           # rank_and_click.py:73,78-79: the same make_model / DataParallel bindings
+        _rebind(saved, "rank_and_click", "make_model", _model.make_model)
+        _rebind(saved, "rank_and_click", "CustomDataParallel", single_process_model)
     if patch_eval:
         _rebind(saved, "train_utils", "metric_on_epoch", _training.metric_on_epoch)
         _rebind(saved, "train_utils", "compute_metrics", _training.compute_metrics)
         _rebind(saved, "inference_utils", "rank_slates", _inference.rank_slates)
+        # inference_utils bound the metrics at import (`from allrank.models.metrics import ndcg, dcg`); its
+        # metrics_on_clicked_slates would call the CUDA metrics with host tensors
+        _rebind(saved, "inference_utils", "metrics_on_clicked_slates", _inference.metrics_on_clicked_slates)
+        if have_rac:
+            _rebind(saved, "rank_and_click", "rank_slates", _inference.rank_slates)
+            _rebind(saved, "rank_and_click", "metrics_on_clicked_slates", _inference.metrics_on_clicked_slates)
+    if patch_clicks:
+        _rebind(saved, "click_utils", "click_on_slates", _click_models.click_on_slates)
+        if have_rac:
+            _rebind(saved, "rank_and_click", "click_on_slates", _click_models.click_on_slates)
     if patch_data:
         for name in ("load_libsvm_dataset", "load_libsvm_dataset_role", "load_libsvm_role", "create_data_loaders"):
             _rebind(saved, "dataset_loading", name, getattr(_data, name))

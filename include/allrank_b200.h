@@ -341,6 +341,65 @@ int32_t arb_assemble_slates(const float* docs_x, const float* docs_y, const int6
 int32_t arb_gather_slates(const float* x, const float* y, const int32_t* order, int32_t B, int32_t S, int32_t F,
                           float* x_out, float* y_out, void* stream);
 
+/* ---------------------------------------------------------------- click models (allrank/click_models)
+ * A click model is a tree of at most ARB_CLICK_MAX_NODES nodes.  Node 0 is the root; the children of a node are the
+ * contiguous nodes [first_child, first_child + n_children), each with a larger index than its parent, and every
+ * non-root node has exactly one parent.  Every model sees the REAL items of a slate (y != pad) in slate order, like
+ * MaskedRemainMasked (click_utils.py:30-53); n is their number and "position" is the index among them.
+ *   FIXED       click the positions list[list_offset .. +n_list] (integers stored as doubles; negative = from the end);
+ *               a position outside [-n, n) sets status ARB_CLICK_INDEX_ERROR
+ *   RANDOM      exactly iparam distinct items, uniformly (the iparam smallest per-item hash keys); iparam > n sets
+ *               status ARB_CLICK_VALUE_ERROR
+ *   RELEVANT    click iff y >= fparam0 (compared in fp32)
+ *   CASCADE     observed iff observe_tables[iparam * S + p] >= u (u a per-item uniform); click iff
+ *               (observed ? y : 0*y) >= fparam1 (fp32).  The table holds 1 / (p+1)**eta, evaluated by the caller.
+ *   MULTIPLE    evaluate only child argmax(u < list[list_offset + k]) (cumulative probabilities, n_list = n_children;
+ *               child 0 when none holds), u one uniform per slate
+ *   CONDITIONED iparam 0: all children click, 1: any child clicks
+ *   MAXCLICKS   the child's clicks whose running count is <= fparam0 (+inf passes everything)
+ *   DUPLICATES  item j clicks iff min_{i<j} dist(i, j) > fparam0, metric iparam (ARB_CLICK_METRIC_*); n = 0 sets status
+ *               ARB_CLICK_VALUE_ERROR
+ *   DIVERSE     margin = linear quantile fparam0 of all pairwise euclidean distances (0 when n < 2); the child's clicks
+ *               are walked top to bottom and kept iff their distance to every kept item is > margin
+ * Distances are computed in fp64 from the fp32 features, summed over the features in order without FMA (scipy's cdist).
+ * Uniforms are counter-based: 53 bits of a hash of (seed, node, slate_offset + slate, position). */
+#define ARB_CLICK_MAX_NODES 32
+#define ARB_CLICK_MAX_SLATE 4096
+#define ARB_CLICK_FIXED 0
+#define ARB_CLICK_RANDOM 1
+#define ARB_CLICK_RELEVANT 2
+#define ARB_CLICK_CASCADE 3
+#define ARB_CLICK_MULTIPLE 4
+#define ARB_CLICK_CONDITIONED 5
+#define ARB_CLICK_MAXCLICKS 6
+#define ARB_CLICK_DUPLICATES 7
+#define ARB_CLICK_DIVERSE 8
+#define ARB_CLICK_METRIC_EUCLIDEAN 0
+#define ARB_CLICK_METRIC_SQEUCLIDEAN 1
+#define ARB_CLICK_METRIC_CITYBLOCK 2
+#define ARB_CLICK_METRIC_CHEBYSHEV 3
+/* per-slate status codes */
+#define ARB_CLICK_OK 0
+#define ARB_CLICK_INDEX_ERROR 1
+#define ARB_CLICK_VALUE_ERROR 2
+
+typedef struct arb_click_node {
+  int32_t kind, first_child, n_children, iparam, list_offset, n_list;
+  double fparam0, fparam1;
+} arb_click_node;
+
+/* Device workspace bytes for processing all B slates in one launch: one fp64 upper triangle of pairwise distances
+ * per slate when the tree has a DIVERSE node, 0 otherwise (the tree itself travels with the launch).  A smaller
+ * workspace is processed in chunks of slates; it must hold at least one slate's triangle. */
+size_t arb_click_workspace_bytes(const arb_click_node* nodes_host, int32_t n_nodes, int32_t B, int32_t S, int32_t F);
+/* y [B,S] fp32 (pad marks padding), x [B,S,F] fp32 (may be NULL when no node measures distances), observe_tables
+ * device fp64 [n_tables, S] for CASCADE nodes (may be NULL without them).  Writes clicks [B,S] fp32 (0/1, pad value
+ * `pad` at padded positions) and status [B] int32 (ARB_CLICK_*).  Never synchronises. */
+int32_t arb_click_slates(const arb_click_node* nodes_host, int32_t n_nodes, const double* list_host, int32_t n_list,
+                         const double* observe_tables, const float* x, const float* y, int32_t B, int32_t S, int32_t F,
+                         float pad, int64_t slate_offset, uint64_t seed, float* clicks, int32_t* status,
+                         void* workspace, size_t ws_bytes, void* stream);
+
 /* Per-launch device timing for bench.py's roofline: enable, run steps, collect per kernel class
  * (0 = tensor-core GEMM [work = flops], 1 = scorer SIMT, 2 = losses, 3 = metrics, 4 = optimiser, 5 = slate assembly /
  * gather [work = bytes]). */
