@@ -1,8 +1,11 @@
 // Batched TF32 GEMM on the Hopper tensor cores:  C[M,N] = epilogue(alpha * A * B^T)
 //
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a STAGES-deep shared-memory ring,
-//   * four consumer warps, each owning 32 rows of the 128-row tile, run warp-level mma.sync (m16n8k8 tf32 / m16n8k16
-//     bf16) straight out of the swizzled ring and keep the fp32 accumulator in registers,
+//   * fp32 operands that are both K-major (every forward and input-gradient linear) run on warpgroup MMA: the four
+//     consumer warps issue wgmma m64nNk8 with A in registers (ldmatrix, rounded to nearest tf32) and B read by the
+//     tensor core straight from the swizzled ring; every other operand pair (MN-major, bf16) runs warp-level mma.sync
+//     (m16n8k8 tf32 / m16n8k16 bf16), each warp owning 32 rows of the 128-row tile.  The fp32 accumulator stays in
+//     registers either way,
 //   * the epilogue turns each 32-column chunk of a warp's accumulator into one row per thread (through a small
 //     per-warp transpose buffer), applies bias / ReLU / residual / ReLU-mask, stages the tile in swizzled shared
 //     memory and writes it with one TMA store per 32-column slab (TMA clips ragged edges, so a 240-row slate or a
@@ -13,8 +16,8 @@
 //   * split-K for the weight gradients (K = all rows of the batch): every split stores its tile into a slot of its own
 //     and the slots are summed in split order (DetParts), so results do not depend on the order splits finish in.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = idle, warps 2-5 = MMA + epilogue (warp w owns rows
-// 32*(w%4) .. +31 of the tile).
+// Warp roles (192 threads): warps 0-3 = MMA + epilogue (one aligned warpgroup, as wgmma needs), warp 4 = TMA producer,
+// warp 5 = idle.
 //
 // This one kernel is the tensor-core workhorse of the scorer: every nn.Linear forward/backward and the
 // generic (unfused) attention contractions go through it.  Reference ops replaced: aten::addmm / aten::bmm
@@ -50,6 +53,7 @@ struct GemmParams {
   int flags;
   int kb_per_split;   // k-blocks per split (split-K), or total k-blocks
   int rnd;            // round fp32 operands to tf32 (nearest) before the MMA; else the tensor core truncates them
+  int rnd_b;          // wgmma path: round the B stages in place (rnd, unless B arrives rounded already)
   float alpha;
   const float* bias;
   float* atomic_out;     // split-K: the splits' slots [split][M][atomic_ld] (DetParts), summed in order afterwards
@@ -114,8 +118,72 @@ __device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], const ui
   }
 }
 
-// The 32 accumulator values of chunk `c` (n-tiles 4c .. 4c+3) of row (row0 + lane) of the warp, one row per thread:
-// the fragments go through the warp's transpose buffer `xp`.
+// fp32 operands with both A and B K-major run on warpgroup MMA (wgmma) instead: the consumer warps form one warpgroup
+// per 128 x WG_N(BLOCK_N) block of the output.  Both kernels issue the same instruction shapes in the same k order, so the
+// one-tile and the persistent kernel give bit-identical results.
+template <int A_MN, int B_MN, bool IN16>
+constexpr bool use_wgmma() { return A_MN == 0 && B_MN == 0 && !IN16; }
+template <int BLOCK_N>
+constexpr int wg_cols() { return BLOCK_N == 128 ? 64 : 32; }
+
+// acc[mt][nt] += rows 64 mt + 16 w .. +15 of A (w: the warp's rank in its warpgroup)  x  columns col0 + 8 nt .. +7 of
+// B over one k-block of the ring, issued by the calling warp's whole warpgroup (128 threads, named barrier `bar`).
+// The A fragments are the m16n8k8 ones (ldmatrix + round to nearest in registers); with rnd_b, the warpgroup first
+// rounds its B rows in place (wgmma reads B from shared memory and would truncate it).  Returns with the MMAs of this
+// k-block complete, so the caller may release the stage.
+template <int NT, int WN>
+__device__ __forceinline__ void wg_mma_kblock(float (&acc)[2][NT][4], const uint8_t* a_s, uint8_t* b_s, int col0,
+                                              int rnd, int rnd_b, int bar) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3, j = lane >> 3;
+  if (rnd_b) {
+    float4* b4 = reinterpret_cast<float4*>(b_s + col0 * 128);
+#pragma unroll
+    for (int i = threadIdx.x & 127; i < NT * 8 * 8; i += 128) {
+      float4 v = b4[i];
+      v.x = __uint_as_float(ptx::cvt_tf32(v.x)); v.y = __uint_as_float(ptx::cvt_tf32(v.y));
+      v.z = __uint_as_float(ptx::cvt_tf32(v.z)); v.w = __uint_as_float(ptx::cvt_tf32(v.w));
+      b4[i] = v;
+    }
+    ptx::fence_proxy_async_smem();
+    ptx::named_bar_sync(bar, 128);
+  }
+  uint32_t a[4][2][4];
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      // lanes 8j .. 8j+7 address block j: rows +8 (j & 1), k +4 (j >> 1) of the 16 x 8 fragment
+      ptx::ldmatrix_x4(a[ks][mt], a_s + ptx::sw128(64 * mt + 16 * w + 8 * (j & 1) + (lane & 7), 32 * ks + 16 * (j >> 1)));
+      if (rnd) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) a[ks][mt][e] = ptx::cvt_tf32(__uint_as_float(a[ks][mt][e]));
+      }
+    }
+  const uint64_t desc = ptx::wgmma_desc_sw128(b_s + col0 * 128);
+  ptx::wgmma_fence_acc(acc[0]);
+  ptx::wgmma_fence_acc(acc[1]);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      const uint64_t d = desc + 2 * ks;                     // +32 bytes (8 tf32) per k8 step
+      if constexpr (WN == 64) {
+        ptx::wgmma_m64n64k8_tf32<0>(acc[mt], a[ks][mt], d);
+        if constexpr (NT == 16) ptx::wgmma_m64n64k8_tf32<8>(acc[mt], a[ks][mt], d + 64 * 128 / 16);
+      } else {
+        ptx::wgmma_m64n32k8_tf32<0>(acc[mt], a[ks][mt], d);
+        if constexpr (NT == 8) ptx::wgmma_m64n32k8_tf32<4>(acc[mt], a[ks][mt], d + 32 * 128 / 16);
+      }
+    }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait0();
+  ptx::wgmma_fence_acc(acc[0]);
+  ptx::wgmma_fence_acc(acc[1]);
+}
+
+// The 32 accumulator values of chunk `c` (n-tiles 4c .. 4c+3) of the warp's accumulator row `lane` (fragment row
+// 16 mt + g), one row per thread: the fragments go through the warp's transpose buffer `xp`.
 template <int NT>
 __device__ __forceinline__ void acc_chunk_row(const float (&acc)[2][NT][4], int c, float* xp, uint32_t (&v)[32]) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -230,7 +298,8 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
   constexpr int STAGES = L::stages();
   constexpr int N_SLABS = BLOCK_N / 32;                       // 32-column accumulator chunks
   constexpr int NT = BLOCK_N / 8;                             // 8-column MMA tiles per warp
-  constexpr int N_CONSUMERS = GEMM_EPI_THREADS / 32;
+  constexpr int N_CONSUMERS = GEMM_EPI_THREADS / 32;          // warps 0 .. N_CONSUMERS-1; the next one is the producer
+  constexpr bool WG = use_wgmma<A_MN, B_MN, IN16>();
   constexpr int OUT_COLS = OUT16 ? 64 : 32;                   // output columns per 128-byte staging slab row
   constexpr int OUT_SLABS = (BLOCK_N + OUT_COLS - 1) / OUT_COLS;
   static_assert(!OUT16 || BLOCK_N >= 64, "bf16 outputs need at least one full 128-byte slab row");
@@ -278,7 +347,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
   arb_pdl_wait();          // everything above overlaps the previous kernel's tail; global memory is touched below
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp == N_CONSUMERS) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       for (int i = 0; i < nkb; ++i) {
@@ -311,13 +380,14 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
           ptx::tma_load_4d(staging + c * (BLOCK_M * 128), &tmAux, aux_bar, n0 + OUT_COLS * c, m0, b2 * p.c_b2, b3 * p.c_b3);
       }
     }
-  } else if (warp >= 2) {
-    // ===================== MMA + epilogue (warps 2..) =====================
-    const int q = warp & 3;                 // 32-row quarter of the tile this warp computes
-    const int row = 32 * q + lane;          // row of the tile owned by this thread in the epilogue
-    const int et = threadIdx.x - 64;        // 0..GEMM_EPI_THREADS-1
-    const int grp = (warp - 2) >> 2;        // which chunks: grp, grp + GEMM_EPI_GROUPS, ...
-    float* xp = reinterpret_cast<float*>(tail + L::XPOSE_OFF) + (warp - 2) * (XPOSE_BYTES / 4);
+  } else if (warp < N_CONSUMERS) {
+    // ===================== MMA + epilogue (warps 0..N_CONSUMERS-1) =====================
+    const int q = warp & 3;                 // mma.sync: 32-row quarter of the tile; wgmma: rank in the warpgroup
+    // row of the tile owned by this thread in the epilogue (wgmma: the warp computes rows 16q.. and 64+16q.., 16 each)
+    const int row = WG ? 64 * (lane >> 4) + 16 * q + (lane & 15) : 32 * q + lane;
+    const int et = threadIdx.x;             // 0..GEMM_EPI_THREADS-1
+    const int grp = warp >> 2;              // which chunks: grp, grp + GEMM_EPI_GROUPS, ...
+    float* xp = reinterpret_cast<float*>(tail + L::XPOSE_OFF) + warp * (XPOSE_BYTES / 4);
     if (p.flags & EPI_BIAS) {
       for (int j = et; j < BLOCK_N; j += GEMM_EPI_THREADS) bias_s[j] = (n0 + j < p.N) ? p.bias[n0 + j] : 0.0f;
     }
@@ -336,8 +406,9 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
     for (int i = 0; i < nkb; ++i) {
       const int s = i % STAGES, round = i / STAGES;
       ptx::mbar_wait(&full_bar[s], round & 1);
-      const uint8_t* a_s = smem + s * L::STAGE_BYTES;
-      warp_mma_kblock<NT, A_MN, B_MN, IN16>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, 0, 1, p.rnd);
+      uint8_t* a_s = smem + s * L::STAGE_BYTES;
+      if constexpr (WG) wg_mma_kblock<NT, wg_cols<BLOCK_N>()>(acc, a_s, a_s + A_STAGE_BYTES, 0, p.rnd, p.rnd_b, 1);
+      else warp_mma_kblock<NT, A_MN, B_MN, IN16>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, 0, 1, p.rnd);
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);      // this warp is done with the stage
     }
@@ -509,6 +580,9 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
   constexpr int NGA = N_SLABS < EPI_GROUPS ? N_SLABS : EPI_GROUPS;   // active consumer groups
   constexpr int SLABS_PER_GROUP = N_SLABS / NGA;
   constexpr int NT = 4 * SLABS_PER_GROUP;                            // 8-column MMA tiles per warp
+  constexpr bool WG = use_wgmma<A_MN, B_MN, false>();
+  static_assert(!WG || 32 * SLABS_PER_GROUP == wg_cols<BLOCK_N>(), "a group's columns are one wgmma instruction wide");
+  constexpr int PRODUCER_WARP = EPI_THREADS / 32;                   // after the consumer warps (whole warpgroups)
 
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
@@ -559,7 +633,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
     }
   };
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t it = 0;          // running k-block counter across tiles (ring position)
@@ -601,18 +675,18 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
         }
       }
     }
-  } else if (warp >= 2) {
-    // ===================== MMA + epilogue (warps 2..9) =====================
-    // NGA = min(EPI_GROUPS, slabs) groups of four warps are active, group g owning the 32-column slabs g, g + NGA, ...
-    // of the tile (each warp: 32 rows of them).  A group turns a slab registers -> swizzled staging and its leader
+  } else if (warp < PRODUCER_WARP) {
+    // ===================== MMA + epilogue (warps 0..7) =====================
+    // NGA = min(EPI_GROUPS, slabs) groups of four warps (warpgroups) are active, group g owning the 32-column slabs
+    // g * SLABS_PER_GROUP .. +SLABS_PER_GROUP-1 of the tile (mma.sync: each warp 32 rows of them; wgmma: see row).  A group turns a slab registers -> swizzled staging and its leader
     // immediately issues that slab's TMA store; the staging slab is reclaimed lazily (cp.async.bulk.wait_group.read)
     // right before the group writes it again one tile later.  No barrier spans more than the 128 threads of a group.
     const int q = warp & 3;
-    const int row = 32 * q + lane;
-    const int grp = (warp - 2) >> 2;                    // 0 .. EPI_GROUPS-1
-    const int gt = threadIdx.x - 64 - 128 * grp;        // 0..127 inside the group
+    const int row = WG ? 64 * (lane >> 4) + 16 * q + (lane & 15) : 32 * q + lane;   // as in gemm_tf32_kernel
+    const int grp = warp >> 2;                          // 0 .. EPI_GROUPS-1
+    const int gt = threadIdx.x - 128 * grp;             // 0..127 inside the group
     const bool leader = gt == 0;
-    float* xp = reinterpret_cast<float*>(smem + L::XPOSE_OFF) + (warp - 2) * (XPOSE_BYTES / 4);
+    float* xp = reinterpret_cast<float*>(smem + L::XPOSE_OFF) + warp * (XPOSE_BYTES / 4);
     if (grp < NGA) {
       uint32_t it = 0;
       int local = 0;
@@ -624,7 +698,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
         ptx::named_bar_sync(1 + grp, 128);            // the group's previous epilogue is done with the bias row
         if (p.flags & EPI_BIAS) {                     // this group's columns only (ordered by the group barriers)
           for (int j = gt; j < 32 * SLABS_PER_GROUP; j += 128) {
-            const int col = 32 * (grp + NGA * (j >> 5)) + (j & 31);
+            const int col = 32 * (grp * SLABS_PER_GROUP + (j >> 5)) + (j & 31);
             bias_s[col] = (n0 + col < p.N) ? p.bias[n0 + col] : 0.0f;
           }
         }
@@ -633,7 +707,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
         if ((p.flags & EPI_MASK_BITS) && m0 + row < p.M) {
 #pragma unroll
           for (int ci = 0; ci < (SLABS_PER_GROUP < 2 ? SLABS_PER_GROUP : 2); ++ci) {
-            const int c = grp + NGA * ci;
+            const int c = grp * SLABS_PER_GROUP + ci;
             if (n0 + 32 * c < p.N) mword[ci] = p.bits[(long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c)];
           }
         }
@@ -646,15 +720,18 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
           const int s = it % STAGES;
           const uint32_t round = it / STAGES;
           ptx::mbar_wait(&full_bar[s], round & 1);
-          const uint8_t* a_s = smem + s * L::STAGE_BYTES;
-          warp_mma_kblock<NT, A_MN, B_MN, false>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, grp, NGA, p.rnd);
+          uint8_t* a_s = smem + s * L::STAGE_BYTES;
+          if constexpr (WG)
+            wg_mma_kblock<NT, wg_cols<BLOCK_N>()>(acc, a_s, a_s + A_STAGE_BYTES, 32 * SLABS_PER_GROUP * grp, p.rnd, p.rnd_b,
+                                                  1 + grp);
+          else warp_mma_kblock<NT, A_MN, B_MN, false>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, SLABS_PER_GROUP * grp, 1, p.rnd);
           __syncwarp();
           if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);
         }
         if (has_aux) ptx::mbar_wait(aux_full, local & 1);
 #pragma unroll 1
         for (int ci = 0; ci < SLABS_PER_GROUP; ++ci) {
-          const int c = grp + NGA * ci;
+          const int c = grp * SLABS_PER_GROUP + ci;
           // reclaim the slab: every store this leader committed except the most recent (SLABS_PER_GROUP - 1) ones has
           // been read out of shared memory -- in particular the one that used slab c a tile ago.  With an aux tile
           // the leader already drained its stores before the producer refilled the staging area.
@@ -804,7 +881,7 @@ int make_tmap_4d(void* out, const TRef& t, TmapBox box, int unswizzled) {
 
 // launch name for the per-kernel profile table: shape, operand layouts and what the epilogue does
 static void gemm_prof_name(char (&out)[56], const GemmDesc& d, const char* variant) {
-  const char* kind = (d.flags & EPI_ATOMIC) ? "wgrad" : (d.nb2 * d.nb3 > 1 ? "batched" : (d.b_mn ? "dgrad" : "fwd"));
+  const char* kind = (d.flags & EPI_ATOMIC) ? "wgrad" : (d.nb2 * d.nb3 > 1 ? "batched" : (d.b_mn || d.dgrad ? "dgrad" : "fwd"));
   std::snprintf(out, sizeof out, "gemm_%s%s[%s M%d N%d K%d%s%s%s]", variant, d.A.bf16 ? (d.C.bf16 ? "_bf16o" : "_bf16") : "",
                 kind, d.M, d.N, d.K, (d.flags & EPI_RELU) ? " relu" : "", (d.flags & EPI_ADD_AUX) ? " +res" : "",
                 (d.flags & EPI_MASK_AUX) ? " mask" : "");
@@ -949,6 +1026,7 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   p.rows_dev = d.rows_dev;
   p.bits = d.bits;
   p.rnd = g_round_on_load;
+  p.rnd_b = g_round_on_load && !d.b_tf32;
   if (d.flags & (EPI_RELU_BITS | EPI_MASK_BITS)) {
     if (!d.bits || d.N % 32 || out16 || split || d.nb2 != 1 || d.nb3 != 1 || (d.flags & (EPI_DROPOUT | EPI_ADD_AUX | EPI_MASK_AUX)) ||
         ((d.flags & EPI_RELU_BITS) && !(d.flags & EPI_RELU))) {

@@ -32,6 +32,8 @@ enum : int {
 struct GemmDesc {
   int M = 0, N = 0, K = 0;      // C[M,N] = alpha * sum_k A[m,k] B[n,k]
   int a_mn = 0, b_mn = 0;       // 0: operand stored K-contiguous ("K-major"); 1: stored M/N-contiguous ("MN-major")
+  int b_tf32 = 0;               // fp32 B already holds tf32-rounded values (the scorer's weight copy): not rounded again
+  int dgrad = 0;                // an input-gradient product (label of the per-kernel profile only)
   TRef A, B, C, Aux;            // K-major operand: dim = (K, rows, b2, b3); MN-major: dim = (rows, K, b2, b3);
                                 // C/Aux: dim = (N, M, b2, b3)
   int nb2 = 1, nb3 = 1;         // batch grid: blockIdx.z = b3 * nb2 + b2

@@ -155,6 +155,8 @@ struct WsLayout {
   int64_t kext;                     // [B] ints: key extent of every slate (keys at or beyond it are all masked)
   int64_t xc, poff, plan, rowmap;   // packed rows: features of the packed rows, off [B+1], plan [2], rowmap [B*S] (ints)
   int64_t wb16;                     // bf16 mode: bfloat16 shadow of the whole parameter buffer (same element offsets)
+  int64_t wt32, wt32t;              // TF32 mode: the parameters rounded to tf32, and every weight matrix W [out,in]
+                                    // rounded and transposed to [in,out] (same element offsets; written by the forward)
   int64_t meanf, stdf, xf, total;   // xf: final-norm output, kept only for the multi-output head
   int Sp;
   bool fused;
@@ -190,6 +192,8 @@ static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int
   // bf16 mode: tensors that only feed products (LayerNorm outputs, context, FFN hidden) are bfloat16: half the floats
   const int64_t op = (c.bf16 && c.n_layers > 0) ? 2 : 1;
   W.wb16 = op == 2 ? take((L.total + 1) / 2) : 0;
+  W.wt32 = op == 1 ? take(L.total) : 0;
+  W.wt32t = op == 1 ? take(L.total) : 0;
   WsLayout::Layer shared{};
   for (int l = 0; l < c.n_layers; ++l) {
     auto& y = W.layer[l];
@@ -234,10 +238,12 @@ struct Ctx {
 struct V {
   const void* p;
   int bf16;
+  int tf32 = 0;    // a weight from the TF32 copy (WsLayout::wt32 / wt32t): already rounded
   V(const float* q = nullptr) : p(q), bf16(0) {}
   V(const void* q, int is16) : p(q), bf16(is16) {}
 };
 static inline V b16(const void* q) { return V(q, 1); }
+static inline V t32(const float* q) { V v(q); v.tf32 = 1; return v; }
 
 static TRef rows_view(V v, int64_t inner, int64_t rows, int64_t pitch) {
   TRef t; t.ptr = v.p; t.bf16 = v.bf16; t.dim[0] = inner; t.dim[1] = rows; t.stride[0] = 1; t.stride[1] = pitch; return t;
@@ -254,6 +260,7 @@ static int linear_fwd(const Ctx& k, V X, int64_t x_pitch, int in, V Wt, const fl
   if (drop.thresh != 0) flags |= EPI_DROPOUT;
   g.A = rows_view(X, in, k.R, x_pitch);
   g.B = rows_view(Wt, in, out, in);
+  g.b_tf32 = Wt.tf32;
   g.C = rows_view(Y, out, k.R, y_pitch);
   if (aux.p) g.Aux = rows_view(aux, out, k.R, aux_pitch);
   g.bias = bias; g.flags = flags | (bias ? EPI_BIAS : 0);
@@ -263,7 +270,8 @@ static int linear_fwd(const Ctx& k, V X, int64_t x_pitch, int in, V Wt, const fl
   g.rows_dev = k.rows_dev;
   return launch_gemm_tf32(g, k.st);
 }
-// dX[R,in] = epi( dY[R,out] W[out,in] )      (W read as an MN-major B operand)
+// dX[R,in] = epi( dY[R,out] W[out,in] ): `Wt` is W^T [in,out] from the TF32 copy (a K-major B operand, Wt.tf32 set) or
+// else W itself, read as an MN-major B operand (bf16 mode)
 static int linear_bwd_input(const Ctx& k, V dY, int64_t dy_pitch, int out, V Wt, int in, V dX,
                             int64_t dx_pitch, int flags, V aux, int64_t aux_pitch, float alpha = 1.0f,
                             float* colsum_out = nullptr, const uint32_t* mask_bits = nullptr) {
@@ -271,9 +279,15 @@ static int linear_bwd_input(const Ctx& k, V dY, int64_t dy_pitch, int out, V Wt,
   g.alpha = alpha;
   g.colsum_out = colsum_out;
   if (!colsum_out) flags &= ~EPI_COLSUM;     // (no parameter gradients requested)
-  g.M = int(k.R); g.N = in; g.K = out; g.b_mn = 1;
+  g.M = int(k.R); g.N = in; g.K = out; g.dgrad = 1;
   g.A = rows_view(dY, out, k.R, dy_pitch);
-  g.B = rows_view(Wt, in, out, in);          // dim0 = in (N, contiguous), dim1 = out (K)
+  if (Wt.tf32) {
+    g.B = rows_view(Wt, out, in, out);       // dim0 = out (K, contiguous), dim1 = in (N)
+    g.b_tf32 = 1;
+  } else {
+    g.b_mn = 1;
+    g.B = rows_view(Wt, in, out, in);        // dim0 = in (N, contiguous), dim1 = out (K)
+  }
   g.C = rows_view(dX, in, k.R, dx_pitch);
   if (aux.p) g.Aux = rows_view(aux, in, k.R, aux_pitch);
   g.flags = flags;
@@ -320,6 +334,22 @@ static void batch_all(GemmDesc& g, int h, int B) {
   g.a_b2 = g.a_b3 = g.b_b2 = g.b_b3 = g.c_b2 = g.c_b3 = 1;
 }
 
+static WeightMats weight_mats(const arb_scorer_config& c, const ParamLayout& L) {
+  WeightMats m{};
+  m.n_fc = L.n_fc;
+  for (int i = 0; i < L.n_fc; ++i) {
+    m.fc_w[i] = L.fc_w[i]; m.fc_out[i] = L.fc_size[i]; m.fc_in[i] = i == 0 ? c.n_features : L.fc_size[i - 1];
+  }
+  m.n_layers = c.n_layers; m.d = c.d_model; m.f = c.d_ff;
+  if (c.n_layers > 0) {
+    const auto& y = L.layer[0];
+    m.enc0 = y.wqkv;
+    m.enc_stride = y.ln2_b + c.d_model - y.wqkv;     // the layers follow each other with the same layout
+    m.o_wo = y.wo - y.wqkv; m.o_w1 = y.w1 - y.wqkv; m.o_w2 = y.w2 - y.wqkv;
+  }
+  return m;
+}
+
 #define ARB_TRY(expr) do { int rc__ = (expr); if (rc__ != ARB_OK) return rc__; } while (0)
 
 // Exactly one of `scores` (the model's output) and `hidden` (the encoder's output, [B, S, d]; the head is not run) is
@@ -349,8 +379,13 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
       return ARB_E_UNSUPPORTED;
     }
     ARB_TRY(convert_to_bf16(P, Pb, L.total, st));      // refresh the GEMM-operand shadow of the master weights
+  } else {
+    // refresh the GEMM-operand copy of the master weights (rounded once here instead of in every GEMM; the transposed
+    // matrices make every input-gradient product K-major); the backward of this call reads it too
+    ARB_TRY(tf32_weight_copy(P, L.total, weight_mats(c, L), tf32_round_on_load(), ws + W.wt32, ws + W.wt32t, st));
   }
-  auto wt = [&](int64_t off) { return bf ? b16(Pb + off) : V(P + off); };
+  auto wt = [&](int64_t off) { return bf ? b16(Pb + off) : t32(ws + W.wt32 + off); };
+  auto wfc = [&](int64_t off) { return bf ? V(P + off) : t32(ws + W.wt32 + off); };   // FC weights stay fp32 in bf16 mode
   auto act = [&](float* q) { return bf ? b16(q) : V(q); };   // a product-only activation buffer of this mode
   float* xcur = ws + W.x0;
   int* kext = reinterpret_cast<int*>(ws + W.kext);
@@ -410,10 +445,10 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
       float* hout = last ? (W.fc_last ? ws + W.fc_last : xcur) : ws + W.fch[i];
       const DropSite site = make_drop_site(seed, i, SITE_FC, p_fc);
       if (c.fc_act == ARB_ACT_NONE || c.fc_act == ARB_ACT_RELU) {
-        ARB_TRY(linear_fwd(k, hin, in, in, P + L.fc_w[i], P + L.fc_b[i], out, hout, out,
+        ARB_TRY(linear_fwd(k, hin, in, in, wfc(L.fc_w[i]), P + L.fc_b[i], out, hout, out,
                            c.fc_act == ARB_ACT_RELU ? EPI_RELU : 0, nullptr, 0, site));
       } else {
-        ARB_TRY(linear_fwd(k, hin, in, in, P + L.fc_w[i], P + L.fc_b[i], out, hout, out, 0, nullptr, 0));
+        ARB_TRY(linear_fwd(k, hin, in, in, wfc(L.fc_w[i]), P + L.fc_b[i], out, hout, out, 0, nullptr, 0));
         ARB_TRY(act_forward(hout, k.R, out, c.fc_act, site, st, plan));
       }
       hin = hout; in = out;
@@ -599,7 +634,9 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   }
   const uint16_t* Pb = bf ? reinterpret_cast<const uint16_t*>(ws + W.wb16) : nullptr;
   void* dy16 = bf ? static_cast<void*>(scratch + Z.dy16) : nullptr;
-  auto wt = [&](int64_t off) { return bf ? b16(Pb + off) : V(P + off); };
+  // the weight operand of the input-gradient products: W^T from the forward's TF32 copy, or W's bf16 shadow
+  auto wt = [&](int64_t off) { return bf ? b16(Pb + off) : t32(ws + W.wt32t + off); };
+  auto wfc = [&](int64_t off) { return bf ? V(P + off) : t32(ws + W.wt32t + off); };
   auto act = [&](const float* q) { return bf ? b16(q) : V(q); };
   // site whose mask the gradient of the residual stream must pass through right below the head / final norm
   // The last FC layer's dropout mask (and its bias gradient) is folded into the kernel that emits the gradient of the
@@ -804,12 +841,12 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     if (i > 0) {
       const DropSite site = make_drop_site(seed, i - 1, SITE_FC, p_fc);
       if (c.fc_act == ARB_ACT_RELU) {        // h > 0 <=> ReLU active and kept by the dropout: mask tile + 1/(1-p)
-        ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, EPI_MASK_AUX | EPI_COLSUM, hin, in,
+        ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[i]), in, dfa, in, EPI_MASK_AUX | EPI_COLSUM, hin, in,
                                  site.scale, g(L.fc_b[i - 1])));
       } else if (c.fc_act == ARB_ACT_NONE && site.thresh == 0) {
-        ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, EPI_COLSUM, nullptr, 0, 1.0f, g(L.fc_b[i - 1])));
+        ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[i]), in, dfa, in, EPI_COLSUM, nullptr, 0, 1.0f, g(L.fc_b[i - 1])));
       } else {
-        ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[i], in, dfa, in, 0, nullptr, 0));
+        ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[i]), in, dfa, in, 0, nullptr, 0));
         ARB_TRY(act_backward(dfa, hin, dfa, k.R, in, c.fc_act, site, 1.0f, g(L.fc_b[i - 1]), st, plan));
       }
       dz = dfa; std::swap(dfa, dfb);
@@ -818,11 +855,11 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     // the first layer's input: d loss / d x goes to dX (dense rows) or to a packed buffer scattered into dX below
     float* const dxin = dX ? (pack ? scratch + Z.dxin : dX) : nullptr;
     if (c.fc_input_norm && (G || dX)) {      // the LayerNorm's backward emits d x (kept only when asked for)
-      ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[0], in, dfa, in, 0, nullptr, 0));
+      ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[0]), in, dfa, in, 0, nullptr, 0));
       ARB_TRY(ln_backward(dfa, x, P + L.in_a, ws + W.in_mean, ws + W.in_std, 0.0f, nullptr, k.R, F, dxin ? dxin : dfb,
                           g(L.in_a), g(L.in_b), st, nullptr, none_site, nullptr, 1, nullptr, nullptr, plan));
     } else if (dX) {                         // dX = dZ0 W0
-      ARB_TRY(linear_bwd_input(k, dz, out, out, P + L.fc_w[0], in, dxin, in, 0, nullptr, 0));
+      ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[0]), in, dxin, in, 0, nullptr, 0));
     }
   }
   if (dX && pack) {   // items beyond their slate's packed rows get 0, like their score

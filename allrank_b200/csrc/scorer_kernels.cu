@@ -441,6 +441,36 @@ __global__ void __launch_bounds__(256) to_bf16_kernel(const float4* __restrict__
   }
 }
 
+__global__ void __launch_bounds__(256) tf32_weight_copy_kernel(const float* __restrict__ P, long long n, WeightMats m,
+                                                              int rnd, float* __restrict__ pr, float* __restrict__ pt) {
+  arb_pdl_wait();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float v = P[i];
+    if (rnd) {
+      uint32_t r;
+      asm("cvt.rn.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+      v = __uint_as_float(r);
+    }
+    pr[i] = v;
+    long long o = -1;     // the matrix holding element i: offset, rows (out), columns (in)
+    int rows = 0, cols = 0;
+    for (int j = 0; j < m.n_fc; ++j)
+      if (i >= m.fc_w[j] && i < m.fc_w[j] + (long long)m.fc_out[j] * m.fc_in[j]) { o = m.fc_w[j]; rows = m.fc_out[j]; cols = m.fc_in[j]; }
+    if (o < 0 && m.n_layers > 0 && i >= m.enc0 && i < m.enc0 + m.n_layers * m.enc_stride) {
+      const long long base = m.enc0 + (i - m.enc0) / m.enc_stride * m.enc_stride, j = i - base;
+      const long long d = m.d, f = m.f;
+      if (j < 3 * d * d) { o = base; rows = int(3 * d); cols = int(d); }
+      else if (j >= m.o_wo && j < m.o_wo + d * d) { o = base + m.o_wo; rows = int(d); cols = int(d); }
+      else if (j >= m.o_w1 && j < m.o_w1 + f * d) { o = base + m.o_w1; rows = int(f); cols = int(d); }
+      else if (j >= m.o_w2 && j < m.o_w2 + d * f) { o = base + m.o_w2; rows = int(d); cols = int(f); }
+    }
+    if (o >= 0) {
+      const long long e = i - o, r = e / cols, c = e % cols;
+      pt[o + c * rows + r] = v;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ slate extents
 __global__ void __launch_bounds__(256) slate_extent_kernel(const uint8_t* __restrict__ mask,
                                                            const float* __restrict__ dscores, int n_out, int B, int S,
@@ -1737,6 +1767,12 @@ int convert_to_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
   ProfScope ps(ARB_PROF_SCORER_SIMT, 6.0 * double(n), st);
   return launch(to_bf16_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n4 + 255) / 256, 132 * 8)))), dim3(256), 0, st,
                 /*pdl=*/true, reinterpret_cast<const float4*>(src), static_cast<uint2*>(dst), n);
+}
+
+int tf32_weight_copy(const float* P, long long n, const WeightMats& m, int rnd, float* pr, float* pt, cudaStream_t st) {
+  ProfScope ps(ARB_PROF_SCORER_SIMT, 12.0 * double(n), st);
+  return launch(tf32_weight_copy_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 8)))),
+                dim3(256), 0, st, /*pdl=*/true, P, n, m, rnd, pr, pt);
 }
 
 int colsum_accumulate(const float* in, long long rows, int width, long long ld, float* out, cudaStream_t st) {

@@ -47,6 +47,19 @@ int softmax_backward(float* dp, float* prob, long long rows, int S, int pitch, c
 int slate_extents(const uint8_t* mask, const float* dscores, int n_out, int B, int S, int* extent, cudaStream_t st);
 // flat fp32 -> bfloat16 copy (the GEMM-operand shadow of the parameter buffer in bf16 mode); n multiple of 4
 int convert_to_bf16(const float* src, void* dst, long long n, cudaStream_t st);
+// The weight matrices inside the flat parameter buffer: FC layer i at fc_w[i] ([fc_out[i], fc_in[i]] row-major) and the
+// four of encoder layer l at enc0 + l * enc_stride + {0, o_wo, o_w1, o_w2} ([3d, d], [d, d], [f, d], [d, f]).
+struct WeightMats {
+  int n_fc;
+  long long fc_w[8];
+  int fc_out[8], fc_in[8];
+  int n_layers, d, f;
+  long long enc0, enc_stride, o_wo, o_w1, o_w2;
+};
+// The GEMM-operand copy of the parameter buffer in TF32 mode, one launch: pr[i] = P[i] and, for every weight matrix
+// W [out, in] at offset o, pt[o + c * out + r] = W[r][c] (W^T, the K-major B operand of the input gradient); values
+// rounded to tf32 (nearest even) when rnd != 0, else copied as they are (the tensor core then truncates them).
+int tf32_weight_copy(const float* P, long long n, const WeightMats& m, int rnd, float* pr, float* pt, cudaStream_t st);
 int colsum_accumulate(const float* in, long long rows, int width, long long ld, float* out, cudaStream_t st);
 int head_forward(const float* x, const float* a, const float* b, float eps, const float* w, const float* wb,
                  int has_norm, int act, long long rows, int width, float* score, float* mean, float* sd,

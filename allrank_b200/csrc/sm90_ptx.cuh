@@ -119,6 +119,59 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
+// Four 8x4 fp32 blocks from shared memory (ldmatrix of 8x8 b16 matrices): lanes 8j..8j+7 give the 16-byte row
+// addresses of block j; lane (g = lane / 4, t = lane % 4) receives element (g, t) of every block.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* row_addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(smem_u32(row_addr)));
+}
+
+// ------------------------------------------------------------------ warpgroup MMA (wgmma)
+// Shared-memory matrix descriptor of a K-major operand tile written by TMA with SWIZZLE_128B: rows of 128 bytes, 8-row
+// swizzle atoms 1024 bytes apart (stride byte offset), the tile 1024-byte aligned.  A k-step inside the 128-byte row
+// advances the start address by its byte offset (the hardware applies the swizzle to the final address).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(const void* tile) {
+  const uint64_t addr = smem_u32(tile);
+  return ((addr & 0x3FFFFull) >> 4) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Keeps the compiler from moving accumulator accesses across the asynchronous MMA (no code emitted).
+template <int NT>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[NT][4]) {
+#pragma unroll
+  for (int j = 0; j < NT; ++j) asm volatile("" : "+f"(d[j][0]), "+f"(d[j][1]), "+f"(d[j][2]), "+f"(d[j][3])::"memory");
+}
+
+// D[64 x WN] += A[64 x 8] B[WN x 8]^T, tf32 operands, fp32 accumulation, issued by a whole warpgroup.  A comes from
+// registers: warp w of the warpgroup holds rows 16w .. 16w+15 in the m16n8k8 A fragment layout above.  B is a K-major
+// tile in shared memory (descriptor).  The accumulator of 8-column block j lives in d[J0 + j] in the m16n8k8 D layout.
+#define ARB_D4(j) "+f"(d[J0 + j][0]), "+f"(d[J0 + j][1]), "+f"(d[J0 + j][2]), "+f"(d[J0 + j][3])
+template <int J0, int NT>
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[NT][4], const uint32_t (&a)[4], uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : ARB_D4(0), ARB_D4(1), ARB_D4(2), ARB_D4(3)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+template <int J0, int NT>
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[NT][4], const uint32_t (&a)[4], uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : ARB_D4(0), ARB_D4(1), ARB_D4(2), ARB_D4(3), ARB_D4(4), ARB_D4(5), ARB_D4(6), ARB_D4(7)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+#undef ARB_D4
+
 // An accumulator fragment {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]} of an 8-column block, reused as the tf32
 // A fragment of the next product (contraction over those 8 columns): lane t needs columns t and t + 4 of its rows.
 __device__ __forceinline__ void acc_to_a_tf32(const float (&c)[4], uint32_t (&a)[4], int lane) {
