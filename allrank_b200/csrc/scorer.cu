@@ -465,17 +465,15 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     ARB_TRY(pos_forward(xcur, reinterpret_cast<const long long*>(indices), mask, table, c.pe_rows, sqrtf(float(d)), k.R, d, st));
   }
   if (pack) {
-    // The attention kernels' 128-row boxes overrun the last slates: 256 finite rows behind the packed rows of every
-    // layer's Q|K|V; and the context of the alignment rows (no slate writes them) feeds the output projection: zero.
-    // Nothing else writes those rows, so one launch serves all layers (eval mode: the layers share one buffer set).
+    // The context of the alignment rows (no slate writes them) feeds the output projection: zero.  Nothing else
+    // writes those rows, so one launch serves all layers (eval mode: the layers share one buffer set).
     ZeroRegions z;
     for (int l = 0; l < c.n_layers; ++l) {
       if (l > 0 && !training) break;
       const auto& wl = W.layer[l];
-      if (!z.add(ws + wl.qkv, 3 * d, 3 * d, 0, 256) || !z.add(ws + wl.ctx, bf ? d / 2 : d, bf ? d / 2 : d, 1, 0)) {
+      if (!z.add(ws + wl.ctx, bf ? d / 2 : d, bf ? d / 2 : d, 1, 0)) {
         ARB_TRY(zero_rows(z, plan, k.R, st));
         z = ZeroRegions{};
-        z.add(ws + wl.qkv, 3 * d, 3 * d, 0, 256);
         z.add(ws + wl.ctx, bf ? d / 2 : d, bf ? d / 2 : d, 1, 0);
       }
     }

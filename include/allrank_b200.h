@@ -254,9 +254,10 @@ int32_t arb_scorer_backward_ex(const arb_scorer_config* cfg, const float* params
  * head width <= 32); other shapes use the unfused path automatically.  Process-wide; exists for A/B tests. */
 void arb_set_attention_mode(int32_t mode);
 
-/* 1 (default): the fused attention kernels skip the 128-item tiles that lie entirely inside a slate's padding -- keys
- * beyond the last real item have probability exactly 0 and rows beyond the last item that is real or carries a score
- * gradient have exactly zero activation gradients, so results are unchanged; 0: dense tiles.  For A/B measurements. */
+/* 1 (default): the fused attention kernels stop at each slate's extent -- the 16-row strips of keys (and, where their
+ * gradients are exactly zero, of query rows) beyond round_up(last real item + 1, 16) are skipped: keys beyond the last
+ * real item have probability exactly 0 and rows beyond the last item that is real or carries a score gradient have
+ * exactly zero activation gradients, so results are unchanged; 0: all keys and all queries.  For A/B measurements. */
 void arb_set_attention_skip_padding(int32_t on);
 
 /* Packed rows (padding removal).  1: the encoder -- every LayerNorm, linear, attention and head kernel and every
