@@ -3,16 +3,18 @@
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a STAGES-deep shared-memory ring,
 //   * fp32 operands that are both K-major (every forward and input-gradient linear) run on warpgroup MMA: the four
 //     consumer warps issue wgmma m64nNk8 with A in registers (ldmatrix, rounded to nearest tf32) and B read by the
-//     tensor core straight from the swizzled ring; every other operand pair (MN-major, bf16) runs warp-level mma.sync
-//     (m16n8k8 tf32 / m16n8k16 bf16), each warp owning 32 rows of the 128-row tile.  The fp32 accumulator stays in
-//     registers either way,
+//     tensor core straight from the swizzled ring.  fp32 operands that are both MN-major (the split-K weight
+//     gradients) run on wgmma as well, with both operands read from shared memory: the warpgroup rewrites each ring
+//     stage K-major (and rounded) into one of two on-chip stages, and the MMAs of one stage run while it rewrites the
+//     next.  The mixed fp32 pairs and bf16 run warp-level mma.sync (m16n8k8 tf32 / m16n8k16 bf16), each warp owning 32
+//     rows of the 128-row tile.  The fp32 accumulator stays in registers either way,
 //   * the epilogue turns each 32-column chunk of a warp's accumulator into one row per thread (through a small
 //     per-warp transpose buffer), applies bias / ReLU / residual / ReLU-mask, stages the tile in swizzled shared
 //     memory and writes it with one TMA store per 32-column slab (TMA clips ragged edges, so a 240-row slate or a
 //     136-wide feature matrix needs no masking code),
 //   * either operand may be "K-major" (rows of K contiguous, e.g. nn.Linear weights [out,in]) or "MN-major"
-//     (the transpose), which is what the backward GEMMs dX = dY W and dW = dY^T X need; the fragment loads address
-//     either layout directly, so no transposition pass is needed,
+//     (the transpose), which is what the backward GEMMs dX = dY W and dW = dY^T X need; the mma.sync fragment loads
+//     address either layout directly,
 //   * split-K for the weight gradients (K = all rows of the batch): every split stores its tile into a slot of its own
 //     and the slots are summed in split order (DetParts), so results do not depend on the order splits finish in.
 //
@@ -120,9 +122,13 @@ __device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], const ui
 
 // fp32 operands with both A and B K-major run on warpgroup MMA (wgmma) instead: the consumer warps form one warpgroup
 // per 128 x WG_N(BLOCK_N) block of the output.  Both kernels issue the same instruction shapes in the same k order, so the
-// one-tile and the persistent kernel give bit-identical results.
+// one-tile and the persistent kernel give bit-identical results.  fp32 operands that are both MN-major (the split-K
+// weight gradients, some batched attention products) run on wgmma too, in the one-tile kernel only: the warpgroup
+// first rewrites each ring stage K-major (wg_kmajor_stage).
 template <int A_MN, int B_MN, bool IN16>
-constexpr bool use_wgmma() { return A_MN == 0 && B_MN == 0 && !IN16; }
+constexpr bool use_wgmma() { return A_MN == B_MN && !IN16; }
+template <int A_MN, int B_MN, bool IN16>
+constexpr bool wgmma_transposed() { return A_MN == 1 && B_MN == 1 && !IN16; }
 template <int BLOCK_N>
 constexpr int wg_cols() { return BLOCK_N == 128 ? 64 : 32; }
 
@@ -180,6 +186,78 @@ __device__ __forceinline__ void wg_mma_kblock(float (&acc)[2][NT][4], const uint
   ptx::wgmma_wait0();
   ptx::wgmma_fence_acc(acc[0]);
   ptx::wgmma_fence_acc(acc[1]);
+}
+
+// Both operands MN-major: tf32 wgmma reads only K-major tiles from shared memory, so the warpgroup (128 threads)
+// rewrites a ring stage K-major into `kt`, rounded to nearest tf32 on the way when `rnd` (else the tensor core
+// truncates).  The stage is NSLAB slabs (4 of A, then those of B) of 32 k-rows x 128 bytes, element (k, m) of a slab at
+// sw128(k, 4 m).  In `kt` slab sl becomes rows 32 sl .. 32 sl + 31 of 128 bytes, element (m, k) at sw128(m, 4 k) of the
+// slab's 4 KB: the A tile (rows 0..127) and then the B tile, both in the layout TMA gives K-major operands.
+//
+// A thread moves 4 x 4 blocks: k-rows 4 kc .. 4 kc + 3 of 16-byte chunk c (MN-elements 4 c .. 4 c + 3) come in as four
+// 16-byte loads, and the rows m = 4 c .. 4 c + 3 of 16-byte chunk kc go out as four 16-byte stores.  Bank conflicts: a
+// warp's 16-byte access is served 8 lanes (128 bytes) at a time, conflict-free when those 8 lanes touch the 8 distinct
+// 16-byte bank groups of a 128-byte row.  Lane l (0..7) of each 8-lane group takes kc = l and c = l ^ d, d being the
+// group's diagonal of the slab's 8 x 8 blocks.  Load j (k = 4 l + j) hits bank group c ^ (k & 7) = P(l) ^ d ^ j, store j
+// (m = 4 c + j) hits kc ^ (m & 7) = P(l) ^ 4 (d & 1) ^ j, with P(l) = l ^ 4 (l & 1) a permutation of 0..7: 8 distinct
+// groups either way.  The 16 groups of a warpgroup walk the 8 NSLAB (slab, diagonal) pairs.
+template <int NSLAB>
+__device__ __forceinline__ void wg_kmajor_stage(const uint8_t* ring, uint8_t* kt, int rnd) {
+  constexpr int TASKS = 8 * NSLAB, PER = (TASKS + 15) / 16;
+  const int l = threadIdx.x & 7, grp = (threadIdx.x & 127) >> 3;
+  const uint32_t src0 = ptx::smem_u32(ring), dst0 = ptx::smem_u32(kt);
+  float v[PER][4][4];                       // [task][k][m]
+#pragma unroll
+  for (int u = 0; u < PER; ++u) {
+    const int task = grp + 16 * u;
+    if (TASKS % 16 != 0 && task >= TASKS) continue;
+    const uint32_t src = src0 + (task >> 3) * 4096;
+    const int c = l ^ (task & 7);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = 4 * l + j;
+      const float4 x = ptx::lds128(src + k * 128 + ((c ^ (k & 7)) << 4));
+      v[u][j][0] = x.x; v[u][j][1] = x.y; v[u][j][2] = x.z; v[u][j][3] = x.w;
+    }
+  }
+#pragma unroll
+  for (int u = 0; u < PER; ++u) {
+    const int task = grp + 16 * u;
+    if (TASKS % 16 != 0 && task >= TASKS) continue;
+    const uint32_t dst = dst0 + (task >> 3) * 4096;
+    const int c = l ^ (task & 7);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int m = 4 * c + j;
+      float o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[e] = rnd ? __uint_as_float(ptx::cvt_tf32(v[u][e][j])) : v[u][e][j];
+      ptx::sts128(dst + m * 128 + ((l ^ (m & 7)) << 4), make_float4(o[0], o[1], o[2], o[3]));
+    }
+  }
+}
+
+// acc += the K-major stage `kt` written by wg_kmajor_stage (A: rows 0..127, B: the BLOCK_N rows after them), both
+// operands read by the tensor core from shared memory; same instruction shapes, accumulator layout and k8 order as
+// wg_mma_kblock.  Issued and committed, not waited for.
+template <int NT, int WN>
+__device__ __forceinline__ void wg_mma_kmajor(float (&acc)[2][NT][4], const uint8_t* kt) {
+  const uint64_t da = ptx::wgmma_desc_sw128(kt), db = ptx::wgmma_desc_sw128(kt + A_STAGE_BYTES);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      const uint64_t a = da + mt * (64 * 128 / 16) + 2 * ks, b = db + 2 * ks;
+      if constexpr (WN == 64) {
+        ptx::wgmma_m64n64k8_tf32_ss<0>(acc[mt], a, b);
+        if constexpr (NT == 16) ptx::wgmma_m64n64k8_tf32_ss<8>(acc[mt], a, b + 64 * 128 / 16);
+      } else {
+        ptx::wgmma_m64n32k8_tf32_ss<0>(acc[mt], a, b);
+        if constexpr (NT == 8) ptx::wgmma_m64n32k8_tf32_ss<4>(acc[mt], a, b + 32 * 128 / 16);
+      }
+    }
+  ptx::wgmma_commit();
 }
 
 // The 32 accumulator values of chunk `c` (n-tiles 4c .. 4c+3) of the warp's accumulator row `lane` (fragment row
@@ -272,7 +350,7 @@ __device__ __forceinline__ bool epi_chunk_dispatch(int flags, const uint32_t (&v
   }
 }
 
-template <int BLOCK_N, int NST = 2>
+template <int BLOCK_N, int NST = 2, bool KM = false>
 struct SmemLayout {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 4;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
@@ -281,9 +359,13 @@ struct SmemLayout {
   // weight-gradient GEMMs (both operands MN-major, K = all rows of the batch) run a long K loop per CTA: 4 stages
   static constexpr int stages() { return NST; }
   static constexpr int pipe_bytes() { return stages() * STAGE_BYTES; }
+  // KM (fp32, both operands MN-major): after the ring, the two K-major stages wgmma reads (wg_kmajor_stage)
+  static constexpr int kmajor_bytes() { return KM ? 2 * STAGE_BYTES : 0; }
   // The output staging tile (and the residual / mask tile, fetched only after the last MMA) aliases the operand
   // ring: both are touched only once every consumer warp has finished reading it.
-  static constexpr int body_bytes() { return pipe_bytes() > STAGING_BYTES ? pipe_bytes() : STAGING_BYTES; }
+  static constexpr int body_bytes() {
+    return pipe_bytes() + kmajor_bytes() > STAGING_BYTES ? pipe_bytes() + kmajor_bytes() : STAGING_BYTES;
+  }
   static constexpr int XPOSE_OFF = 256 + BLOCK_N * 4;     // after the barriers and the bias row, in the tail
   static constexpr int total() { return body_bytes() + XPOSE_OFF + (GEMM_EPI_THREADS / 32) * XPOSE_BYTES + 1024; }
 };
@@ -294,12 +376,14 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
                                                                  const __grid_constant__ CUtensorMap tmC,
                                                                  const __grid_constant__ CUtensorMap tmAux,
                                                                  const GemmParams p) {
-  using L = SmemLayout<BLOCK_N, NST>;
+  constexpr bool WG = use_wgmma<A_MN, B_MN, IN16>();
+  constexpr bool WG_T = wgmma_transposed<A_MN, B_MN, IN16>();
+  using L = SmemLayout<BLOCK_N, NST, WG_T>;
   constexpr int STAGES = L::stages();
   constexpr int N_SLABS = BLOCK_N / 32;                       // 32-column accumulator chunks
   constexpr int NT = BLOCK_N / 8;                             // 8-column MMA tiles per warp
   constexpr int N_CONSUMERS = GEMM_EPI_THREADS / 32;          // warps 0 .. N_CONSUMERS-1; the next one is the producer
-  constexpr bool WG = use_wgmma<A_MN, B_MN, IN16>();
+  static_assert(!WG_T || N_CONSUMERS == 4, "the K-major rewrite is one warpgroup's");
   constexpr int OUT_COLS = OUT16 ? 64 : 32;                   // output columns per 128-byte staging slab row
   constexpr int OUT_SLABS = (BLOCK_N + OUT_COLS - 1) / OUT_COLS;
   static_assert(!OUT16 || BLOCK_N >= 64, "bf16 outputs need at least one full 128-byte slab row");
@@ -403,14 +487,38 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
     for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.f;
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % STAGES, round = i / STAGES;
-      ptx::mbar_wait(&full_bar[s], round & 1);
-      uint8_t* a_s = smem + s * L::STAGE_BYTES;
-      if constexpr (WG) wg_mma_kblock<NT, wg_cols<BLOCK_N>()>(acc, a_s, a_s + A_STAGE_BYTES, 0, p.rnd, p.rnd_b, 1);
-      else warp_mma_kblock<NT, A_MN, B_MN, IN16>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, 0, 1, p.rnd);
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);      // this warp is done with the stage
+    if constexpr (WG_T) {
+      // ring stage i -> K-major stage i & 1 (which frees the ring stage at once); the MMAs of stage i then run while
+      // the warpgroup rewrites stage i + 1.  Each warp waits for its MMAs of stage i - 1 before the barrier of stage i,
+      // so no warp rewrites a K-major stage that the tensor core may still read.
+      uint8_t* kmajor = smem + L::pipe_bytes();
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % STAGES, round = i / STAGES;
+        ptx::mbar_wait(&full_bar[s], round & 1);
+        uint8_t* kt = kmajor + (i & 1) * L::STAGE_BYTES;
+        wg_kmajor_stage<4 + N_SLABS>(smem + s * L::STAGE_BYTES, kt, p.rnd);
+        ptx::fence_proxy_async_smem();                     // generic-proxy writes -> the tensor core's reads
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);
+        ptx::wgmma_wait0();
+        ptx::wgmma_fence_acc(acc[0]);
+        ptx::wgmma_fence_acc(acc[1]);
+        ptx::named_bar_sync(1, GEMM_EPI_THREADS);
+        wg_mma_kmajor<NT, wg_cols<BLOCK_N>()>(acc, kt);
+      }
+      ptx::wgmma_wait0();
+      ptx::wgmma_fence_acc(acc[0]);
+      ptx::wgmma_fence_acc(acc[1]);
+    } else {
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % STAGES, round = i / STAGES;
+        ptx::mbar_wait(&full_bar[s], round & 1);
+        uint8_t* a_s = smem + s * L::STAGE_BYTES;
+        if constexpr (WG) wg_mma_kblock<NT, wg_cols<BLOCK_N>()>(acc, a_s, a_s + A_STAGE_BYTES, 0, p.rnd, p.rnd_b, 1);
+        else warp_mma_kblock<NT, A_MN, B_MN, IN16>(acc, a_s, a_s + A_STAGE_BYTES, 32 * q, 0, 1, p.rnd);
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);      // this warp is done with the stage
+      }
     }
     if (lane == 0) ptx::mbar_arrive(ring_done_bar);
     // the staging tile aliases the ring: no warp writes it before every warp has finished its MMAs (this barrier also
@@ -581,6 +689,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
   constexpr int SLABS_PER_GROUP = N_SLABS / NGA;
   constexpr int NT = 4 * SLABS_PER_GROUP;                            // 8-column MMA tiles per warp
   constexpr bool WG = use_wgmma<A_MN, B_MN, false>();
+  static_assert(!wgmma_transposed<A_MN, B_MN, false>(), "both operands MN-major: one-tile kernel only");
   static_assert(!WG || 32 * SLABS_PER_GROUP == wg_cols<BLOCK_N>(), "a group's columns are one wgmma instruction wide");
   constexpr int PRODUCER_WARP = EPI_THREADS / 32;                   // after the consumer warps (whole warpgroups)
 
@@ -949,27 +1058,31 @@ template <int BLOCK_N, int A_MN, int B_MN>
 static int launch_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
                     const CUtensorMap& tX, const GemmParams& p, dim3 grid, cudaStream_t st) {
   if (d.A.bf16) return launch_bf16_t<BLOCK_N, A_MN, B_MN>(d, tA, tB, tC, tX, p, grid, st);
+  // Mode 1: the persistent pipeline for every shape it supports, i.e. all but those with both operands MN-major, which
+  // always take the one-tile kernel (its K-major rewrite for wgmma).
   // Mode 2 (default): the persistent pipeline for every unbatched, non-split shape EXCEPT short-K products with a
   // residual / mask tile, whose aux load it can only issue once the previous tile's stores have left the staging area.
-  const bool has_aux_tile = (p.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) != 0;
   // Mode 3 (measurement): as 2, but the short-K products with an aux tile go to the persistent kernel too (under packed
   // rows half of a one-tile grid are CTAs of dead tiles that only exit; the persistent kernel has none).
-  const bool pick = !(A_MN == 1 && B_MN == 1) && !(p.flags & EPI_ATOMIC) && d.nb2 == 1 && d.nb3 == 1 &&
-                    (d.K >= 256 || !has_aux_tile || g_persistent == 3);
-  if (g_persistent == 1 || (g_persistent >= 2 && pick))
-    return launch_persistent_t<BLOCK_N, A_MN, B_MN>(d, tA, tB, tC, tX, p, grid, st);
+  constexpr bool WGRAD = (A_MN == 1 && B_MN == 1);
+  if constexpr (!WGRAD) {
+    const bool has_aux_tile = (p.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) != 0;
+    const bool pick = !(p.flags & EPI_ATOMIC) && d.nb2 == 1 && d.nb3 == 1 &&
+                      (d.K >= 256 || !has_aux_tile || g_persistent == 3);
+    if (g_persistent == 1 || (g_persistent >= 2 && pick))
+      return launch_persistent_t<BLOCK_N, A_MN, B_MN>(d, tA, tB, tC, tX, p, grid, st);
+  }
   // dropout epilogue is a separate instantiation (forward linears only) so the common path carries no mask code;
   // ring depth: 4 stages for the long split-K loops of the weight gradients (1 CTA/SM), 3 for K >= 256
   // (2 CTAs/SM), 2 for the short contractions (3-4 CTAs/SM)
   constexpr bool CAN_DROP = (A_MN == 0 && B_MN == 0);
-  constexpr bool WGRAD = (A_MN == 1 && B_MN == 1);
   const bool drop = (p.flags & EPI_DROPOUT) != 0;
   if (drop && !CAN_DROP) { arb_set_error("gemm_tf32: dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
   const bool deep = !WGRAD && d.K >= 256;
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
   int smem;
-  if (WGRAD) {
-    kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 4>; smem = SmemLayout<BLOCK_N, 4>::total();
+  if constexpr (WGRAD) {
+    kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 4>; smem = SmemLayout<BLOCK_N, 4, true>::total();
   } else if (drop) {
     if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); }
     else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, CAN_DROP, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); }

@@ -87,6 +87,15 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 __device__ __forceinline__ uint32_t sw128(int r, int b) {
   return uint32_t(r) * 128u + ((uint32_t((b >> 4) ^ (r & 7))) << 4) + uint32_t(b & 15);
 }
+// 16-byte shared-memory load / store at a shared-window address (smem_u32)
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
 // fp32 element (r, c) of a [rows][32] tile (c < 32: the contiguous dimension)
 __device__ __forceinline__ float ld_f32(const uint8_t* tile, int r, int c) {
   return *reinterpret_cast<const float*>(tile + sw128(r, 4 * c));
@@ -169,6 +178,29 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[NT][4], const uin
       "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
       : ARB_D4(0), ARB_D4(1), ARB_D4(2), ARB_D4(3), ARB_D4(4), ARB_D4(5), ARB_D4(6), ARB_D4(7)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+// The same with A also read from shared memory (a K-major tile, descriptor as for B); every warp's 16 rows of D are as
+// above.
+template <int J0, int NT>
+__device__ __forceinline__ void wgmma_m64n32k8_tf32_ss(float (&d)[NT][4], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1;\n\t}"
+      : ARB_D4(0), ARB_D4(1), ARB_D4(2), ARB_D4(3)
+      : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+template <int J0, int NT>
+__device__ __forceinline__ void wgmma_m64n64k8_tf32_ss(float (&d)[NT][4], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : ARB_D4(0), ARB_D4(1), ARB_D4(2), ARB_D4(3), ARB_D4(4), ARB_D4(5), ARB_D4(6), ARB_D4(7)
+      : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 #undef ARB_D4
 

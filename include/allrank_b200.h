@@ -286,7 +286,7 @@ void arb_set_pdl(int32_t on);
 void arb_set_attention_fwd_two_pass(int32_t on);
 
 /* GEMM kernel choice.  0: one CTA per output tile everywhere; 1: the persistent, decoupled-pipeline kernel (one CTA per
- * SM walking all tiles) wherever it is supported; 2 (default): persistent for every unbatched, non-split product except
+ * SM walking all tiles) wherever it is supported (not for fp32 products whose operands are both MN-major); 2 (default): persistent for every unbatched, non-split product except
  * short-K ones (K < 256) with a residual / mask tile.  Process-wide; exists
  * for A/B measurements. */
 void arb_set_gemm_persistent(int32_t on);
