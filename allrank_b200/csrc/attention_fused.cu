@@ -187,6 +187,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) attn_fwd_kernel(
   }
 
   // ===== compute warps
+  if constexpr (DROP) drop.seed = drop_seed(drop);
   auto strip = [&](const Item& it, uint32_t region, const uint32_t* bits, int s) {
     const int r0 = 16 * s, qA = r0 + g, qB = qA + 8;
     const uint32_t q_s = region, k_s = q_s + NKB * it.qrows * 128, v_s = k_s + NKB * it.krows * 128;

@@ -139,6 +139,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
   ptx::fence_proxy_async_smem();
   arb_pdl_wait();
   __syncthreads();
+  if constexpr (DROP) drop.seed = drop_seed(drop);
 
   // Rows at or beyond a slate's extent are masked keys (probability exactly 0) whose d ctx rows are exactly zero:
   // neither their key strips nor their query strips contribute anything, and their dQ / dK / dV rows are zero.  Only

@@ -57,14 +57,17 @@ struct GemmParams {
   int rnd;            // round fp32 operands to tf32 (nearest) before the MMA; else the tensor core truncates them
   int rnd_b;          // wgmma path: round the B stages in place (rnd, unless B arrives rounded already)
   float alpha;
+  int atomic_ld;
   const float* bias;
   float* atomic_out;     // split-K: the splits' slots [split][M][atomic_ld] (DetParts), summed in order afterwards
-  long long atomic_ld;
   DropSite drop;
   float* colsum_out;
   const int* rows_dev;   // packed rows: device-resident live row count -- bounds M, or K for the split-K weight gradients
   uint32_t* bits;        // EPI_RELU_BITS / EPI_MASK_BITS: [M, N / 32] words
 };
+// The compiler keeps a kernel's by-value parameter struct of up to 128 bytes in registers; a larger GemmParams is
+// read through its address instead, which costs most GEMM kernels registers and several of them spills.
+static_assert(sizeof(GemmParams) <= 128, "GemmParams must stay within 128 bytes");
 
 // ---- MMA main loop ------------------------------------------------------------------------------------------------
 // One 32-bit operand word of a ring stage: an fp32 element (tf32 mode) or the bf16 pair (k, k+1) (k even) of row /
@@ -525,6 +528,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
     // publishes the bias row)
     ptx::named_bar_sync(1, GEMM_EPI_THREADS);
     if (has_aux) ptx::mbar_wait(aux_bar, 0);
+    const uint32_t drop_s = DROP ? drop_seed(p.drop) : 0u;
 #pragma unroll 1
     for (int c = grp; c < N_SLABS; c += GEMM_EPI_GROUPS) {
       const uint32_t word_in = word_next;
@@ -547,7 +551,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
             if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
             if constexpr (DROP) {
               const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
-              x = drop_keep(idx, p.drop.seed, p.drop.thresh) ? x * p.drop.scale : 0.0f;
+              x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
             }
             o[e] = x;
           }
@@ -587,7 +591,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
           if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
           if constexpr (DROP) {
             const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
-            x = drop_keep(idx, p.drop.seed, p.drop.thresh) ? x * p.drop.scale : 0.0f;
+            x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
           }
           o[e] = x;
         }
@@ -856,6 +860,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
                                   ? p.bits + (long long)(m0 + row) * (p.N >> 5) + ((n0 >> 5) + c) : nullptr;
           const uint32_t word_in = ci == 0 ? mword[0] : mword[1];
           if (!epi_chunk_dispatch(p.flags, v, slab_row, row, bias_s + 32 * c, p.alpha, bits_at, word_in)) {
+          const uint32_t drop_s = (p.flags & EPI_DROPOUT) ? drop_seed(p.drop) : 0u;
 #pragma unroll
           for (int piece = 0; piece < 8; ++piece) {
             float4* dst = reinterpret_cast<float4*>(slab_row + ((piece ^ (row & 7)) << 4));
@@ -868,7 +873,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
               if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
               if (p.flags & EPI_DROPOUT) {
                 const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
-                x = drop_keep(idx, p.drop.seed, p.drop.thresh) ? x * p.drop.scale : 0.0f;
+                x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
               }
               o[e] = x;
             }
@@ -1133,7 +1138,7 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   GemmParams p;
   p.M = d.M; p.N = d.N; p.K = d.K; p.nb2 = d.nb2;
   p.a_b2 = d.a_b2; p.a_b3 = d.a_b3; p.b_b2 = d.b_b2; p.b_b3 = d.b_b3; p.c_b2 = d.c_b2; p.c_b3 = d.c_b3;
-  p.flags = d.flags; p.alpha = d.alpha; p.bias = d.bias; p.atomic_out = d.atomic_out; p.atomic_ld = d.atomic_ld;
+  p.flags = d.flags; p.alpha = d.alpha; p.bias = d.bias; p.atomic_out = d.atomic_out; p.atomic_ld = int(d.atomic_ld);
   p.drop = d.drop;
   p.colsum_out = d.colsum_out;
   p.rows_dev = d.rows_dev;

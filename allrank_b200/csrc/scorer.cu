@@ -13,6 +13,7 @@
 // synchronisation and only stream-ordered allocations (the reduction slots, common.h: DetParts), so a training step can
 // be captured into a CUDA graph by the host layer.
 #include <cstdint>
+#include <string>
 #include <vector>
 #include <cuda_runtime.h>
 
@@ -356,7 +357,7 @@ static WeightMats weight_mats(const arb_scorer_config& c, const ParamLayout& L) 
 // non-null.
 static int forward_impl(const arb_scorer_config& c, const float* P, const float* x, const uint8_t* mask,
                         const int64_t* indices, const float* pe_table, int B, int S,
-                        float* scores, float* hidden, float* ws, int64_t ws_floats, int training, uint64_t seed,
+                        float* scores, float* hidden, float* ws, int64_t ws_floats, int training, CallSeed seed,
                         cudaStream_t st) {
   ParamLayout L;
   ARB_TRY(make_param_layout(c, L));
@@ -598,7 +599,7 @@ static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L
 static int backward_impl(const arb_scorer_config& c, const float* P, const float* x, const uint8_t* mask,
                          const int64_t* indices, int B, int S,
                          const float* scores, const float* dscores, const float* dhidden, float* G, float* dX,
-                         float* ws, int64_t ws_floats, float* scratch, int64_t scratch_floats, uint64_t seed,
+                         float* ws, int64_t ws_floats, float* scratch, int64_t scratch_floats, CallSeed seed,
                          cudaStream_t st) {
   ParamLayout L;
   ARB_TRY(make_param_layout(c, L));
@@ -907,27 +908,72 @@ extern "C" int64_t arb_scorer_backward_ex_scratch_floats(const arb_scorer_config
   make_scratch_layout(*cfg, L, B, S, Z, want_dx != 0);
   return Z.total;
 }
+// The entry points below take the per-call dropout seed as a host value (arb_scorer_forward, ...) or as a device word
+// (..._dseed); both are the same code with a CallSeed (dropout.cuh).
+static int forward_entry(const char* name, const arb_scorer_config* cfg, const float* params, const float* x,
+                         const uint8_t* mask, const int64_t* indices, const float* pe_table, int32_t B, int32_t S,
+                         float* scores, float* hidden, float* workspace, int64_t workspace_floats, int32_t training,
+                         CallSeed seed, void* stream) {
+  if (!cfg || !params || !x || !mask || !(scores || hidden) || !workspace || B <= 0 || S <= 0) {
+    std::string msg = std::string(name) + ": null pointer or bad shape";
+    arb_set_error(msg.c_str());
+    return ARB_E_INVALID_ARG;
+  }
+  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, scores, hidden, workspace, workspace_floats,
+                      training, seed, static_cast<cudaStream_t>(stream));
+}
+static int backward_ex_entry(const char* name, const arb_scorer_config* cfg, const float* params, const float* x,
+                             const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S, const float* scores,
+                             const float* d_scores, const float* d_hidden, float* grads, float* d_x, float* workspace,
+                             int64_t workspace_floats, float* scratch, int64_t scratch_floats, CallSeed seed,
+                             void* stream) {
+  if (!cfg || !params || !x || !mask || !workspace || !scratch || B <= 0 || S <= 0 || (!d_scores == !d_hidden) ||
+      (d_scores && !scores)) {
+    std::string msg = std::string(name) + ": null pointer, bad shape, or not exactly one of d_scores / d_hidden";
+    arb_set_error(msg.c_str());
+    return ARB_E_INVALID_ARG;
+  }
+  return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, d_hidden, grads, d_x, workspace,
+                       workspace_floats, scratch, scratch_floats, seed, static_cast<cudaStream_t>(stream));
+}
+static bool null_seed(const char* name, const uint64_t* seed_dev) {
+  if (seed_dev) return false;
+  std::string msg = std::string(name) + ": seed_dev is null";
+  arb_set_error(msg.c_str());
+  return true;
+}
+
 extern "C" int32_t arb_scorer_forward(const arb_scorer_config* cfg, const float* params, const float* x,
                                       const uint8_t* mask, const int64_t* indices, const float* pe_table, int32_t B,
                                       int32_t S, float* scores, float* workspace, int64_t workspace_floats,
                                       int32_t training, uint64_t seed, void* stream) {
-  if (!cfg || !params || !x || !mask || !scores || !workspace || B <= 0 || S <= 0) {
-    arb_set_error("arb_scorer_forward: null pointer or bad shape");
-    return ARB_E_INVALID_ARG;
-  }
-  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, scores, nullptr, workspace, workspace_floats,
-                      training, seed, static_cast<cudaStream_t>(stream));
+  return forward_entry("arb_scorer_forward", cfg, params, x, mask, indices, pe_table, B, S, scores, nullptr, workspace,
+                       workspace_floats, training, CallSeed{seed, nullptr}, stream);
+}
+extern "C" int32_t arb_scorer_forward_dseed(const arb_scorer_config* cfg, const float* params, const float* x,
+                                            const uint8_t* mask, const int64_t* indices, const float* pe_table,
+                                            int32_t B, int32_t S, float* scores, float* workspace,
+                                            int64_t workspace_floats, int32_t training, const uint64_t* seed_dev,
+                                            void* stream) {
+  if (null_seed("arb_scorer_forward_dseed", seed_dev)) return ARB_E_INVALID_ARG;
+  return forward_entry("arb_scorer_forward_dseed", cfg, params, x, mask, indices, pe_table, B, S, scores, nullptr,
+                       workspace, workspace_floats, training, CallSeed{0, seed_dev}, stream);
 }
 extern "C" int32_t arb_scorer_encode(const arb_scorer_config* cfg, const float* params, const float* x,
                                      const uint8_t* mask, const int64_t* indices, const float* pe_table, int32_t B,
                                      int32_t S, float* hidden, float* workspace, int64_t workspace_floats,
                                      int32_t training, uint64_t seed, void* stream) {
-  if (!cfg || !params || !x || !mask || !hidden || !workspace || B <= 0 || S <= 0) {
-    arb_set_error("arb_scorer_encode: null pointer or bad shape");
-    return ARB_E_INVALID_ARG;
-  }
-  return forward_impl(*cfg, params, x, mask, indices, pe_table, B, S, nullptr, hidden, workspace, workspace_floats,
-                      training, seed, static_cast<cudaStream_t>(stream));
+  return forward_entry("arb_scorer_encode", cfg, params, x, mask, indices, pe_table, B, S, nullptr, hidden, workspace,
+                       workspace_floats, training, CallSeed{seed, nullptr}, stream);
+}
+extern "C" int32_t arb_scorer_encode_dseed(const arb_scorer_config* cfg, const float* params, const float* x,
+                                           const uint8_t* mask, const int64_t* indices, const float* pe_table,
+                                           int32_t B, int32_t S, float* hidden, float* workspace,
+                                           int64_t workspace_floats, int32_t training, const uint64_t* seed_dev,
+                                           void* stream) {
+  if (null_seed("arb_scorer_encode_dseed", seed_dev)) return ARB_E_INVALID_ARG;
+  return forward_entry("arb_scorer_encode_dseed", cfg, params, x, mask, indices, pe_table, B, S, nullptr, hidden,
+                       workspace, workspace_floats, training, CallSeed{0, seed_dev}, stream);
 }
 extern "C" int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float* params, const float* x,
                                        const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
@@ -939,18 +985,26 @@ extern "C" int32_t arb_scorer_backward(const arb_scorer_config* cfg, const float
     return ARB_E_INVALID_ARG;
   }
   return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, nullptr, grads, nullptr, workspace,
-                       workspace_floats, scratch, scratch_floats, seed, static_cast<cudaStream_t>(stream));
+                       workspace_floats, scratch, scratch_floats, CallSeed{seed, nullptr},
+                       static_cast<cudaStream_t>(stream));
 }
 extern "C" int32_t arb_scorer_backward_ex(const arb_scorer_config* cfg, const float* params, const float* x,
                                           const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
                                           const float* scores, const float* d_scores, const float* d_hidden,
                                           float* grads, float* d_x, float* workspace, int64_t workspace_floats,
                                           float* scratch, int64_t scratch_floats, uint64_t seed, void* stream) {
-  if (!cfg || !params || !x || !mask || !workspace || !scratch || B <= 0 || S <= 0 || (!d_scores == !d_hidden) ||
-      (d_scores && !scores)) {
-    arb_set_error("arb_scorer_backward_ex: null pointer, bad shape, or not exactly one of d_scores / d_hidden");
-    return ARB_E_INVALID_ARG;
-  }
-  return backward_impl(*cfg, params, x, mask, indices, B, S, scores, d_scores, d_hidden, grads, d_x, workspace,
-                       workspace_floats, scratch, scratch_floats, seed, static_cast<cudaStream_t>(stream));
+  return backward_ex_entry("arb_scorer_backward_ex", cfg, params, x, mask, indices, B, S, scores, d_scores, d_hidden,
+                           grads, d_x, workspace, workspace_floats, scratch, scratch_floats, CallSeed{seed, nullptr},
+                           stream);
+}
+extern "C" int32_t arb_scorer_backward_ex_dseed(const arb_scorer_config* cfg, const float* params, const float* x,
+                                                const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
+                                                const float* scores, const float* d_scores, const float* d_hidden,
+                                                float* grads, float* d_x, float* workspace, int64_t workspace_floats,
+                                                float* scratch, int64_t scratch_floats, const uint64_t* seed_dev,
+                                                void* stream) {
+  if (null_seed("arb_scorer_backward_ex_dseed", seed_dev)) return ARB_E_INVALID_ARG;
+  return backward_ex_entry("arb_scorer_backward_ex_dseed", cfg, params, x, mask, indices, B, S, scores, d_scores,
+                           d_hidden, grads, d_x, workspace, workspace_floats, scratch, scratch_floats,
+                           CallSeed{0, seed_dev}, stream);
 }

@@ -225,6 +225,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
                                                                     const int* __restrict__ rows_dev,
                                                                     const int* __restrict__ rowmap_in) {
   arb_pdl_wait();
+  site.seed = drop_seed(site);
   if (rows_dev) {
     rows = min(rows, (long long)__ldg(rows_dev));
     if ((long long)blockIdx.x * ROWS_PER_BLOCK * rows_per_warp >= rows) return;   // whole block beyond the packed rows
@@ -347,6 +348,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_k
 template <bool DROP>
 __global__ void __launch_bounds__(256) softmax_fwd_kernel(float* __restrict__ sc, const uint8_t* __restrict__ mask,
                                                           int B, int h, int S, int pitch, DropSite site) {
+  if (DROP) site.seed = drop_seed(site);
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const long long total = (long long)B * h * S;
@@ -395,6 +397,7 @@ __global__ void __launch_bounds__(256) softmax_fwd_kernel(float* __restrict__ sc
 template <bool DROP>
 __global__ void __launch_bounds__(256) softmax_bwd_kernel(float* __restrict__ dp, float* __restrict__ prob,
                                                           long long rows, int S, int pitch, DropSite site) {
+  if (DROP) site.seed = drop_seed(site);
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= rows) return;
@@ -688,6 +691,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
     float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out, uint16_t* __restrict__ dy16_out,
     const int* __restrict__ rows_dev, const int* __restrict__ rowmap) {
   arb_pdl_wait();
+  site.seed = drop_seed(site);
   if (rows_dev) {
     rows = min(rows, (long long)__ldg(rows_dev));
     if ((long long)blockIdx.x * ROWS_PER_BLOCK * rows_per_warp >= rows) return;
@@ -882,6 +886,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
   RowRegs<NV> acc, gw;
 #pragma unroll
   for (int k = 0; k < NV; ++k) acc.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (dx_masked) site.seed = drop_seed(site);   // (here rather than at entry: NV = 2 then spills)
   for (int it = 0; it < rows_per_warp; ++it) {
     const long long row = first + it;
     if (row >= rows) break;
@@ -987,6 +992,7 @@ __global__ void __launch_bounds__(256) pos_bwd_kernel(const float* __restrict__ 
 // Element index of the dropout counter = row * width + column (the same as the GEMM epilogue's).
 __global__ void __launch_bounds__(256) act_fwd_kernel(float* __restrict__ h, long long n4, int act, DropSite site,
                                                       const int* __restrict__ rows_dev, int width4) {
+  site.seed = drop_seed(site);
   if (rows_dev) n4 = min(n4, (long long)__ldg(rows_dev) * width4);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = reinterpret_cast<float4*>(h)[i];
@@ -1007,6 +1013,7 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
                                                       int tx_n, int rows_per_block, float* __restrict__ colsum_out,
                                                       const int* __restrict__ rows_dev) {
   extern __shared__ float sh_cols[];     // [ty_n][width]: one row of column partials per row group
+  site.seed = drop_seed(site);
   const int tx = threadIdx.x % tx_n, ty = threadIdx.x / tx_n, ty_n = blockDim.x / tx_n;
   if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
   if (colsum_out) {
@@ -1224,6 +1231,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) ln_bwd_r_kernel(
     const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
     const int* __restrict__ rowmap_in) {
   arb_pdl_wait();
+  site.seed = drop_seed(site);
   constexpr int RW = 32 / LPR, W = 16 * LPR;
   if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
   if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;      // whole block beyond the live rows
@@ -1388,6 +1396,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) head_bwd_r_kernel(
     float* __restrict__ colsum_out, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
     const int* __restrict__ rowmap) {
   arb_pdl_wait();
+  site.seed = drop_seed(site);
   constexpr int RW = 32 / LPR, W = 16 * LPR;
   if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
   if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;

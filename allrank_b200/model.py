@@ -22,6 +22,8 @@ flat optimisers possible.  There is no eager fallback: CPU tensors raise.
 Dropout (transformer.dropout on attention probabilities, sublayer outputs and the FFN hidden layer; fc_model.dropout
 on the input FC) is fused into the kernels with counter-based masks that backward regenerates; like nn.Dropout it is
 active in train() mode only.  The mask stream differs from torch's Philox stream: parity under dropout is statistical.
+The per-call seed is drawn on the host, or inside `with model.dropout_seed_from(seed_tensor):` read by the kernels from
+a device tensor -- what a CUDA-graph replay of a training step needs (allrank_b200.graph).
 
 Positional encodings (allrank/models/positional.py: fixed sinusoidal buffer or learned embedding indexed by `indices`,
 padding row for padded items) are applied by a SIMT kernel after the input FC; the learned table is part of the flat
@@ -37,6 +39,7 @@ slate's packed rows get 0 in `prepare_for_output` and in x.grad, and a gradient 
 the same contract as their score.  Double backward is not supported (it raises).
 Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes.
 """
+import contextlib
 import copy
 import ctypes
 
@@ -70,6 +73,20 @@ _lib.register("arb_scorer_encode", c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i,
 _lib.register("arb_scorer_backward_ex_scratch_floats", c_i64, [c_p, c_i, c_i, c_i])
 _lib.register("arb_scorer_backward_ex", c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p,
                                               c_i64, ctypes.c_uint64, c_p])
+# the same calls with the dropout seed read from a device word (include/allrank_b200.h)
+_lib.register("arb_scorer_forward_dseed", c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i64, c_i, c_p, c_p])
+_lib.register("arb_scorer_encode_dseed", c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i64, c_i, c_p, c_p])
+_lib.register("arb_scorer_backward_ex_dseed", c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p,
+                                                    c_i64, c_p, c_i64, c_p, c_p])
+
+
+def _seed_arg(seed, device):
+    """The C argument of a dropout seed: a host value, or the address of a one-element int64 tensor on `device`."""
+    if not isinstance(seed, torch.Tensor):
+        return ctypes.c_uint64(seed)
+    if seed.device != device:
+        raise ValueError(f"the dropout seed tensor is on {seed.device}, the batch on {device}")
+    return _lib.ptr(seed)
 
 
 # ------------------------------------------------------------------------------------------------ module tree
@@ -171,10 +188,10 @@ class _ScorerFn(torch.autograd.Function):
     def forward(ctx, anchor, x, mask, model, indices):
         keep = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         xin = model._pad_features(x)
-        seed = model._draw_seed()
+        seed, drop = model._call_seed()
         scores, ws = model._launch_forward(xin, mask, keep, seed, indices)
         if keep:
-            ctx.model, ctx.ws, ctx.seed, ctx.indices = model, ws, seed, indices
+            ctx.model, ctx.ws, ctx.seed, ctx.drop, ctx.indices = model, ws, seed, drop, indices
             ctx.x_meta = (x.shape, x.dtype)
             ctx.save_for_backward(xin, mask, scores)
         return scores
@@ -183,7 +200,7 @@ class _ScorerFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, d_scores):
         xin, mask, scores = ctx.saved_tensors
-        dx = ctx.model._launch_backward(xin, mask, scores, d_scores.contiguous().float(), ctx.ws, ctx.seed,
+        dx = ctx.model._launch_backward(xin, mask, scores, d_scores.contiguous().float(), ctx.ws, ctx.seed, ctx.drop,
                                         ctx.indices, want_params=ctx.needs_input_grad[0],
                                         want_dx=ctx.needs_input_grad[1])
         ctx.ws = None
@@ -197,10 +214,10 @@ class _EncodeFn(torch.autograd.Function):
     def forward(ctx, anchor, x, mask, model, indices):
         keep = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         xin = model._pad_features(x)
-        seed = model._draw_seed()
+        seed, drop = model._call_seed()
         hidden, ws = model._launch_forward(xin, mask, keep, seed, indices, encode=True)
         if keep:
-            ctx.model, ctx.ws, ctx.seed, ctx.indices = model, ws, seed, indices
+            ctx.model, ctx.ws, ctx.seed, ctx.drop, ctx.indices = model, ws, seed, drop, indices
             ctx.x_meta = (x.shape, x.dtype)
             ctx.save_for_backward(xin, mask)
         return hidden
@@ -209,9 +226,9 @@ class _EncodeFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, d_hidden):
         xin, mask = ctx.saved_tensors
-        dx = ctx.model._launch_backward(xin, mask, None, d_hidden.contiguous().float(), ctx.ws, ctx.seed, ctx.indices,
-                                        want_params=ctx.needs_input_grad[0], want_dx=ctx.needs_input_grad[1],
-                                        from_hidden=True)
+        dx = ctx.model._launch_backward(xin, mask, None, d_hidden.contiguous().float(), ctx.ws, ctx.seed, ctx.drop,
+                                        ctx.indices, want_params=ctx.needs_input_grad[0],
+                                        want_dx=ctx.needs_input_grad[1], from_hidden=True)
         ctx.ws = None
         return None, ctx.model._input_grad(dx, ctx.x_meta), None, None, None
 
@@ -280,6 +297,7 @@ class LTRModel(nn.Module):
         self._flat_grad = None
         self._views = None
         self._anchor = None
+        self._dropout_seed = None      # the seed tensor of dropout_seed_from(), or None: seeds drawn on the host
 
     # ---- arithmetic of the encoder's matrix products ------------------------------------------------
     @property
@@ -432,8 +450,38 @@ class LTRModel(nn.Module):
             return int(torch.randint(0, 2 ** 62, (1,)).item())
         return 0
 
+    @contextlib.contextmanager
+    def dropout_seed_from(self, seed):
+        """Inside this context, train-mode calls with dropout take their per-call dropout seed from `seed` -- a
+        one-element int64 tensor on the model's CUDA device -- instead of drawing it on the host (_draw_seed).
+
+        Each call snapshots the tensor with a device-side clone() and the kernels read that snapshot when they execute,
+        so a CUDA graph captured here applies new masks whenever the tensor changes between replays (GraphedTrainStep
+        does that).  The backward reads the forward's snapshot: the tensor may be advanced between a step's forward and
+        its backward.  With the same seed value, the masks are bit-identical to those of a host-seeded call (the
+        tensor's 64 bits are read as an unsigned integer)."""
+        dev = next(self.parameters()).device
+        if not (isinstance(seed, torch.Tensor) and seed.is_cuda and seed.device == dev and seed.dtype == torch.int64
+                and seed.numel() == 1):
+            raise ValueError("dropout_seed_from: the seed must be a one-element int64 CUDA tensor on the model's "
+                             f"device ({dev})")
+        prev, self._dropout_seed = self._dropout_seed, seed
+        try:
+            yield
+        finally:
+            self._dropout_seed = prev
+
+    def _call_seed(self):
+        """(seed, dropout on) for one call: an int from _draw_seed() (0 without dropout), or inside dropout_seed_from()
+        with dropout on, a device-side snapshot of the seed tensor."""
+        if self._dropout_seed is not None and self.training and (self.dropout_p > 0.0 or self.fc_dropout_p > 0.0):
+            return self._dropout_seed.clone(), True
+        seed = self._draw_seed()
+        return seed, seed != 0
+
     def _launch_forward(self, x, mask, keep_for_backward, seed=0, indices=None, encode=False):
-        """scores (encode: the encoder output [B,S,d_model]) and the workspace kept for backward (or None)."""
+        """scores (encode: the encoder output [B,S,d_model]) and the workspace kept for backward (or None).
+        seed: an int, or a one-element int64 device tensor read by the kernels (the *_dseed entry points)."""
         training = keep_for_backward
         B, S = x.shape[0], x.shape[1]
         dev = x.device
@@ -451,39 +499,43 @@ class LTRModel(nn.Module):
             shape = (B, S) if self.d_output == 1 else (B, S, self.d_output)   # squeeze(dim=2) is a no-op for n > 1 (model.py:117)
         scores = torch.empty(shape, dtype=torch.float32, device=dev)
         name = "arb_scorer_encode" if encode else "arb_scorer_forward"
+        if isinstance(seed, torch.Tensor):
+            name += "_dseed"
         with torch.cuda.device(dev):
             table = self._pe_table(dev)
             rc = getattr(_lib.lib(), name)(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
                                            _lib.ptr(indices), _lib.ptr(table), B, S,
                                            _lib.ptr(scores), _lib.ptr(ws), n_ws, 1 if training else 0,
-                                           ctypes.c_uint64(seed), _lib.stream_ptr(dev))
+                                           _seed_arg(seed, dev), _lib.stream_ptr(dev))
         _lib.check(rc, name)
         return scores, (ws if training else None)
 
-    def _launch_backward(self, x, mask, scores, d_out, ws, seed=0, indices=None, want_params=True, want_dx=False,
-                         from_hidden=False):
+    def _launch_backward(self, x, mask, scores, d_out, ws, seed=0, dropout=False, indices=None, want_params=True,
+                         want_dx=False, from_hidden=False):
         """Accumulates the parameter gradients (want_params) and returns d loss / d x [B,S,_Fp] (want_dx, else None).
-        d_out is d loss / d scores, or d loss / d hidden (from_hidden)."""
+        d_out is d loss / d scores, or d loss / d hidden (from_hidden).  seed, dropout: what _call_seed() gave the
+        forward."""
         B, S = x.shape[0], x.shape[1]
         dev = x.device
         cfg = ctypes.byref(self._cfg)
         fresh = want_params and any(p.grad is None or p.grad.data_ptr() != gv.data_ptr() for p, _, gv in self._views)
         if fresh:                      # after optimizer.zero_grad(set_to_none=True): start from zero
             self._flat_grad.zero_()
-        self._cfg.dropout = self.dropout_p if seed else 0.0          # same mask configuration as the forward call
-        self._cfg.fc_dropout = self.fc_dropout_p if seed else 0.0
+        self._cfg.dropout = self.dropout_p if dropout else 0.0          # same mask configuration as the forward call
+        self._cfg.fc_dropout = self.fc_dropout_p if dropout else 0.0
         n_sc = int(_lib.lib().arb_scorer_backward_ex_scratch_floats(cfg, B, S, 1 if want_dx else 0))
         scratch = torch.empty(n_sc, dtype=torch.float32, device=dev)
         dx = torch.empty((B, S, self._Fp), dtype=torch.float32, device=dev) if want_dx else None
+        name = "arb_scorer_backward_ex_dseed" if isinstance(seed, torch.Tensor) else "arb_scorer_backward_ex"
         with torch.cuda.device(dev):
-            rc = _lib.lib().arb_scorer_backward_ex(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
-                                                   _lib.ptr(indices), B, S, _lib.ptr(scores),
-                                                   None if from_hidden else _lib.ptr(d_out),
-                                                   _lib.ptr(d_out) if from_hidden else None,
-                                                   _lib.ptr(self._flat_grad) if want_params else None, _lib.ptr(dx),
-                                                   _lib.ptr(ws), ws.numel(), _lib.ptr(scratch), n_sc,
-                                                   ctypes.c_uint64(seed), _lib.stream_ptr(dev))
-        _lib.check(rc, "arb_scorer_backward_ex")
+            rc = getattr(_lib.lib(), name)(cfg, _lib.ptr(self._flat), _lib.ptr(x), _lib.ptr(mask),
+                                           _lib.ptr(indices), B, S, _lib.ptr(scores),
+                                           None if from_hidden else _lib.ptr(d_out),
+                                           _lib.ptr(d_out) if from_hidden else None,
+                                           _lib.ptr(self._flat_grad) if want_params else None, _lib.ptr(dx),
+                                           _lib.ptr(ws), ws.numel(), _lib.ptr(scratch), n_sc,
+                                           _seed_arg(seed, dev), _lib.stream_ptr(dev))
+        _lib.check(rc, name)
         if fresh:
             for p, _, gv in self._views:
                 if p.requires_grad:
@@ -507,7 +559,7 @@ class LTRModel(nn.Module):
         if torch.is_grad_enabled() and (params or x.requires_grad):
             anchor = self._anchor if params else self._anchor.detach()
             return fn_cls.apply(anchor, x, m, self, idx)
-        out, _ = self._launch_forward(self._pad_features(x), m, False, self._draw_seed(), idx,
+        out, _ = self._launch_forward(self._pad_features(x), m, False, self._call_seed()[0], idx,
                                       encode=fn_cls is _EncodeFn)
         return out
 

@@ -249,6 +249,26 @@ int32_t arb_scorer_backward_ex(const arb_scorer_config* cfg, const float* params
                                float* workspace, int64_t workspace_floats, float* scratch, int64_t scratch_floats,
                                uint64_t seed, void* stream);
 
+/* The dropout seed read from device memory: the three calls above with `const uint64_t* seed_dev` (device memory,
+ * non-null) in place of `seed`.  The kernels read *seed_dev when they execute, not when they are enqueued, and give
+ * exactly the masks of the host-seeded call with seed = *seed_dev.  So a CUDA graph that captures them draws new
+ * masks on every replay once the word is advanced (in stream order) between replays.  The word must hold the same
+ * value when a step's backward executes as when its forward did: to advance it between the two, pass the backward a
+ * copy taken before.  With dropout off (cfg->dropout and cfg->fc_dropout 0) the word is not read. */
+int32_t arb_scorer_forward_dseed(const arb_scorer_config* cfg, const float* params, const float* x, const uint8_t* mask,
+                                 const int64_t* indices, const float* pe_table,
+                                 int32_t B, int32_t S, float* scores, float* workspace, int64_t workspace_floats,
+                                 int32_t training, const uint64_t* seed_dev, void* stream);
+int32_t arb_scorer_encode_dseed(const arb_scorer_config* cfg, const float* params, const float* x, const uint8_t* mask,
+                                const int64_t* indices, const float* pe_table,
+                                int32_t B, int32_t S, float* hidden, float* workspace, int64_t workspace_floats,
+                                int32_t training, const uint64_t* seed_dev, void* stream);
+int32_t arb_scorer_backward_ex_dseed(const arb_scorer_config* cfg, const float* params, const float* x,
+                                     const uint8_t* mask, const int64_t* indices, int32_t B, int32_t S,
+                                     const float* scores, const float* d_scores, const float* d_hidden, float* grads,
+                                     float* d_x, float* workspace, int64_t workspace_floats, float* scratch,
+                                     int64_t scratch_floats, const uint64_t* seed_dev, void* stream);
+
 /* 0: unfused attention (materialised logits + generic GEMMs); 1: fused tensor-core attention forward kernel, unfused
  * backward; 2 (default): fused forward and backward kernels.  Fused kernels serve slates of <= 256 items (backward:
  * head width <= 32); other shapes use the unfused path automatically.  Process-wide; exists for A/B tests. */
