@@ -335,6 +335,69 @@ static void batch_all(GemmDesc& g, int h, int B) {
   g.a_b2 = g.a_b3 = g.b_b2 = g.b_b3 = g.c_b2 = g.c_b3 = 1;
 }
 
+// ---- fused attention descriptors ---------------------------------------------------------------
+// The launch descriptors of the fused attention kernels over the buffers the scorer keeps: qkv = the QKV linear's
+// output [rows, 3d] fp32 (Q | K | V, heads side by side in each), the context [rows, d] (bfloat16 in bf16 mode), d ctx
+// [rows, d] fp32 and d qkv [rows, 3d] of the context's element type.  Dense layout: rows = B * S, per-head views
+// (dk, S, h, B); packed rows (pack_off != null): rows = the buffers' row count, views (dk, rows, h, 1).  The scorer and
+// the test entry points (arb_attention_forward / arb_attention_backward) both launch through these, so the tests run
+// the descriptors the scorer uses.
+struct AttnGeom {
+  int B, S, h, dk;
+  int64_t rows;
+  const int* pack_off;
+  TRef view(V v, int64_t pitch) const {
+    return pack_off ? head_view(v, dk, int(rows), h, 1, pitch) : head_view(v, dk, S, h, B, pitch);
+  }
+};
+
+static AttnFwdArgs attn_fwd_args(const AttnGeom& z, const float* qkv, V ctx, const uint8_t* mask, const int* extent,
+                                 float* stat_max, float* stat_sum, DropSite drop) {
+  const int64_t d = int64_t(z.h) * z.dk;
+  AttnFwdArgs a;   // QK^T, key mask, softmax, PV in one kernel; the S x S tile never leaves registers
+  a.q = z.view(qkv, 3 * d);
+  a.k = z.view(qkv + d, 3 * d);
+  a.v = z.view(qkv + 2 * d, 3 * d);
+  a.o = z.view(ctx, d);
+  a.pack_off = z.pack_off;
+  a.mask = mask; a.stat_max = stat_max; a.stat_sum = stat_sum;
+  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.dk));
+  a.drop = drop;
+  a.extent = extent;
+  return a;
+}
+
+// dbias_qkv (nullable): the column sums of dQ | dK | dV are ADDED to it (the bias gradient of the QKV linear)
+static AttnBwdArgs attn_bwd_args(const AttnGeom& z, const float* qkv, V ctx, const float* dctx, void* dqkv,
+                                 const uint8_t* mask, const int* extent, const float* stat_max, const float* stat_sum,
+                                 float* delta, float* dbias_qkv, DropSite drop, const int* rows_dev, const int* rowmap) {
+  const int64_t d = int64_t(z.h) * z.dk;
+  AttnBwdArgs a;   // dQ, dK, dV from d ctx in one kernel; P is recomputed from the saved row statistics
+  a.q = z.view(qkv, 3 * d);
+  a.k = z.view(qkv + d, 3 * d);
+  a.v = z.view(qkv + 2 * d, 3 * d);
+  a.d_o = z.view(dctx, d);
+  if (ctx.bf16) {   // dQ | dK | dV as one packed bfloat16 [rows, 3d] buffer
+    const uint16_t* g16 = static_cast<const uint16_t*>(dqkv);
+    a.dq = z.view(b16(g16), 3 * d);
+    a.dk_ = z.view(b16(g16 + d), 3 * d);
+    a.dv = z.view(b16(g16 + 2 * d), 3 * d);
+  } else {
+    const float* g32 = static_cast<const float*>(dqkv);
+    a.dq = z.view(g32, 3 * d);
+    a.dk_ = z.view(g32 + d, 3 * d);
+    a.dv = z.view(g32 + 2 * d, 3 * d);
+  }
+  a.pack_off = z.pack_off; a.rows_dev = rows_dev; a.rowmap = rowmap;
+  a.o_ptr = ctx.p; a.o_bf16 = ctx.bf16 ? 1 : 0; a.do_ptr = dctx; a.o_pitch = d;
+  a.mask = mask; a.stat_max = stat_max; a.stat_sum = stat_sum; a.delta = delta;
+  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.dk));
+  a.drop = drop;
+  a.dbias_qkv = dbias_qkv; a.d_model = int(d);
+  a.extent = extent;
+  return a;
+}
+
 static WeightMats weight_mats(const arb_scorer_config& c, const ParamLayout& L) {
   WeightMats m{};
   m.n_fc = L.n_fc;
@@ -481,7 +544,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     if (z.count) ARB_TRY(zero_rows(z, plan, k.R, st));
   }
   // per-head views: dense (dk, S, h, B), or packed (dk, rows, h, 1) with per-slate row offsets inside the kernels
-  auto hview = [&](V v, int64_t pitch) { return pack ? head_view(v, dk, int(k.R), h, 1, pitch) : head_view(v, dk, S, h, B, pitch); };
+  const AttnGeom geom{B, S, h, dk, k.R, poff};
   for (int l = 0; l < c.n_layers; ++l) {
     const auto& pl = L.layer[l];
     const auto& wl = W.layer[l];
@@ -492,17 +555,8 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
                        bf ? xn1 : nullptr, plan));
     ARB_TRY(linear_fwd(k, act(xn1), d, d, wt(pl.wqkv), P + pl.bqkv, 3 * d, qkv, 3 * d, 0, nullptr, 0));
     if (W.fused) {
-      AttnFwdArgs a;   // QK^T, key mask, softmax, PV in one kernel; the S x S tile never leaves registers
-      a.q = hview(qkv, 3 * d);
-      a.k = hview(qkv + d, 3 * d);
-      a.v = hview(qkv + 2 * d, 3 * d);
-      a.o = hview(act(ctx), d);
-      a.pack_off = poff;
-      a.mask = mask; a.stat_max = ws + wl.smax; a.stat_sum = ws + wl.ssum;
-      a.B = B; a.h = h; a.S = S; a.dk = dk; a.scale = 1.0f / sqrtf(float(dk));
-      a.drop = make_drop_site(seed, l, SITE_ATTN_P, p_drop);
-      a.extent = g_skip_padding ? kext : nullptr;
-      ARB_TRY(launch_attn_fwd(a, st));
+      ARB_TRY(launch_attn_fwd(attn_fwd_args(geom, qkv, act(ctx), mask, g_skip_padding ? kext : nullptr, ws + wl.smax,
+                                            ws + wl.ssum, make_drop_site(seed, l, SITE_ATTN_P, p_drop)), st));
     } else {
       {
         GemmDesc g;   // logits = Q K^T / sqrt(dk)      (transformer.py:148)
@@ -659,7 +713,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   const int* poff = pack ? reinterpret_cast<const int*>(ws + W.poff) : nullptr;
   if (pack) { k.rows_dev = plan; k.R = buffer_rows(c, B, S); x = ws + W.xc; gext = reinterpret_cast<int*>(ws + W.kext); }
   else if (skip) ARB_TRY(slate_extents(mask, dhidden ? dhidden : dscores, dhidden ? d : n_outputs(c), B, S, gext, st));
-  auto hview = [&](V v, int64_t pitch) { return pack ? head_view(v, dk, int(k.R), h, 1, pitch) : head_view(v, dk, S, h, B, pitch); };
+  const AttnGeom geom{B, S, h, dk, k.R, poff};
   if (pack) {
     // 256 finite rows of d ctx behind the packed rows (the attention backward's boxes overrun the last slates), and
     // zero dQ | dK | dV in the alignment rows no slate writes (the QKV weight gradient sums over them): both buffers
@@ -728,29 +782,10 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     if (G) ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), d, d, G + pl.wo));   // (bo gradient: fused into the LayerNorm backward above)
     ARB_TRY(linear_bwd_input(k, dyo, d, d, wt(pl.wo), d, dctx, d, 0, nullptr, 0));
     if (use_fused_bwd(c, S)) {
-      AttnBwdArgs a;   // dQ, dK, dV from d ctx in one kernel; P is recomputed from the saved row statistics
-      a.q = hview(qkv, 3 * d);
-      a.k = hview(qkv + d, 3 * d);
-      a.v = hview(qkv + 2 * d, 3 * d);
-      a.d_o = hview(dctx, d);
-      if (bf) {   // dQ | dK | dV as one packed bfloat16 [R, 3d] buffer
-        uint16_t* g16 = reinterpret_cast<uint16_t*>(dqkv);
-        a.dq = hview(b16(g16), 3 * d);
-        a.dk_ = hview(b16(g16 + d), 3 * d);
-        a.dv = hview(b16(g16 + 2 * d), 3 * d);
-      } else {
-        a.dq = hview(dqkv, 3 * d);
-        a.dk_ = hview(dqkv + d, 3 * d);
-        a.dv = hview(dqkv + 2 * d, 3 * d);
-      }
-      a.pack_off = poff; a.rows_dev = plan; a.rowmap = rowmap;
-      a.o_ptr = ctx; a.o_bf16 = bf ? 1 : 0; a.do_ptr = dctx; a.o_pitch = d;
-      a.mask = mask; a.stat_max = ws + wl.smax; a.stat_sum = ws + wl.ssum; a.delta = scratch + Z.delta;
-      a.B = B; a.h = h; a.S = S; a.dk = dk; a.scale = alpha;
-      a.drop = make_drop_site(seed, l, SITE_ATTN_P, p_drop);
-      a.dbias_qkv = g(pl.bqkv); a.d_model = d;           // bias gradient of the QKV projection, fused
-      a.extent = (skip || pack) ? gext : nullptr;
-      ARB_TRY(launch_attn_bwd(a, st));
+      // dQ | dK | dV into one [R, 3d] buffer (bfloat16 in bf16 mode); the QKV bias gradient is fused
+      ARB_TRY(launch_attn_bwd(attn_bwd_args(geom, qkv, act(ctx), dctx, dqkv, mask, (skip || pack) ? gext : nullptr,
+                                            ws + wl.smax, ws + wl.ssum, scratch + Z.delta, g(pl.bqkv),
+                                            make_drop_site(seed, l, SITE_ATTN_P, p_drop), plan, rowmap), st));
     } else {
       const DropSite site_p = make_drop_site(seed, l, SITE_ATTN_P, p_drop);
       if (W.fused || site_p.thresh) {
@@ -880,6 +915,49 @@ extern "C" int32_t arb_get_relu_bits(void) { return g_relu_bits; }
 extern "C" void arb_set_pack_rows(int32_t on) { g_pack_rows = on; }
 extern "C" int32_t arb_get_pack_rows(void) { return g_pack_rows; }
 extern "C" void arb_set_attention_fwd_two_pass(int32_t on) { set_attn_fwd_two_pass(on); }
+
+// The fused attention kernels on their own (include/allrank_b200.h), dense layout, launched through the scorer's
+// descriptors (attn_fwd_args / attn_bwd_args) with the dropout site of encoder layer `layer`.
+static int attention_hook_check(const char* what, int B, int S, int h, float p, bool bwd, int dk) {
+  if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
+  if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
+  if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 256; head width 16, 32 or 64, backward 16 or 32)").c_str());
+    return ARB_E_UNSUPPORTED;
+  }
+  return ARB_OK;
+}
+
+extern "C" int32_t arb_attention_forward(const float* qkv, const uint8_t* mask, const int32_t* extent, int32_t B,
+                                         int32_t S, int32_t h, int32_t dk, float p, uint64_t seed, int32_t layer,
+                                         int32_t ctx_bf16, void* ctx, float* stat_max, float* stat_sum, void* stream) {
+  if (!qkv || !mask || !ctx || !stat_max || !stat_sum) { arb_set_error("arb_attention_forward: null pointer"); return ARB_E_INVALID_ARG; }
+  ARB_TRY(attention_hook_check("arb_attention_forward", B, S, h, p, false, dk));
+  if (ctx_bf16 && dk > 32) { arb_set_error("arb_attention_forward: a bf16 context needs head width <= 32"); return ARB_E_UNSUPPORTED; }
+  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
+  const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
+  return launch_attn_fwd(attn_fwd_args(z, qkv, o, mask, extent, stat_max, stat_sum,
+                                       make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p)),
+                         static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int32_t arb_attention_backward(const float* qkv, const void* ctx, int32_t ctx_bf16, const float* d_ctx,
+                                          const uint8_t* mask, const int32_t* extent, const float* stat_max,
+                                          const float* stat_sum, int32_t B, int32_t S, int32_t h, int32_t dk, float p,
+                                          uint64_t seed, int32_t layer, void* d_qkv, float* dbias_qkv,
+                                          float* delta_scratch, void* stream) {
+  if (!qkv || !ctx || !d_ctx || !mask || !stat_max || !stat_sum || !d_qkv || !delta_scratch) {
+    arb_set_error("arb_attention_backward: null pointer");
+    return ARB_E_INVALID_ARG;
+  }
+  ARB_TRY(attention_hook_check("arb_attention_backward", B, S, h, p, true, dk));
+  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
+  const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
+  return launch_attn_bwd(attn_bwd_args(z, qkv, o, d_ctx, d_qkv, mask, extent, stat_max, stat_sum, delta_scratch,
+                                       dbias_qkv, make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p),
+                                       nullptr, nullptr),
+                         static_cast<cudaStream_t>(stream));
+}
 
 extern "C" int64_t arb_scorer_param_count(const arb_scorer_config* cfg) {
   ParamLayout L;

@@ -328,6 +328,31 @@ int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const void* aux, co
                       int32_t K, int32_t a_mn, int32_t b_mn, int32_t block_n, int32_t flags, float alpha,
                       int32_t split_k, int32_t out_bf16, float* colsum_out, void* stream);
 
+/* Building blocks exposed for tests: the fused attention kernels of one encoder layer, dense layout, launched with the
+ * descriptors the scorer uses (csrc/attention_fused.cu, attention_fused_bwd.cu).  Shapes: B slates of S <= 256 items,
+ * h heads of width dk (16, 32 or 64; backward 16 or 32; a bf16 context 16 or 32); d = h * dk.
+ *   qkv       [B*S, 3d] fp32: the QKV linear's output, Q | K | V, head j at columns j*dk ... j*dk + dk - 1 of each
+ *   mask      [B, S] uint8, 1 = padded item (a masked key)
+ *   extent    nullable [B] int32: keys at or beyond extent[b] must be masked; the kernels skip their work (forward:
+ *             keys; backward: keys and queries -- the rows of d_ctx at or beyond it must be zero).  Null: all rows.
+ *   ctx       [B*S, d]: fp32, or bfloat16 (round to nearest even) when ctx_bf16
+ *   stat_max  [B, h, S] fp32: the row maximum of the raw logits Q K^T over the unmasked keys (-inf: none)
+ *   stat_sum  [B, h, S] fp32: sum over the unmasked keys of exp((s - max) / sqrt(dk))
+ *   d_ctx     [B*S, d] fp32;  d_qkv [B*S, 3d], dQ | dK | dV in the layout of qkv, of the context's element type
+ *   dbias_qkv nullable [3d] fp32: the column sums of d_qkv are ADDED to it (the bias gradient of the QKV linear)
+ *   delta_scratch [B, h, S] fp32
+ * Dropout on the probabilities with rate p uses the scorer's site of encoder layer `layer` under the call seed `seed`:
+ * element ((b*h + head)*S + query)*S + key.  The backward reads the forward's statistics and context.  An all-padded
+ * slate gets NaN context rows (as the reference) and zero gradients.  Returns ARB_E_UNSUPPORTED for other shapes. */
+int32_t arb_attention_forward(const float* qkv, const uint8_t* mask, const int32_t* extent, int32_t B, int32_t S,
+                              int32_t h, int32_t dk, float p, uint64_t seed, int32_t layer, int32_t ctx_bf16,
+                              void* ctx, float* stat_max, float* stat_sum, void* stream);
+int32_t arb_attention_backward(const float* qkv, const void* ctx, int32_t ctx_bf16, const float* d_ctx,
+                               const uint8_t* mask, const int32_t* extent, const float* stat_max,
+                               const float* stat_sum, int32_t B, int32_t S, int32_t h, int32_t dk, float p,
+                               uint64_t seed, int32_t layer, void* d_qkv, float* dbias_qkv, float* delta_scratch,
+                               void* stream);
+
 /* ---------------------------------------------------------------- optimiser + profiling helpers
  * Flat Adam over the scorer's flat parameter/gradient buffers: torch.optim.Adam semantics (the optimiser the
  * reference instantiates from its config, allrank/main.py:82), one launch.  grads are multiplied by grad_scale

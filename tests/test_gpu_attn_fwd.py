@@ -5,7 +5,8 @@ row-local and reads the forward's row statistics (max, sum) through the attentio
 
 Extents cover one item, both sides of every 16-row strip and 128-row boundary, full slates of 240 and 256 items and
 (packed rows) empty slates; head widths 16, 32 and 64 (64 at S = 256: two items do not fit the operand pool side by
-side), the bf16 context, and batches of several hundred slates (many items per CTA)."""
+side), the bf16 context, and batches of several hundred slates (many items per CTA).  The values themselves are checked
+element by element against an fp64 reference in tests/test_gpu_attention_kernels.py."""
 import pytest
 import torch
 
