@@ -7,5 +7,4 @@
 #define ARB_DEFAULT_GEMM_PERSISTENT 2     // 0 never, 1 everywhere, 2 all unbatched non-split shapes but short-K + aux tile (arb_set_gemm_persistent)
 #define ARB_DEFAULT_PACK_ROWS 1           // encoder over the unpadded rows only (arb_set_pack_rows, ARB_PACK_ROWS)
 #define ARB_DEFAULT_ATTN_BWD_PERSISTENT 1 // attention backward: one CTA per SM walks the (slate, head) items (arb_set_attention_bwd_persistent)
-#define ARB_DEFAULT_ROW_LAYOUT 15         // bit mask: row kernels with several rows per warp step for W = 128 / 256 (ARB_ROW_LAYOUT)
 #define ARB_DEFAULT_RELU_BITS 1           // FFN ReLU backward from a 1-bit-per-unit mask written by the W1 epilogue (arb_set_relu_bits)

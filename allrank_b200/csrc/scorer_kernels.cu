@@ -2,15 +2,15 @@
 //   row LayerNorm forward / backward (the reference's custom LayerNorm: unbiased std, eps added to the std,
 //   allrank/models/transformer.py:59-81), key-masked row softmax forward / backward (transformer.py:148-153),
 //   bias-gradient column sums, final LayerNorm + linear head forward / backward (model.py:111-117).
-// All are one-warp-per-row, coalesced 128-bit accesses where the width allows, warp-shuffle reductions;
-// they are HBM-bound (DESIGN.md section 3 lists bytes per row).
+// The LayerNorm and head kernels give each row 8, 16 or 32 lanes by width (the row layout below), the others a warp per
+// row; coalesced 128-bit accesses where the width allows, warp-shuffle reductions; they are HBM-bound (DESIGN.md
+// section 3 lists bytes per row).
 #include <cstdint>
-#include <cstdlib>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "block_utils.cuh"
 #include "common.h"
-#include "defaults.h"
 #include "dropout.cuh"
 #include "scorer_kernels.h"
 
@@ -18,26 +18,38 @@ namespace arb {
 
 constexpr int ROWS_PER_BLOCK = 8;   // 8 warps
 
-// Each lane owns columns lane*4 + 128*k .. +3 (float4), k < NV; width must be a multiple of 4 and <= 128*NV.
-template <int NV>
-struct RowRegs {
-  float4 v[NV];
-};
-
-template <int NV>
-__device__ __forceinline__ void load_row(const float* __restrict__ p, int width, int lane, RowRegs<NV>& r) {
+// ------------------------------------------------------------------------------------------------ row layout
+// The row kernels give each row LPR lanes: a lane owns NJ float4 of ONE row, float4 j at column
+// ((lane % LPR) + LPR * j) * 4, so that the LPR lanes of a row read LPR * 16 contiguous bytes per instruction and a
+// warp holds 32 / LPR rows at once.  A row reduction is log2(LPR) shuffle steps that serve all rows of the warp at once
+// (one row per warp needs five steps per row and reduction: ncu put the LayerNorm forward at 75 % issue-active with
+// shuffles and their adds a third of it).  A lane's columns reach the capacity 4 * LPR * NJ; those at or beyond the
+// width are masked: loads give 0, stores skip them.
+// LayerNorm and the head take (LPR, NJ) = (8, 4) up to W = 128, (16, 4) up to 256, (32, 4) up to 512 and (32, 8) up
+// to 1024 (with_row_layout); the column sums and the multi-output head keep one row per warp (LPR = 32,
+// NJ = ceil(W / 128)).
+template <int LPR>
+__device__ __forceinline__ int r_col(int lane, int j) { return ((lane % LPR) + LPR * j) * 4; }
+template <int LPR>
+__device__ __forceinline__ float r_sum(float v) {
 #pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    const int c = lane * 4 + 128 * k;
-    r.v[k] = (c < width) ? *reinterpret_cast<const float4*>(p + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int off = 1; off < LPR; off <<= 1) v += __shfl_xor_sync(FULL, v, off);
+  return v;
+}
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_load(const float* __restrict__ row, int width, int lane, float4 (&v)[NJ]) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int c = r_col<LPR>(lane, j);
+    v[j] = c < width ? *reinterpret_cast<const float4*>(row + c) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
-template <int NV>
-__device__ __forceinline__ void store_row(float* __restrict__ p, int width, int lane, const RowRegs<NV>& r) {
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_store(float* __restrict__ row, int width, int lane, const float4 (&v)[NJ]) {
 #pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    const int c = lane * 4 + 128 * k;
-    if (c < width) *reinterpret_cast<float4*>(p + c) = r.v[k];
+  for (int j = 0; j < NJ; ++j) {
+    const int c = r_col<LPR>(lane, j);
+    if (c < width) *reinterpret_cast<float4*>(row + c) = v[j];
   }
 }
 
@@ -48,159 +60,145 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
-template <int NV>
-__device__ __forceinline__ void load_row_bf16(const uint16_t* __restrict__ p, int width, int lane, RowRegs<NV>& r) {
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_load_bf16(const uint16_t* __restrict__ row, int width, int lane, float4 (&v)[NJ]) {
 #pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    const int c = lane * 4 + 128 * k;
+  for (int j = 0; j < NJ; ++j) {
+    const int c = r_col<LPR>(lane, j);
     if (c < width) {
-      const uint2 u = *reinterpret_cast<const uint2*>(p + c);
-      r.v[k] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u),
-                           __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xffff0000u));
+      const uint2 u = *reinterpret_cast<const uint2*>(row + c);
+      v[j] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                         __uint_as_float(u.y & 0xffff0000u));
     } else {
-      r.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
 }
-template <int NV>
-__device__ __forceinline__ void store_row_bf16(uint16_t* __restrict__ p, int width, int lane, const RowRegs<NV>& r) {
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_store_bf16(uint16_t* __restrict__ row, int width, int lane, const float4 (&v)[NJ]) {
 #pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    const int c = lane * 4 + 128 * k;
+  for (int j = 0; j < NJ; ++j) {
+    const int c = r_col<LPR>(lane, j);
     if (c < width)
-      *reinterpret_cast<uint2*>(p + c) = make_uint2(pack_bf16x2(r.v[k].x, r.v[k].y), pack_bf16x2(r.v[k].z, r.v[k].w));
+      *reinterpret_cast<uint2*>(row + c) = make_uint2(pack_bf16x2(v[j].x, v[j].y), pack_bf16x2(v[j].z, v[j].w));
   }
 }
-
-template <int NV>
-__device__ __forceinline__ void apply_drop(RowRegs<NV>& r, long long row, int width, int lane, const DropSite& site) {
+template <int NJ>
+__device__ __forceinline__ void r_zero(float4 (&v)[NJ]) {
 #pragma unroll
-  for (int k = 0; k < NV; ++k) {
-    const int c = lane * 4 + 128 * k;
-    float* v = &r.v[k].x;
+  for (int j = 0; j < NJ; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+// dropout counter row * width + column: the same as the GEMM epilogues'
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_drop(float4 (&v)[NJ], long long row, int width, int lane, const DropSite& site) {
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const unsigned long long idx = (unsigned long long)row * (unsigned long long)width + (c + e);
-      v[e] = drop_keep(idx, site.seed, site.thresh) ? v[e] * site.scale : 0.0f;
+  for (int j = 0; j < NJ; ++j) {
+    float* e = &v[j].x;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const unsigned long long idx = (unsigned long long)row * (unsigned long long)width + (r_col<LPR>(lane, j) + t);
+      e[t] = drop_keep(idx, site.seed, site.thresh) ? e[t] * site.scale : 0.0f;
     }
   }
+}
+// sum the per-column accumulators of the warp's row groups, then over the block's warps, then into the block's slot of
+// `dst` (DetParts)
+template <int LPR, int NJ>
+__device__ __forceinline__ void r_reduce_columns(float4 (&acc)[NJ], float (*sh)[4 * LPR * NJ + 4], int width, int lane,
+                                                 int wid, float* __restrict__ dst) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    float* e = &acc[j].x;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+#pragma unroll
+      for (int off = LPR; off < 32; off <<= 1) e[t] += __shfl_xor_sync(FULL, e[t], off);
+    }
+  }
+  if (lane < LPR) {
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) *reinterpret_cast<float4*>(&sh[wid][r_col<LPR>(lane, j)]) = acc[j];
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < width; c += blockDim.x) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < ROWS_PER_BLOCK; ++w) t += sh[w][c];
+    dst[size_t(blockIdx.x) * width + c] = t;        // this block's slot (DetParts)
+  }
+  __syncthreads();
 }
 
 // ------------------------------------------------------------------------------------------------ LayerNorm fwd
 // y = a * (x - mean) / (std_unbiased + eps) + b ; saves mean and std per row.
-// A warp owns FWD_RPW consecutive rows and issues all their loads before the first reduction: one row per warp leaves
-// only 512 B in flight per warp at d_model = 128, far too little to cover the HBM latency (Little's law).
-constexpr int FWD_RPW = 4;
-// ... and it walks FWD_NB such batches, the loads of the next batch issued before the arithmetic of the current one: a
-// warp that retires after a single batch spends a third of its life waiting for its first loads and for a new block
-// to be scheduled (ln_forward sat at 0.66 of the HBM roof, the head at 0.31).  Wide rows (NV > 2) keep one batch: two
-// batches of them do not fit the register file.
-template <int NV>
-struct FwdBatches { static constexpr int value = NV <= 2 ? 4 : 1; };
-// (small launches keep one batch per warp: more batches would leave SMs without a block -- B = 64 has 8 k live rows)
-static inline int fwd_batches_for(int width, long long rows) { return (width <= 256 && rows >= (1 << 17)) ? 4 : 1; }
-
+// A warp walks `steps` steps of 32 / LPR rows, the loads of the next step issued before the arithmetic of the current
+// one: one row per warp leaves only 512 B in flight per warp at d_model = 128, far too little to cover the HBM latency
+// (Little's law), and a warp that retires after a single step spends a third of its life waiting for its first loads
+// and for a new block to be scheduled.
 // MAP: packed rows with a row-mapped output (rowmap_out); a template flag so that the plain kernels compile unchanged
-template <int NV, bool MAP>
+template <int LPR, int NJ, bool FILLED, bool MAP>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float* __restrict__ x,
                                                                     const float* __restrict__ a,
                                                                     const float* __restrict__ b, float eps,
-                                                                    long long rows, int width,
-                                                                    float* __restrict__ y, float* __restrict__ mean_o,
+                                                                    long long rows, int width, float* __restrict__ y,
+                                                                    float* __restrict__ mean_o,
                                                                     float* __restrict__ std_o, int torch_mode,
                                                                     uint16_t* __restrict__ y16,
-                                                                    const int* __restrict__ rows_dev, int n_batches,
+                                                                    const int* __restrict__ rows_dev, int steps,
                                                                     const int* __restrict__ rowmap_out) {
+  if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
   arb_pdl_wait();
-  constexpr int NBMAX = FwdBatches<NV>::value;
-  const int NB = NBMAX > 1 ? n_batches : 1;
-  const int lane = threadIdx.x & 31;
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (FWD_RPW * NB);
+  constexpr int RW = 32 / LPR;
+  const int lane = threadIdx.x & 31, rg = lane / LPR;
+  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (RW * steps);
   if (base >= rows) return;
-  // packed rows: the live row count lives on the device.  Its load is issued WITH the first row loads (every row below
-  // the host-side bound is readable) and consulted afterwards.
-  const long long live = rows_dev ? (long long)__ldg(rows_dev) : rows;
-  // (a multi-batch warp amortises the wait for the count over 16 rows and must not fetch rows beyond it: the dead half
-  // of a packed launch would otherwise read 12 % extra; a single-batch warp overlaps it with its only fetch)
-  if (NB > 1) { rows = min(rows, live); if (base >= rows) return; }
-  RowRegs<NV> r[FWD_RPW], rn[FWD_RPW], ga, gb;
-  auto fetch = [&](long long r0, RowRegs<NV>(&dst)[FWD_RPW]) {
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      if (r0 + q < rows) load_row<NV>(x + (r0 + q) * width, width, lane, dst[q]);
-      else {
-#pragma unroll
-        for (int k = 0; k < NV; ++k) dst[q].v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-  };
-  fetch(base, r);
-  load_row<NV>(a, width, lane, ga);
-  load_row<NV>(b, width, lane, gb);
-  rows = min(rows, live);
+  if (rows_dev) { rows = min(rows, (long long)__ldg(rows_dev)); if (base >= rows) return; }
+  float4 ga[NJ], gb[NJ], cur[NJ], nxt[NJ];
+  r_load<LPR>(a, width, lane, ga);
+  r_load<LPR>(b, width, lane, gb);
+  if (base + rg < rows) r_load<LPR>(x + (base + rg) * width, width, lane, cur); else r_zero(cur);
 #pragma unroll 1
-  for (int nb = 0; nb < NB; ++nb) {
-    const long long row0 = base + nb * FWD_RPW;
-    if (row0 >= rows) break;
-    if (NBMAX > 1 && nb + 1 < NB) fetch(row0 + FWD_RPW, rn);
-    float mean[FWD_RPW], sd[FWD_RPW];
+  for (int s = 0; s < steps; ++s) {
+    if (base + (long long)s * RW >= rows) break;
+    const long long row = base + (long long)s * RW + rg;
+    if (s + 1 < steps) { if (row + RW < rows) r_load<LPR>(x + (row + RW) * width, width, lane, nxt); else r_zero(nxt); }
+    float sum = 0.f;
 #pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      float s = 0.f;
+    for (int j = 0; j < NJ; ++j) sum += cur[j].x + cur[j].y + cur[j].z + cur[j].w;
+    const float m = r_sum<LPR>(sum) / float(width);
+    float ss = 0.f;
 #pragma unroll
-      for (int k = 0; k < NV; ++k) s += r[q].v[k].x + r[q].v[k].y + r[q].v[k].z + r[q].v[k].w;
-      mean[q] = s;
-    }
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) mean[q] = warp_sum(mean[q]) / float(width);
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      float ss = 0.f;
-#pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        const int c = lane * 4 + 128 * k;
-        if (c < width) {
-          const float d0 = r[q].v[k].x - mean[q], d1 = r[q].v[k].y - mean[q], d2 = r[q].v[k].z - mean[q],
-                      d3 = r[q].v[k].w - mean[q];
-          ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
-        }
+    for (int j = 0; j < NJ; ++j) {
+      if (r_col<LPR>(lane, j) < width) {
+        const float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
+        ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
       }
-      sd[q] = ss;
     }
+    ss = r_sum<LPR>(ss);
+    // torch_mode: nn.LayerNorm (biased variance, eps inside the root; FCModel's input_norm, model.py:27) -- the saved
+    // "std" is then sqrt(var + eps) and the backward is called with eps = 0
+    const float sdq = torch_mode ? sqrtf(ss / float(width) + eps) : sqrtf(ss / float(width - 1));
+    // one reciprocal per row instead of a division per element: the kernel is bound by instruction issue as much as
+    // by HBM (an IEEE division is ~10 instructions), and a * (x - mean) * (1 / (std + eps)) differs from the
+    // reference's a * (x - mean) / (std + eps) by one rounding (6e-8 relative)
+    const float rinv = 1.0f / (torch_mode ? sdq : sdq + eps);
 #pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) sd[q] = warp_sum(sd[q]);
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      if (row0 + q >= rows) break;
-      // torch_mode: nn.LayerNorm (biased variance, eps inside the root; FCModel's input_norm, model.py:27) -- the saved
-      // "std" is then sqrt(var + eps) and the backward is called with eps = 0
-      const float sdq = torch_mode ? sqrtf(sd[q] / float(width) + eps) : sqrtf(sd[q] / float(width - 1));
-      // one reciprocal per row instead of a division per element: the kernel is bound by instruction issue as much as
-      // by HBM (an IEEE division is ~10 instructions), and a * (x - mean) * (1 / (std + eps)) differs from the
-      // reference's a * (x - mean) / (std + eps) by one rounding (6e-8 relative)
-      const float rinv = 1.0f / (torch_mode ? sdq : sdq + eps);
-      const float m = mean[q];
-#pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        r[q].v[k].x = ga.v[k].x * (r[q].v[k].x - m) * rinv + gb.v[k].x;
-        r[q].v[k].y = ga.v[k].y * (r[q].v[k].y - m) * rinv + gb.v[k].y;
-        r[q].v[k].z = ga.v[k].z * (r[q].v[k].z - m) * rinv + gb.v[k].z;
-        r[q].v[k].w = ga.v[k].w * (r[q].v[k].w - m) * rinv + gb.v[k].w;
-      }
-      if (y16) store_row_bf16<NV>(y16 + (row0 + q) * width, width, lane, r[q]);   // bf16 mode: the GEMM operand copy only
+    for (int j = 0; j < NJ; ++j) {
+      cur[j].x = ga[j].x * (cur[j].x - m) * rinv + gb[j].x;
+      cur[j].y = ga[j].y * (cur[j].y - m) * rinv + gb[j].y;
+      cur[j].z = ga[j].z * (cur[j].z - m) * rinv + gb[j].z;
+      cur[j].w = ga[j].w * (cur[j].w - m) * rinv + gb[j].w;
+    }
+    if (row < rows) {
+      if (y16) r_store_bf16<LPR>(y16 + row * width, width, lane, cur);   // bf16 mode: the GEMM operand copy only
       else {   // packed rows with rowmap_out: row r goes to y[rowmap_out[r]] (alignment rows: nowhere)
-        const long long yr = MAP ? (long long)rowmap_out[row0 + q] : row0 + q;
-        if (!MAP || yr >= 0) store_row<NV>(y + yr * width, width, lane, r[q]);
+        const long long yr = MAP ? (long long)rowmap_out[row] : row;
+        if (!MAP || yr >= 0) r_store<LPR>(y + yr * width, width, lane, cur);
       }
-      if (lane == 0) { mean_o[row0 + q] = m; std_o[row0 + q] = sdq; }
+      if (lane % LPR == 0) { mean_o[row] = m; std_o[row] = sdq; }
     }
-    if (NBMAX > 1) {
 #pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-#pragma unroll
-        for (int k = 0; k < NV; ++k) r[q].v[k] = rn[q].v[k];
-      }
-    }
+    for (int j = 0; j < NJ; ++j) cur[j] = nxt[j];
   }
 }
 
@@ -208,135 +206,101 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
 // dx = [dres +] r (dxh - mean(dxh)) - r^2 (sum_k dxh_k c_k) / ((d-1) std) * c,   dxh = dy * a, c = x - mean,
 // r = 1/(std+eps).   grad_a += sum_rows dy * xhat,  grad_b += sum_rows dy  (block partials -> DetParts slots).
 // MAP: packed rows reading a row-mapped gradient (rowmap_in); a template flag as in ln_fwd_kernel
-template <int NV, bool MAP>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NV == 1 ? 4 : 1) ln_bwd_kernel(const float* __restrict__ dy,
-                                                                    const float* __restrict__ x,
-                                                                    const float* __restrict__ a,
-                                                                    const float* __restrict__ mean_i,
-                                                                    const float* __restrict__ std_i, float eps,
-                                                                    const float* __restrict__ dres, long long rows,
-                                                                    int width, int rows_per_warp,
-                                                                    float* __restrict__ dx, float* __restrict__ grad_a,
-                                                                    float* __restrict__ grad_b,
-                                                                    float* __restrict__ dx_masked, DropSite site,
-                                                                    float* __restrict__ colsum_out, int torch_mode,
-                                                                    const uint16_t* __restrict__ dy16_in,
-                                                                    uint16_t* __restrict__ dy16_out,
-                                                                    const int* __restrict__ rows_dev,
-                                                                    const int* __restrict__ rowmap_in) {
+template <int LPR, int NJ, bool FILLED, bool MAP>
+__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) ln_bwd_kernel(
+    const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ a,
+    const float* __restrict__ mean_i, const float* __restrict__ std_i, float eps, const float* __restrict__ dres,
+    long long rows, int width, int steps, float* __restrict__ dx, float* __restrict__ grad_a,
+    float* __restrict__ grad_b, float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out,
+    int torch_mode, const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out,
+    const int* __restrict__ rows_dev, const int* __restrict__ rowmap_in) {
+  if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
   arb_pdl_wait();
   site.seed = drop_seed(site);
-  if (rows_dev) {
-    rows = min(rows, (long long)__ldg(rows_dev));
-    if ((long long)blockIdx.x * ROWS_PER_BLOCK * rows_per_warp >= rows) return;   // whole block beyond the packed rows
-  }
-  __shared__ float sh[ROWS_PER_BLOCK][128 * NV + 4];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  RowRegs<NV> ga, acc_a, acc_b, acc_c;
-  load_row<NV>(a, width, lane, ga);
-#pragma unroll
-  for (int k = 0; k < NV; ++k) acc_a.v[k] = acc_b.v[k] = acc_c.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-  const long long first = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * rows_per_warp;
-  // Software pipeline over the warp's rows: the loads of row it+1 (dy, x, residual gradient, statistics) are issued
-  // before the reductions of row it, so two rows of traffic are in flight per warp.
-  RowRegs<NV> g, xr, res, g_n, xr_n, res_n;
-  float mean = 0.f, sd = 1.f, mean_n = 0.f, sd_n = 1.f;
-  auto fetch = [&](long long row, RowRegs<NV>& gg, RowRegs<NV>& xx, RowRegs<NV>& rr, float& mm, float& ss) {
-    if (dy16_in) load_row_bf16<NV>(dy16_in + row * width, width, lane, gg);
-    else if (MAP) {   // packed rows: dy of row r is dy[rowmap_in[r]]; alignment rows have a zero gradient
-      const long long src = rowmap_in[row];
-      if (src >= 0) load_row<NV>(dy + src * width, width, lane, gg);
-      else {
-#pragma unroll
-        for (int k = 0; k < NV; ++k) gg.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    } else load_row<NV>(dy + row * width, width, lane, gg);
-    load_row<NV>(x + row * width, width, lane, xx);
-    if (dres) load_row<NV>(dres + row * width, width, lane, rr);
-    mm = mean_i[row]; ss = std_i[row];
-  };
-  if (first < rows) fetch(first, g, xr, res, mean, sd);
-  for (int it = 0; it < rows_per_warp; ++it) {
-    const long long row = first + it;
-    if (row >= rows) break;
-    const bool more = it + 1 < rows_per_warp && row + 1 < rows;
-    if (more) fetch(row + 1, g_n, xr_n, res_n, mean_n, sd_n);
+  constexpr int RW = 32 / LPR;
+  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
+  if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;      // whole block beyond the live rows
+  __shared__ float sh[ROWS_PER_BLOCK][4 * LPR * NJ + 4];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, rg = lane / LPR;
+  float4 ga[NJ], acc_a[NJ], acc_b[NJ], acc_c[NJ];
+  r_load<LPR>(a, width, lane, ga);
+  r_zero(acc_a); r_zero(acc_b); r_zero(acc_c);
+  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * (RW * steps);
+#pragma unroll 1
+  for (int s = 0; s < steps; ++s) {
+    if (base + (long long)s * RW >= rows) break;
+    const long long row = base + (long long)s * RW + rg;
+    const bool ok = row < rows;
+    float4 g[NJ], xr[NJ], res[NJ];
+    float mean = 0.f, sd = 1.f;
+    r_zero(g); r_zero(xr); r_zero(res);
+    if (ok) {
+      if (dy16_in) r_load_bf16<LPR>(dy16_in + row * width, width, lane, g);
+      else if (MAP) {   // packed rows: dy of row r is dy[rowmap_in[r]]; alignment rows have a zero gradient
+        const long long src = rowmap_in[row];
+        if (src >= 0) r_load<LPR>(dy + src * width, width, lane, g);
+      } else r_load<LPR>(dy + row * width, width, lane, g);
+      r_load<LPR>(x + row * width, width, lane, xr);
+      if (dres) r_load<LPR>(dres + row * width, width, lane, res);
+      mean = mean_i[row]; sd = std_i[row];
+    }
     const float r = 1.0f / (sd + eps);
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-    for (int k = 0; k < NV; ++k) {
-      const int c = lane * 4 + 128 * k;
-      float* gv = &g.v[k].x;
-      float* xv = &xr.v[k].x;
-      const float* av = &ga.v[k].x;
-      float* aa = &acc_a.v[k].x;
-      float* ab = &acc_b.v[k].x;
+    for (int j = 0; j < NJ; ++j) {
+      const bool in = ok && r_col<LPR>(lane, j) < width;
+      float* gv = &g[j].x;
+      float* xv = &xr[j].x;
+      const float* av = &ga[j].x;
+      float* aa = &acc_a[j].x;
+      float* ab = &acc_b[j].x;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float cc = (c < width) ? xv[e] - mean : 0.f;
-        const float dyv = gv[e];
-        aa[e] += dyv * cc * r;     // dy * xhat
-        ab[e] += dyv;
-        const float dxh = dyv * av[e];
-        gv[e] = dxh;
-        xv[e] = cc;
+      for (int t = 0; t < 4; ++t) {
+        const float cc = in ? xv[t] - mean : 0.f;
+        const float dyv = gv[t];
+        aa[t] += dyv * cc * r;     // dy * xhat
+        ab[t] += dyv;
+        const float dxh = dyv * av[t];
+        gv[t] = dxh;
+        xv[t] = cc;
         s1 += dxh;
         s2 += dxh * cc;
       }
     }
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
+    s1 = r_sum<LPR>(s1);
+    s2 = r_sum<LPR>(s2);
     const float m1 = s1 / float(width);
     const float coef = torch_mode ? r * r * r * s2 / float(width)
                                   : ((sd > 0.f) ? r * r * s2 / (float(width - 1) * sd) : 0.f);
 #pragma unroll
-    for (int k = 0; k < NV; ++k) {
-      float* gv = &g.v[k].x;
-      const float* xv = &xr.v[k].x;
-      const float* rv = &res.v[k].x;
+    for (int j = 0; j < NJ; ++j) {
+      float* gv = &g[j].x;
+      const float* xv = &xr[j].x;
+      const float* rv = &res[j].x;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        float o = r * (gv[e] - m1) - coef * xv[e];
-        if (dres) o += rv[e];
-        gv[e] = o;
+      for (int t = 0; t < 4; ++t) {
+        float o = r * (gv[t] - m1) - coef * xv[t];
+        if (dres) o += rv[t];
+        gv[t] = o;
       }
     }
-    store_row<NV>(dx + row * width, width, lane, g);
-    if (dx_masked) {   // the same gradient through the dropout of the sublayer below (mask regenerated)
-      apply_drop<NV>(g, row, width, lane, site);
-      store_row<NV>(dx_masked + row * width, width, lane, g);
-    }
-    // bf16 mode: the copy the weight / input-gradient GEMMs of the sublayer below read (after its dropout mask)
-    if (dy16_out) store_row_bf16<NV>(dy16_out + row * width, width, lane, g);
-    if (colsum_out) {  // bias gradient of the linear below = column sums of what that linear receives
+    if (ok) {
+      r_store<LPR>(dx + row * width, width, lane, g);
+      if (dx_masked) {   // the same gradient through the dropout of the sublayer below (mask regenerated)
+        r_drop<LPR>(g, row, width, lane, site);
+        r_store<LPR>(dx_masked + row * width, width, lane, g);
+      }
+      // bf16 mode: the copy the weight / input-gradient GEMMs of the sublayer below read (after its dropout mask)
+      if (dy16_out) r_store_bf16<LPR>(dy16_out + row * width, width, lane, g);
+      if (colsum_out) {  // bias gradient of the linear below = column sums of what that linear receives
 #pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        acc_c.v[k].x += g.v[k].x; acc_c.v[k].y += g.v[k].y; acc_c.v[k].z += g.v[k].z; acc_c.v[k].w += g.v[k].w;
+        for (int j = 0; j < NJ; ++j) { acc_c[j].x += g[j].x; acc_c[j].y += g[j].y; acc_c[j].z += g[j].z; acc_c[j].w += g[j].w; }
       }
     }
-    if (more) {
-#pragma unroll
-      for (int k = 0; k < NV; ++k) { g.v[k] = g_n.v[k]; xr.v[k] = xr_n.v[k]; res.v[k] = res_n.v[k]; }
-      mean = mean_n; sd = sd_n;
-    }
   }
-  // block-level reduction of the gain/bias gradients
-#pragma unroll
-  for (int pass = 0; pass < 3; ++pass) {
-    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : colsum_out);
-    if (!dst) continue;      // (no parameter gradients requested: grad_a / grad_b are null)
-    const RowRegs<NV>& src = pass == 0 ? acc_a : (pass == 1 ? acc_b : acc_c);
-#pragma unroll
-    for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = src.v[k];
-    __syncthreads();
-    for (int c = threadIdx.x; c < width; c += blockDim.x) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < ROWS_PER_BLOCK; ++w) t += sh[w][c];
-      dst[size_t(blockIdx.x) * width + c] = t;      // this block's slot (DetParts)
-    }
-    __syncthreads();
-  }
+  if (grad_a) r_reduce_columns<LPR>(acc_a, sh, width, lane, wid, grad_a);
+  if (grad_b) r_reduce_columns<LPR>(acc_b, sh, width, lane, wid, grad_b);
+  if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, width, lane, wid, colsum_out);
 }
 
 // ------------------------------------------------------------------------------------------------ softmax fwd
@@ -501,45 +465,36 @@ __global__ void __launch_bounds__(256) slate_extent_kernel(const uint8_t* __rest
 template <int NV>
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ in, long long rows, int width,
                                                      long long ld, int rows_per_block, float* __restrict__ out) {
-  __shared__ float sh[8][128 * NV + 4];
+  __shared__ float sh[ROWS_PER_BLOCK][128 * NV + 4];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const long long r0 = (long long)blockIdx.x * rows_per_block;
   const long long r1 = min(rows, r0 + rows_per_block);
-  RowRegs<NV> acc;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) acc.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 acc[NV];
+  r_zero(acc);
   long long r = r0 + wid;
   for (; r + 24 < r1; r += 32) {
-    RowRegs<NV> a0, a1, a2, a3;
-    load_row<NV>(in + r * ld, width, lane, a0);
-    load_row<NV>(in + (r + 8) * ld, width, lane, a1);
-    load_row<NV>(in + (r + 16) * ld, width, lane, a2);
-    load_row<NV>(in + (r + 24) * ld, width, lane, a3);
+    float4 a0[NV], a1[NV], a2[NV], a3[NV];
+    r_load<32>(in + r * ld, width, lane, a0);
+    r_load<32>(in + (r + 8) * ld, width, lane, a1);
+    r_load<32>(in + (r + 16) * ld, width, lane, a2);
+    r_load<32>(in + (r + 24) * ld, width, lane, a3);
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
-      acc.v[k].x += (a0.v[k].x + a1.v[k].x) + (a2.v[k].x + a3.v[k].x);
-      acc.v[k].y += (a0.v[k].y + a1.v[k].y) + (a2.v[k].y + a3.v[k].y);
-      acc.v[k].z += (a0.v[k].z + a1.v[k].z) + (a2.v[k].z + a3.v[k].z);
-      acc.v[k].w += (a0.v[k].w + a1.v[k].w) + (a2.v[k].w + a3.v[k].w);
+      acc[k].x += (a0[k].x + a1[k].x) + (a2[k].x + a3[k].x);
+      acc[k].y += (a0[k].y + a1[k].y) + (a2[k].y + a3[k].y);
+      acc[k].z += (a0[k].z + a1[k].z) + (a2[k].z + a3[k].z);
+      acc[k].w += (a0[k].w + a1[k].w) + (a2[k].w + a3[k].w);
     }
   }
   for (; r < r1; r += 8) {
-    RowRegs<NV> a0;
-    load_row<NV>(in + r * ld, width, lane, a0);
+    float4 a0[NV];
+    r_load<32>(in + r * ld, width, lane, a0);
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
-      acc.v[k].x += a0.v[k].x; acc.v[k].y += a0.v[k].y; acc.v[k].z += a0.v[k].z; acc.v[k].w += a0.v[k].w;
+      acc[k].x += a0[k].x; acc[k].y += a0[k].y; acc[k].z += a0[k].z; acc[k].w += a0[k].w;
     }
   }
-#pragma unroll
-  for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = acc.v[k];
-  __syncthreads();
-  for (int c = threadIdx.x; c < width; c += blockDim.x) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += sh[w][c];
-    out[size_t(blockIdx.x) * width + c] = t;        // this block's slot (DetParts)
-  }
+  r_reduce_columns<32>(acc, sh, width, lane, wid, out);
 }
 
 // ------------------------------------------------------------------------------------------------ head fwd
@@ -557,284 +512,196 @@ __device__ __forceinline__ float act_bwd(float out, float z, int act) {
   return 1.0f;
 }
 
-template <int NV>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_fwd_kernel(const float* __restrict__ x,
-                                                                      const float* __restrict__ a,
-                                                                      const float* __restrict__ b, float eps,
-                                                                      const float* __restrict__ w,
-                                                                      const float* __restrict__ wb, int has_norm,
-                                                                      int act, long long rows, int width,
-                                                                      float* __restrict__ score,
-                                                                      float* __restrict__ mean_o,
-                                                                      float* __restrict__ std_o,
-                                                                      const int* __restrict__ rows_dev,
-                                                                      const int* __restrict__ rowmap, int n_batches) {
+template <int LPR, int NJ, bool FILLED>
+__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_fwd_kernel(
+    const float* __restrict__ x, const float* __restrict__ a, const float* __restrict__ b, float eps,
+    const float* __restrict__ w, const float* __restrict__ wb, int has_norm, int act, long long rows, int width,
+    float* __restrict__ score, float* __restrict__ mean_o, float* __restrict__ std_o,
+    const int* __restrict__ rows_dev, const int* __restrict__ rowmap, int steps) {
+  if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
   arb_pdl_wait();
-  constexpr int NBMAX = FwdBatches<NV>::value;
-  const int NB = NBMAX > 1 ? n_batches : 1;
-  const int lane = threadIdx.x & 31;
-  // n_batches batches of FWD_RPW rows per warp, the next batch's loads (rows and their row-map entries) issued before
-  // the arithmetic of the current one (see ln_fwd_kernel); the device-side row count is loaded with the first batch
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (FWD_RPW * NB);
+  constexpr int RW = 32 / LPR;
+  const int lane = threadIdx.x & 31, rg = lane / LPR;
+  // `steps` steps of 32 / LPR rows per warp, the next step's loads (rows and their row-map entries) issued before the
+  // arithmetic of the current one (see ln_fwd_kernel)
+  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (RW * steps);
   if (base >= rows) return;
-  const long long live = rows_dev ? (long long)__ldg(rows_dev) : rows;
-  if (NB > 1) { rows = min(rows, live); if (base >= rows) return; }   // (see ln_fwd_kernel)
-  RowRegs<NV> r[FWD_RPW], rn[FWD_RPW], ga, gb, gw;
-  long long at[FWD_RPW], atn[FWD_RPW];
-  auto fetch = [&](long long r0, RowRegs<NV>(&dst)[FWD_RPW], long long(&dat)[FWD_RPW]) {
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      dat[q] = (rowmap && r0 + q < rows) ? (long long)rowmap[r0 + q] : r0 + q;
-      if (r0 + q < rows) load_row<NV>(x + (r0 + q) * width, width, lane, dst[q]);
-      else {
-#pragma unroll
-        for (int k = 0; k < NV; ++k) dst[q].v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-  };
-  fetch(base, r, at);
-  load_row<NV>(w, width, lane, gw);
-  if (has_norm) {
-    load_row<NV>(a, width, lane, ga);
-    load_row<NV>(b, width, lane, gb);
-  }
+  if (rows_dev) { rows = min(rows, (long long)__ldg(rows_dev)); if (base >= rows) return; }
+  float4 ga[NJ], gb[NJ], gw[NJ], cur[NJ], nxt[NJ];
+  r_load<LPR>(w, width, lane, gw);
+  if (has_norm) { r_load<LPR>(a, width, lane, ga); r_load<LPR>(b, width, lane, gb); } else { r_zero(ga); r_zero(gb); }
   const float bias = wb[0];
-  rows = min(rows, live);
+  long long at = -1, at_n = -1;
+  if (base + rg < rows) {
+    r_load<LPR>(x + (base + rg) * width, width, lane, cur);
+    at = rowmap ? (long long)rowmap[base + rg] : base + rg;
+  } else {
+    r_zero(cur);
+  }
 #pragma unroll 1
-  for (int nb = 0; nb < NB; ++nb) {
-    const long long row0 = base + nb * FWD_RPW;
-    if (row0 >= rows) break;
-    if (NBMAX > 1 && nb + 1 < NB) fetch(row0 + FWD_RPW, rn, atn);
-    float mean[FWD_RPW], sd[FWD_RPW];
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) mean[q] = sd[q] = 0.f;
+  for (int s = 0; s < steps; ++s) {
+    if (base + (long long)s * RW >= rows) break;
+    const long long row = base + (long long)s * RW + rg;
+    if (s + 1 < steps) {
+      at_n = -1;
+      if (row + RW < rows) {
+        r_load<LPR>(x + (row + RW) * width, width, lane, nxt);
+        at_n = rowmap ? (long long)rowmap[row + RW] : row + RW;
+      } else {
+        r_zero(nxt);
+      }
+    }
+    float m = 0.f, sdv = 0.f;
     if (has_norm) {
+      float sum = 0.f;
 #pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-        float s = 0.f;
+      for (int j = 0; j < NJ; ++j) sum += cur[j].x + cur[j].y + cur[j].z + cur[j].w;
+      m = r_sum<LPR>(sum) / float(width);
+      float ss = 0.f;
 #pragma unroll
-        for (int k = 0; k < NV; ++k) s += r[q].v[k].x + r[q].v[k].y + r[q].v[k].z + r[q].v[k].w;
-        mean[q] = s;
-      }
-#pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) mean[q] = warp_sum(mean[q]) / float(width);
-#pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-        float ss = 0.f;
-#pragma unroll
-        for (int k = 0; k < NV; ++k) {
-          const int c = lane * 4 + 128 * k;
-          if (c < width) {
-            const float d0 = r[q].v[k].x - mean[q], d1 = r[q].v[k].y - mean[q], d2 = r[q].v[k].z - mean[q],
-                        d3 = r[q].v[k].w - mean[q];
-            ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
-          }
-        }
-        sd[q] = ss;
-      }
-#pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) sd[q] = sqrtf(warp_sum(sd[q]) / float(width - 1));
-#pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-        const float rinv = 1.0f / (sd[q] + eps), m = mean[q];      // (one reciprocal per row: see ln_fwd_kernel)
-#pragma unroll
-        for (int k = 0; k < NV; ++k) {
-          r[q].v[k].x = ga.v[k].x * (r[q].v[k].x - m) * rinv + gb.v[k].x;
-          r[q].v[k].y = ga.v[k].y * (r[q].v[k].y - m) * rinv + gb.v[k].y;
-          r[q].v[k].z = ga.v[k].z * (r[q].v[k].z - m) * rinv + gb.v[k].z;
-          r[q].v[k].w = ga.v[k].w * (r[q].v[k].w - m) * rinv + gb.v[k].w;
+      for (int j = 0; j < NJ; ++j) {
+        if (r_col<LPR>(lane, j) < width) {
+          const float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
+          ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
         }
       }
-    }
-    float dot[FWD_RPW];
+      sdv = sqrtf(r_sum<LPR>(ss) / float(width - 1));
+      const float rinv = 1.0f / (sdv + eps);      // (one reciprocal per row: see ln_fwd_kernel)
 #pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) {
-      float t = 0.f;
-#pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        const int c = lane * 4 + 128 * k;
-        if (c < width)
-          t += r[q].v[k].x * gw.v[k].x + r[q].v[k].y * gw.v[k].y + r[q].v[k].z * gw.v[k].z + r[q].v[k].w * gw.v[k].w;
-      }
-      dot[q] = t;
-    }
-#pragma unroll
-    for (int q = 0; q < FWD_RPW; ++q) dot[q] = warp_sum(dot[q]);
-    if (lane == 0) {
-#pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-        if (row0 + q >= rows) break;
-        // packed rows: the score goes to the item's place in the [B, S] tensor (alignment rows have none)
-        if (at[q] >= 0) score[at[q]] = act_fwd(dot[q] + bias, act);
-        if (has_norm && mean_o) { mean_o[row0 + q] = mean[q]; std_o[row0 + q] = sd[q]; }
+      for (int j = 0; j < NJ; ++j) {
+        cur[j].x = ga[j].x * (cur[j].x - m) * rinv + gb[j].x;
+        cur[j].y = ga[j].y * (cur[j].y - m) * rinv + gb[j].y;
+        cur[j].z = ga[j].z * (cur[j].z - m) * rinv + gb[j].z;
+        cur[j].w = ga[j].w * (cur[j].w - m) * rinv + gb[j].w;
       }
     }
-    if (NBMAX > 1) {
+    // (masked columns hold 0: their gain and bias are loaded as 0)
+    float dot = 0.f;
 #pragma unroll
-      for (int q = 0; q < FWD_RPW; ++q) {
-        at[q] = atn[q];
-#pragma unroll
-        for (int k = 0; k < NV; ++k) r[q].v[k] = rn[q].v[k];
-      }
+    for (int j = 0; j < NJ; ++j) dot += cur[j].x * gw[j].x + cur[j].y * gw[j].y + cur[j].z * gw[j].z + cur[j].w * gw[j].w;
+    dot = r_sum<LPR>(dot);
+    if (row < rows && lane % LPR == 0) {
+      // packed rows: the score goes to the item's place in the [B, S] tensor (alignment rows have none)
+      if (at >= 0) score[at] = act_fwd(dot + bias, act);
+      if (has_norm && mean_o) { mean_o[row] = m; std_o[row] = sdv; }
     }
+    at = at_n;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) cur[j] = nxt[j];
   }
 }
 
 // head backward: dz = dscore * act'(z);  d xf = dz * w;  grad_w += dz * xf;  grad_wb += dz;  then LayerNorm bwd.
-template <int NV>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_bwd_kernel(
+template <int LPR, int NJ, bool FILLED>
+__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) head_bwd_kernel(
     const float* __restrict__ dscore, const float* __restrict__ score, const float* __restrict__ x,
     const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ mean_i,
-    const float* __restrict__ std_i, float eps, const float* __restrict__ w, const float* __restrict__ wb,
-    int has_norm, int act, long long rows, int width, int rows_per_warp, float* __restrict__ dx,
-    float* __restrict__ grad_a, float* __restrict__ grad_b, float* __restrict__ grad_w, float* __restrict__ grad_wb,
-    float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out, uint16_t* __restrict__ dy16_out,
-    const int* __restrict__ rows_dev, const int* __restrict__ rowmap) {
+    const float* __restrict__ std_i, float eps, const float* __restrict__ w, int has_norm, int act, long long rows,
+    int width, int steps, float* __restrict__ dx, float* __restrict__ grad_a, float* __restrict__ grad_b,
+    float* __restrict__ grad_w, float* __restrict__ grad_wb, float* __restrict__ dx_masked, DropSite site,
+    float* __restrict__ colsum_out, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
+    const int* __restrict__ rowmap) {
+  if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
   arb_pdl_wait();
   site.seed = drop_seed(site);
-  if (rows_dev) {
-    rows = min(rows, (long long)__ldg(rows_dev));
-    if ((long long)blockIdx.x * ROWS_PER_BLOCK * rows_per_warp >= rows) return;
-  }
-  __shared__ float sh[ROWS_PER_BLOCK][128 * NV + 4];
+  constexpr int RW = 32 / LPR;
+  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
+  if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;
+  __shared__ float sh[ROWS_PER_BLOCK][4 * LPR * NJ + 4];
   __shared__ float shb[ROWS_PER_BLOCK];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  RowRegs<NV> ga, gb, gw, acc_a, acc_b, acc_w, acc_c;
-  load_row<NV>(w, width, lane, gw);
-  if (has_norm) { load_row<NV>(a, width, lane, ga); load_row<NV>(b, width, lane, gb); }
-#pragma unroll
-  for (int k = 0; k < NV; ++k) acc_a.v[k] = acc_b.v[k] = acc_w.v[k] = acc_c.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, rg = lane / LPR;
+  float4 ga[NJ], gb[NJ], gw[NJ], acc_a[NJ], acc_b[NJ], acc_w[NJ], acc_c[NJ];
+  r_load<LPR>(w, width, lane, gw);
+  if (has_norm) { r_load<LPR>(a, width, lane, ga); r_load<LPR>(b, width, lane, gb); } else { r_zero(ga); r_zero(gb); }
+  r_zero(acc_a); r_zero(acc_b); r_zero(acc_w); r_zero(acc_c);
   float acc_wb = 0.f;
-  const long long first = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * rows_per_warp;
-  // The warp's rows go in batches of HB: the loads of a whole batch -- rows, row-map entries, statistics, then the
-  // scores and their gradients -- are issued before the first row's arithmetic (one row at a time left 12 KB in flight
-  // per SM at 73 registers).  Per-row arithmetic and accumulation order are unchanged.
-  constexpr int HB = NV <= 2 ? 2 : 1;
+  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * (RW * steps);
 #pragma unroll 1
-  for (int it0 = 0; it0 < rows_per_warp; it0 += HB) {
-    if (first + it0 >= rows) break;
-    RowRegs<NV> xb[HB];
-    long long atb[HB];
-    float meanb[HB], sdb[HB], outb[HB], dsb[HB];
-#pragma unroll
-    for (int q = 0; q < HB; ++q) {
-      const long long row = first + it0 + q;
-      const bool ok = it0 + q < rows_per_warp && row < rows;
-      atb[q] = -1;
-      meanb[q] = 0.f; sdb[q] = 1.f;
-      if (ok) {
-        load_row<NV>(x + row * width, width, lane, xb[q]);
-        // packed rows: score and its gradient sit at the item's place in the [B, S] tensors; alignment rows have neither
-        atb[q] = rowmap ? (long long)rowmap[row] : row;
-        if (has_norm) { meanb[q] = mean_i[row]; sdb[q] = std_i[row]; }
-      }
+  for (int s = 0; s < steps; ++s) {
+    if (base + (long long)s * RW >= rows) break;
+    const long long row = base + (long long)s * RW + rg;
+    const bool ok = row < rows;
+    float4 xr[NJ], g[NJ];
+    r_zero(xr);
+    long long at = -1;
+    float mean = 0.f, sd = 1.f;
+    if (ok) {
+      r_load<LPR>(x + row * width, width, lane, xr);
+      // packed rows: score and its gradient sit at the item's place in the [B, S] tensors; alignment rows have neither
+      at = rowmap ? (long long)rowmap[row] : row;
+      if (has_norm) { mean = mean_i[row]; sd = std_i[row]; }
     }
-#pragma unroll
-    for (int q = 0; q < HB; ++q) {
-      outb[q] = atb[q] >= 0 ? score[atb[q]] : 0.f;
-      dsb[q] = atb[q] >= 0 ? dscore[atb[q]] : 0.f;
-    }
-#pragma unroll
-    for (int q = 0; q < HB; ++q) {
-    const long long row = first + it0 + q;
-    if (it0 + q >= rows_per_warp || row >= rows) break;
-    RowRegs<NV>& xr = xb[q];
-    RowRegs<NV> g;
-    const float out = outb[q];
+    const float out = at >= 0 ? score[at] : 0.f;
     float z = 0.f;
     if (act == ARB_ACT_RELU) z = out;   // relu: out > 0 <=> z > 0
-    const float dz = atb[q] >= 0 ? dsb[q] * act_bwd(out, z, act) : 0.f;
-    if (lane == 0) acc_wb += dz;
+    const float dz = at >= 0 ? dscore[at] * act_bwd(out, z, act) : 0.f;
+    if (lane % LPR == 0) acc_wb += dz;
     if (!has_norm) {
 #pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        const float* xv = &xr.v[k].x;
-        const float* wv = &gw.v[k].x;
-        float* gv = &g.v[k].x;
-        float* aw = &acc_w.v[k].x;
+      for (int j = 0; j < NJ; ++j) {
+        const float* xv = &xr[j].x;
+        const float* wv = &gw[j].x;
+        float* gv = &g[j].x;
+        float* aw = &acc_w[j].x;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { gv[e] = dz * wv[e]; aw[e] += dz * xv[e]; }
+        for (int t = 0; t < 4; ++t) { gv[t] = dz * wv[t]; aw[t] += dz * xv[t]; }
       }
-      store_row<NV>(dx + row * width, width, lane, g);
-      if (dx_masked) { apply_drop<NV>(g, row, width, lane, site); store_row<NV>(dx_masked + row * width, width, lane, g); }
-      if (dy16_out) store_row_bf16<NV>(dy16_out + row * width, width, lane, g);
-      if (colsum_out) {
+    } else {
+      const float r = 1.0f / (sd + eps);
+      float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-        for (int k = 0; k < NV; ++k) {
-          acc_c.v[k].x += g.v[k].x; acc_c.v[k].y += g.v[k].y; acc_c.v[k].z += g.v[k].z; acc_c.v[k].w += g.v[k].w;
+      for (int j = 0; j < NJ; ++j) {
+        const bool in = ok && r_col<LPR>(lane, j) < width;
+        float* xv = &xr[j].x;
+        const float* wv = &gw[j].x;
+        const float* av = &ga[j].x;
+        const float* bv = &gb[j].x;
+        float* gv = &g[j].x;
+        float* aa = &acc_a[j].x;
+        float* ab = &acc_b[j].x;
+        float* aw = &acc_w[j].x;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const float cc = in ? xv[t] - mean : 0.f;
+          const float xh = cc * r;
+          const float xf = av[t] * xh + bv[t];     // the final norm's output, recomputed (xh = (x - mean) / (std + eps))
+          const float dyv = dz * wv[t];            // d loss / d xf
+          aw[t] += dz * xf;
+          aa[t] += dyv * xh;
+          ab[t] += dyv;
+          const float dxh = dyv * av[t];
+          gv[t] = dxh;
+          xv[t] = cc;
+          s1 += dxh;
+          s2 += dxh * cc;
         }
       }
-      continue;
-    }
-    const float mean = meanb[q], sd = sdb[q];
-    const float r = 1.0f / (sd + eps);
-    float s1 = 0.f, s2 = 0.f;
+      s1 = r_sum<LPR>(s1);
+      s2 = r_sum<LPR>(s2);
+      const float m1 = s1 / float(width);
+      const float coef = (sd > 0.f) ? r * r * s2 / (float(width - 1) * sd) : 0.f;
 #pragma unroll
-    for (int k = 0; k < NV; ++k) {
-      const int c = lane * 4 + 128 * k;
-      float* xv = &xr.v[k].x;
-      const float* wv = &gw.v[k].x;
-      const float* av = &ga.v[k].x;
-      const float* bv = &gb.v[k].x;
-      float* gv = &g.v[k].x;
-      float* aa = &acc_a.v[k].x;
-      float* ab = &acc_b.v[k].x;
-      float* aw = &acc_w.v[k].x;
+      for (int j = 0; j < NJ; ++j) {
+        float* gv = &g[j].x;
+        const float* xv = &xr[j].x;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float cc = (c < width) ? xv[e] - mean : 0.f;
-        const float xh = cc * r;
-        const float xf = av[e] * xh + bv[e];     // the final norm's output, recomputed (xh = (x - mean) / (std + eps))
-        const float dyv = dz * wv[e];          // d loss / d xf
-        aw[e] += dz * xf;
-        aa[e] += dyv * xh;
-        ab[e] += dyv;
-        const float dxh = dyv * av[e];
-        gv[e] = dxh;
-        xv[e] = cc;
-        s1 += dxh;
-        s2 += dxh * cc;
+        for (int t = 0; t < 4; ++t) gv[t] = r * (gv[t] - m1) - coef * xv[t];
       }
     }
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    const float m1 = s1 / float(width);
-    const float coef = (sd > 0.f) ? r * r * s2 / (float(width - 1) * sd) : 0.f;
+    if (ok) {
+      r_store<LPR>(dx + row * width, width, lane, g);
+      if (dx_masked) { r_drop<LPR>(g, row, width, lane, site); r_store<LPR>(dx_masked + row * width, width, lane, g); }
+      if (dy16_out) r_store_bf16<LPR>(dy16_out + row * width, width, lane, g);
+      if (colsum_out) {
 #pragma unroll
-    for (int k = 0; k < NV; ++k) {
-      float* gv = &g.v[k].x;
-      const float* xv = &xr.v[k].x;
-#pragma unroll
-      for (int e = 0; e < 4; ++e) gv[e] = r * (gv[e] - m1) - coef * xv[e];
-    }
-    store_row<NV>(dx + row * width, width, lane, g);
-    if (dx_masked) { apply_drop<NV>(g, row, width, lane, site); store_row<NV>(dx_masked + row * width, width, lane, g); }
-    if (dy16_out) store_row_bf16<NV>(dy16_out + row * width, width, lane, g);
-    if (colsum_out) {
-#pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        acc_c.v[k].x += g.v[k].x; acc_c.v[k].y += g.v[k].y; acc_c.v[k].z += g.v[k].z; acc_c.v[k].w += g.v[k].w;
+        for (int j = 0; j < NJ; ++j) { acc_c[j].x += g[j].x; acc_c[j].y += g[j].y; acc_c[j].z += g[j].z; acc_c[j].w += g[j].w; }
       }
     }
-    }
   }
-#pragma unroll
-  for (int pass = 0; pass < 4; ++pass) {
-    if (!has_norm && pass < 2) continue;
-    float* dst = pass == 0 ? grad_a : (pass == 1 ? grad_b : (pass == 2 ? grad_w : colsum_out));
-    if (!dst) continue;      // (no parameter gradients requested: the gradient outputs are null)
-    const RowRegs<NV>& src = pass == 0 ? acc_a : (pass == 1 ? acc_b : (pass == 2 ? acc_w : acc_c));
-#pragma unroll
-    for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = src.v[k];
-    __syncthreads();
-    for (int c = threadIdx.x; c < width; c += blockDim.x) {
-      float t = 0.f;
-#pragma unroll
-      for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += sh[ww][c];
-      dst[size_t(blockIdx.x) * width + c] = t;      // this block's slot (DetParts)
-    }
-    __syncthreads();
-  }
+  if (has_norm && grad_a) r_reduce_columns<LPR>(acc_a, sh, width, lane, wid, grad_a);
+  if (has_norm && grad_b) r_reduce_columns<LPR>(acc_b, sh, width, lane, wid, grad_b);
+  if (grad_w) r_reduce_columns<LPR>(acc_w, sh, width, lane, wid, grad_w);
+  if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, width, lane, wid, colsum_out);
   acc_wb = warp_sum(acc_wb);
   if (lane == 0) shb[wid] = acc_wb;
   __syncthreads();
@@ -858,13 +725,13 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_fwd_kernel(con
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5);
   if (row >= rows) return;
-  RowRegs<NV> r, gw;
-  load_row<NV>(xf + row * width, width, lane, r);
+  float4 r[NV], gw[NV];
+  r_load<32>(xf + row * width, width, lane, r);
   for (int j = 0; j < n; ++j) {
-    load_row<NV>(w + (long long)j * width, width, lane, gw);
+    r_load<32>(w + (long long)j * width, width, lane, gw);
     float dot = 0.f;
 #pragma unroll
-    for (int k = 0; k < NV; ++k) dot += r.v[k].x * gw.v[k].x + r.v[k].y * gw.v[k].y + r.v[k].z * gw.v[k].z + r.v[k].w * gw.v[k].w;
+    for (int k = 0; k < NV; ++k) dot += r[k].x * gw[k].x + r[k].y * gw[k].y + r[k].z * gw[k].z + r[k].w * gw[k].w;
     dot = warp_sum(dot);
     if (lane == 0) score[row * n + j] = act_fwd(dot + wb[j], act);
   }
@@ -883,31 +750,29 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
   __shared__ float shb[ROWS_PER_BLOCK];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const long long first = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * rows_per_warp;
-  RowRegs<NV> acc, gw;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) acc.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 acc[NV], gw[NV];
+  r_zero(acc);
   if (dx_masked) site.seed = drop_seed(site);   // (here rather than at entry: NV = 2 then spills)
   for (int it = 0; it < rows_per_warp; ++it) {
     const long long row = first + it;
     if (row >= rows) break;
-    RowRegs<NV> g;
-#pragma unroll
-    for (int k = 0; k < NV; ++k) g.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 g[NV];
+    r_zero(g);
     for (int j = 0; j < n; ++j) {
       const float out = score[row * n + j];
       const float dz = dscore[row * n + j] * act_bwd(out, out, act);   // relu: out > 0 <=> z > 0
-      load_row<NV>(w + (long long)j * width, width, lane, gw);
+      r_load<32>(w + (long long)j * width, width, lane, gw);
 #pragma unroll
       for (int k = 0; k < NV; ++k) {
-        g.v[k].x += dz * gw.v[k].x; g.v[k].y += dz * gw.v[k].y; g.v[k].z += dz * gw.v[k].z; g.v[k].w += dz * gw.v[k].w;
+        g[k].x += dz * gw[k].x; g[k].y += dz * gw[k].y; g[k].z += dz * gw[k].z; g[k].w += dz * gw[k].w;
       }
     }
-    store_row<NV>(dxf + row * width, width, lane, g);
-    if (dx_masked) { apply_drop<NV>(g, row, width, lane, site); store_row<NV>(dx_masked + row * width, width, lane, g); }
+    r_store<32>(dxf + row * width, width, lane, g);
+    if (dx_masked) { r_drop<32>(g, row, width, lane, site); r_store<32>(dx_masked + row * width, width, lane, g); }
     if (colsum_out) {
 #pragma unroll
       for (int k = 0; k < NV; ++k) {
-        acc.v[k].x += g.v[k].x; acc.v[k].y += g.v[k].y; acc.v[k].z += g.v[k].z; acc.v[k].w += g.v[k].w;
+        acc[k].x += g[k].x; acc[k].y += g[k].y; acc[k].z += g[k].z; acc[k].w += g[k].w;
       }
     }
   }
@@ -915,23 +780,22 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
   for (int j = colsum_out ? -1 : 0; j < (grad_w ? n : 0); ++j) {
     float acc_b = 0.f;
     if (j >= 0) {
-#pragma unroll
-      for (int k = 0; k < NV; ++k) acc.v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      r_zero(acc);
       for (int it = 0; it < rows_per_warp; ++it) {
         const long long row = first + it;
         if (row >= rows) break;
         const float out = score[row * n + j];
         const float dz = dscore[row * n + j] * act_bwd(out, out, act);
-        load_row<NV>(xf + row * width, width, lane, gw);
+        r_load<32>(xf + row * width, width, lane, gw);
         acc_b += dz;
 #pragma unroll
         for (int k = 0; k < NV; ++k) {
-          acc.v[k].x += dz * gw.v[k].x; acc.v[k].y += dz * gw.v[k].y; acc.v[k].z += dz * gw.v[k].z; acc.v[k].w += dz * gw.v[k].w;
+          acc[k].x += dz * gw[k].x; acc[k].y += dz * gw[k].y; acc[k].z += dz * gw[k].z; acc[k].w += dz * gw[k].w;
         }
       }
     }
 #pragma unroll
-    for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][lane * 4 + 128 * k]) = acc.v[k];
+    for (int k = 0; k < NV; ++k) *reinterpret_cast<float4*>(&sh[wid][r_col<32>(lane, k)]) = acc[k];
     if (lane == 0) shb[wid] = acc_b;
     __syncthreads();
     // this block's slots (DetParts): colsum_out [block][width], grad_w [block][n][width], grad_wb [block][n]
@@ -1056,6 +920,7 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
 // ------------------------------------------------------------------------------------------------ host launchers
 static int nv_for(int width) { return (width + 127) / 128; }
 
+// NV of the one-row-per-warp kernels (column sums, multi-output head)
 #define ARB_DISPATCH_NV(width, CALL)                                  \
   switch (nv_for(width)) {                                            \
     case 1: { constexpr int NV = 1; CALL; } break;                    \
@@ -1065,459 +930,28 @@ static int nv_for(int width) { return (width + 127) / 128; }
     default: arb_set_error("row kernels support widths up to 1024"); return ARB_E_UNSUPPORTED; \
   }
 
-// rows per warp of the backward row kernels (LayerNorm, head): more rows per warp = fewer block-level reductions and
-// block slots of the gain / bias gradients per byte moved.  ARB_ROWS_PER_WARP overrides (measurement knob).
-static int bwd_rows_per_warp() {
-  static int v = 0;
-  if (!v) {
-    const char* e = getenv("ARB_ROWS_PER_WARP");
-    v = e ? std::max(1, std::min(256, atoi(e))) : 8;
-  }
-  return v;
+// Returns f(LPR, NJ, FILLED) with std::integral_constant arguments: the row layout of the LayerNorm and head kernels
+// for `width`, and whether the width fills it.  A filled width is a compile-time constant of the kernel: its row
+// statistics then divide by a constant, as kernels written for one width do (a run-time divisor costs registers and
+// changes which products the compiler fuses into FMAs, and so the last bits of W = 128 / 256).
+template <class F>
+static int with_row_layout(int width, F&& f) {
+  using std::integral_constant;
+  auto layout = [&](auto LPR, auto NJ) {
+    if (width == 4 * LPR * NJ) return f(LPR, NJ, std::true_type());
+    return f(LPR, NJ, std::false_type());
+  };
+  if (width <= 128) return layout(integral_constant<int, 8>(), integral_constant<int, 4>());
+  if (width <= 256) return layout(integral_constant<int, 16>(), integral_constant<int, 4>());
+  if (width <= 512) return layout(integral_constant<int, 32>(), integral_constant<int, 4>());
+  if (width <= 1024) return layout(integral_constant<int, 32>(), integral_constant<int, 8>());
+  arb_set_error("row kernels support widths up to 1024");
+  return ARB_E_UNSUPPORTED;
 }
-
-
-// ------------------------------------------------------------------------------------------------ rows of 128 / 256
-// "R" layout of the row kernels for the common model widths W = 128 (LPR = 8 lanes per row, 4 rows per warp step)
-// and W = 256 (LPR = 16, 2 rows per step): a lane owns 16 elements of ONE row -- float4 j at column
-// ((lane % LPR) + LPR * j) * 4, so that the LPR lanes of a row read LPR * 16 contiguous bytes per instruction --
-// and a row reduction is log2(LPR) shuffle steps that serve all rows of the step at once (one row per warp needs five
-// steps per row and reduction: ncu put ln_fwd at 75 % issue-active with shuffles and their adds a third of it).
-// Same arithmetic per element as the generic kernels; the summation trees differ.
-template <int LPR>
-__device__ __forceinline__ int r_col(int lane, int j) { return ((lane % LPR) + LPR * j) * 4; }
-template <int LPR>
-__device__ __forceinline__ float r_sum(float v) {
-#pragma unroll
-  for (int off = 1; off < LPR; off <<= 1) v += __shfl_xor_sync(FULL, v, off);
-  return v;
-}
-template <int LPR>
-__device__ __forceinline__ void r_load(const float* __restrict__ row, int lane, float4 (&v)[4]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j) v[j] = *reinterpret_cast<const float4*>(row + r_col<LPR>(lane, j));
-}
-template <int LPR>
-__device__ __forceinline__ void r_load_bf16(const uint16_t* __restrict__ row, int lane, float4 (&v)[4]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const uint2 u = *reinterpret_cast<const uint2*>(row + r_col<LPR>(lane, j));
-    v[j] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
-                       __uint_as_float(u.y & 0xffff0000u));
-  }
-}
-template <int LPR>
-__device__ __forceinline__ void r_store(float* __restrict__ row, int lane, const float4 (&v)[4]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j) *reinterpret_cast<float4*>(row + r_col<LPR>(lane, j)) = v[j];
-}
-template <int LPR>
-__device__ __forceinline__ void r_store_bf16(uint16_t* __restrict__ row, int lane, const float4 (&v)[4]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    *reinterpret_cast<uint2*>(row + r_col<LPR>(lane, j)) = make_uint2(pack_bf16x2(v[j].x, v[j].y), pack_bf16x2(v[j].z, v[j].w));
-}
-__device__ __forceinline__ void r_zero(float4 (&v)[4]) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-}
-template <int LPR>
-__device__ __forceinline__ void r_drop(float4 (&v)[4], long long row, int lane, const DropSite& site) {
-  constexpr int W = 16 * LPR;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float* e = &v[j].x;
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const unsigned long long idx = (unsigned long long)row * W + (r_col<LPR>(lane, j) + t);
-      e[t] = drop_keep(idx, site.seed, site.thresh) ? e[t] * site.scale : 0.0f;
-    }
-  }
-}
-// sum the per-column accumulators of the warp's row groups, then over the block's warps, then into the block's slot of
-// `dst` (DetParts)
-template <int LPR>
-__device__ __forceinline__ void r_reduce_columns(float4 (&acc)[4], float (*sh)[16 * LPR + 4], int lane, int wid,
-                                                 float* __restrict__ dst) {
-  constexpr int W = 16 * LPR;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float* e = &acc[j].x;
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-#pragma unroll
-      for (int off = LPR; off < 32; off <<= 1) e[t] += __shfl_xor_sync(FULL, e[t], off);
-    }
-  }
-  if (lane < LPR) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) *reinterpret_cast<float4*>(&sh[wid][r_col<LPR>(lane, j)]) = acc[j];
-  }
-  __syncthreads();
-  for (int c = threadIdx.x; c < W; c += blockDim.x) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < ROWS_PER_BLOCK; ++w) t += sh[w][c];
-    dst[size_t(blockIdx.x) * W + c] = t;            // this block's slot (DetParts)
-  }
-  __syncthreads();
-}
-
-template <int LPR, bool MAP>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_r_kernel(const float* __restrict__ x,
-                                                                      const float* __restrict__ a,
-                                                                      const float* __restrict__ b, float eps,
-                                                                      long long rows, float* __restrict__ y,
-                                                                      float* __restrict__ mean_o,
-                                                                      float* __restrict__ std_o, int torch_mode,
-                                                                      uint16_t* __restrict__ y16,
-                                                                      const int* __restrict__ rows_dev, int steps,
-                                                                      const int* __restrict__ rowmap_out) {
-  arb_pdl_wait();
-  constexpr int RW = 32 / LPR, W = 16 * LPR;
-  const int lane = threadIdx.x & 31, rg = lane / LPR;
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (RW * steps);
-  if (base >= rows) return;
-  if (rows_dev) { rows = min(rows, (long long)__ldg(rows_dev)); if (base >= rows) return; }
-  float4 ga[4], gb[4], cur[4], nxt[4];
-  r_load<LPR>(a, lane, ga);
-  r_load<LPR>(b, lane, gb);
-  if (base + rg < rows) r_load<LPR>(x + (base + rg) * W, lane, cur); else r_zero(cur);
-#pragma unroll 1
-  for (int s = 0; s < steps; ++s) {
-    if (base + (long long)s * RW >= rows) break;
-    const long long row = base + (long long)s * RW + rg;
-    if (s + 1 < steps) { if (row + RW < rows) r_load<LPR>(x + (row + RW) * W, lane, nxt); else r_zero(nxt); }
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) sum += cur[j].x + cur[j].y + cur[j].z + cur[j].w;
-    const float m = r_sum<LPR>(sum) / float(W);
-    float ss = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
-      ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
-    }
-    ss = r_sum<LPR>(ss);
-    // (torch_mode and the reciprocal: see ln_fwd_kernel)
-    const float sdq = torch_mode ? sqrtf(ss / float(W) + eps) : sqrtf(ss / float(W - 1));
-    const float rinv = 1.0f / (torch_mode ? sdq : sdq + eps);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      cur[j].x = ga[j].x * (cur[j].x - m) * rinv + gb[j].x;
-      cur[j].y = ga[j].y * (cur[j].y - m) * rinv + gb[j].y;
-      cur[j].z = ga[j].z * (cur[j].z - m) * rinv + gb[j].z;
-      cur[j].w = ga[j].w * (cur[j].w - m) * rinv + gb[j].w;
-    }
-    if (row < rows) {
-      if (y16) r_store_bf16<LPR>(y16 + row * W, lane, cur);
-      else {   // (rowmap_out: see ln_fwd_kernel)
-        const long long yr = MAP ? (long long)rowmap_out[row] : row;
-        if (!MAP || yr >= 0) r_store<LPR>(y + yr * W, lane, cur);
-      }
-      if (lane % LPR == 0) { mean_o[row] = m; std_o[row] = sdq; }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) cur[j] = nxt[j];
-  }
-}
-
-template <int LPR, bool MAP>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) ln_bwd_r_kernel(
-    const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ a,
-    const float* __restrict__ mean_i, const float* __restrict__ std_i, float eps, const float* __restrict__ dres,
-    long long rows, int steps, float* __restrict__ dx, float* __restrict__ grad_a, float* __restrict__ grad_b,
-    float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out, int torch_mode,
-    const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
-    const int* __restrict__ rowmap_in) {
-  arb_pdl_wait();
-  site.seed = drop_seed(site);
-  constexpr int RW = 32 / LPR, W = 16 * LPR;
-  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
-  if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;      // whole block beyond the live rows
-  __shared__ float sh[ROWS_PER_BLOCK][W + 4];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, rg = lane / LPR;
-  float4 ga[4], acc_a[4], acc_b[4], acc_c[4];
-  r_load<LPR>(a, lane, ga);
-  r_zero(acc_a); r_zero(acc_b); r_zero(acc_c);
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * (RW * steps);
-#pragma unroll 1
-  for (int s = 0; s < steps; ++s) {
-    if (base + (long long)s * RW >= rows) break;
-    const long long row = base + (long long)s * RW + rg;
-    const bool ok = row < rows;
-    float4 g[4], xr[4], res[4];
-    float mean = 0.f, sd = 1.f;
-    r_zero(g); r_zero(xr); r_zero(res);
-    if (ok) {
-      if (dy16_in) r_load_bf16<LPR>(dy16_in + row * W, lane, g);
-      else if (MAP) { const long long src = rowmap_in[row]; if (src >= 0) r_load<LPR>(dy + src * W, lane, g); }
-      else r_load<LPR>(dy + row * W, lane, g);
-      r_load<LPR>(x + row * W, lane, xr);
-      if (dres) r_load<LPR>(dres + row * W, lane, res);
-      mean = mean_i[row]; sd = std_i[row];
-    }
-    const float r = 1.0f / (sd + eps);
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float* gv = &g[j].x;
-      float* xv = &xr[j].x;
-      const float* av = &ga[j].x;
-      float* aa = &acc_a[j].x;
-      float* ab = &acc_b[j].x;
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float cc = ok ? xv[t] - mean : 0.f;
-        const float dyv = gv[t];
-        aa[t] += dyv * cc * r;     // dy * xhat
-        ab[t] += dyv;
-        const float dxh = dyv * av[t];
-        gv[t] = dxh;
-        xv[t] = cc;
-        s1 += dxh;
-        s2 += dxh * cc;
-      }
-    }
-    s1 = r_sum<LPR>(s1);
-    s2 = r_sum<LPR>(s2);
-    const float m1 = s1 / float(W);
-    const float coef = torch_mode ? r * r * r * s2 / float(W) : ((sd > 0.f) ? r * r * s2 / (float(W - 1) * sd) : 0.f);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float* gv = &g[j].x;
-      const float* xv = &xr[j].x;
-      const float* rv = &res[j].x;
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        float o = r * (gv[t] - m1) - coef * xv[t];
-        if (dres) o += rv[t];
-        gv[t] = o;
-      }
-    }
-    if (ok) {
-      r_store<LPR>(dx + row * W, lane, g);
-      if (dx_masked) {   // the same gradient through the dropout of the sublayer below (mask regenerated)
-        r_drop<LPR>(g, row, lane, site);
-        r_store<LPR>(dx_masked + row * W, lane, g);
-      }
-      if (dy16_out) r_store_bf16<LPR>(dy16_out + row * W, lane, g);
-      if (colsum_out) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { acc_c[j].x += g[j].x; acc_c[j].y += g[j].y; acc_c[j].z += g[j].z; acc_c[j].w += g[j].w; }
-      }
-    }
-  }
-  if (grad_a) r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
-  if (grad_b) r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
-  if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, lane, wid, colsum_out);
-}
-
-template <int LPR>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_fwd_r_kernel(
-    const float* __restrict__ x, const float* __restrict__ a, const float* __restrict__ b, float eps,
-    const float* __restrict__ w, const float* __restrict__ wb, int has_norm, int act, long long rows,
-    float* __restrict__ score, float* __restrict__ mean_o, float* __restrict__ std_o,
-    const int* __restrict__ rows_dev, const int* __restrict__ rowmap, int steps) {
-  arb_pdl_wait();
-  constexpr int RW = 32 / LPR, W = 16 * LPR;
-  const int lane = threadIdx.x & 31, rg = lane / LPR;
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5)) * (RW * steps);
-  if (base >= rows) return;
-  if (rows_dev) { rows = min(rows, (long long)__ldg(rows_dev)); if (base >= rows) return; }
-  float4 ga[4], gb[4], gw[4], cur[4], nxt[4];
-  r_load<LPR>(w, lane, gw);
-  if (has_norm) { r_load<LPR>(a, lane, ga); r_load<LPR>(b, lane, gb); } else { r_zero(ga); r_zero(gb); }
-  const float bias = wb[0];
-  long long at = -1, at_n = -1;
-  if (base + rg < rows) {
-    r_load<LPR>(x + (base + rg) * W, lane, cur);
-    at = rowmap ? (long long)rowmap[base + rg] : base + rg;
-  } else {
-    r_zero(cur);
-  }
-#pragma unroll 1
-  for (int s = 0; s < steps; ++s) {
-    if (base + (long long)s * RW >= rows) break;
-    const long long row = base + (long long)s * RW + rg;
-    if (s + 1 < steps) {
-      at_n = -1;
-      if (row + RW < rows) {
-        r_load<LPR>(x + (row + RW) * W, lane, nxt);
-        at_n = rowmap ? (long long)rowmap[row + RW] : row + RW;
-      } else {
-        r_zero(nxt);
-      }
-    }
-    float m = 0.f, sdv = 0.f;
-    if (has_norm) {
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) sum += cur[j].x + cur[j].y + cur[j].z + cur[j].w;
-      m = r_sum<LPR>(sum) / float(W);
-      float ss = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
-        ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
-      }
-      sdv = sqrtf(r_sum<LPR>(ss) / float(W - 1));
-      const float rinv = 1.0f / (sdv + eps);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        cur[j].x = ga[j].x * (cur[j].x - m) * rinv + gb[j].x;
-        cur[j].y = ga[j].y * (cur[j].y - m) * rinv + gb[j].y;
-        cur[j].z = ga[j].z * (cur[j].z - m) * rinv + gb[j].z;
-        cur[j].w = ga[j].w * (cur[j].w - m) * rinv + gb[j].w;
-      }
-    }
-    float dot = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) dot += cur[j].x * gw[j].x + cur[j].y * gw[j].y + cur[j].z * gw[j].z + cur[j].w * gw[j].w;
-    dot = r_sum<LPR>(dot);
-    if (row < rows && lane % LPR == 0) {
-      // packed rows: the score goes to the item's place in the [B, S] tensor (alignment rows have none)
-      if (at >= 0) score[at] = act_fwd(dot + bias, act);
-      if (has_norm && mean_o) { mean_o[row] = m; std_o[row] = sdv; }
-    }
-    at = at_n;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) cur[j] = nxt[j];
-  }
-}
-
-template <int LPR>
-__global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, 2) head_bwd_r_kernel(
-    const float* __restrict__ dscore, const float* __restrict__ score, const float* __restrict__ x,
-    const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ mean_i,
-    const float* __restrict__ std_i, float eps, const float* __restrict__ w, int has_norm, int act, long long rows,
-    int steps, float* __restrict__ dx, float* __restrict__ grad_a, float* __restrict__ grad_b,
-    float* __restrict__ grad_w, float* __restrict__ grad_wb, float* __restrict__ dx_masked, DropSite site,
-    float* __restrict__ colsum_out, uint16_t* __restrict__ dy16_out, const int* __restrict__ rows_dev,
-    const int* __restrict__ rowmap) {
-  arb_pdl_wait();
-  site.seed = drop_seed(site);
-  constexpr int RW = 32 / LPR, W = 16 * LPR;
-  if (rows_dev) rows = min(rows, (long long)__ldg(rows_dev));
-  if ((long long)blockIdx.x * ROWS_PER_BLOCK * RW * steps >= rows) return;
-  __shared__ float sh[ROWS_PER_BLOCK][W + 4];
-  __shared__ float shb[ROWS_PER_BLOCK];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, rg = lane / LPR;
-  float4 ga[4], gb[4], gw[4], acc_a[4], acc_b[4], acc_w[4], acc_c[4];
-  r_load<LPR>(w, lane, gw);
-  if (has_norm) { r_load<LPR>(a, lane, ga); r_load<LPR>(b, lane, gb); } else { r_zero(ga); r_zero(gb); }
-  r_zero(acc_a); r_zero(acc_b); r_zero(acc_w); r_zero(acc_c);
-  float acc_wb = 0.f;
-  const long long base = ((long long)blockIdx.x * ROWS_PER_BLOCK + wid) * (RW * steps);
-#pragma unroll 1
-  for (int s = 0; s < steps; ++s) {
-    if (base + (long long)s * RW >= rows) break;
-    const long long row = base + (long long)s * RW + rg;
-    const bool ok = row < rows;
-    float4 xr[4], g[4];
-    r_zero(xr);
-    long long at = -1;
-    float mean = 0.f, sd = 1.f;
-    if (ok) {
-      r_load<LPR>(x + row * W, lane, xr);
-      // packed rows: score and its gradient sit at the item's place in the [B, S] tensors; alignment rows have neither
-      at = rowmap ? (long long)rowmap[row] : row;
-      if (has_norm) { mean = mean_i[row]; sd = std_i[row]; }
-    }
-    const float out = at >= 0 ? score[at] : 0.f;
-    float z = 0.f;
-    if (act == ARB_ACT_RELU) z = out;   // relu: out > 0 <=> z > 0
-    const float dz = at >= 0 ? dscore[at] * act_bwd(out, z, act) : 0.f;
-    if (lane % LPR == 0) acc_wb += dz;
-    if (!has_norm) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float* xv = &xr[j].x;
-        const float* wv = &gw[j].x;
-        float* gv = &g[j].x;
-        float* aw = &acc_w[j].x;
-#pragma unroll
-        for (int t = 0; t < 4; ++t) { gv[t] = dz * wv[t]; aw[t] += dz * xv[t]; }
-      }
-    } else {
-      const float r = 1.0f / (sd + eps);
-      float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float* xv = &xr[j].x;
-        const float* wv = &gw[j].x;
-        const float* av = &ga[j].x;
-        const float* bv = &gb[j].x;
-        float* gv = &g[j].x;
-        float* aa = &acc_a[j].x;
-        float* ab = &acc_b[j].x;
-        float* aw = &acc_w[j].x;
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float cc = ok ? xv[t] - mean : 0.f;
-          const float xh = cc * r;
-          const float xf = av[t] * xh + bv[t];     // the final norm's output, recomputed
-          const float dyv = dz * wv[t];            // d loss / d xf
-          aw[t] += dz * xf;
-          aa[t] += dyv * xh;
-          ab[t] += dyv;
-          const float dxh = dyv * av[t];
-          gv[t] = dxh;
-          xv[t] = cc;
-          s1 += dxh;
-          s2 += dxh * cc;
-        }
-      }
-      s1 = r_sum<LPR>(s1);
-      s2 = r_sum<LPR>(s2);
-      const float m1 = s1 / float(W);
-      const float coef = (sd > 0.f) ? r * r * s2 / (float(W - 1) * sd) : 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float* gv = &g[j].x;
-        const float* xv = &xr[j].x;
-#pragma unroll
-        for (int t = 0; t < 4; ++t) gv[t] = r * (gv[t] - m1) - coef * xv[t];
-      }
-    }
-    if (ok) {
-      r_store<LPR>(dx + row * W, lane, g);
-      if (dx_masked) { r_drop<LPR>(g, row, lane, site); r_store<LPR>(dx_masked + row * W, lane, g); }
-      if (dy16_out) r_store_bf16<LPR>(dy16_out + row * W, lane, g);
-      if (colsum_out) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { acc_c[j].x += g[j].x; acc_c[j].y += g[j].y; acc_c[j].z += g[j].z; acc_c[j].w += g[j].w; }
-      }
-    }
-  }
-  if (has_norm && grad_a) r_reduce_columns<LPR>(acc_a, sh, lane, wid, grad_a);
-  if (has_norm && grad_b) r_reduce_columns<LPR>(acc_b, sh, lane, wid, grad_b);
-  if (grad_w) r_reduce_columns<LPR>(acc_w, sh, lane, wid, grad_w);
-  if (colsum_out) r_reduce_columns<LPR>(acc_c, sh, lane, wid, colsum_out);
-  acc_wb = warp_sum(acc_wb);
-  if (lane == 0) shb[wid] = acc_wb;
-  __syncthreads();
-  if (threadIdx.x == 0 && grad_wb) {
-    float t = 0.f;
-    for (int ww = 0; ww < ROWS_PER_BLOCK; ++ww) t += shb[ww];
-    grad_wb[blockIdx.x] = t;                        // this block's slot (DetParts)
-  }
-}
-
-// Which row kernels use the layout above for W = 128 / 256 (else the generic one-row-per-warp kernels): bit 0 ln_fwd,
-// bit 1 ln_bwd, bit 2 head_fwd, bit 3 head_bwd.  ARB_ROW_LAYOUT overrides (measurement knob).
-enum { R_LN_FWD = 1, R_LN_BWD = 2, R_HEAD_FWD = 4, R_HEAD_BWD = 8 };
-static int row_layout_r() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ARB_ROW_LAYOUT"); v = e ? atoi(e) : ARB_DEFAULT_ROW_LAYOUT; }
-  return v;
-}
-static inline int r_lpr(int width, int which) {
-  return ((row_layout_r() & which) && (width == 128 || width == 256)) ? width / 16 : 0;
-}
-// steps per warp of the forward R kernels: 4 (16 / 8 rows per warp) for large launches, 1 for small ones
+// steps per warp of the forward row kernels: 4 for large launches, 1 for small ones (more steps would leave SMs without
+// a block -- B = 64 has 8 k live rows)
 static inline int r_fwd_steps(long long rows) { return rows >= (1 << 17) ? 4 : 1; }
-// rows per warp of the backward R kernels (a multiple of 4): the per-warp column reduction at the end costs 2 shuffles
+// rows per warp of the backward row kernels (a multiple of 4): the per-warp column reduction at the end costs 2 shuffles
 // per accumulator element, so large launches amortise it over 32 rows; small ones keep every SM busy with 8
 static inline int r_bwd_rows_per_warp(long long rows) { return rows >= (1 << 17) ? 32 : 8; }
 
@@ -1667,18 +1101,13 @@ int ln_forward(const float* x, const float* a, const float* b, float eps, long l
   if (rowmap_out && y16) { arb_set_error("ln_forward: a row-mapped output is fp32 only"); return ARB_E_INVALID_ARG; }
   if (width % 4) { arb_set_error("LayerNorm width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * ((y16 ? 6.0 : 8.0) * width + 8), st);
-  if (const int lpr = r_lpr(width, R_LN_FWD)) {      // W = 128 / 256: several rows per warp step (see ln_fwd_r_kernel)
-    const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
+  return with_row_layout(width, [&](auto LPR, auto NJ, auto FILLED) {
+    const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / LPR) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    if (lpr == 8) return launch(rowmap_out ? ln_fwd_r_kernel<8, true> : ln_fwd_r_kernel<8, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
-    return launch(rowmap_out ? ln_fwd_r_kernel<16, true> : ln_fwd_r_kernel<16, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
-  }
-  const int nb = fwd_batches_for(width, rows);
-  const int per_block = ROWS_PER_BLOCK * FWD_RPW * nb;
-  const unsigned blocks = unsigned((rows + per_block - 1) / per_block);
-  int rc;
-  ARB_DISPATCH_NV(width, (rc = launch(rowmap_out ? ln_fwd_kernel<NV, true> : ln_fwd_kernel<NV, false>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode, static_cast<uint16_t*>(y16), rows_dev, nb, rowmap_out)));
-  return rc;
+    return launch(rowmap_out ? ln_fwd_kernel<LPR, NJ, FILLED, true> : ln_fwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
+                  dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode,
+                  static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
+  });
 }
 
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
@@ -1690,24 +1119,20 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
   if (dy16_out && dx_masked == nullptr && (site.thresh != 0 || site.scale != 1.0f)) {
     arb_set_error("ln_backward: a masked bf16 copy needs the masked fp32 buffer too"); return ARB_E_INVALID_ARG;
   }   // thresh 0 with a scale = pure rescale (positional encoding)
-  const int rpw = bwd_rows_per_warp();
-  const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * ((dres ? 16.0 : 12.0) * width + 8), st);
-  const int lpr = r_lpr(width, R_LN_BWD);
-  const int steps = lpr ? r_bwd_rows_per_warp(rows) / (32 / lpr) : 0;
-  const unsigned nblk = lpr ? unsigned((rows + ROWS_PER_BLOCK * (32 / lpr) * steps - 1) / (ROWS_PER_BLOCK * (32 / lpr) * steps)) : blocks;
-  DetParts dp;
-  dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width);
-  int rc = dp.begin(st);
-  if (rc) return rc;
-  if (lpr) {
-    if (lpr == 8) rc = launch(rowmap_in ? ln_bwd_r_kernel<8, true> : ln_bwd_r_kernel<8, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in);
-    else rc = launch(rowmap_in ? ln_bwd_r_kernel<16, true> : ln_bwd_r_kernel<16, false>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in);
-  } else {
-    ARB_DISPATCH_NV(width, (rc = launch(rowmap_in ? ln_bwd_kernel<NV, true> : ln_bwd_kernel<NV, false>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width, rpw, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode, static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in)));
-  }
-  if (rc) return rc;
-  return dp.finish(st);
+  return with_row_layout(width, [&](auto LPR, auto NJ, auto FILLED) {
+    const int steps = r_bwd_rows_per_warp(rows) / (32 / LPR), per_block = ROWS_PER_BLOCK * (32 / LPR) * steps;
+    const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
+    DetParts dp;
+    dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width);
+    if (int rc = dp.begin(st)) return rc;
+    if (int rc = launch(rowmap_in ? ln_bwd_kernel<LPR, NJ, FILLED, true> : ln_bwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
+                        dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width,
+                        steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode,
+                        static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in))
+      return rc;
+    return dp.finish(st);
+  });
 }
 
 int pos_forward(float* x, const long long* indices, const uint8_t* mask, const float* pe, int pe_rows, float scale,
@@ -1803,18 +1228,12 @@ int head_forward(const float* x, const float* a, const float* b, float eps, cons
                  cudaStream_t st, const int* rows_dev, const int* rowmap) {
   if (width % 4) { arb_set_error("model width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * (4.0 * width + 12), st);
-  if (const int lpr = r_lpr(width, R_HEAD_FWD)) {
-    const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / lpr) * steps;
+  return with_row_layout(width, [&](auto LPR, auto NJ, auto FILLED) {
+    const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / LPR) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    if (lpr == 8) return launch(head_fwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
-    return launch(head_fwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, score, mean, sd, rows_dev, rowmap, steps);
-  }
-  const int nb = fwd_batches_for(width, rows);
-  const int per_block = ROWS_PER_BLOCK * FWD_RPW * nb;
-  const unsigned blocks = unsigned((rows + per_block - 1) / per_block);
-  int rc;
-  ARB_DISPATCH_NV(width, (rc = launch(head_fwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, w, wb, has_norm, act, rows, width, score, mean, sd, rows_dev, rowmap, nb)));
-  return rc;
+    return launch(head_fwd_kernel<LPR, NJ, FILLED>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps,
+                  w, wb, has_norm, act, rows, width, score, mean, sd, rows_dev, rowmap, steps);
+  });
 }
 
 int head_backward(const float* dscore, const float* score, const float* x, const float* a, const float* b,
@@ -1823,25 +1242,20 @@ int head_backward(const float* dscore, const float* score, const float* x, const
                   float* grad_wb, cudaStream_t st, float* dx_masked, DropSite site, float* colsum_out, void* dy16_out,
                   const int* rows_dev, const int* rowmap) {
   if (site.thresh == 0) dx_masked = nullptr;
-  const int rpw = bwd_rows_per_warp();
-  const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * (8.0 * width + 16), st);
-  const int lpr = r_lpr(width, R_HEAD_BWD);
-  const int steps = lpr ? r_bwd_rows_per_warp(rows) / (32 / lpr) : 0;
-  const unsigned nblk = lpr ? unsigned((rows + ROWS_PER_BLOCK * (32 / lpr) * steps - 1) / (ROWS_PER_BLOCK * (32 / lpr) * steps)) : blocks;
-  DetParts dp;
-  if (has_norm) { dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); }
-  dp.add(grad_w, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width); dp.add(grad_wb, nblk, 1, 1, 1);
-  int rc = dp.begin(st);
-  if (rc) return rc;
-  if (lpr) {
-    if (lpr == 8) rc = launch(head_bwd_r_kernel<8>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
-    else rc = launch(head_bwd_r_kernel<16>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, has_norm, act, rows, steps, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap);
-  } else {
-    ARB_DISPATCH_NV(width, (rc = launch(head_bwd_kernel<NV>, dim3(blocks), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore, score, x, a, b, mean, sd, eps, w, wb, has_norm, act, rows, width, rpw, dx, grad_a, grad_b, grad_w, grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap)));
-  }
-  if (rc) return rc;
-  return dp.finish(st);
+  return with_row_layout(width, [&](auto LPR, auto NJ, auto FILLED) {
+    const int steps = r_bwd_rows_per_warp(rows) / (32 / LPR), per_block = ROWS_PER_BLOCK * (32 / LPR) * steps;
+    const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
+    DetParts dp;
+    if (has_norm) { dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); }
+    dp.add(grad_w, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width); dp.add(grad_wb, nblk, 1, 1, 1);
+    if (int rc = dp.begin(st)) return rc;
+    if (int rc = launch(head_bwd_kernel<LPR, NJ, FILLED>, dim3(nblk), dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dscore,
+                        score, x, a, b, mean, sd, eps, w, has_norm, act, rows, width, steps, dx, grad_a, grad_b, grad_w,
+                        grad_wb, dx_masked, site, colsum_out, static_cast<uint16_t*>(dy16_out), rows_dev, rowmap))
+      return rc;
+    return dp.finish(st);
+  });
 }
 
 int head_multi_forward(const float* xf, const float* w, const float* wb, int act, long long rows, int width, int n,
@@ -1858,7 +1272,7 @@ int head_multi_backward(const float* dscore, const float* score, const float* xf
                         long long rows, int width, int n, float* dxf, float* grad_w, float* grad_wb, cudaStream_t st,
                         float* dx_masked, DropSite site, float* colsum_out) {
   if (site.thresh == 0) dx_masked = nullptr;
-  const int rpw = bwd_rows_per_warp();
+  const int rpw = 8;    // rows per warp: more = fewer block slots of grad_w per byte moved
   const unsigned blocks = unsigned((rows + ROWS_PER_BLOCK * rpw - 1) / (ROWS_PER_BLOCK * rpw));
   ProfScope ps(ARB_PROF_SCORER_SIMT, double(rows) * (8.0 * width + 8.0 * n), st);
   DetParts dp;

@@ -16,6 +16,12 @@ CASES = [
     (20, [24, 32], "ReLU", False, 2, 2, 64, ("fixed", 15), 1, "Tanh"),
     (20, [40, 32], "Tanh", False, 1, 2, 64, ("learned", 15), 1, None),
     (20, [32, 32, 32, 32], None, True, 1, 4, 32, None, 1, None),
+    # widths of each row layout of the LayerNorm and head kernels beyond 256, and a ragged one below: d_model 300,
+    # input_norm over F = 300 in front of d_model 200, input_norm over F = 1000 and a head over 1000 (FC only: an
+    # encoder's QKV bias gradient is limited to 3 * d_model <= 1024 columns)
+    (20, [300], "ReLU", False, 1, 3, 64, None, 1, None),
+    (300, [200], "Tanh", True, 1, 2, 64, None, 1, None),
+    (1000, [1000], "ReLU", True, 0, 1, 4, None, 1, None),
 ]
 
 
