@@ -72,7 +72,9 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// until at most N of this thread's most recent store groups still read their shared-memory source
+template <int N = 0>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
 // two fp32 -> packed bf16x2 (round to nearest even); `lo` lands in the low half
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
