@@ -6,6 +6,7 @@
 // row; coalesced 128-bit accesses where the width allows, warp-shuffle reductions; they are HBM-bound (DESIGN.md
 // section 3 lists bytes per row).
 #include <cstdint>
+#include <string>
 #include <type_traits>
 #include <cuda_runtime.h>
 
@@ -1286,3 +1287,111 @@ int head_multi_backward(const float* dscore, const float* score, const float* xf
 }
 
 }  // namespace arb
+
+// ------------------------------------------------------------------------------------------------ test entry points
+// The row kernels on their own (include/allrank_b200.h): argument checks, then the launchers above, so that the steps
+// per warp, the row layout and the DetParts slots are the ones the scorer gets for the same row count.
+using namespace arb;
+
+static int row_args(const char* what, bool ptrs_ok, long long rows, int width, float p) {
+  if (!ptrs_ok) { arb_set_error((std::string(what) + ": null pointer").c_str()); return ARB_E_INVALID_ARG; }
+  if (rows < 0) { arb_set_error((std::string(what) + ": rows must be >= 0").c_str()); return ARB_E_INVALID_ARG; }
+  if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
+  if (width <= 0 || width % 4 || width > 1024) {
+    arb_set_error((std::string(what) + ": the width must be a positive multiple of 4, at most 1024").c_str());
+    return ARB_E_UNSUPPORTED;
+  }
+  return ARB_OK;
+}
+#define ARB_ROW_ARGS(what, ptrs_ok, rows, width, p) \
+  do { if (int rc__ = row_args(what, ptrs_ok, rows, width, p)) return rc__; if ((rows) == 0) return ARB_OK; } while (0)
+
+static DropSite test_site(uint64_t seed, int layer, int site, float p) {
+  return make_drop_site(CallSeed{seed, nullptr}, layer, site, p);
+}
+
+extern "C" int32_t arb_layernorm_forward(const float* x, const float* a, const float* b, float eps, int32_t torch_mode,
+                                         int64_t rows, int32_t width, float* y, void* y16, float* mean, float* sd,
+                                         const int32_t* rows_dev, const int32_t* rowmap, void* stream) {
+  ARB_ROW_ARGS("arb_layernorm_forward", x && a && b && (y || y16) && mean && sd, rows, width, 0.0f);
+  return ln_forward(x, a, b, eps, rows, width, y, mean, sd, static_cast<cudaStream_t>(stream), torch_mode, y16,
+                    rows_dev, rowmap);
+}
+
+extern "C" int32_t arb_layernorm_backward(const float* dy, const void* dy16_in, const float* x, const float* a,
+                                          const float* mean, const float* sd, float eps, int32_t torch_mode,
+                                          const float* dres, int64_t rows, int32_t width, float* dx, float* grad_a,
+                                          float* grad_b, float* dx_masked, void* dy16_out, float* colsum_out, float p,
+                                          uint64_t seed, int32_t layer, int32_t site, const int32_t* rows_dev,
+                                          const int32_t* rowmap, void* stream) {
+  ARB_ROW_ARGS("arb_layernorm_backward", (dy || dy16_in) && x && a && mean && sd && dx, rows, width, p);
+  return ln_backward(dy, x, a, mean, sd, eps, dres, rows, width, dx, grad_a, grad_b, static_cast<cudaStream_t>(stream),
+                     dx_masked, test_site(seed, layer, site, p), colsum_out, torch_mode, dy16_in, dy16_out, rows_dev,
+                     rowmap);
+}
+
+extern "C" int32_t arb_head_forward(const float* x, const float* a, const float* b, float eps, const float* w,
+                                    const float* wb, int32_t has_norm, int32_t act, int64_t rows, int32_t width,
+                                    float* score, float* mean, float* sd, const int32_t* rows_dev,
+                                    const int32_t* rowmap, void* stream) {
+  ARB_ROW_ARGS("arb_head_forward", x && w && wb && score && (!has_norm || (a && b)) && !mean == !sd, rows, width, 0.0f);
+  return head_forward(x, a, b, eps, w, wb, has_norm, act, rows, width, score, mean, sd,
+                      static_cast<cudaStream_t>(stream), rows_dev, rowmap);
+}
+
+extern "C" int32_t arb_head_backward(const float* dscore, const float* score, const float* x, const float* a,
+                                     const float* b, const float* mean, const float* sd, float eps, const float* w,
+                                     int32_t has_norm, int32_t act, int64_t rows, int32_t width, float* dx,
+                                     float* grad_a, float* grad_b, float* grad_w, float* grad_wb, float* dx_masked,
+                                     void* dy16_out, float* colsum_out, float p, uint64_t seed, int32_t layer,
+                                     int32_t site, const int32_t* rows_dev, const int32_t* rowmap, void* stream) {
+  ARB_ROW_ARGS("arb_head_backward",
+               dscore && score && x && w && dx && (!has_norm || (a && b && mean && sd)),
+               rows, width, p);
+  return head_backward(dscore, score, x, a, b, mean, sd, eps, w, nullptr, has_norm, act, rows, width, dx, grad_a,
+                       grad_b, grad_w, grad_wb, static_cast<cudaStream_t>(stream), dx_masked,
+                       test_site(seed, layer, site, p), colsum_out, dy16_out, rows_dev, rowmap);
+}
+
+extern "C" int32_t arb_head_multi_forward(const float* xf, const float* w, const float* wb, int32_t act, int64_t rows,
+                                          int32_t width, int32_t n, float* score, void* stream) {
+  ARB_ROW_ARGS("arb_head_multi_forward", xf && w && wb && score && n >= 1, rows, width, 0.0f);
+  return head_multi_forward(xf, w, wb, act, rows, width, n, score, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int32_t arb_head_multi_backward(const float* dscore, const float* score, const float* xf, const float* w,
+                                           int32_t act, int64_t rows, int32_t width, int32_t n, float* dxf,
+                                           float* grad_w, float* grad_wb, float* dx_masked, float* colsum_out, float p,
+                                           uint64_t seed, int32_t layer, int32_t site, void* stream) {
+  ARB_ROW_ARGS("arb_head_multi_backward",
+               dscore && score && xf && w && dxf && n >= 1 && !grad_w == !grad_wb, rows, width, p);
+  return head_multi_backward(dscore, score, xf, w, act, rows, width, n, dxf, grad_w, grad_wb,
+                             static_cast<cudaStream_t>(stream), dx_masked, test_site(seed, layer, site, p), colsum_out);
+}
+
+extern "C" int32_t arb_column_sums(const float* in, int64_t rows, int32_t width, int64_t ld, float* out, void* stream) {
+  ARB_ROW_ARGS("arb_column_sums", in && out && ld >= width, rows, width, 0.0f);
+  return colsum_accumulate(in, rows, width, ld, out, static_cast<cudaStream_t>(stream));
+}
+
+static int softmax_args(const char* what, bool ptrs_ok, int S, int pitch, float p) {
+  if (!ptrs_ok) { arb_set_error((std::string(what) + ": null pointer or no rows").c_str()); return ARB_E_INVALID_ARG; }
+  if (S <= 0 || pitch < S) { arb_set_error((std::string(what) + ": S >= 1 and pitch >= S").c_str()); return ARB_E_INVALID_ARG; }
+  if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
+  return ARB_OK;
+}
+
+extern "C" int32_t arb_softmax_forward(float* scores, const uint8_t* mask, int32_t B, int32_t h, int32_t S,
+                                       int32_t pitch, float p, uint64_t seed, int32_t layer, void* stream) {
+  if (int rc = softmax_args("arb_softmax_forward", scores && mask && B >= 1 && h >= 1, S, pitch, p))
+    return rc;
+  return softmax_forward(scores, mask, B, h, S, pitch, static_cast<cudaStream_t>(stream),
+                         test_site(seed, layer, SITE_ATTN_P, p));
+}
+
+extern "C" int32_t arb_softmax_backward(float* dprob, float* prob, int64_t rows, int32_t S, int32_t pitch, float p,
+                                        uint64_t seed, int32_t layer, void* stream) {
+  if (int rc = softmax_args("arb_softmax_backward", dprob && prob && rows >= 1, S, pitch, p)) return rc;
+  return softmax_backward(dprob, prob, rows, S, pitch, static_cast<cudaStream_t>(stream),
+                          test_site(seed, layer, SITE_ATTN_P, p));
+}

@@ -353,6 +353,57 @@ int32_t arb_attention_backward(const float* qkv, const void* ctx, int32_t ctx_bf
                                uint64_t seed, int32_t layer, void* d_qkv, float* dbias_qkv, float* delta_scratch,
                                void* stream);
 
+/* Building blocks exposed for tests: the SIMT row kernels (csrc/scorer_kernels.cu), launched by the scorer's own
+ * launchers, so that the steps per warp, the row layout and the reduction slots depend on `rows` as in the scorer
+ * (launches of 2^17 rows or more take the large-launch path).  Rows are `width` floats apart; width is a multiple of 4,
+ * at most 1024 (else ARB_E_UNSUPPORTED).  Nullable arguments: y16, dy16_in, dy16_out, dres, dx_masked, colsum_out, the
+ * gradient outputs grad_*, rows_dev and rowmap (both device int32); a null output is not computed.
+ *   - Gradients and column sums are ACCUMULATED: grad_*, colsum_out and the multi-head grad_w / grad_wb += their sums.
+ *   - rows_dev: rows at or beyond *rows_dev (live rows <= rows) are not read and not written.
+ *   - rowmap [rows]: layer norm forward writes row r to y[rowmap[r]], its backward reads dy[rowmap[r]]; the head reads
+ *     and writes score / dscore [rowmap[r]].  rowmap[r] < 0: no destination, or a zero gradient.  fp32 rows only.
+ *   - Dropout with rate p uses make_drop_site(seed, layer, site) as the scorer does; the row kernels' element counter
+ *     is row * width + column.  dx_masked = dx through that mask (not written when p = 0); dy16_out is the bfloat16
+ *     copy (nearest even) of dx_masked, or of dx when p = 0; dy16_in replaces dy with bfloat16 values.
+ *   - torch_mode: nn.LayerNorm (biased variance, eps under the root); sd receives sqrt(var + eps), and the backward is
+ *     then called with eps = 0 as the scorer calls it.  Otherwise the reference's LayerNorm (unbiased std, eps added to
+ *     the std).  A row with sd = 0 (a constant row) gets y = b, and in the backward the std term of dx is 0.
+ *   - act: ARB_ACT_*; has_norm = 0 is the FC-only head score = act(w . x + wb[0]).
+ *   - the multi-output head: score [rows, n] = act(xf w^T + wb), w [n, width]; grad_w and grad_wb both or neither.
+ * Softmax: in place on scores [B, h, S] rows of `pitch` >= S floats (S <= 1536, else ARB_E_UNSUPPORTED), keys with
+ * mask [B, S] = 1 get probability 0, an all-masked slate gets NaN rows.  Dropout on the probabilities with the
+ * attention site of `layer`, counter row * S + key (independent of pitch), as in the fused kernels.  The backward
+ * turns dprob (the gradient w.r.t. the dropped probabilities) into dS = P (dP - sum P dP) in place and overwrites
+ * prob (the undropped P) with the dropped probabilities.  Columns from S to pitch are neither read nor written. */
+int32_t arb_layernorm_forward(const float* x, const float* a, const float* b, float eps, int32_t torch_mode,
+                              int64_t rows, int32_t width, float* y, void* y16, float* mean, float* sd,
+                              const int32_t* rows_dev, const int32_t* rowmap, void* stream);
+int32_t arb_layernorm_backward(const float* dy, const void* dy16_in, const float* x, const float* a, const float* mean,
+                               const float* sd, float eps, int32_t torch_mode, const float* dres, int64_t rows,
+                               int32_t width, float* dx, float* grad_a, float* grad_b, float* dx_masked,
+                               void* dy16_out, float* colsum_out, float p, uint64_t seed, int32_t layer, int32_t site,
+                               const int32_t* rows_dev, const int32_t* rowmap, void* stream);
+int32_t arb_head_forward(const float* x, const float* a, const float* b, float eps, const float* w, const float* wb,
+                         int32_t has_norm, int32_t act, int64_t rows, int32_t width, float* score, float* mean,
+                         float* sd, const int32_t* rows_dev, const int32_t* rowmap, void* stream);
+int32_t arb_head_backward(const float* dscore, const float* score, const float* x, const float* a, const float* b,
+                          const float* mean, const float* sd, float eps, const float* w, int32_t has_norm, int32_t act,
+                          int64_t rows, int32_t width, float* dx, float* grad_a, float* grad_b, float* grad_w,
+                          float* grad_wb, float* dx_masked, void* dy16_out, float* colsum_out, float p, uint64_t seed,
+                          int32_t layer, int32_t site, const int32_t* rows_dev, const int32_t* rowmap, void* stream);
+int32_t arb_head_multi_forward(const float* xf, const float* w, const float* wb, int32_t act, int64_t rows,
+                               int32_t width, int32_t n, float* score, void* stream);
+int32_t arb_head_multi_backward(const float* dscore, const float* score, const float* xf, const float* w, int32_t act,
+                                int64_t rows, int32_t width, int32_t n, float* dxf, float* grad_w, float* grad_wb,
+                                float* dx_masked, float* colsum_out, float p, uint64_t seed, int32_t layer,
+                                int32_t site, void* stream);
+/* out[c] += sum over rows r of in[r * ld + c], c < width; ld >= width, a multiple of 4 */
+int32_t arb_column_sums(const float* in, int64_t rows, int32_t width, int64_t ld, float* out, void* stream);
+int32_t arb_softmax_forward(float* scores, const uint8_t* mask, int32_t B, int32_t h, int32_t S, int32_t pitch,
+                            float p, uint64_t seed, int32_t layer, void* stream);
+int32_t arb_softmax_backward(float* dprob, float* prob, int64_t rows, int32_t S, int32_t pitch, float p,
+                             uint64_t seed, int32_t layer, void* stream);
+
 /* ---------------------------------------------------------------- optimiser + profiling helpers
  * Flat Adam over the scorer's flat parameter/gradient buffers: torch.optim.Adam semantics (the optimiser the
  * reference instantiates from its config, allrank/main.py:82), one launch.  grads are multiplied by grad_scale

@@ -20,7 +20,8 @@ def _site(call_seed, layer, site, p):
     z = ((z ^ (z >> 27)) * 0x94d049bb133111eb) & m64
     z ^= z >> 31
     seed = (z & 0xFFFFFFFF) ^ (z >> 32)
-    thresh = max(1, min(int(p * 4294967296.0), 0xFFFFFFFF))
+    # the library takes the rate as a float: p = 0.1 gives thresh 429496736, not the 429496729 of the double 0.1
+    thresh = max(1, min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF))
     return np.uint64(seed), np.uint64(thresh), 1.0 / (1.0 - p)
 
 

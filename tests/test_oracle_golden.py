@@ -78,6 +78,27 @@ def build_from_golden(g):
     return model.eval()
 
 
+def zero_by_symmetry(k):
+    """The key projection's bias: its gradient is analytically zero, because the softmax is invariant to a per-query
+    constant (transformer.py:148-153).  What the reference and the oracle hold there is fp32 rounding noise, whose
+    pattern depends on the CPU's summation order (the thread count), not on the maths."""
+    return k.endswith("self_attn.linears.1.bias")
+
+
+def check_param_grads(model, g, prefix="g:"):
+    """Every parameter gradient within 1e-4 of the reference's largest entry; a gradient that is zero by symmetry is
+    held, in the oracle and in the reference alike, below 1e-5 of its weight's largest gradient entry (the noise is
+    ~4e-8 of it; a real key-bias gradient would be of the weight's order)."""
+    grads = dict(model.named_parameters())
+    for k, p in grads.items():
+        ref = g[prefix + k]
+        if zero_by_symmetry(k):
+            level = 1e-5 * np.abs(g[prefix + k[:-len("bias")] + "weight"]).max()
+            assert np.abs(p.grad.numpy()).max() <= level and np.abs(ref).max() <= level, k
+            continue
+        assert np.abs(p.grad.numpy() - ref).max() <= 1e-4 * max(np.abs(ref).max(), 1e-6), k
+
+
 @pytest.mark.parametrize("name", ["tiny", "mid", "cfg2"])
 def test_scorer_matches_reference(golden, name):
     g = golden("scorer_" + name)
@@ -88,9 +109,7 @@ def test_scorer_matches_reference(golden, name):
     assert np.allclose(scores.detach().numpy(), g["scores"], rtol=1e-5, atol=2e-6)
     assert np.allclose(model.score(x, mask, None).detach().numpy(), g["scores"], rtol=1e-5, atol=2e-6)
     (scores * torch.tensor(g["w"])).sum().backward()
-    for k, p in model.named_parameters():
-        ref = g["g:" + k]
-        assert np.abs(p.grad.numpy() - ref).max() <= 1e-4 * max(np.abs(ref).max(), 1e-6), k
+    check_param_grads(model, g)
 
 
 @pytest.mark.parametrize("name", ["dout4", "dout3_fc"])
@@ -104,9 +123,7 @@ def test_multi_output_scorer_matches_reference(golden, name):
     assert np.allclose(out.detach().numpy(), g["scores"], rtol=1e-5, atol=2e-6)
     assert np.allclose(model.score(x, mask, None).detach().numpy(), g["score_sum"], rtol=1e-5, atol=4e-6)
     (out * torch.tensor(g["w"])).sum().backward()
-    for k, p in model.named_parameters():
-        ref = g["g:" + k]
-        assert np.abs(p.grad.numpy() - ref).max() <= 1e-4 * max(np.abs(ref).max(), 1e-6), k
+    check_param_grads(model, g)
 
 
 def test_ordinal_matches_reference(golden):
@@ -146,6 +163,4 @@ def test_scorer_with_positional_encoding_matches_reference(golden, strategy):
     scores = model(x, y == -1, idx)
     assert np.allclose(scores.detach().numpy(), g["scores"], rtol=1e-5, atol=2e-6)
     (scores * torch.tensor(g["w"])).sum().backward()
-    for k, p in model.named_parameters():
-        ref = g["g:" + k]
-        assert np.abs(p.grad.numpy() - ref).max() <= 1e-4 * max(np.abs(ref).max(), 1e-6), k
+    check_param_grads(model, g)
