@@ -59,6 +59,32 @@ struct GemmDesc {
 
 int launch_gemm_tf32(const GemmDesc& d, cudaStream_t stream);   // 0 or ARB_E_*
 
+// The FFN sublayer's two linears chained in one kernel (ffn_chain.cu), fp32 operands on the tf32 tensor cores, all
+// matrices row-major and dense:  Y[rows, d] = epi2( sum_j epi1( X[rows, d] A_j^T ) B_j^T ),  A [f, d], B [d, f].
+//   forward (bwd = 0): A = W1, B = W2;  epi1 = + b1, ReLU (H -> h, bit words -> bits, either nullable);
+//                      epi2 = + b2 + aux (the residual; may alias y)
+//   backward (bwd = 1): X = dY, A = W2^T, B = W1^T;  epi1 = mask by bits (dH -> h, nullable);  colsum (nullable) +=
+//                      the column sums of dH (the b1 gradient)
+// The weights are read as given (the scorer's tf32-rounded copy); X and the chunk of the hidden layer are rounded as
+// the GEMMs round their register operands.  Bit-identical to the two launch_gemm_tf32 products it replaces.
+struct FfnChain {
+  int rows = 0, d = 0, f = 0;
+  const float* x = nullptr;
+  const float* a = nullptr;
+  const float* b = nullptr;
+  const float* b1 = nullptr;
+  const float* b2 = nullptr;
+  const float* aux = nullptr;
+  float* y = nullptr;
+  float* h = nullptr;
+  uint32_t* bits = nullptr;
+  float* colsum = nullptr;
+  const int* rows_dev = nullptr;   // packed rows: device-side live row count; tiles beyond it are not touched
+  int bwd = 0;
+};
+bool ffn_chain_supported(int d, int f);   // d a multiple of 32 up to 256, f a multiple of 64
+int launch_ffn_chain(const FfnChain& c, cudaStream_t stream);   // 0 or ARB_E_*
+
 // 4-D tiled tensor map with 128-byte swizzle; box[0] must span 128 bytes (32 fp32 / 64 bf16 elements).
 struct TmapBox { uint32_t b[4]; };
 // unswizzled = 0: SWIZZLE_128B (16-byte chunks); 1: no swizzle (dense rows narrower than 128 bytes: the bf16 outputs

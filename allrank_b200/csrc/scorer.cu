@@ -53,6 +53,14 @@ static int g_relu_bits = ARB_DEFAULT_RELU_BITS;
 static bool relu_bits(const arb_scorer_config& c) {
   return g_relu_bits && c.n_layers > 0 && !c.bf16 && c.dropout == 0.0f && c.d_ff % 32 == 0;
 }
+// The FFN's two linears run as one chained kernel per direction (ffn_chain.cu) where the bit mask serves the ReLU
+// backward; it gives the same bits as the two GEMMs and saves their re-read of the hidden layer.  It pays off only with
+// d_model <= 128 and at least four 128-row tiles per SM (DESIGN.md 4.13: at d_model 256 and at 64 slates per batch,
+// measured on an H100, the two GEMMs are faster), so the choice follows the width and the launch's row count.
+static bool use_ffn_chain(const arb_scorer_config& c, int64_t rows) {
+  return relu_bits(c) && ffn_chain_supported(c.d_model, c.d_ff) && c.d_model <= 128 &&
+         rows >= int64_t(4) * 128 * sm_count();
+}
 
 // Packed rows need both fused attention kernels (they take per-slate row offsets) and, so far, a call without dropout
 // (its counters index the dense layout), without a positional encoding and with a single output per item.
@@ -585,11 +593,21 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     // ---- feed-forward sublayer: x + W2 relu(W1 LN(x))   (transformer.py:134, :227)
     ARB_TRY(ln_forward(xmid, P + pl.ln2_a, P + pl.ln2_b, c.ln_eps, k.R, d, xn2, ws + wl.mean2, ws + wl.std2, st, 0,
                        bf ? xn2 : nullptr, plan));
-    ARB_TRY(linear_fwd(k, act(xn2), d, d, wt(pl.w1), P + pl.b1, f, act(hdn), f, EPI_RELU, nullptr, 0,
-                       make_drop_site(seed, l, SITE_FFN_HID, p_drop),
-                       wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr));
-    ARB_TRY(linear_fwd(k, act(hdn), f, f, wt(pl.w2), P + pl.b2, d, xout, d, EPI_ADD_AUX, xmid, d,
-                       make_drop_site(seed, l, SITE_FFN_OUT, p_drop)));
+    if (use_ffn_chain(c, k.R)) {      // both linears in one kernel; H is kept for the backward only
+      FfnChain fc;
+      fc.rows = int(k.R); fc.d = d; fc.f = f; fc.rows_dev = k.rows_dev;
+      fc.x = xn2; fc.a = ws + W.wt32 + pl.w1; fc.b = ws + W.wt32 + pl.w2;
+      fc.b1 = P + pl.b1; fc.b2 = P + pl.b2; fc.aux = xmid; fc.y = xout;
+      fc.h = training ? hdn : nullptr;
+      fc.bits = wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr;
+      ARB_TRY(launch_ffn_chain(fc, st));
+    } else {
+      ARB_TRY(linear_fwd(k, act(xn2), d, d, wt(pl.w1), P + pl.b1, f, act(hdn), f, EPI_RELU, nullptr, 0,
+                         make_drop_site(seed, l, SITE_FFN_HID, p_drop),
+                         wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr));
+      ARB_TRY(linear_fwd(k, act(hdn), f, f, wt(pl.w2), P + pl.b2, d, xout, d, EPI_ADD_AUX, xmid, d,
+                         make_drop_site(seed, l, SITE_FFN_OUT, p_drop)));
+    }
     xcur = xout;
   }
   const int has_norm = c.n_layers > 0;
@@ -764,14 +782,25 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     if (G) ARB_TRY(linear_bwd_weight(k, dyv, d, d, act(hdn), f, f, G + pl.w2));   // (b2 gradient: fused into the kernel that emitted dy)
     // hdn <- d hdn in place; hdn > 0 <=> ReLU active AND kept by the hidden dropout, so the mask tile also carries
     // the dropout mask and only the 1/(1-p) scale is needed
-    if (wl.hbits)    // ReLU mask from the forward's bit mask (1 bit per unit) instead of the fp32 activation tile
-      ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_COLSUM, nullptr, 0, 1.0f, g(pl.b1),
-                               reinterpret_cast<const uint32_t*>(ws + wl.hbits)));
-    else
-    ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_MASK_AUX | EPI_COLSUM, act(hdn), f,
-                             drop_on ? 1.0f / (1.0f - p_drop) : 1.0f, g(pl.b1)));   // b1 gradient in the epilogue
-    if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
-    ARB_TRY(linear_bwd_input(k, act(hdn), f, f, wt(pl.w1), d, act(dxn), d, 0, nullptr, 0));
+    if (use_ffn_chain(c, k.R)) {
+      // d hdn (in place, masked by the forward's bit words; b1 gradient in the kernel) and dxn in one kernel
+      FfnChain fc;
+      fc.rows = int(k.R); fc.d = d; fc.f = f; fc.rows_dev = k.rows_dev; fc.bwd = 1;
+      fc.x = dy; fc.a = ws + W.wt32t + pl.w2; fc.b = ws + W.wt32t + pl.w1;
+      fc.bits = reinterpret_cast<uint32_t*>(ws + wl.hbits);
+      fc.h = hdn; fc.colsum = g(pl.b1); fc.y = dxn;
+      ARB_TRY(launch_ffn_chain(fc, st));
+      if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
+    } else {
+      if (wl.hbits)    // ReLU mask from the forward's bit mask (1 bit per unit) instead of the fp32 activation tile
+        ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_COLSUM, nullptr, 0, 1.0f, g(pl.b1),
+                                 reinterpret_cast<const uint32_t*>(ws + wl.hbits)));
+      else
+        ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_MASK_AUX | EPI_COLSUM, act(hdn), f,
+                                 drop_on ? 1.0f / (1.0f - p_drop) : 1.0f, g(pl.b1)));   // b1 gradient in the epilogue
+      if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
+      ARB_TRY(linear_bwd_input(k, act(hdn), f, f, wt(pl.w1), d, act(dxn), d, 0, nullptr, 0));
+    }
     const DropSite site_ao = make_drop_site(seed, l, SITE_ATTN_OUT, p_drop);
     ARB_TRY(ln_backward(dxn, xmid, P + pl.ln2_a, ws + wl.mean2, ws + wl.std2, c.ln_eps, dx, k.R, d, dx_alt,
                         g(pl.ln2_a), g(pl.ln2_b), st, dxm, site_ao, g(pl.bo), 0, bf ? dxn : nullptr, dy16, plan));

@@ -353,6 +353,26 @@ int32_t arb_attention_backward(const float* qkv, const void* ctx, int32_t ctx_bf
                                uint64_t seed, int32_t layer, void* d_qkv, float* dbias_qkv, float* delta_scratch,
                                void* stream);
 
+/* Building blocks exposed for tests: the encoder's feed-forward sublayer as the scorer runs it in TF32 mode without
+ * dropout, both linears chained in one kernel per direction (csrc/ffn_chain.cu).  All matrices are dense row-major
+ * fp32; d is a multiple of 32 up to 256 and d_ff a multiple of 64 (else ARB_E_UNSUPPORTED).  The weights are read as
+ * given: pass them tf32-rounded, as the scorer's weight copy holds them.  The activations are rounded (or truncated,
+ * arb_set_tf32_round_on_load(0)) as the GEMMs round their operands, so the results equal bit for bit those of the two
+ * arb_gemm_tf32 products they replace.
+ *   forward:  h = relu(x w1^T + b1), bits[r][u / 32] bit u % 32 = (h[r][u] > 0), y = h w2^T + b2 + res
+ *             x, res, y [rows, d] (res may alias y); w1 [d_ff, d]; w2 [d, d_ff]; h [rows, d_ff] and bits
+ *             [rows, d_ff / 32] are nullable (not written).
+ *   backward: dh = (dy w2) masked by bits, dx = dh w1;  w2t = w2^T [d_ff, d], w1t = w1^T [d, d_ff]; dh nullable;
+ *             grad_b1 (nullable) += the column sums of dh, per 128-row tile in the EPI_COLSUM epilogue's order.
+ *   rows_dev (nullable, device int32): the live row count; the 128-row tiles at or beyond it are neither read nor
+ *   written. */
+int32_t arb_ffn_forward(const float* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                        const float* res, int32_t rows, int32_t d, int32_t d_ff, float* y, float* h, uint32_t* bits,
+                        const int32_t* rows_dev, void* stream);
+int32_t arb_ffn_backward_input(const float* dy, const float* w2t, const float* w1t, const uint32_t* bits,
+                               int32_t rows, int32_t d, int32_t d_ff, float* dx, float* dh, float* grad_b1,
+                               const int32_t* rows_dev, void* stream);
+
 /* Building blocks exposed for tests: the SIMT row kernels (csrc/scorer_kernels.cu), launched by the scorer's own
  * launchers, so that the steps per warp, the row layout and the reduction slots depend on `rows` as in the scorer
  * (launches of 2^17 rows or more take the large-launch path).  Rows are `width` floats apart; width is a multiple of 4,
