@@ -12,8 +12,8 @@
 // saves one [rows, d_ff] fp32 read per direction and layer.  H / dH are still written: the weight gradients read them.
 //
 // Results are bit-identical to the two GEMMs (DESIGN.md 4.13): the same wgmma m64 x k8 tf32 instructions in ascending
-// k order into one accumulator per product (the second one across chunks, in chunk order), A operands loaded by
-// ldmatrix and rounded in registers exactly as wg_mma_kblock does, the chunk staged unrounded in the 128-byte-swizzled
+// k order into one accumulator per product (the second one across chunks, in chunk order), A operands loaded and
+// rounded in registers by the GEMM's own ptx::load_a_tf32, the chunk staged unrounded in the 128-byte-swizzled
 // K-major layout the second GEMM read from its ring, and the epilogue operations in epi_chunk_f32's order.
 //
 // Structure: one CTA per SM walks the 128-row tiles (bounded by the device-side live row count); warp 8 is the TMA
@@ -75,20 +75,6 @@ struct ChainParams {
   float* colsum;         // backward: per-tile slots [tiles][F] of the b1 gradient (nullable)
   const int* rows_dev;   // packed rows: device-side live row count (nullable)
 };
-
-// A fragments of one 32-wide k-block for rows r0 .. r0+15 of a [rows][32 fp32] swizzled slab, as wg_mma_kblock
-// loads them (ldmatrix, then round to nearest tf32 unless truncating).
-__device__ __forceinline__ void load_a(uint32_t (&a)[4][4], const uint8_t* slab, int r0, int rnd) {
-  const int lane = threadIdx.x & 31, j = lane >> 3;
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    ptx::ldmatrix_x4(a[ks], slab + ptx::sw128(r0 + 8 * (j & 1) + (lane & 7), 32 * ks + 16 * (j >> 1)));
-    if (rnd) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) a[ks][e] = ptx::cvt_tf32(__uint_as_float(a[ks][e]));
-    }
-  }
-}
 
 // acc[:, all D columns] += A (64 x 8, registers) x the k8 step at byte offset 32 ks of the second product's k-block,
 // whose weight rows 64 u .. 64 u + 63 are in ring unit desc[u].  d a multiple of 64: m64n64 per unit, as the W2 GEMM's
@@ -214,7 +200,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) ffn_chain_kernel(const __grid_c
           ptx::mbar_wait(&full[s], (it / NU) & 1);
           if (j == 0) ptx::mbar_wait(&xfull[kb], local & 1);
           uint32_t a[4][4];
-          load_a(a, xs + kb * X_SLAB_BYTES, 64 * g + 16 * w, p.rnd);
+          ptx::load_a_tf32(a, xs + kb * X_SLAB_BYTES, 64 * g + 16 * w, p.rnd);
           const uint64_t desc = ptx::wgmma_desc_sw128(ring + s * UNIT_BYTES);
           ptx::wgmma_fence_acc(accH);
           ptx::wgmma_fence();
@@ -306,7 +292,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) ffn_chain_kernel(const __grid_c
 #pragma unroll 1
         for (int kb2 = 0; kb2 < 2; ++kb2, it += NBU) {
           uint32_t a[4][4];
-          load_a(a, hs + kb2 * H_SLAB_BYTES, 16 * w, p.rnd);
+          ptx::load_a_tf32(a, hs + kb2 * H_SLAB_BYTES, 16 * w, p.rnd);
           uint64_t desc[NBU];
 #pragma unroll
           for (int u = 0; u < NBU; ++u) {

@@ -137,13 +137,13 @@ constexpr int wg_cols() { return BLOCK_N == 128 ? 64 : 32; }
 
 // acc[mt][nt] += rows 64 mt + 16 w .. +15 of A (w: the warp's rank in its warpgroup)  x  columns col0 + 8 nt .. +7 of
 // B over one k-block of the ring, issued by the calling warp's whole warpgroup (128 threads, named barrier `bar`).
-// The A fragments are the m16n8k8 ones (ldmatrix + round to nearest in registers); with rnd_b, the warpgroup first
+// The A fragments come from ptx::load_a_tf32 (ldmatrix + round to nearest in registers); with rnd_b, the warpgroup first
 // rounds its B rows in place (wgmma reads B from shared memory and would truncate it).  Returns with the MMAs of this
 // k-block complete, so the caller may release the stage.
 template <int NT, int WN>
 __device__ __forceinline__ void wg_mma_kblock(float (&acc)[2][NT][4], const uint8_t* a_s, uint8_t* b_s, int col0,
                                               int rnd, int rnd_b, int bar) {
-  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3, j = lane >> 3;
+  const int w = (threadIdx.x >> 5) & 3;
   if (rnd_b) {
     float4* b4 = reinterpret_cast<float4*>(b_s + col0 * 128);
 #pragma unroll
@@ -156,18 +156,9 @@ __device__ __forceinline__ void wg_mma_kblock(float (&acc)[2][NT][4], const uint
     ptx::fence_proxy_async_smem();
     ptx::named_bar_sync(bar, 128);
   }
-  uint32_t a[4][2][4];
+  uint32_t a[2][4][4];
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      // lanes 8j .. 8j+7 address block j: rows +8 (j & 1), k +4 (j >> 1) of the 16 x 8 fragment
-      ptx::ldmatrix_x4(a[ks][mt], a_s + ptx::sw128(64 * mt + 16 * w + 8 * (j & 1) + (lane & 7), 32 * ks + 16 * (j >> 1)));
-      if (rnd) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) a[ks][mt][e] = ptx::cvt_tf32(__uint_as_float(a[ks][mt][e]));
-      }
-    }
+  for (int mt = 0; mt < 2; ++mt) ptx::load_a_tf32(a[mt], a_s, 64 * mt + 16 * w, rnd);
   const uint64_t desc = ptx::wgmma_desc_sw128(b_s + col0 * 128);
   ptx::wgmma_fence_acc(acc[0]);
   ptx::wgmma_fence_acc(acc[1]);
@@ -178,11 +169,11 @@ __device__ __forceinline__ void wg_mma_kblock(float (&acc)[2][NT][4], const uint
     for (int mt = 0; mt < 2; ++mt) {
       const uint64_t d = desc + 2 * ks;                     // +32 bytes (8 tf32) per k8 step
       if constexpr (WN == 64) {
-        ptx::wgmma_m64n64k8_tf32<0>(acc[mt], a[ks][mt], d);
-        if constexpr (NT == 16) ptx::wgmma_m64n64k8_tf32<8>(acc[mt], a[ks][mt], d + 64 * 128 / 16);
+        ptx::wgmma_m64n64k8_tf32<0>(acc[mt], a[mt][ks], d);
+        if constexpr (NT == 16) ptx::wgmma_m64n64k8_tf32<8>(acc[mt], a[mt][ks], d + 64 * 128 / 16);
       } else {
-        ptx::wgmma_m64n32k8_tf32<0>(acc[mt], a[ks][mt], d);
-        if constexpr (NT == 8) ptx::wgmma_m64n32k8_tf32<4>(acc[mt], a[ks][mt], d + 32 * 128 / 16);
+        ptx::wgmma_m64n32k8_tf32<0>(acc[mt], a[mt][ks], d);
+        if constexpr (NT == 8) ptx::wgmma_m64n32k8_tf32<4>(acc[mt], a[mt][ks], d + 32 * 128 / 16);
       }
     }
   ptx::wgmma_commit();
@@ -353,6 +344,41 @@ __device__ __forceinline__ bool epi_chunk_dispatch(int flags, const uint32_t (&v
   }
 }
 
+// ---- TMA producer loads -------------------------------------------------------------------------------------------
+// One k-block (elements k0 ..) of A (tile rows m0 ..) and B (tile rows n0 ..) of batch (b2, b3) into the ring stage at
+// a_s (B after the A_STAGE_BYTES of A), completing on `bar`.  An MN-major operand comes as slabs of 32 fp32 / 64 bf16
+// MN-elements x one k-block; a K-major one as one box of 128-byte rows.
+template <int A_MN, int B_MN, bool IN16, int BLOCK_N>
+__device__ __forceinline__ void load_stage(uint8_t* a_s, uint64_t* bar, const CUtensorMap* tmA, const CUtensorMap* tmB,
+                                           const GemmParams& p, int m0, int n0, int k0, int b2, int b3) {
+  constexpr int MN_SLAB = IN16 ? 64 : 32;                     // MN-elements per MN-major slab (128 bytes)
+  constexpr int MN_SLAB_BYTES = MN_SLAB * 128;                // the k-block's 32 / 64 k-rows of 128 bytes: 4096 / 8192
+  uint8_t* b_s = a_s + A_STAGE_BYTES;
+  ptx::mbar_expect_tx(bar, A_STAGE_BYTES + BLOCK_N * 128);
+  if (A_MN) {
+    for (int c = 0; c < BLOCK_M / MN_SLAB; ++c)
+      ptx::tma_load_4d(a_s + c * MN_SLAB_BYTES, tmA, bar, m0 + MN_SLAB * c, k0, b2 * p.a_b2, b3 * p.a_b3);
+  } else {
+    ptx::tma_load_4d(a_s, tmA, bar, k0, m0, b2 * p.a_b2, b3 * p.a_b3);
+  }
+  if (B_MN) {
+    for (int c = 0; c < BLOCK_N / MN_SLAB; ++c)
+      ptx::tma_load_4d(b_s + c * MN_SLAB_BYTES, tmB, bar, n0 + MN_SLAB * c, k0, b2 * p.b_b2, b3 * p.b_b3);
+  } else {
+    ptx::tma_load_4d(b_s, tmB, bar, k0, n0, b2 * p.b_b2, b3 * p.b_b3);
+  }
+}
+// The residual / ReLU-mask tile of output tile (m0, n0) into the staging slabs, completing on `bar`.  It has the
+// output's element type: 128-byte slab rows hold 32 fp32 or 64 bf16 columns.
+template <int BLOCK_N, bool OUT16>
+__device__ __forceinline__ void load_aux_tile(uint8_t* staging, uint64_t* bar, const CUtensorMap* tmAux,
+                                              const GemmParams& p, int m0, int n0, int b2, int b3) {
+  constexpr int OUT_COLS = OUT16 ? 64 : 32, OUT_SLABS = BLOCK_N / OUT_COLS;
+  ptx::mbar_expect_tx(bar, OUT_SLABS * BLOCK_M * 128);
+  for (int c = 0; c < OUT_SLABS; ++c)
+    ptx::tma_load_4d(staging + c * (BLOCK_M * 128), tmAux, bar, n0 + OUT_COLS * c, m0, b2 * p.c_b2, b3 * p.c_b3);
+}
+
 template <int BLOCK_N, int NST = 2, bool KM = false>
 struct SmemLayout {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 4;
@@ -407,8 +433,6 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
   const bool split = (p.flags & EPI_ATOMIC) != 0;
   const int b2 = split ? 0 : int(blockIdx.z) % p.nb2, b3 = split ? 0 : int(blockIdx.z) / p.nb2;
   constexpr int KELEMS = IN16 ? BLOCK_K_BF16 : BLOCK_K;       // elements of K per k-block (128 bytes either way)
-  constexpr int MN_SLAB = IN16 ? 64 : 32;                     // MN-elements per MN-major slab (128 bytes)
-  constexpr int MN_SLAB_BYTES = MN_SLAB * KELEMS * (IN16 ? 2 : 4);   // 8192 (bf16) / 4096 (tf32)
   // Packed rows: the live row count is on the device (written at least two launches upstream, so it may be read
   // before the PDL wait).  It bounds M -- CTAs of tiles beyond it leave at once -- or, for the split-K weight gradients,
   // K, which is then divided evenly over the grid's splits here.
@@ -440,31 +464,14 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
       for (int i = 0; i < nkb; ++i) {
         const int s = i % STAGES, round = i / STAGES;
         if (round > 0) ptx::mbar_wait(&empty_bar[s], (round - 1) & 1);
-        uint8_t* a_s = smem + s * L::STAGE_BYTES;
-        uint8_t* b_s = a_s + A_STAGE_BYTES;
-        const int k0 = (kb_begin + i) * KELEMS;
-        ptx::mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-        if (A_MN) {
-          for (int c = 0; c < BLOCK_M / MN_SLAB; ++c)
-            ptx::tma_load_4d(a_s + c * MN_SLAB_BYTES, &tmA, &full_bar[s], m0 + MN_SLAB * c, k0, b2 * p.a_b2, b3 * p.a_b3);
-        } else {
-          ptx::tma_load_4d(a_s, &tmA, &full_bar[s], k0, m0, b2 * p.a_b2, b3 * p.a_b3);
-        }
-        if (B_MN) {
-          for (int c = 0; c < BLOCK_N / MN_SLAB; ++c)
-            ptx::tma_load_4d(b_s + c * MN_SLAB_BYTES, &tmB, &full_bar[s], n0 + MN_SLAB * c, k0, b2 * p.b_b2, b3 * p.b_b3);
-        } else {
-          ptx::tma_load_4d(b_s, &tmB, &full_bar[s], k0, n0, b2 * p.b_b2, b3 * p.b_b3);
-        }
+        load_stage<A_MN, B_MN, IN16, BLOCK_N>(smem + s * L::STAGE_BYTES, &full_bar[s], &tmA, &tmB, p, m0, n0,
+                                              (kb_begin + i) * KELEMS, b2, b3);
       }
       if (has_aux) {
         // the residual / ReLU-mask tile goes into the staging area, i.e. over the operand ring: wait until every
-        // consumer warp has finished reading it.  It has the output's element type: 128-byte slab rows hold 32 fp32
-        // or 64 bf16 columns.
+        // consumer warp has finished reading it
         if (nkb > 0) ptx::mbar_wait(ring_done_bar, 0);
-        ptx::mbar_expect_tx(aux_bar, OUT16 ? L::STAGING_BYTES / 2 : L::STAGING_BYTES);
-        for (int c = 0; c < OUT_SLABS; ++c)
-          ptx::tma_load_4d(staging + c * (BLOCK_M * 128), &tmAux, aux_bar, n0 + OUT_COLS * c, m0, b2 * p.c_b2, b3 * p.c_b3);
+        load_aux_tile<BLOCK_N, OUT16>(staging, aux_bar, &tmAux, p, m0, n0, b2, b3);
       }
     }
   } else if (warp < N_CONSUMERS) {
@@ -760,31 +767,15 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
           const int s = it % STAGES;
           const uint32_t round = it / STAGES;
           if (round > 0) ptx::mbar_wait(&empty_bar[s], (round - 1) & 1);
-          uint8_t* a_s = smem + s * L::STAGE_BYTES;
-          uint8_t* b_s = a_s + A_STAGE_BYTES;
-          const int k0 = (kb0 + i) * BLOCK_K;
-          ptx::mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          if (A_MN) {
-            for (int c = 0; c < BLOCK_M / 32; ++c)
-              ptx::tma_load_4d(a_s + c * 4096, &tmA, &full_bar[s], m0 + 32 * c, k0, b2 * p.a_b2, b3 * p.a_b3);
-          } else {
-            ptx::tma_load_4d(a_s, &tmA, &full_bar[s], k0, m0, b2 * p.a_b2, b3 * p.a_b3);
-          }
-          if (B_MN) {
-            for (int c = 0; c < N_SLABS; ++c)
-              ptx::tma_load_4d(b_s + c * 4096, &tmB, &full_bar[s], n0 + 32 * c, k0, b2 * p.b_b2, b3 * p.b_b3);
-          } else {
-            ptx::tma_load_4d(b_s, &tmB, &full_bar[s], k0, n0, b2 * p.b_b2, b3 * p.b_b3);
-          }
+          load_stage<A_MN, B_MN, false, BLOCK_N>(smem + s * L::STAGE_BYTES, &full_bar[s], &tmA, &tmB, p, m0, n0,
+                                                 (kb0 + i) * BLOCK_K, b2, b3);
         }
         if (has_aux) {
           // the residual / mask tile goes into the staging area, which is reused tile after tile: wait until the
           // previous tile's TMA store has read it (issued AFTER this tile's operand loads so the ring never stalls
           // behind the epilogue)
           if (local > 0) ptx::mbar_wait(stage_free, (local - 1) & 1);
-          ptx::mbar_expect_tx(aux_full, L::STAGING_BYTES);
-          for (int c = 0; c < N_SLABS; ++c)
-            ptx::tma_load_4d(staging + c * (BLOCK_M * 128), &tmAux, aux_full, n0 + 32 * c, m0, b2 * p.c_b2, b3 * p.c_b3);
+          load_aux_tile<BLOCK_N, false>(staging, aux_full, &tmAux, p, m0, n0, b2, b3);
         }
       }
     }
@@ -1004,6 +995,17 @@ static void gemm_prof_name(char (&out)[56], const GemmDesc& d, const char* varia
 // accounting only: a launch over packed rows (rows_dev) processes arb_row_frac() of its nominal M (or K, split-K)
 static double live_m(const GemmDesc& d) { return double(d.M) * ((d.rows_dev && !(d.flags & EPI_ATOMIC)) ? arb_row_frac() : 1.0); }
 static double live_k(const GemmDesc& d) { return double(d.K) * ((d.rows_dev && (d.flags & EPI_ATOMIC)) ? arb_row_frac() : 1.0); }
+// the profile record of one GEMM launch: 2 M N K flops per batch; bytes: both operands once, the output and any aux
+// tile, at their element sizes
+static ProfScope gemm_prof(const GemmDesc& d, const char* variant, cudaStream_t st) {
+  const double nb = double(d.nb2) * double(d.nb3), dM = live_m(d), dK = live_k(d);
+  const double isz = d.A.bf16 ? 2.0 : 4.0, osz = d.C.bf16 ? 2.0 : 4.0;
+  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
+  char pname[56];
+  gemm_prof_name(pname, d, variant);
+  return ProfScope(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
+                   nb * (isz * (dM * dK + double(d.N) * dK) + osz * (1.0 + has_x) * dM * d.N), pname);
+}
 static int g_persistent = ARB_DEFAULT_GEMM_PERSISTENT;   // 0: never, 1: wherever supported, 2: auto
 void set_gemm_persistent(int on) { g_persistent = on; }
 
@@ -1012,13 +1014,7 @@ static int launch_persistent_t(const GemmDesc& d, const CUtensorMap& tA, const C
                                const CUtensorMap& tX, const GemmParams& p, dim3 tiles, cudaStream_t st) {
   const long long n_tiles = (long long)tiles.x * tiles.y * tiles.z;
   const int grid = int(std::min<long long>(n_tiles, sm_count()));
-  const double nb = double(d.nb2) * double(d.nb3);
-  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-  char pname[56];
-  gemm_prof_name(pname, d, "persist");
-  const double dM = live_m(d), dK = live_k(d);
-  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-               4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
+  const ProfScope ps = gemm_prof(d, "persist", st);
   return launch(gemm_tf32_persistent<BLOCK_N, A_MN, B_MN>, dim3(grid), dim3(PERSIST_THREADS),
                 PersistLayout<BLOCK_N>::total(), st, /*pdl=*/true, tA, tB, tC, tX, p, int(tiles.x), int(tiles.y),
                 int(tiles.z));
@@ -1048,14 +1044,7 @@ static int launch_bf16_t(const GemmDesc& d, const CUtensorMap& tA, const CUtenso
     smem = SmemLayout<BLOCK_N, 3>::total();
   }
   if (!kern) { arb_set_error("gemm_bf16: block_n must be 64 or 128"); return ARB_E_UNSUPPORTED; }
-  const double nb = double(d.nb2) * double(d.nb3);
-  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-  const double osz = d.C.bf16 ? 2.0 : 4.0;
-  char pname[56];
-  gemm_prof_name(pname, d, "tile");
-  const double dM = live_m(d), dK = live_k(d);
-  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-               nb * (2.0 * (dM * dK + double(d.N) * dK) + osz * (1.0 + has_x) * dM * d.N), pname);
+  const ProfScope ps = gemm_prof(d, "tile", st);
   return launch(kern, grid, dim3(GEMM_THREADS), smem, st, /*pdl=*/true, tA, tB, tC, tX, p);
 }
 
@@ -1095,13 +1084,7 @@ static int launch_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap&
     if (deep) { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 3>; smem = SmemLayout<BLOCK_N, 3>::total(); }
     else      { kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, false, 2>; smem = SmemLayout<BLOCK_N, 2>::total(); }
   }
-  const double nb = double(d.nb2) * double(d.nb3);
-  const double has_x = (d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) ? 1.0 : 0.0;
-  char pname[56];
-  gemm_prof_name(pname, d, "tile");
-  const double dM = live_m(d), dK = live_k(d);
-  ProfScope ps(ARB_PROF_GEMM, 2.0 * dM * double(d.N) * dK * nb, st,
-               4.0 * nb * (dM * dK + double(d.N) * dK + (1.0 + has_x) * dM * d.N), pname);
+  const ProfScope ps = gemm_prof(d, "tile", st);
   return launch(kern, grid, dim3(GEMM_THREADS), smem, st, /*pdl=*/true, tA, tB, tC, tX, p);
 }
 

@@ -137,6 +137,21 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* row_ad
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
                : "r"(smem_u32(row_addr)));
 }
+// The tf32 A fragments (m16n8k8 layout above) of rows r0 .. r0+15 of a [rows][32 fp32] 128-byte-swizzled tile, one per
+// k8 step of its 32-wide k-block: ldmatrix, then round to nearest tf32 unless `rnd` is 0 (the tensor core then
+// truncates).  Every register-A tf32 wgmma loads its operand here, so the kernels that must agree bit for bit agree.
+__device__ __forceinline__ void load_a_tf32(uint32_t (&a)[4][4], const uint8_t* tile, int r0, int rnd) {
+  const int lane = threadIdx.x & 31, j = lane >> 3;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    // lanes 8j .. 8j+7 address block j: rows +8 (j & 1), k +4 (j >> 1) of the 16 x 8 fragment
+    ldmatrix_x4(a[ks], tile + sw128(r0 + 8 * (j & 1) + (lane & 7), 32 * ks + 16 * (j >> 1)));
+    if (rnd) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) a[ks][e] = cvt_tf32(__uint_as_float(a[ks][e]));
+    }
+  }
+}
 
 // ------------------------------------------------------------------ warpgroup MMA (wgmma)
 // Shared-memory matrix descriptor of a K-major operand tile written by TMA with SWIZZLE_128B: rows of 128 bytes, 8-row

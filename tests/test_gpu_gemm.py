@@ -158,6 +158,10 @@ def test_persistent_modes_are_bit_identical_to_the_tile_kernel(gemm, mode, K, bl
         C = torch.empty(M, N, device="cuda")
         gemm(A, W, C, X, None, M, N, K, 0, 0, 1, 0, 0, 0, block_n, EPI_MASK_AUX, 0.5)
         outs.append(C)
+        # no specialised epilogue for this combination: both kernels run their generic per-element path
+        Xc = X.clone()
+        gemm(A, W, Xc, Xc, None, M, N, K, 0, 0, 1, 0, 0, 0, block_n, EPI_RELU | EPI_ADD_AUX, 0.5)
+        outs.append(Xc)
         return outs
 
     try:
