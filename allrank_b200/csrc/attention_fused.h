@@ -21,9 +21,12 @@ struct AttnFwdArgs {
                                  // only the first round_up(extent[b], 16) rows of every slate, slate b at row pack_off[b]
 };
 
+// S <= 256 at head width 16, 32 or 64 (attention_fused.cu), or 256 < S <= 4096 at head width 16 or 32, fp32 context,
+// dense layout (attention_long.cu)
 bool attn_fused_supported(int S, int dk);
 void set_attn_fwd_two_pass(int on);   // accepted for the C ABI; every setting runs the same kernel
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st);
+int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st);   // 256 < S <= 4096 (attention_long.cu)
 
 }  // namespace arb
 
@@ -54,8 +57,10 @@ struct AttnBwdArgs {
   const int* rowmap = nullptr;   // packed rows: item index of every packed row (for the delta kernel)
 };
 
+// S <= 4096 at head width 16 or 32; beyond 256 items fp32 operands and the dense layout only
 bool attn_fused_bwd_supported(int S, int dk);
 void set_attn_bwd_persistent(int on);   // 1: one CTA per SM walks the (slate, head) items; 0: one CTA per item
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st);
+int launch_attn_long_bwd(const AttnBwdArgs& a, cudaStream_t st);   // 256 < S <= 4096, after delta (attention_long.cu)
 
 }  // namespace arb

@@ -562,6 +562,17 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
 static int g_attn_bwd_persistent = ARB_DEFAULT_ATTN_BWD_PERSISTENT;
 void set_attn_bwd_persistent(int on) { g_attn_bwd_persistent = on; }
 
+// delta = rowsum(dO * O) per (slate, head, query), for either backward
+static int launch_delta(const AttnBwdArgs& a, cudaStream_t st) {
+  const bool packed = a.pack_off != nullptr;
+  const double rf = packed ? arb_row_frac() : 1.0;
+  ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
+  const long long rows = packed ? (long long)a.q.dim[1] : (long long)a.B * a.S;   // packed: the buffers' row count
+  return launch(attn_delta_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0, st,
+                /*pdl=*/true, a.do_ptr, static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.B, a.S, a.h,
+                a.dk, a.delta, a.o_bf16, a.rows_dev, a.rowmap, rows);
+}
+
 template <int DK>
 static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   alignas(64) CUtensorMap tQ, tK, tV, tDO, tDQ, tDK, tDV;
@@ -579,14 +590,7 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   if ((rc = make_tmap_4d(&tDK, a.dk_, box, out16 ? 1 : 0))) return rc;
   if ((rc = make_tmap_4d(&tDV, a.dv, box, out16 ? 1 : 0))) return rc;
   const double rf = packed ? arb_row_frac() : 1.0;
-  {
-    ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
-    const long long rows = packed ? (long long)a.q.dim[1] : (long long)a.B * a.S;   // packed: the buffers' row count
-    if ((rc = launch(attn_delta_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0, st,
-                     /*pdl=*/true, a.do_ptr, static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.B, a.S, a.h,
-                     a.dk, a.delta, a.o_bf16, a.rows_dev, a.rowmap, rows)))
-      return rc;
-  }
+  if ((rc = launch_delta(a, st))) return rc;
   const bool drop = a.drop.thresh != 0;
   auto kern = out16 ? (drop ? attn_bwd_kernel<DK, true, true> : attn_bwd_kernel<DK, false, true>)
                     : (drop ? attn_bwd_kernel<DK, true> : attn_bwd_kernel<DK, false>);
@@ -617,10 +621,18 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 
-bool attn_fused_bwd_supported(int S, int dk) { return S >= 1 && S <= 256 && (dk == 16 || dk == 32); }
+bool attn_fused_bwd_supported(int S, int dk) { return S >= 1 && S <= 4096 && (dk == 16 || dk == 32); }
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
   if (!attn_fused_bwd_supported(a.S, a.dk)) { arb_set_error("fused attention backward: unsupported shape"); return ARB_E_UNSUPPORTED; }
+  if (a.S > 256) {
+    if (a.o_bf16 || a.dq.bf16 || a.dk_.bf16 || a.dv.bf16 || a.pack_off) {
+      arb_set_error("fused attention backward: bf16 operands and packed rows need slate_length <= 256");
+      return ARB_E_UNSUPPORTED;
+    }
+    int rc = launch_delta(a, st);
+    return rc ? rc : launch_attn_long_bwd(a, st);
+  }
   return a.dk == 16 ? launch_bwd_t<16>(a, st) : launch_bwd_t<32>(a, st);
 }
 

@@ -37,8 +37,10 @@ static int g_skip_padding = ARB_DEFAULT_SKIP_PADDING;
 // for every real item and every parameter gradient; scores of padded items are then 0 instead of what the network
 // computes for an all-zero feature row, which every consumer in allRank masks: DESIGN.md 4.12); 0: dense [B*S] rows
 static int g_pack_rows = ARB_DEFAULT_PACK_ROWS;
+// Beyond 256 items the fused kernels (attention_long.cu) read and write fp32 only: bf16 mode keeps the unfused path
+// there (which it does not support, so such a call fails as before).
 static bool use_fused(const arb_scorer_config& c, int S) {
-  return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, c.d_model / c.n_heads);
+  return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, c.d_model / c.n_heads) && !(c.bf16 && S > 256);
 }
 static bool use_fused_bwd(const arb_scorer_config& c, int S) {
   return g_attn_mode >= 2 && use_fused(c, S) && attn_fused_bwd_supported(S, c.d_model / c.n_heads);
@@ -62,10 +64,12 @@ static bool use_ffn_chain(const arb_scorer_config& c, int64_t rows) {
          rows >= int64_t(4) * 128 * sm_count();
 }
 
-// Packed rows need both fused attention kernels (they take per-slate row offsets) and, so far, a call without dropout
-// (its counters index the dense layout), without a positional encoding and with a single output per item.
+// Packed rows need both fused attention kernels of slates up to 256 items (they take per-slate row offsets; the
+// longer slates' kernels run the dense layout, which scores padded items as the reference does) and, so far, a call
+// without dropout (its counters index the dense layout), without a positional encoding and with a single output per
+// item.
 static bool pack_eligible(const arb_scorer_config& c, int S) {
-  return c.n_layers > 0 && use_fused_bwd(c, S) && c.dropout == 0.0f && c.fc_dropout == 0.0f && c.pe_mode == 0 &&
+  return c.n_layers > 0 && S <= 256 && use_fused_bwd(c, S) && c.dropout == 0.0f && c.fc_dropout == 0.0f && c.pe_mode == 0 &&
          n_outputs(c) == 1;
 }
 static bool use_pack(const arb_scorer_config& c, int S) { return g_pack_rows && g_skip_padding && pack_eligible(c, S); }
@@ -951,7 +955,7 @@ static int attention_hook_check(const char* what, int B, int S, int h, float p, 
   if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
   if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
   if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
-    arb_set_error((std::string(what) + ": unsupported shape (S <= 256; head width 16, 32 or 64, backward 16 or 32)").c_str());
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 256 at head width 16, 32 or 64, backward 16 or 32; S <= 4096 at head width 16 or 32)").c_str());
     return ARB_E_UNSUPPORTED;
   }
   return ARB_OK;
@@ -963,6 +967,7 @@ extern "C" int32_t arb_attention_forward(const float* qkv, const uint8_t* mask, 
   if (!qkv || !mask || !ctx || !stat_max || !stat_sum) { arb_set_error("arb_attention_forward: null pointer"); return ARB_E_INVALID_ARG; }
   ARB_TRY(attention_hook_check("arb_attention_forward", B, S, h, p, false, dk));
   if (ctx_bf16 && dk > 32) { arb_set_error("arb_attention_forward: a bf16 context needs head width <= 32"); return ARB_E_UNSUPPORTED; }
+  if (ctx_bf16 && S > 256) { arb_set_error("arb_attention_forward: a bf16 context needs S <= 256"); return ARB_E_UNSUPPORTED; }
   const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
   const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
   return launch_attn_fwd(attn_fwd_args(z, qkv, o, mask, extent, stat_max, stat_sum,
