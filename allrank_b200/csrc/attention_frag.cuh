@@ -67,6 +67,11 @@ __device__ __forceinline__ void ld_a_head(uint32_t op, int r0, int lane, uint32_
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) ldsm_x4(op + uint32_t(r) * 128u + (uint32_t((2 * ks + (m >> 1)) ^ (r & 7)) << 4), a[ks]);
 }
+// a[ks] of ld_a_head alone (the wide streaming kernels re-read the tile's fragments one k-step at a time)
+__device__ __forceinline__ void ld_a_step(uint32_t op, int r0, int lane, int ks, uint32_t (&a)[4]) {
+  const int m = lane >> 3, r = r0 + (lane & 7) + 8 * (m & 1);
+  ldsm_x4(op + uint32_t(r) * 128u + (uint32_t((2 * ks + (m >> 1)) ^ (r & 7)) << 4), a);
+}
 // B fragments over the head dimension of the 8 rows r0 + sigma(n): b[ks] = {X[r0 + sigma(g)][8ks + t], ...[8ks + t + 4]}
 template <int KS>
 __device__ __forceinline__ void ld_b_head(uint32_t op, int r0, int lane, uint32_t (&b)[KS][2]) {

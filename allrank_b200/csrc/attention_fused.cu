@@ -376,13 +376,15 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
                 tf32_round_on_load(), pool_units);
 }
 
+// attn_fwd_kernel: S <= 256 at head width 16, 32 or 64; attention_long.cu: S <= 4096 at 16, 32 and 36 ... 96 in steps
+// of 4 (every width but 64 at S <= 256 runs there)
 bool attn_fused_supported(int S, int dk) {
-  return S >= 1 && ((S <= 256 && (dk == 16 || dk == 32 || dk == 64)) || (S <= 4096 && (dk == 16 || dk == 32)));
+  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 96 && dk % 4 == 0));
 }
 
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
   if (!attn_fused_supported(a.S, a.dk)) { arb_set_error("fused attention: unsupported shape"); return ARB_E_UNSUPPORTED; }
-  if (a.S > 256) return launch_attn_long_fwd(a, st);
+  if (a.S > 256 || (a.dk > 32 && a.dk != 64)) return launch_attn_long_fwd(a, st);
   switch (a.dk) {
     case 16: return launch_fwd_t<16>(a, st);
     case 32: return launch_fwd_t<32>(a, st);

@@ -1,4 +1,5 @@
-// Fused self-attention backward for slates of up to 256 items and head width <= 32.
+// Fused self-attention backward for slates of up to 256 items and head width 16 or 32 (other shapes:
+// attention_long.cu).
 //
 // Reference: autograd of attention() allrank/models/transformer.py:137-156.  Given d ctx it produces dQ, dK, dV
 // without ever materialising the S x S probabilities in HBM: they are recomputed from Q, K and the row statistics
@@ -21,7 +22,8 @@ constexpr int BWD_WARPS = 8;                          // compute warps: one 16-r
 constexpr int BWD_THREADS = 32 * (BWD_WARPS + 2);     // + one load warp, one store warp
 
 // delta[b,h,q] = sum_e dO[b,q,h,e] * O[b,q,h,e]: one warp per row of the [B*S, d_model] activations, 128-bit loads,
-// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32}: 4 or 8 lanes per head).
+// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32, 64}: 4, 8 or 16 lanes per head);
+// other widths (36 ... 96) reduce one head at a time over the whole warp.
 constexpr int DELTA_RPW = 4;     // rows per warp of the delta kernel
 __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ d_o, const float* __restrict__ o,
                                                          long long pitch, int B, int S, int h, int dk,
@@ -40,6 +42,30 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
   long long item[DELTA_RPW];
 #pragma unroll
   for (int q = 0; q < DELTA_RPW; ++q) item[q] = (row0 + q < rows) ? (rowmap ? (long long)rowmap[row0 + q] : row0 + q) : -1;
+  if (dk & (dk - 1)) {
+    // a width that is not a power of two (36 ... 96, dense fp32 rows): one head at a time, lane l takes its columns
+    // 4l ... 4l + 3 (dk / 4 <= 24 lanes), reduced over the whole warp
+    for (int head = 0; head < h; ++head) {
+      const int c = head * dk + lane * 4;
+      const bool on = lane < lanes_per_head;
+#pragma unroll
+      for (int q = 0; q < DELTA_RPW; ++q) {
+        float acc = 0.f;
+        if (on && item[q] >= 0) {
+          const long long row = row0 + q;
+          const float4 x = *reinterpret_cast<const float4*>(d_o + row * pitch + c);
+          const float4 y = *reinterpret_cast<const float4*>(o + row * pitch + c);
+          acc = x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
+        }
+        for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(FULL, acc, off);
+        if (item[q] >= 0 && lane == 0) {
+          const int b = int(item[q] / S), qi = int(item[q] - (long long)b * S);
+          delta[((long long)b * h + head) * S + qi] = acc;
+        }
+      }
+    }
+    return;
+  }
   for (int c0 = 0; c0 < width; c0 += 128) {
     const int c = c0 + lane * 4;
     float4 a[DELTA_RPW], bq[DELTA_RPW];
@@ -621,13 +647,18 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 
-bool attn_fused_bwd_supported(int S, int dk) { return S >= 1 && S <= 4096 && (dk == 16 || dk == 32); }
+// head widths 16 and 32, and 36 ... 96 in steps of 4 (attention_long.cu)
+bool attn_fused_bwd_supported(int S, int dk) {
+  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 96 && dk % 4 == 0));
+}
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
   if (!attn_fused_bwd_supported(a.S, a.dk)) { arb_set_error("fused attention backward: unsupported shape"); return ARB_E_UNSUPPORTED; }
-  if (a.S > 256) {
+  // the long kernels: slates beyond 256 items, and every width above 32 (whose statistics the short forward writes in
+  // the same [B, h, S] format at width 64)
+  if (a.S > 256 || a.dk > 32) {
     if (a.o_bf16 || a.dq.bf16 || a.dk_.bf16 || a.dv.bf16 || a.pack_off) {
-      arb_set_error("fused attention backward: bf16 operands and packed rows need slate_length <= 256");
+      arb_set_error("fused attention backward: bf16 operands and packed rows need slate_length <= 256 and head width 16 or 32");
       return ARB_E_UNSUPPORTED;
     }
     int rc = launch_delta(a, st);

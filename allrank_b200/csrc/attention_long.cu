@@ -1,7 +1,8 @@
-// Fused self-attention for slates of 257 ... 4096 items at head width 16 or 32, forward and backward, without the
-// S x S matrix.  attention_fused.cu / attention_fused_bwd.cu serve S <= 256 by holding a whole (slate, head) in shared
-// memory; that stops fitting beyond 256 rows, so here a work item is one 128-row tile of a (slate, head) and the other
-// side of its products streams through a ring of shared-memory stages:
+// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 96 (w % 4 == 0)
+// for slates of 1 ... 4096 items, forward and backward, without the S x S matrix.  attention_fused.cu /
+// attention_fused_bwd.cu serve S <= 256 at width <= 32 (the forward also 64) by holding a whole (slate, head) in shared
+// memory; that stops fitting beyond 256 rows or 32 columns, so here a work item is one 128-row tile of a (slate, head)
+// and the other side of its products streams through a ring of shared-memory stages:
 //   attn_long_fwd_kernel   tile of 128 queries;  streams K (pass A), then K and V (pass B)          -> ctx, row stats
 //   attn_long_dkdv_kernel  tile of 128 keys;     streams Q, dO and the queries' {nm, delta}         -> dK, dV
 //   attn_long_dq_kernel    tile of 128 queries;  streams K, V                                      -> dQ
@@ -10,6 +11,7 @@
 // context, row statistics and dQ / dK / dV.  Only the QKV bias gradient is summed in another order.
 #include <algorithm>
 #include <cstdint>
+#include <type_traits>
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -24,32 +26,52 @@ namespace arb {
 
 constexpr int LONG_WARPS = 8;                         // compute warps: one 16-row strip of the tile each
 constexpr int LONG_THREADS = 32 * (LONG_WARPS + 1);   // + one load warp
-constexpr int LONG_BLK = 128;                         // rows of a tile and of a streamed block
-constexpr int LONG_NST = 4;                           // stages of the ring
-constexpr int LONG_OP = LONG_BLK * 128;               // one operand of a buffer: 128 rows of 128 bytes
-constexpr int LONG_BUF = 2 * LONG_OP + 1024;          // two operands + aux (key bits, or float2 {nm, delta} per query)
-constexpr int LONG_OUT = 2 * 2048;                    // per compute warp: two 16-row output boxes
+constexpr int LONG_BLK = 128;                         // rows of a tile
 
+// An operand row of DK columns is NKB slabs of 128 bytes (32 fp32 columns; TMA zero-fills the columns past the head
+// width), each slab of a buffer 128B-swizzled in its own 16-row boxes.  A buffer holds two operands, slab after slab,
+// and an aux region (key bits, or float2 {nm, delta} per query).
+//   DK <= 32: 128-row streamed blocks in four stages; the fragments of the tile's rows stay in registers, the tile is
+//             free again once they are loaded, and each compute warp stages its strips in two boxes of its own.
+//   DK 64, 96 (wide): 64-row streamed blocks in four / two stages; the tile stays resident for the whole item: the dK /
+//             dV and dQ strips re-read its fragments for every k-step (they would not fit in registers beside the
+//             accumulators), and each warp stages its finished strip over its own 16 rows of the tile.
+template <int DK>
 struct LongSmem {
-  // [tile buffer] [ring: LONG_NST buffers] [output boxes] [mbarriers: full[NST] empty[NST] res_full res_empty]
-  static constexpr int ring = LONG_BUF;
-  static constexpr int out = ring + LONG_NST * LONG_BUF;
-  static constexpr int bars = out + LONG_WARPS * LONG_OUT;
-  static constexpr int total = bars + 8 * (2 * LONG_NST + 2) + 1024;
+  static constexpr bool WIDE = DK > 32;
+  static constexpr int NKB = (DK + 31) / 32;          // 128-byte slabs per operand row
+  static constexpr int KSB = DK / 8 / NKB;            // k8 steps per slab
+  static constexpr int SBLK = WIDE ? 64 : 128;        // rows of a streamed block
+  static constexpr int NST = DK <= 64 ? 4 : 2;        // stages of the ring
+  static constexpr int TSLAB = LONG_BLK * 128;        // one slab of a tile operand
+  static constexpr int SSLAB = SBLK * 128;            // one slab of a streamed operand
+  static constexpr int TOP = NKB * TSLAB, SOP = NKB * SSLAB;
+  static constexpr int TBUF = 2 * TOP + 1024, SBUF = 2 * SOP + 1024;
+  static constexpr int OUT = WIDE ? 0 : 2 * 2048;     // per compute warp: two 16-row output boxes (wide: none)
+  // [tile buffer] [ring: NST buffers] [output boxes] [mbarriers: full[NST] empty[NST] res_full res_empty]
+  static constexpr int ring = TBUF;
+  static constexpr int out = ring + NST * SBUF;
+  static constexpr int bars = out + LONG_WARPS * OUT;
+  static constexpr int total = bars + 8 * (2 * NST + 2) + 1024;
+  static_assert(total <= 227 * 1024, "attention_long: shared memory");
+  static_assert(DK % 32 == 0 || DK == 16, "attention_long: DK is 16 or a multiple of 32");
 };
-static_assert(LongSmem::total <= 227 * 1024, "attention_long: shared memory");
 
 enum { LONG_FWD = 0, LONG_DKDV = 1, LONG_DQ = 2 };
 enum { AUX_NONE = 0, AUX_BITS = 1, AUX_STATS = 2 };
 
 // One CTA per SM walks the items blockIdx.x, blockIdx.x + gridDim.x, ...; item ((b * h) + head) * tiles + tile.
 // The last warp loads.  Per item it TMA-loads the tile's rows (forward: Q; dK / dV: K, V; dQ: Q, dO) into the tile
-// buffer (res_full; free again once every compute warp has taken its fragments: res_empty), then the streamed blocks
-// into the ring, in 16-row boxes up to the extent, each stage completing on full[stage] and freed by one arrival per
-// compute warp on empty[stage].  With the rows it writes a buffer's aux: the real-key bits of its keys, or the
-// per-query {nm = -max c - log2 sum, delta} of its queries (c = log2(e) / sqrt(dk)).  Operands are rounded to tf32
-// (cvt.rn) after every fragment load, which gives the values the short kernels round in place; with rounding off the
-// tensor core truncates.
+// buffer (res_full; free again once every compute warp is done with it: res_empty), then the streamed blocks into the
+// ring, in 16-row boxes up to the extent, each stage completing on full[stage] and freed by one arrival per compute
+// warp on empty[stage].  With the rows it writes a buffer's aux: the real-key bits of its keys, or the per-query
+// {nm = -max c - log2 sum, delta} of its queries (c = log2(e) / sqrt(w)).  Operands are rounded to tf32 (cvt.rn) after
+// every fragment load, which gives the values the short kernels round in place; with rounding off the tensor core
+// truncates.  Products run slab by slab and k-step by k-step, i.e. over the head columns in order, as the short
+// kernels do.
+//
+// Head widths w that are not a slab multiple run on the next DK up: the tensor maps have w columns, so TMA loads give
+// exact zeros in columns w ... DK - 1 (they add exact zeros to every product) and TMA stores clip at w.
 //
 // Extents: keys at or beyond a slate's extent are masked (probability exactly 0) and not streamed, so the work is
 // proportional to S * extent.  The forward computes every query row below round_up(S, 16) (padded items get the
@@ -61,13 +83,18 @@ __device__ __forceinline__ void attn_long_body(
     const CUtensorMap* tmO0, const CUtensorMap* tmO1, const uint8_t* __restrict__ mask, float* __restrict__ stat_max,
     float* __restrict__ stat_sum, const float* __restrict__ delta, int S, int n_heads, float scale, DropSite drop,
     float* __restrict__ dbias, int d_model, const int* __restrict__ extent, int n_items, int rnd) {
-  constexpr int KS = DK / 8;
+  using L = LongSmem<DK>;
+  constexpr int NKB = L::NKB, KSB = L::KSB, SBLK = L::SBLK, NST = L::NST;
+  constexpr bool WIDE = L::WIDE;
+  // the tile's fragments stay in registers for the whole item (the forward's Q at every width)
+  constexpr bool KEEP = !WIDE || MODE == LONG_FWD;
+  constexpr int DKDV_NB = DK > 64 ? 1 : 2;      // 8-query blocks in flight in dK / dV
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
   const uint32_t sbase = (ptx::smem_u32(smem_dyn) + 1023u) & ~1023u;
   uint8_t* smem = smem_dyn + (sbase - ptx::smem_u32(smem_dyn));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + LongSmem::bars);
-  uint64_t* empty = full + LONG_NST;
-  uint64_t* res_full = empty + LONG_NST;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::bars);
+  uint64_t* empty = full + NST;
+  uint64_t* res_full = empty + NST;
   uint64_t* res_empty = res_full + 1;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -76,7 +103,7 @@ __device__ __forceinline__ void attn_long_body(
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(tmR0); ptx::prefetch_tmap(tmR1); ptx::prefetch_tmap(tmS0); ptx::prefetch_tmap(tmS1);
-    for (int s = 0; s < LONG_NST; ++s) {
+    for (int s = 0; s < NST; ++s) {
       ptx::mbar_init(full + s, 33);         // the expect_tx arrival + every load lane after its aux stores
       ptx::mbar_init(empty + s, LONG_WARPS);
     }
@@ -98,36 +125,36 @@ __device__ __forceinline__ void attn_long_body(
     it.rows16 = (it.e + 15) & ~15;
     it.ns = min(LONG_WARPS, (S + 15) / 16 - LONG_WARPS * it.tile);       // strips of the tile below round_up(S, 16)
     it.live = MODE == LONG_FWD ? it.ns : max(0, min(it.ns, it.rows16 / 16 - LONG_WARPS * it.tile));
-    it.nblk = it.live > 0 ? (it.rows16 + LONG_BLK - 1) / LONG_BLK : 0;  // streamed blocks (keys, or queries for dK / dV)
+    it.nblk = it.live > 0 ? (it.rows16 + SBLK - 1) / SBLK : 0;          // streamed blocks (keys, or queries for dK / dV)
     return it;
   };
   constexpr int NPASS = MODE == LONG_FWD ? 2 : 1;
 
   if (warp == LONG_WARPS) {
     // ===== load warp
-    // rows row0 ... row0 + rows - 1 of `ops` operands into buffer `buf` (operand o at buf + o * LONG_OP), its aux, and
-    // the arrivals on `bar`
-    auto fill = [&](uint8_t* buf, uint64_t* bar, const Item& it, int row0, int rows, int ops, const CUtensorMap* m0,
-                    const CUtensorMap* m1, int aux) {
+    // rows row0 ... row0 + rows - 1 of `ops` operands into buffer `buf` (operand o, slab kb at buf + (o NKB + kb) slab),
+    // its aux (for `cap` rows), and the arrivals on `bar`
+    auto fill = [&](uint8_t* buf, uint64_t* bar, const Item& it, int row0, int rows, int ops, int slab, int cap,
+                    const CUtensorMap* m0, const CUtensorMap* m1, int aux) {
       ptx::fence_proxy_async_smem();
-      if (lane == 0) ptx::mbar_expect_tx(bar, uint32_t(rows * ops * 128));
+      if (lane == 0) ptx::mbar_expect_tx(bar, uint32_t(rows * ops * NKB * 128));
       __syncwarp();
       const int nb = rows >> 4;
-      for (int j = lane; j < ops * nb; j += 32) {
-        const int o = j / nb, i = j - o * nb;
-        ptx::tma_load_4d(buf + o * LONG_OP + i * 2048, o ? m1 : m0, bar, 0, row0 + 16 * i, it.head, it.b);
+      for (int j = lane; j < ops * NKB * nb; j += 32) {
+        const int o = j / (NKB * nb), r = j - o * (NKB * nb), kb = r / nb, i = r - kb * nb;
+        ptx::tma_load_4d(buf + (o * NKB + kb) * slab + i * 2048, o ? m1 : m0, bar, 32 * kb, row0 + 16 * i, it.head, it.b);
       }
-      uint8_t* ax = buf + 2 * LONG_OP;
+      uint8_t* ax = buf + 2 * NKB * slab;
       if (aux == AUX_BITS) {          // bit j of word w: key row0 + 32 w + j is real
-#pragma unroll
-        for (int w = 0; w < LONG_BLK / 32; ++w) {
+#pragma unroll 4
+        for (int w = 0; w < cap / 32; ++w) {
           const int key = row0 + 32 * w + lane;
           const uint32_t bw = __ballot_sync(FULL, key < S && mask[size_t(it.b) * S + key] == 0);
           if (lane == 0) reinterpret_cast<uint32_t*>(ax)[w] = bw;
         }
       } else if (aux == AUX_STATS) {  // queries the slate does not have: nm = -inf (probability 0)
-#pragma unroll
-        for (int w = 0; w < LONG_BLK / 32; ++w) {
+#pragma unroll 4
+        for (int w = 0; w < cap / 32; ++w) {
           const int qi = row0 + 32 * w + lane;
           float2 st = make_float2(-CUDART_INF_F, 0.f);
           if (qi < S) {
@@ -146,13 +173,13 @@ __device__ __forceinline__ void attn_long_body(
     for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k) {
       const Item it = item_info(item);
       if (k >= 1) ptx::mbar_wait(res_empty, (k - 1) & 1);
-      fill(smem, res_full, it, LONG_BLK * it.tile, 16 * it.live, RES_OPS, tmR0, tmR1, RES_AUX);
+      fill(smem, res_full, it, LONG_BLK * it.tile, 16 * it.live, RES_OPS, L::TSLAB, LONG_BLK, tmR0, tmR1, RES_AUX);
       for (int pass = 0; pass < NPASS; ++pass) {
         for (int blk = 0; blk < it.nblk; ++blk, ++cnt) {
-          const int st = cnt % LONG_NST;
-          if (cnt >= LONG_NST) ptx::mbar_wait(empty + st, ((cnt / LONG_NST) - 1) & 1);
-          fill(smem + LongSmem::ring + st * LONG_BUF, full + st, it, LONG_BLK * blk,
-               min(LONG_BLK, it.rows16 - LONG_BLK * blk), (MODE == LONG_FWD && pass == 0) ? 1 : 2, tmS0, tmS1, STR_AUX);
+          const int st = cnt % NST;
+          if (cnt >= NST) ptx::mbar_wait(empty + st, ((cnt / NST) - 1) & 1);
+          fill(smem + L::ring + st * L::SBUF, full + st, it, SBLK * blk, min(SBLK, it.rows16 - SBLK * blk),
+               (MODE == LONG_FWD && pass == 0) ? 1 : 2, L::SSLAB, SBLK, tmS0, tmS1, STR_AUX);
         }
       }
     }
@@ -162,21 +189,50 @@ __device__ __forceinline__ void attn_long_body(
   // ===== compute warps
   if constexpr (DROP) drop.seed = drop_seed(drop);
   auto rt = [&](uint32_t& x) { if (rnd) x = ptx::cvt_tf32(__uint_as_float(x)); };
-  const uint32_t res_s = sbase, box_s = sbase + LongSmem::out + warp * LONG_OUT;
-  uint8_t* box = smem + LongSmem::out + warp * LONG_OUT;
+  const int r0 = 16 * warp;                                            // the warp's strip rows in the tile buffer
+  const uint32_t res_s = sbase;
+  // output boxes: operand o, slab kb at ob_s + o * OB_OP + kb * L::TSLAB (wide: the warp's own tile rows)
+  constexpr int OB_OP = WIDE ? L::TOP : 2048;
+  const uint32_t ob_s = WIDE ? res_s + r0 * 128 : sbase + L::out + warp * L::OUT;
+  uint8_t* ob = smem + (ob_s - sbase);
+  // A fragment of k-step ks of slab kb of tile operand o, rows r0 ... r0 + 15 (wide dK / dV and dQ: from shared memory)
+  uint32_t ta[KEEP ? NKB : 1][KSB][4], tb[KEEP && MODE != LONG_FWD ? NKB : 1][KSB][4];
+  auto tfrag = [&](int o, int kb, int ks, uint32_t (&a)[4]) {
+    if constexpr (KEEP) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = o ? tb[kb][ks][i] : ta[kb][ks][i];
+    } else {
+      ld_a_step(res_s + o * L::TOP + kb * L::TSLAB, r0, lane, ks, a);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) rt(a[i]);
+    }
+  };
+  auto load_tile_frags = [&](int ops) {
+    if constexpr (KEEP) {
+#pragma unroll
+      for (int kb = 0; kb < NKB; ++kb) {
+        ld_a_head<KSB>(res_s + kb * L::TSLAB, r0, lane, ta[kb]);
+        if (ops > 1) ld_a_head<KSB>(res_s + L::TOP + kb * L::TSLAB, r0, lane, tb[kb]);
+#pragma unroll
+        for (int ks = 0; ks < KSB; ++ks)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) { rt(ta[kb][ks][i]); if (ops > 1) rt(tb[kb][ks][i]); }
+      }
+    }
+  };
   int cnt = 0, k = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k) {
     const Item it = item_info(item);
     const bool has = warp < it.ns, live = warp < it.live;
-    const int strip = LONG_WARPS * it.tile + warp, r0 = 16 * warp;      // r0: the strip's rows in the tile buffer
+    const int strip = LONG_WARPS * it.tile + warp;
     const unsigned long long dbase = (unsigned long long)(it.b * n_heads + it.head) * S;
     // the streamed blocks of this item: fn(block, buffer address) on the warps that have a live strip; every warp
     // frees every stage
     auto consume = [&](auto&& fn) {
       for (int blk = 0; blk < it.nblk; ++blk, ++cnt) {
-        const int st = cnt % LONG_NST;
-        ptx::mbar_wait(full + st, (cnt / LONG_NST) & 1);
-        if (live) fn(blk, sbase + LongSmem::ring + st * LONG_BUF);
+        const int st = cnt % NST;
+        ptx::mbar_wait(full + st, (cnt / NST) & 1);
+        if (live) fn(blk, sbase + L::ring + st * L::SBUF);
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(empty + st);
       }
@@ -185,30 +241,41 @@ __device__ __forceinline__ void attn_long_body(
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(res_empty);
     };
-    // a finished 16-row strip (rows g, g + 8 of acc, x mul) into the 128B-swizzled output box at `b`
-    auto stage_strip = [&](uint32_t b, const float (&acc)[KS][4], float mul) {
+    // a finished 16-row strip (rows g, g + 8 of acc, x mul) into the 128B-swizzled output box of operand o
+    auto stage_strip = [&](int o, const float (&acc)[NKB][KSB][4], float mul) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = g + 8 * h;
-        float v[2][KS];      // v[0]: head columns of output column 2t, v[1]: of 2t + 1 (n-tile order)
 #pragma unroll
-        for (int nt = 0; nt < KS; ++nt) { v[0][nt] = acc[nt][2 * h] * mul; v[1][nt] = acc[nt][2 * h + 1] * mul; }
-        if constexpr (KS == 4) {
-          sts128(b + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[0][2]), __float_as_uint(v[0][3])));
-          sts128(b + ptx::sw128(r, 64 + 16 * t), make_uint4(__float_as_uint(v[1][0]), __float_as_uint(v[1][1]), __float_as_uint(v[1][2]), __float_as_uint(v[1][3])));
-        } else {
-          sts128(b + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[1][0]), __float_as_uint(v[1][1])));
+        for (int kb = 0; kb < NKB; ++kb) {
+          const uint32_t b = ob_s + o * OB_OP + kb * L::TSLAB;
+          float v[2][KSB];      // v[0]: head columns of output column 2t, v[1]: of 2t + 1 (n-tile order)
+#pragma unroll
+          for (int nt = 0; nt < KSB; ++nt) { v[0][nt] = acc[kb][nt][2 * h] * mul; v[1][nt] = acc[kb][nt][2 * h + 1] * mul; }
+          if constexpr (KSB == 4) {
+            sts128(b + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[0][2]), __float_as_uint(v[0][3])));
+            sts128(b + ptx::sw128(r, 64 + 16 * t), make_uint4(__float_as_uint(v[1][0]), __float_as_uint(v[1][1]), __float_as_uint(v[1][2]), __float_as_uint(v[1][3])));
+          } else {
+            sts128(b + ptx::sw128(r, 16 * t), make_uint4(__float_as_uint(v[0][0]), __float_as_uint(v[0][1]), __float_as_uint(v[1][0]), __float_as_uint(v[1][1])));
+          }
         }
       }
     };
-    // QKV bias gradient: the staged strip's column sums (rows in order) added to this warp's own slot -- one slot per
-    // (CTA, warp), its items in a fixed order; DetParts sums the slots in order
-    auto bias_add = [&](int bx, int col0) {
-      if (dbias == nullptr || lane >= DK) return;
-      float s = 0.f;
+    // QKV bias gradient: the staged strip's column sums (rows in order) of the head's w real columns, added to this
+    // warp's own slot -- one slot per (CTA, warp), its items in a fixed order; DetParts sums the slots in order
+    auto bias_add = [&](int o, int col0) {
+      if (dbias == nullptr) return;
+      const int w = WIDE ? d_model / n_heads : DK;
 #pragma unroll
-      for (int r = 0; r < 16; ++r) s += *reinterpret_cast<const float*>(box + bx * 2048 + ptx::sw128(r, 4 * lane));
-      dbias[(size_t(blockIdx.x) * LONG_WARPS + warp) * 3 * d_model + col0 + it.head * DK + lane] += s;
+      for (int kb = 0; kb < NKB; ++kb) {
+        const int c = 32 * kb + lane;
+        if (c >= w) break;
+        const uint8_t* b = ob + o * OB_OP + kb * L::TSLAB;
+        float s = 0.f;
+#pragma unroll
+        for (int r = 0; r < 16; ++r) s += *reinterpret_cast<const float*>(b + ptx::sw128(r, 4 * lane));
+        dbias[(size_t(blockIdx.x) * LONG_WARPS + warp) * 3 * d_model + col0 + it.head * w + c] += s;
+      }
     };
     auto store_wait = [&]() {   // this warp's previous strip must have been read out of its boxes
       if (lane == 0) ptx::tma_store_wait_read();
@@ -218,9 +285,19 @@ __device__ __forceinline__ void attn_long_body(
       ptx::fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) {
-        ptx::tma_store_4d(tmO0, box, 0, 16 * strip, it.head, it.b);
-        if (nbox > 1) ptx::tma_store_4d(tmO1, box + 2048, 0, 16 * strip, it.head, it.b);
+        for (int o = 0; o < nbox; ++o)
+#pragma unroll
+          for (int kb = 0; kb < NKB; ++kb)
+            ptx::tma_store_4d(o ? tmO1 : tmO0, ob + o * OB_OP + kb * L::TSLAB, 32 * kb, 16 * strip, it.head, it.b);
         ptx::tma_store_commit();
+      }
+    };
+    // the narrow kernels free the tile as soon as its fragments are in registers; the wide ones once the strip's
+    // output has been read out of the tile rows
+    auto finish_tile = [&]() {
+      if constexpr (WIDE) {
+        store_wait();
+        release_tile();
       }
     };
     ptx::mbar_wait(res_full, k & 1);
@@ -228,26 +305,24 @@ __device__ __forceinline__ void attn_long_body(
     if constexpr (MODE == LONG_FWD) {
       // ===== 16 queries: pass A masked row maxima, pass B probabilities and O = P V (attn_fwd_kernel's strip)
       const int qA = 16 * strip + g, qB = qA + 8;
-      uint32_t qa[KS][4];
-      if (live) {
-        ld_a_head<KS>(res_s, r0, lane, qa);
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks) { rt(qa[ks][0]); rt(qa[ks][1]); rt(qa[ks][2]); rt(qa[ks][3]); }
-      }
-      release_tile();
+      if (live) load_tile_frags(1);
+      if constexpr (!WIDE) release_tile();
       // raw scores of keys 8j + t, 8j + t + 4 of the block at k_s for rows qA, qB
       auto scores = [&](uint32_t k_s, int j, float (&s4)[4]) {
         s4[0] = s4[1] = s4[2] = s4[3] = 0.f;
-        uint32_t kf[KS][2];
-        ld_b_head<KS>(k_s, 8 * j, lane, kf);
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) { rt(kf[ks][0]); rt(kf[ks][1]); ptx::mma_tf32(s4, qa[ks], kf[ks]); }
+        for (int kb = 0; kb < NKB; ++kb) {
+          uint32_t kf[KSB][2];
+          ld_b_head<KSB>(k_s + kb * L::SSLAB, 8 * j, lane, kf);
+#pragma unroll
+          for (int ks = 0; ks < KSB; ++ks) { rt(kf[ks][0]); rt(kf[ks][1]); ptx::mma_tf32(s4, ta[kb][ks], kf[ks]); }
+        }
       };
       const int nj_all = (it.e + 7) >> 3;
       float mxA = -CUDART_INF_F, mxB = -CUDART_INF_F;
       consume([&](int blk, uint32_t buf) {
-        const uint32_t* bits = reinterpret_cast<const uint32_t*>(smem + (buf - sbase) + 2 * LONG_OP);
-        const int nj = min(LONG_BLK / 8, nj_all - LONG_BLK / 8 * blk);
+        const uint32_t* bits = reinterpret_cast<const uint32_t*>(smem + (buf - sbase) + 2 * L::SOP);
+        const int nj = min(SBLK / 8, nj_all - SBLK / 8 * blk);
 #pragma unroll 2
         for (int j = 0; j < nj; ++j) {
           float s4[4];
@@ -262,13 +337,15 @@ __device__ __forceinline__ void attn_long_body(
       const float mxsA = mxA * c_log2e, mxsB = mxB * c_log2e;
       const bool odd = (t & 1) != 0;
       float sumA = 0.f, sumB = 0.f;
-      float o[KS][4];
+      float o[NKB][KSB][4];
 #pragma unroll
-      for (int nt = 0; nt < KS; ++nt) o[nt][0] = o[nt][1] = o[nt][2] = o[nt][3] = 0.f;
+      for (int kb = 0; kb < NKB; ++kb)
+#pragma unroll
+        for (int nt = 0; nt < KSB; ++nt) o[kb][nt][0] = o[kb][nt][1] = o[kb][nt][2] = o[kb][nt][3] = 0.f;
       consume([&](int blk, uint32_t buf) {
-        const uint32_t* bits = reinterpret_cast<const uint32_t*>(smem + (buf - sbase) + 2 * LONG_OP);
-        const uint32_t v_s = buf + LONG_OP;
-        const int nj = min(LONG_BLK / 8, nj_all - LONG_BLK / 8 * blk);
+        const uint32_t* bits = reinterpret_cast<const uint32_t*>(smem + (buf - sbase) + 2 * L::SOP);
+        const uint32_t v_s = buf + L::SOP;
+        const int nj = min(SBLK / 8, nj_all - SBLK / 8 * blk);
 #pragma unroll 2
         for (int j = 0; j < nj; ++j) {
           float s4[4];
@@ -286,7 +363,7 @@ __device__ __forceinline__ void attn_long_body(
           sumA += odd ? xA + p[1] : p[0] + xA;
           sumB += odd ? xB + p[3] : p[2] + xB;
           if constexpr (DROP) {
-            const int key0 = LONG_BLK * blk + 8 * j + t;
+            const int key0 = SBLK * blk + 8 * j + t;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const unsigned long long idx = (dbase + (i < 2 ? qA : qB)) * (unsigned long long)S + (key0 + 4 * (i & 1));
@@ -295,14 +372,17 @@ __device__ __forceinline__ void attn_long_body(
           }
           const uint32_t pa[4] = {__float_as_uint(round_tf32(p[0])), __float_as_uint(round_tf32(p[2])),
                                   __float_as_uint(round_tf32(p[1])), __float_as_uint(round_tf32(p[3]))};
-          uint32_t v0[KS], v1[KS];
-          ld_b_out<KS>(v_s, 8 * j + t, g, v0);
-          ld_b_out<KS>(v_s, 8 * j + t + 4, g, v1);
 #pragma unroll
-          for (int nt = 0; nt < KS; ++nt) {
-            rt(v0[nt]); rt(v1[nt]);
-            const uint32_t vb[2] = {v0[nt], v1[nt]};
-            ptx::mma_tf32(o[nt], pa, vb);
+          for (int kb = 0; kb < NKB; ++kb) {
+            uint32_t v0[KSB], v1[KSB];
+            ld_b_out<KSB>(v_s + kb * L::SSLAB, 8 * j + t, g, v0);
+            ld_b_out<KSB>(v_s + kb * L::SSLAB, 8 * j + t + 4, g, v1);
+#pragma unroll
+            for (int nt = 0; nt < KSB; ++nt) {
+              rt(v0[nt]); rt(v1[nt]);
+              const uint32_t vb[2] = {v0[nt], v1[nt]};
+              ptx::mma_tf32(o[kb][nt], pa, vb);
+            }
           }
         }
       });
@@ -316,54 +396,67 @@ __device__ __forceinline__ void attn_long_body(
         }
         store_wait();
         // O / rowsum, per row (one reciprocal each, as attn_fwd_kernel)
-        float oA[KS][4];
         const float invA = 1.0f / sumA, invB = 1.0f / sumB;
 #pragma unroll
-        for (int nt = 0; nt < KS; ++nt) {
-          oA[nt][0] = o[nt][0] * invA; oA[nt][1] = o[nt][1] * invA;
-          oA[nt][2] = o[nt][2] * invB; oA[nt][3] = o[nt][3] * invB;
-        }
-        stage_strip(box_s, oA, 1.0f);
+        for (int kb = 0; kb < NKB; ++kb)
+#pragma unroll
+          for (int nt = 0; nt < KSB; ++nt) {
+            o[kb][nt][0] *= invA; o[kb][nt][1] *= invA;
+            o[kb][nt][2] *= invB; o[kb][nt][3] *= invB;
+          }
+        stage_strip(0, o, 1.0f);
         store(1);
       }
+      finish_tile();
     } else if constexpr (MODE == LONG_DKDV) {
       // ===== 16 keys kA = 16 strip + g, kB = kA + 8: dV, dK over the streamed queries (attn_bwd_kernel's key strip)
       const int kA = 16 * strip + g, kB = kA + 8;
-      uint32_t ka[KS][4], va[KS][4];
       bool liveA = false, liveB = false;
       if (live) {
-        const uint32_t kw = reinterpret_cast<const uint32_t*>(smem + 2 * LONG_OP)[warp >> 1];
+        const uint32_t kw = reinterpret_cast<const uint32_t*>(smem + 2 * L::TOP)[warp >> 1];
         liveA = (kw >> ((r0 + g) & 31)) & 1u;
         liveB = (kw >> ((r0 + g + 8) & 31)) & 1u;
-        ld_a_head<KS>(res_s, r0, lane, ka);
-        ld_a_head<KS>(res_s + LONG_OP, r0, lane, va);
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { rt(ka[ks][i]); rt(va[ks][i]); }
+        load_tile_frags(2);
       }
-      release_tile();
-      float dv[KS][4], dk[KS][4];
+      if constexpr (!WIDE) release_tile();
+      float dv[NKB][KSB][4], dk[NKB][KSB][4];
 #pragma unroll
-      for (int nt = 0; nt < KS; ++nt)
+      for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
-        for (int i = 0; i < 4; ++i) dv[nt][i] = dk[nt][i] = 0.f;
+        for (int nt = 0; nt < KSB; ++nt)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) dv[kb][nt][i] = dk[kb][nt][i] = 0.f;
       const int nq8 = (it.e + 7) & ~7;     // queries at or beyond the extent have zero d ctx rows
       consume([&](int blk, uint32_t buf) {
-        const uint32_t q_s = buf, do_s = buf + LONG_OP, st_s = buf + 2 * LONG_OP;
-        const int qbase = LONG_BLK * blk, nq = min(LONG_BLK, nq8 - qbase);
-        // S^T, dP^T of the 8-query block q0 (of the buffer)
-        auto products = [&](int q0, float (&s)[4], float (&dp)[4]) {
+        const uint32_t q_s = buf, do_s = buf + L::SOP, st_s = buf + 2 * L::SOP;
+        const int qbase = SBLK * blk, nq = min(SBLK, nq8 - qbase);
+        // S^T, dP^T of the NB 8-query blocks q0, q0 + 8 (of the buffer)
+        auto products = [&](auto nbc, int q0, float (&s)[2][4], float (&dp)[2][4]) {
+          constexpr int NB = decltype(nbc)::value;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) s[i] = dp[i] = 0.f;
-          uint32_t qb[KS][2], ob[KS][2];
-          ld_b_head<KS>(q_s, q0, lane, qb);
-          ld_b_head<KS>(do_s, q0, lane, ob);
+          for (int n = 0; n < NB; ++n)
 #pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-            rt(qb[ks][0]); rt(qb[ks][1]); rt(ob[ks][0]); rt(ob[ks][1]);
-            ptx::mma_tf32(s, ka[ks], qb[ks]);
-            ptx::mma_tf32(dp, va[ks], ob[ks]);
+            for (int i = 0; i < 4; ++i) s[n][i] = dp[n][i] = 0.f;
+#pragma unroll
+          for (int kb = 0; kb < NKB; ++kb) {
+            uint32_t qb[NB][KSB][2], ob2[NB][KSB][2];
+#pragma unroll
+            for (int n = 0; n < NB; ++n) {
+              ld_b_head<KSB>(q_s + kb * L::SSLAB, q0 + 8 * n, lane, qb[n]);
+              ld_b_head<KSB>(do_s + kb * L::SSLAB, q0 + 8 * n, lane, ob2[n]);
+            }
+#pragma unroll
+            for (int ks = 0; ks < KSB; ++ks) {
+              uint32_t ka[4], va[4];
+              tfrag(0, kb, ks, ka);
+              tfrag(1, kb, ks, va);
+#pragma unroll
+              for (int n = 0; n < NB; ++n) {
+                rt(qb[n][ks][0]); rt(qb[n][ks][1]); rt(ob2[n][ks][0]); rt(ob2[n][ks][1]);
+                ptx::mma_tf32(s[n], ka, qb[n][ks]);
+                ptx::mma_tf32(dp[n], va, ob2[n][ks]);
+              }
+            }
           }
         };
         // P^T, dS^T of the block and its dV, dK products
@@ -387,76 +480,90 @@ __device__ __forceinline__ void attn_long_body(
           }
           const uint32_t pa[4] = {__float_as_uint(pu[0]), __float_as_uint(pu[2]), __float_as_uint(pu[1]), __float_as_uint(pu[3])};
           const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
-          uint32_t o0[KS], o1[KS], q0v[KS], q1v[KS];
-          ld_b_out<KS>(do_s, q0 + t, g, o0); ld_b_out<KS>(do_s, q0 + t + 4, g, o1);
-          ld_b_out<KS>(q_s, q0 + t, g, q0v); ld_b_out<KS>(q_s, q0 + t + 4, g, q1v);
 #pragma unroll
-          for (int nt = 0; nt < KS; ++nt) {
-            rt(o0[nt]); rt(o1[nt]); rt(q0v[nt]); rt(q1v[nt]);
-            const uint32_t ob[2] = {o0[nt], o1[nt]}, qb[2] = {q0v[nt], q1v[nt]};
-            ptx::mma_tf32(dv[nt], pa, ob);
-            ptx::mma_tf32(dk[nt], dsa, qb);
+          for (int kb = 0; kb < NKB; ++kb) {
+            uint32_t o0[KSB], o1[KSB], q0v[KSB], q1v[KSB];
+            ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t, g, o0); ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t + 4, g, o1);
+            ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t, g, q0v); ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t + 4, g, q1v);
+#pragma unroll
+            for (int nt = 0; nt < KSB; ++nt) {
+              rt(o0[nt]); rt(o1[nt]); rt(q0v[nt]); rt(q1v[nt]);
+              const uint32_t obv[2] = {o0[nt], o1[nt]}, qbv[2] = {q0v[nt], q1v[nt]};
+              ptx::mma_tf32(dv[kb][nt], pa, obv);
+              ptx::mma_tf32(dk[kb][nt], dsa, qbv);
+            }
           }
         };
-        // two blocks in flight
+        // two blocks in flight (DK 96: one, or the accumulators spill)
         int q0 = 0;
-        for (; q0 + 16 <= nq; q0 += 16) {
-          float s0[4], dp0[4], s1[4], dp1[4];
-          products(q0, s0, dp0);
-          products(q0 + 8, s1, dp1);
-          accumulate(q0, s0, dp0);
-          accumulate(q0 + 8, s1, dp1);
+        for (; q0 + 8 * DKDV_NB <= nq; q0 += 8 * DKDV_NB) {
+          float s[2][4], dp[2][4];
+          products(std::integral_constant<int, DKDV_NB>{}, q0, s, dp);
+#pragma unroll
+          for (int n = 0; n < DKDV_NB; ++n) accumulate(q0 + 8 * n, s[n], dp[n]);
         }
         if (q0 < nq) {
-          float s0[4], dp0[4];
-          products(q0, s0, dp0);
-          accumulate(q0, s0, dp0);
+          float s[2][4], dp[2][4];
+          products(std::integral_constant<int, 1>{}, q0, s, dp);
+          accumulate(q0, s[0], dp[0]);
         }
       });
       if (has) {
         store_wait();
-        stage_strip(box_s, dv, 1.0f);
-        stage_strip(box_s + 2048, dk, scale);
+        stage_strip(0, dv, 1.0f);
+        stage_strip(1, dk, scale);
         __syncwarp();
         if (live) { bias_add(0, 2 * d_model); bias_add(1, d_model); }
         store(2);
       }
+      finish_tile();
     } else {
       // ===== 16 queries qA = 16 strip + g, qB = qA + 8: dQ over the streamed keys (attn_bwd_kernel's query strip)
       const int qA = 16 * strip + g, qB = qA + 8;
-      uint32_t qa[KS][4], oa[KS][4];
       float2 stA = make_float2(0.f, 0.f), stB = stA;
       if (live) {
-        const float2* qst = reinterpret_cast<const float2*>(smem + 2 * LONG_OP);
+        const float2* qst = reinterpret_cast<const float2*>(smem + 2 * L::TOP);
         stA = qst[r0 + g];
         stB = qst[r0 + g + 8];
-        ld_a_head<KS>(res_s, r0, lane, qa);
-        ld_a_head<KS>(res_s + LONG_OP, r0, lane, oa);
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { rt(qa[ks][i]); rt(oa[ks][i]); }
+        load_tile_frags(2);
       }
-      release_tile();
-      float dq[KS][4];
+      if constexpr (!WIDE) release_tile();
+      float dq[NKB][KSB][4];
 #pragma unroll
-      for (int nt = 0; nt < KS; ++nt) dq[nt][0] = dq[nt][1] = dq[nt][2] = dq[nt][3] = 0.f;
+      for (int kb = 0; kb < NKB; ++kb)
+#pragma unroll
+        for (int nt = 0; nt < KSB; ++nt) dq[kb][nt][0] = dq[kb][nt][1] = dq[kb][nt][2] = dq[kb][nt][3] = 0.f;
       const int nk8 = (it.e + 7) & ~7;     // keys at or beyond the extent are masked
       consume([&](int blk, uint32_t buf) {
-        const uint32_t k_s = buf, v_s = buf + LONG_OP, kb_s = buf + 2 * LONG_OP;
-        const int kbase = LONG_BLK * blk, nk = min(LONG_BLK, nk8 - kbase);
-        // S, dP of the 8-key block k0 (of the buffer)
-        auto products = [&](int k0, float (&s)[4], float (&dp)[4]) {
+        const uint32_t k_s = buf, v_s = buf + L::SOP, kb_s = buf + 2 * L::SOP;
+        const int kbase = SBLK * blk, nk = min(SBLK, nk8 - kbase);
+        // S, dP of the NB 8-key blocks k0, k0 + 8 (of the buffer)
+        auto products = [&](auto nbc, int k0, float (&s)[2][4], float (&dp)[2][4]) {
+          constexpr int NB = decltype(nbc)::value;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) s[i] = dp[i] = 0.f;
-          uint32_t kb[KS][2], vb[KS][2];
-          ld_b_head<KS>(k_s, k0, lane, kb);
-          ld_b_head<KS>(v_s, k0, lane, vb);
+          for (int n = 0; n < NB; ++n)
 #pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-            rt(kb[ks][0]); rt(kb[ks][1]); rt(vb[ks][0]); rt(vb[ks][1]);
-            ptx::mma_tf32(s, qa[ks], kb[ks]);
-            ptx::mma_tf32(dp, oa[ks], vb[ks]);
+            for (int i = 0; i < 4; ++i) s[n][i] = dp[n][i] = 0.f;
+#pragma unroll
+          for (int kb = 0; kb < NKB; ++kb) {
+            uint32_t kbf[NB][KSB][2], vbf[NB][KSB][2];
+#pragma unroll
+            for (int n = 0; n < NB; ++n) {
+              ld_b_head<KSB>(k_s + kb * L::SSLAB, k0 + 8 * n, lane, kbf[n]);
+              ld_b_head<KSB>(v_s + kb * L::SSLAB, k0 + 8 * n, lane, vbf[n]);
+            }
+#pragma unroll
+            for (int ks = 0; ks < KSB; ++ks) {
+              uint32_t qa[4], oa[4];
+              tfrag(0, kb, ks, qa);
+              tfrag(1, kb, ks, oa);
+#pragma unroll
+              for (int n = 0; n < NB; ++n) {
+                rt(kbf[n][ks][0]); rt(kbf[n][ks][1]); rt(vbf[n][ks][0]); rt(vbf[n][ks][1]);
+                ptx::mma_tf32(s[n], qa, kbf[n][ks]);
+                ptx::mma_tf32(dp[n], oa, vbf[n][ks]);
+              }
+            }
           }
         };
         // dS of the block and its dQ products
@@ -476,36 +583,39 @@ __device__ __forceinline__ void attn_long_body(
             ds[i] = round_tf32(p * (dpv - st.y));
           }
           const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
-          uint32_t k0v[KS], k1v[KS];
-          ld_b_out<KS>(k_s, k0 + t, g, k0v); ld_b_out<KS>(k_s, k0 + t + 4, g, k1v);
 #pragma unroll
-          for (int nt = 0; nt < KS; ++nt) {
-            rt(k0v[nt]); rt(k1v[nt]);
-            const uint32_t kb[2] = {k0v[nt], k1v[nt]};
-            ptx::mma_tf32(dq[nt], dsa, kb);
+          for (int kb = 0; kb < NKB; ++kb) {
+            uint32_t k0v[KSB], k1v[KSB];
+            ld_b_out<KSB>(k_s + kb * L::SSLAB, k0 + t, g, k0v); ld_b_out<KSB>(k_s + kb * L::SSLAB, k0 + t + 4, g, k1v);
+#pragma unroll
+            for (int nt = 0; nt < KSB; ++nt) {
+              rt(k0v[nt]); rt(k1v[nt]);
+              const uint32_t kbv[2] = {k0v[nt], k1v[nt]};
+              ptx::mma_tf32(dq[kb][nt], dsa, kbv);
+            }
           }
         };
         int k0 = 0;
         for (; k0 + 16 <= nk; k0 += 16) {
-          float s0[4], dp0[4], s1[4], dp1[4];
-          products(k0, s0, dp0);
-          products(k0 + 8, s1, dp1);
-          accumulate(k0, s0, dp0);
-          accumulate(k0 + 8, s1, dp1);
+          float s[2][4], dp[2][4];
+          products(std::integral_constant<int, 2>{}, k0, s, dp);
+          accumulate(k0, s[0], dp[0]);
+          accumulate(k0 + 8, s[1], dp[1]);
         }
         if (k0 < nk) {
-          float s0[4], dp0[4];
-          products(k0, s0, dp0);
-          accumulate(k0, s0, dp0);
+          float s[2][4], dp[2][4];
+          products(std::integral_constant<int, 1>{}, k0, s, dp);
+          accumulate(k0, s[0], dp[0]);
         }
       });
       if (has) {
         store_wait();
-        stage_strip(box_s, dq, scale);
+        stage_strip(0, dq, scale);
         __syncwarp();
         if (live) bias_add(0, 0);
         store(1);
       }
+      finish_tile();
     }
   }
   if (lane == 0) ptx::tma_store_wait_all();
@@ -540,6 +650,9 @@ static double long_bytes(int S, int dk, int tile_ops, int stream_ops, int out_op
   return 4.0 * S * dk * (tile_ops + out_ops + tiles * stream_ops);
 }
 
+// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96)
+static int long_dk(int dk) { return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : 96; }
+
 template <int DK>
 static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   alignas(64) CUtensorMap tQ, tK, tV, tO;
@@ -554,15 +667,20 @@ static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   dim3 grid(std::max(1, std::min(n_items, sm_count())));
   ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 4.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                double(a.B) * a.h * (long_bytes(a.S, a.dk, 1, 3, 1) + 8.0 * a.S), "attn_long_fwd_kernel");
-  return launch(kern, grid, dim3(LONG_THREADS), size_t(LongSmem::total), st, /*pdl=*/true, tQ, tQ, tK, tV, tO, tO,
+  return launch(kern, grid, dim3(LONG_THREADS), size_t(LongSmem<DK>::total), st, /*pdl=*/true, tQ, tQ, tK, tV, tO, tO,
                 a.mask, a.stat_max, a.stat_sum, static_cast<const float*>(nullptr), a.S, a.h, a.scale, a.drop,
                 static_cast<float*>(nullptr), 0, a.extent, n_items, tf32_round_on_load());
 }
 
 int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st) {
-  if (a.o.bf16) { arb_set_error("attn_fwd: a bf16 context needs slate_length <= 256"); return ARB_E_UNSUPPORTED; }
-  if (a.pack_off) { arb_set_error("attn_fwd: packed rows need slate_length <= 256"); return ARB_E_UNSUPPORTED; }
-  return a.dk == 16 ? launch_long_fwd_t<16>(a, st) : launch_long_fwd_t<32>(a, st);
+  if (a.o.bf16) { arb_set_error("attn_fwd: a bf16 context needs slate_length <= 256 and head width 16, 32 or 64"); return ARB_E_UNSUPPORTED; }
+  if (a.pack_off) { arb_set_error("attn_fwd: packed rows need slate_length <= 256 and head width 16, 32 or 64"); return ARB_E_UNSUPPORTED; }
+  switch (long_dk(a.dk)) {
+    case 16: return launch_long_fwd_t<16>(a, st);
+    case 32: return launch_long_fwd_t<32>(a, st);
+    case 64: return launch_long_fwd_t<64>(a, st);
+    default: return launch_long_fwd_t<96>(a, st);
+  }
 }
 
 template <int DK>
@@ -580,6 +698,7 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const bool drop = a.drop.thresh != 0;
   const LongKernel kdkdv = drop ? attn_long_dkdv_kernel<DK, true> : attn_long_dkdv_kernel<DK, false>;
   const LongKernel kdq = drop ? attn_long_dq_kernel<DK, true> : attn_long_dq_kernel<DK, false>;
+  constexpr size_t smem = size_t(LongSmem<DK>::total);
   const int n_items = long_items(a.B, a.h, a.S);
   const int n_ctas = std::max(1, std::min(n_items, sm_count()));
   // the QKV bias gradient: one slot per (CTA, compute warp), summed in order afterwards
@@ -593,7 +712,7 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   {
     ProfScope ps(ARB_PROF_GEMM, frac * 8.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                  double(a.B) * a.h * (long_bytes(a.S, a.dk, 2, 2, 2) + 8.0 * a.S), "attn_long_dkdv_kernel");
-    if ((rc = launch(kdkdv, dim3(n_ctas), dim3(LONG_THREADS), size_t(LongSmem::total), st, /*pdl=*/true, tK, tV, tQ,
+    if ((rc = launch(kdkdv, dim3(n_ctas), dim3(LONG_THREADS), smem, st, /*pdl=*/true, tK, tV, tQ,
                      tDO, tDV, tDK, a.mask, smax, ssum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent,
                      n_items, tf32_round_on_load())))
       return rc;
@@ -601,7 +720,7 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   {
     ProfScope ps(ARB_PROF_GEMM, frac * 6.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
                  double(a.B) * a.h * (long_bytes(a.S, a.dk, 2, 2, 1) + 12.0 * a.S), "attn_long_dq_kernel");
-    if ((rc = launch(kdq, dim3(n_ctas), dim3(LONG_THREADS), size_t(LongSmem::total), st, /*pdl=*/true, tQ, tDO, tK,
+    if ((rc = launch(kdq, dim3(n_ctas), dim3(LONG_THREADS), smem, st, /*pdl=*/true, tQ, tDO, tK,
                      tV, tDQ, tDQ, a.mask, smax, ssum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent,
                      n_items, tf32_round_on_load())))
       return rc;
@@ -610,7 +729,12 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 int launch_attn_long_bwd(const AttnBwdArgs& a, cudaStream_t st) {
-  return a.dk == 16 ? launch_long_bwd_t<16>(a, st) : launch_long_bwd_t<32>(a, st);
+  switch (long_dk(a.dk)) {
+    case 16: return launch_long_bwd_t<16>(a, st);
+    case 32: return launch_long_bwd_t<32>(a, st);
+    case 64: return launch_long_bwd_t<64>(a, st);
+    default: return launch_long_bwd_t<96>(a, st);
+  }
 }
 
 }  // namespace arb

@@ -38,7 +38,8 @@ static int g_skip_padding = ARB_DEFAULT_SKIP_PADDING;
 // computes for an all-zero feature row, which every consumer in allRank masks: DESIGN.md 4.12); 0: dense [B*S] rows
 static int g_pack_rows = ARB_DEFAULT_PACK_ROWS;
 // Beyond 256 items the fused kernels (attention_long.cu) read and write fp32 only: bf16 mode keeps the unfused path
-// there (which it does not support, so such a call fails as before).
+// there (which it does not support, so such a call fails as before).  At head widths above 32 the fused kernels refuse
+// a bf16 context, so bf16 mode fails there too.
 static bool use_fused(const arb_scorer_config& c, int S) {
   return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, c.d_model / c.n_heads) && !(c.bf16 && S > 256);
 }
@@ -64,13 +65,13 @@ static bool use_ffn_chain(const arb_scorer_config& c, int64_t rows) {
          rows >= int64_t(4) * 128 * sm_count();
 }
 
-// Packed rows need both fused attention kernels of slates up to 256 items (they take per-slate row offsets; the
-// longer slates' kernels run the dense layout, which scores padded items as the reference does) and, so far, a call
+// Packed rows need both fused attention kernels of slates up to 256 items at head width 16 or 32 (they take per-slate
+// row offsets; attention_long.cu runs the dense layout, which scores padded items as the reference does) and, so far, a call
 // without dropout (its counters index the dense layout), without a positional encoding and with a single output per
 // item.
 static bool pack_eligible(const arb_scorer_config& c, int S) {
-  return c.n_layers > 0 && S <= 256 && use_fused_bwd(c, S) && c.dropout == 0.0f && c.fc_dropout == 0.0f && c.pe_mode == 0 &&
-         n_outputs(c) == 1;
+  return c.n_layers > 0 && S <= 256 && c.d_model / c.n_heads <= 32 && use_fused_bwd(c, S) && c.dropout == 0.0f &&
+         c.fc_dropout == 0.0f && c.pe_mode == 0 && n_outputs(c) == 1;
 }
 static bool use_pack(const arb_scorer_config& c, int S) { return g_pack_rows && g_skip_padding && pack_eligible(c, S); }
 
@@ -955,7 +956,7 @@ static int attention_hook_check(const char* what, int B, int S, int h, float p, 
   if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
   if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
   if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
-    arb_set_error((std::string(what) + ": unsupported shape (S <= 256 at head width 16, 32 or 64, backward 16 or 32; S <= 4096 at head width 16 or 32)").c_str());
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 96 in steps of 4)").c_str());
     return ARB_E_UNSUPPORTED;
   }
   return ARB_OK;

@@ -1,0 +1,117 @@
+"""Training steps of the shipped Transformer configurations whose heads are wider than 32 columns -- local_config
+(d 64, h 1: width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96,
+h 1: width 96) -- and of a d = 256, h = 4 model (width 64), each with its own dropout and loss: the fused attention
+kernels (attention mode 2; csrc/attention_long.cu serves these widths) against the unfused sequence
+(arb_set_attention_mode(0): [B, h, S, S] probabilities in HBM) where the latter exists (S <= 1536).
+
+    python tools/bench_head_widths.py [--steps 5] [--warmup 2] [--runs 3] [--json out.json]
+
+Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the width-96 model at S = 1024, 2048, 4096
+(B = 245760 / S slates, fewer where the unfused path would not fit in memory).  Slate lengths ~ N(S/2, S/4) clamped to
+[1, S].  Step time is the host clock around `steps` training steps that end in a device synchronise, per run; the
+modes alternate run by run.  Peak memory is torch.cuda.max_memory_allocated over a run.  The attention kernels' times
+come from torch.profiler in a separate run per shape.  The GPU's name and power limit are printed with the numbers."""
+import argparse
+import json
+import os
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from tools.bench_long_slates import gpu_info, kernel_times, set_mode, timed  # noqa: E402
+
+# the `model` and `loss` sections of the shipped configurations (d_256_h4: a wider model at the same width as local_config)
+MODELS = {
+    "local_config": (dict(fc_model={"sizes": [64], "input_norm": False, "activation": None, "dropout": 0.0},
+                          transformer={"N": 1, "d_ff": 64, "h": 1, "positional_encoding": None, "dropout": 0.0},
+                          post_model={"output_activation": "Sigmoid", "d_output": 4}), ("ordinal", {"n": 4})),
+    "ordinal": (dict(fc_model={"sizes": [144], "input_norm": False, "activation": None, "dropout": 0.0},
+                     transformer={"N": 4, "d_ff": 512, "h": 2, "positional_encoding": None, "dropout": 0.4},
+                     post_model={"output_activation": "Sigmoid", "d_output": 4}), ("ordinal", {"n": 4})),
+    "approxndcg": (dict(fc_model={"sizes": [96], "input_norm": False, "activation": None, "dropout": 0.0},
+                        transformer={"N": 2, "d_ff": 384, "h": 1, "positional_encoding": None, "dropout": 0.1},
+                        post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
+    "d256_h4": (dict(fc_model={"sizes": [256], "input_norm": False, "activation": None, "dropout": 0.0},
+                     transformer={"N": 2, "d_ff": 1024, "h": 4, "positional_encoding": None, "dropout": 0.1},
+                     post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
+}
+SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [("approxndcg", 245760 // S, S)
+                                                                     for S in (1024, 2048, 4096)]
+
+
+def make_batch(B, S, seed=7):
+    from allrank_b200.synth import make_slates
+    x, y, _ = make_slates(B, S, n_features=136, seed=seed, mean_len=S / 2, std_len=S / 4)
+    return x.cuda(), y.cuda()
+
+
+def make_step(name):
+    from allrank_b200 import losses
+    from allrank_b200.model import make_model
+    from allrank_b200.optim import FlatAdam
+    cfg, (loss_name, loss_args) = MODELS[name]
+    torch.manual_seed(0)
+    model = make_model(**cfg, n_features=136).cuda().train()
+    opt = FlatAdam(model, lr=1e-3)
+    loss_fn = getattr(losses, loss_name)
+
+    def step(x, y):
+        loss = loss_fn(model(x, y == -1, None), y, **loss_args)
+        opt.zero_grad()
+        loss.backward()
+        opt.step()
+        return loss
+    return step
+
+
+def fits_unfused(name, B, S):
+    """The unfused path's [B, h, S, S] buffers: one per layer in the workspace plus two in the backward scratch."""
+    t = MODELS[name][0]["transformer"]
+    return S <= 1536 and (t["N"] + 2) * B * t["h"] * S * S * 4 < 0.7 * torch.cuda.get_device_properties(0).total_memory
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    name_gpu, power = gpu_info()
+    print(f"GPU: {name_gpu}; power limit, max SM clock: {power}", flush=True)
+    rows = []
+    for name, B, S in SHAPES:
+        step = make_step(name)
+        modes = (2, 0) if fits_unfused(name, B, S) else (2,)
+        x, y = make_batch(B, S)
+        res = {m: [] for m in modes}
+        for _ in range(args.runs):
+            for m in modes:
+                set_mode(m)
+                res[m].append(timed(step, x, y, args.steps, args.warmup))
+        kt = {}
+        for m in modes:
+            set_mode(m)
+            kt[m] = kernel_times(step, x, y)
+        set_mode(2)
+        for m in modes:
+            ms = [r[0] for r in res[m]]
+            mem = max(r[1] for r in res[m])
+            row = dict(model=name, B=B, S=S, path="fused" if m == 2 else "unfused", step_ms=ms, peak_gib=mem,
+                       attention_kernel_ms=kt[m])
+            rows.append(row)
+            print(f"{name:12s} B={B:5d} S={S:5d} {row['path']:7s} step ms " + " / ".join(f"{v:8.2f}" for v in ms) +
+                  f"   peak {mem:6.2f} GiB   kernels " + ", ".join(f"{k} {v:.2f}" for k, v in sorted(kt[m].items())),
+                  flush=True)
+        del x, y, step
+        torch.cuda.empty_cache()
+    if args.json:
+        with open(args.json, "w") as fh:
+            json.dump(dict(gpu=name_gpu, power=power, steps=args.steps, rows=rows), fh, indent=1)
+
+
+if __name__ == "__main__":
+    main()
