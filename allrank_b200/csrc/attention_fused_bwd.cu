@@ -22,8 +22,8 @@ constexpr int BWD_WARPS = 8;                          // compute warps: one 16-r
 constexpr int BWD_THREADS = 32 * (BWD_WARPS + 2);     // + one load warp, one store warp
 
 // delta[b,h,q] = sum_e dO[b,q,h,e] * O[b,q,h,e]: one warp per row of the [B*S, d_model] activations, 128-bit loads,
-// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32, 64}: 4, 8 or 16 lanes per head);
-// other widths (36 ... 96) reduce one head at a time over the whole warp.
+// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32, 64, 128}: 4, 8, 16 or 32 lanes per
+// head); other widths (36 ... 124) reduce one head at a time over the whole warp.
 constexpr int DELTA_RPW = 4;     // rows per warp of the delta kernel
 __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ d_o, const float* __restrict__ o,
                                                          long long pitch, int B, int S, int h, int dk,
@@ -43,8 +43,8 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
 #pragma unroll
   for (int q = 0; q < DELTA_RPW; ++q) item[q] = (row0 + q < rows) ? (rowmap ? (long long)rowmap[row0 + q] : row0 + q) : -1;
   if (dk & (dk - 1)) {
-    // a width that is not a power of two (36 ... 96, dense fp32 rows): one head at a time, lane l takes its columns
-    // 4l ... 4l + 3 (dk / 4 <= 24 lanes), reduced over the whole warp
+    // a width that is not a power of two (36 ... 124, dense fp32 rows): one head at a time, lane l takes its columns
+    // 4l ... 4l + 3 (dk / 4 <= 31 lanes), reduced over the whole warp
     for (int head = 0; head < h; ++head) {
       const int c = head * dk + lane * 4;
       const bool on = lane < lanes_per_head;
@@ -647,9 +647,9 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 
-// head widths 16 and 32, and 36 ... 96 in steps of 4 (attention_long.cu)
+// head widths 16 and 32, and 36 ... 128 in steps of 4 (attention_long.cu)
 bool attn_fused_bwd_supported(int S, int dk) {
-  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 96 && dk % 4 == 0));
+  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 128 && dk % 4 == 0));
 }
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {

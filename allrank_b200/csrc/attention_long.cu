@@ -1,4 +1,4 @@
-// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 96 (w % 4 == 0)
+// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 128 (w % 4 == 0)
 // for slates of 1 ... 4096 items, forward and backward, without the S x S matrix.  attention_fused.cu /
 // attention_fused_bwd.cu serve S <= 256 at width <= 32 (the forward also 64) by holding a whole (slate, head) in shared
 // memory; that stops fitting beyond 256 rows or 32 columns, so here a work item is one 128-row tile of a (slate, head)
@@ -33,15 +33,16 @@ constexpr int LONG_BLK = 128;                         // rows of a tile
 // and an aux region (key bits, or float2 {nm, delta} per query).
 //   DK <= 32: 128-row streamed blocks in four stages; the fragments of the tile's rows stay in registers, the tile is
 //             free again once they are loaded, and each compute warp stages its strips in two boxes of its own.
-//   DK 64, 96 (wide): 64-row streamed blocks in four / two stages; the tile stays resident for the whole item: the dK /
-//             dV and dQ strips re-read its fragments for every k-step (they would not fit in registers beside the
-//             accumulators), and each warp stages its finished strip over its own 16 rows of the tile.
+//   DK 64, 96, 128 (wide): 64-row streamed blocks in four / two stages (DK 128: 32-row blocks in two stages, since a
+//             tile of 2 x 4 slabs takes 129 KB); the tile stays resident for the whole item: the dK / dV and dQ strips
+//             re-read its fragments for every k-step (they would not fit in registers beside the accumulators), and
+//             each warp stages its finished strip over its own 16 rows of the tile.
 template <int DK>
 struct LongSmem {
   static constexpr bool WIDE = DK > 32;
   static constexpr int NKB = (DK + 31) / 32;          // 128-byte slabs per operand row
   static constexpr int KSB = DK / 8 / NKB;            // k8 steps per slab
-  static constexpr int SBLK = WIDE ? 64 : 128;        // rows of a streamed block
+  static constexpr int SBLK = DK > 96 ? 32 : WIDE ? 64 : 128;   // rows of a streamed block
   static constexpr int NST = DK <= 64 ? 4 : 2;        // stages of the ring
   static constexpr int TSLAB = LONG_BLK * 128;        // one slab of a tile operand
   static constexpr int SSLAB = SBLK * 128;            // one slab of a streamed operand
@@ -86,9 +87,12 @@ __device__ __forceinline__ void attn_long_body(
   using L = LongSmem<DK>;
   constexpr int NKB = L::NKB, KSB = L::KSB, SBLK = L::SBLK, NST = L::NST;
   constexpr bool WIDE = L::WIDE;
-  // the tile's fragments stay in registers for the whole item (the forward's Q at every width)
-  constexpr bool KEEP = !WIDE || MODE == LONG_FWD;
+  // the tile's fragments stay in registers for the whole item (the forward's Q up to DK 96: at 128 Q's 64 registers
+  // and O's 64 would spill)
+  constexpr bool KEEP = !WIDE || (MODE == LONG_FWD && DK <= 96);
   constexpr int DKDV_NB = DK > 64 ? 1 : 2;      // 8-query blocks in flight in dK / dV
+  // DK 128: dK and dV are two passes over the streamed queries (dK, then dV), one 64-register accumulator each
+  constexpr bool SPLIT = MODE == LONG_DKDV && DK > 96;
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
   const uint32_t sbase = (ptx::smem_u32(smem_dyn) + 1023u) & ~1023u;
   uint8_t* smem = smem_dyn + (sbase - ptx::smem_u32(smem_dyn));
@@ -128,7 +132,7 @@ __device__ __forceinline__ void attn_long_body(
     it.nblk = it.live > 0 ? (it.rows16 + SBLK - 1) / SBLK : 0;          // streamed blocks (keys, or queries for dK / dV)
     return it;
   };
-  constexpr int NPASS = MODE == LONG_FWD ? 2 : 1;
+  constexpr int NPASS = (MODE == LONG_FWD || SPLIT) ? 2 : 1;
 
   if (warp == LONG_WARPS) {
     // ===== load warp
@@ -315,7 +319,12 @@ __device__ __forceinline__ void attn_long_body(
           uint32_t kf[KSB][2];
           ld_b_head<KSB>(k_s + kb * L::SSLAB, 8 * j, lane, kf);
 #pragma unroll
-          for (int ks = 0; ks < KSB; ++ks) { rt(kf[ks][0]); rt(kf[ks][1]); ptx::mma_tf32(s4, ta[kb][ks], kf[ks]); }
+          for (int ks = 0; ks < KSB; ++ks) {
+            uint32_t qa[4];
+            tfrag(0, kb, ks, qa);
+            rt(kf[ks][0]); rt(kf[ks][1]);
+            ptx::mma_tf32(s4, qa, kf[ks]);
+          }
         }
       };
       const int nj_all = (it.e + 7) >> 3;
@@ -419,99 +428,129 @@ __device__ __forceinline__ void attn_long_body(
         load_tile_frags(2);
       }
       if constexpr (!WIDE) release_tile();
-      float dv[NKB][KSB][4], dk[NKB][KSB][4];
-#pragma unroll
-      for (int kb = 0; kb < NKB; ++kb)
-#pragma unroll
-        for (int nt = 0; nt < KSB; ++nt)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) dv[kb][nt][i] = dk[kb][nt][i] = 0.f;
       const int nq8 = (it.e + 7) & ~7;     // queries at or beyond the extent have zero d ctx rows
-      consume([&](int blk, uint32_t buf) {
-        const uint32_t q_s = buf, do_s = buf + L::SOP, st_s = buf + 2 * L::SOP;
-        const int qbase = SBLK * blk, nq = min(SBLK, nq8 - qbase);
-        // S^T, dP^T of the NB 8-query blocks q0, q0 + 8 (of the buffer)
-        auto products = [&](auto nbc, int q0, float (&s)[2][4], float (&dp)[2][4]) {
-          constexpr int NB = decltype(nbc)::value;
+      // one pass over the streamed queries that adds their dV products to dv (with_dv) and / or their dK products to dk
+      // (with_dk), in the same query order either way; a dV-only pass needs neither dP nor the tile's V.  The flags are
+      // constants at every call, so each call compiles to its own loop.
+      auto dkdv_pass = [&](bool with_dv, bool with_dk, float (&dv)[NKB][KSB][4], float (&dk)[NKB][KSB][4]) {
 #pragma unroll
-          for (int n = 0; n < NB; ++n)
+        for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) s[n][i] = dp[n][i] = 0.f;
+          for (int nt = 0; nt < KSB; ++nt)
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb) {
-            uint32_t qb[NB][KSB][2], ob2[NB][KSB][2];
-#pragma unroll
-            for (int n = 0; n < NB; ++n) {
-              ld_b_head<KSB>(q_s + kb * L::SSLAB, q0 + 8 * n, lane, qb[n]);
-              ld_b_head<KSB>(do_s + kb * L::SSLAB, q0 + 8 * n, lane, ob2[n]);
+            for (int i = 0; i < 4; ++i) {
+              if (with_dv) dv[kb][nt][i] = 0.f;
+              if (with_dk) dk[kb][nt][i] = 0.f;
             }
+        consume([&](int blk, uint32_t buf) {
+          const uint32_t q_s = buf, do_s = buf + L::SOP, st_s = buf + 2 * L::SOP;
+          const int qbase = SBLK * blk, nq = min(SBLK, nq8 - qbase);
+          // S^T, dP^T of the NB 8-query blocks q0, q0 + 8 (of the buffer)
+          auto products = [&](auto nbc, int q0, float (&s)[2][4], float (&dp)[2][4]) {
+            constexpr int NB = decltype(nbc)::value;
 #pragma unroll
-            for (int ks = 0; ks < KSB; ++ks) {
-              uint32_t ka[4], va[4];
-              tfrag(0, kb, ks, ka);
-              tfrag(1, kb, ks, va);
+            for (int n = 0; n < NB; ++n)
+#pragma unroll
+              for (int i = 0; i < 4; ++i) s[n][i] = dp[n][i] = 0.f;
+#pragma unroll
+            for (int kb = 0; kb < NKB; ++kb) {
+              uint32_t qb[NB][KSB][2], ob2[NB][KSB][2];
 #pragma unroll
               for (int n = 0; n < NB; ++n) {
-                rt(qb[n][ks][0]); rt(qb[n][ks][1]); rt(ob2[n][ks][0]); rt(ob2[n][ks][1]);
-                ptx::mma_tf32(s[n], ka, qb[n][ks]);
-                ptx::mma_tf32(dp[n], va, ob2[n][ks]);
+                ld_b_head<KSB>(q_s + kb * L::SSLAB, q0 + 8 * n, lane, qb[n]);
+                if (with_dk) ld_b_head<KSB>(do_s + kb * L::SSLAB, q0 + 8 * n, lane, ob2[n]);
+              }
+#pragma unroll
+              for (int ks = 0; ks < KSB; ++ks) {
+                uint32_t ka[4], va[4];
+                tfrag(0, kb, ks, ka);
+                if (with_dk) tfrag(1, kb, ks, va);
+#pragma unroll
+                for (int n = 0; n < NB; ++n) {
+                  rt(qb[n][ks][0]); rt(qb[n][ks][1]);
+                  if (with_dk) { rt(ob2[n][ks][0]); rt(ob2[n][ks][1]); }
+                  ptx::mma_tf32(s[n], ka, qb[n][ks]);
+                  if (with_dk) ptx::mma_tf32(dp[n], va, ob2[n][ks]);
+                }
               }
             }
-          }
-        };
-        // P^T, dS^T of the block and its dV, dK products
-        auto accumulate = [&](int q0, const float (&s)[4], const float (&dp)[4]) {
-          const uint2 st0 = lds64(st_s + 8 * (q0 + t)), st1 = lds64(st_s + 8 * (q0 + t + 4));
-          float pu[4], ds[4];
+          };
+          // P^T, dS^T of the block and its dV, dK products
+          auto accumulate = [&](int q0, const float (&s)[4], const float (&dp)[4]) {
+            const uint2 st0 = lds64(st_s + 8 * (q0 + t)), st1 = lds64(st_s + 8 * (q0 + t + 4));
+            float pu[4], ds[4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int q = qbase + q0 + t + 4 * (i & 1);
-            const float nm = __uint_as_float((i & 1) ? st1.x : st0.x), dl = __uint_as_float((i & 1) ? st1.y : st0.y);
-            const float p = (i < 2 ? liveA : liveB) ? ex2_approx(fmaf(s[i], c_log2e, nm)) : 0.0f;
-            float p_used = p, dpv = dp[i];
-            if constexpr (DROP) {
-              const unsigned long long idx = (dbase + q) * (unsigned long long)S + (i < 2 ? kA : kB);
-              const float m = drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
-              p_used = p * m;
-              dpv *= m;
+            for (int i = 0; i < 4; ++i) {
+              const int q = qbase + q0 + t + 4 * (i & 1);
+              const float nm = __uint_as_float((i & 1) ? st1.x : st0.x), dl = __uint_as_float((i & 1) ? st1.y : st0.y);
+              const float p = (i < 2 ? liveA : liveB) ? ex2_approx(fmaf(s[i], c_log2e, nm)) : 0.0f;
+              float p_used = p, dpv = dp[i];
+              if constexpr (DROP) {
+                const unsigned long long idx = (dbase + q) * (unsigned long long)S + (i < 2 ? kA : kB);
+                const float m = drop_keep(idx, drop.seed, drop.thresh) ? drop.scale : 0.0f;
+                p_used = p * m;
+                dpv *= m;
+              }
+              pu[i] = round_tf32(p_used);
+              ds[i] = round_tf32(p * (dpv - dl));
             }
-            pu[i] = round_tf32(p_used);
-            ds[i] = round_tf32(p * (dpv - dl));
-          }
-          const uint32_t pa[4] = {__float_as_uint(pu[0]), __float_as_uint(pu[2]), __float_as_uint(pu[1]), __float_as_uint(pu[3])};
-          const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
+            const uint32_t pa[4] = {__float_as_uint(pu[0]), __float_as_uint(pu[2]), __float_as_uint(pu[1]), __float_as_uint(pu[3])};
+            const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb) {
-            uint32_t o0[KSB], o1[KSB], q0v[KSB], q1v[KSB];
-            ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t, g, o0); ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t + 4, g, o1);
-            ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t, g, q0v); ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t + 4, g, q1v);
+            for (int kb = 0; kb < NKB; ++kb) {
+              uint32_t o0[KSB], o1[KSB], q0v[KSB], q1v[KSB];
+              if (with_dv) { ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t, g, o0); ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t + 4, g, o1); }
+              if (with_dk) { ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t, g, q0v); ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t + 4, g, q1v); }
 #pragma unroll
-            for (int nt = 0; nt < KSB; ++nt) {
-              rt(o0[nt]); rt(o1[nt]); rt(q0v[nt]); rt(q1v[nt]);
-              const uint32_t obv[2] = {o0[nt], o1[nt]}, qbv[2] = {q0v[nt], q1v[nt]};
-              ptx::mma_tf32(dv[kb][nt], pa, obv);
-              ptx::mma_tf32(dk[kb][nt], dsa, qbv);
+              for (int nt = 0; nt < KSB; ++nt) {
+                if (with_dv) {
+                  rt(o0[nt]); rt(o1[nt]);
+                  const uint32_t obv[2] = {o0[nt], o1[nt]};
+                  ptx::mma_tf32(dv[kb][nt], pa, obv);
+                }
+                if (with_dk) {
+                  rt(q0v[nt]); rt(q1v[nt]);
+                  const uint32_t qbv[2] = {q0v[nt], q1v[nt]};
+                  ptx::mma_tf32(dk[kb][nt], dsa, qbv);
+                }
+              }
             }
-          }
-        };
-        // two blocks in flight (DK 96: one, or the accumulators spill)
-        int q0 = 0;
-        for (; q0 + 8 * DKDV_NB <= nq; q0 += 8 * DKDV_NB) {
-          float s[2][4], dp[2][4];
-          products(std::integral_constant<int, DKDV_NB>{}, q0, s, dp);
+          };
+          // two blocks in flight (DK 96, 128: one, or the accumulators spill)
+          int q0 = 0;
+          for (; q0 + 8 * DKDV_NB <= nq; q0 += 8 * DKDV_NB) {
+            float s[2][4], dp[2][4];
+            products(std::integral_constant<int, DKDV_NB>{}, q0, s, dp);
 #pragma unroll
-          for (int n = 0; n < DKDV_NB; ++n) accumulate(q0 + 8 * n, s[n], dp[n]);
+            for (int n = 0; n < DKDV_NB; ++n) accumulate(q0 + 8 * n, s[n], dp[n]);
+          }
+          if (q0 < nq) {
+            float s[2][4], dp[2][4];
+            products(std::integral_constant<int, 1>{}, q0, s, dp);
+            accumulate(q0, s[0], dp[0]);
+          }
+        });
+      };
+      if constexpr (SPLIT) {
+        // dK first, staged over the warp's own V rows (the dV pass reads only K), then dV over its K rows
+        float acc[NKB][KSB][4];
+        dkdv_pass(false, true, acc, acc);
+        if (has) {
+          store_wait();
+          stage_strip(1, acc, scale);
         }
-        if (q0 < nq) {
-          float s[2][4], dp[2][4];
-          products(std::integral_constant<int, 1>{}, q0, s, dp);
-          accumulate(q0, s[0], dp[0]);
+        dkdv_pass(true, false, acc, acc);
+        if (has) stage_strip(0, acc, 1.0f);
+      } else {
+        float dv[NKB][KSB][4], dk[NKB][KSB][4];
+        dkdv_pass(true, true, dv, dk);
+        if (has) {
+          store_wait();
+          stage_strip(0, dv, 1.0f);
+          stage_strip(1, dk, scale);
         }
-      });
+      }
       if (has) {
-        store_wait();
-        stage_strip(0, dv, 1.0f);
-        stage_strip(1, dk, scale);
         __syncwarp();
         if (live) { bias_add(0, 2 * d_model); bias_add(1, d_model); }
         store(2);
@@ -650,8 +689,8 @@ static double long_bytes(int S, int dk, int tile_ops, int stream_ops, int out_op
   return 4.0 * S * dk * (tile_ops + out_ops + tiles * stream_ops);
 }
 
-// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96)
-static int long_dk(int dk) { return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : 96; }
+// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96, 128)
+static int long_dk(int dk) { return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : dk <= 96 ? 96 : 128; }
 
 template <int DK>
 static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
@@ -679,7 +718,8 @@ int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st) {
     case 16: return launch_long_fwd_t<16>(a, st);
     case 32: return launch_long_fwd_t<32>(a, st);
     case 64: return launch_long_fwd_t<64>(a, st);
-    default: return launch_long_fwd_t<96>(a, st);
+    case 96: return launch_long_fwd_t<96>(a, st);
+    default: return launch_long_fwd_t<128>(a, st);
   }
 }
 
@@ -733,7 +773,8 @@ int launch_attn_long_bwd(const AttnBwdArgs& a, cudaStream_t st) {
     case 16: return launch_long_bwd_t<16>(a, st);
     case 32: return launch_long_bwd_t<32>(a, st);
     case 64: return launch_long_bwd_t<64>(a, st);
-    default: return launch_long_bwd_t<96>(a, st);
+    case 96: return launch_long_bwd_t<96>(a, st);
+    default: return launch_long_bwd_t<128>(a, st);
   }
 }
 

@@ -956,7 +956,7 @@ static int attention_hook_check(const char* what, int B, int S, int h, float p, 
   if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
   if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
   if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
-    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 96 in steps of 4)").c_str());
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 128 in steps of 4)").c_str());
     return ARB_E_UNSUPPORTED;
   }
   return ARB_OK;

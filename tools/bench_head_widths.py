@@ -1,12 +1,14 @@
 """Training steps of the shipped Transformer configurations whose heads are wider than 32 columns -- local_config
 (d 64, h 1: width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96,
-h 1: width 96) -- and of a d = 256, h = 4 model (width 64), each with its own dropout and loss: the fused attention
+h 1: width 96) -- of a d = 256, h = 4 model (width 64), and of two width-128 models (d 128, h 1 and d 256, h 2), each
+with its own dropout and loss: the fused attention
 kernels (attention mode 2; csrc/attention_long.cu serves these widths) against the unfused sequence
 (arb_set_attention_mode(0): [B, h, S, S] probabilities in HBM) where the latter exists (S <= 1536).
 
-    python tools/bench_head_widths.py [--steps 5] [--warmup 2] [--runs 3] [--json out.json]
+    python tools/bench_head_widths.py [--steps 5] [--warmup 2] [--runs 3] [--models a,b] [--json out.json]
 
-Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the width-96 model at S = 1024, 2048, 4096
+Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the width-96 and width-128 models at S = 1024,
+2048, 4096
 (B = 245760 / S slates, fewer where the unfused path would not fit in memory).  Slate lengths ~ N(S/2, S/4) clamped to
 [1, S].  Step time is the host clock around `steps` training steps that end in a device synchronise, per run; the
 modes alternate run by run.  Peak memory is torch.cuda.max_memory_allocated over a run.  The attention kernels' times
@@ -36,8 +38,15 @@ MODELS = {
     "d256_h4": (dict(fc_model={"sizes": [256], "input_norm": False, "activation": None, "dropout": 0.0},
                      transformer={"N": 2, "d_ff": 1024, "h": 4, "positional_encoding": None, "dropout": 0.1},
                      post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
+    "d128_h1": (dict(fc_model={"sizes": [128], "input_norm": False, "activation": None, "dropout": 0.0},
+                     transformer={"N": 2, "d_ff": 512, "h": 1, "positional_encoding": None, "dropout": 0.1},
+                     post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
+    "d256_h2": (dict(fc_model={"sizes": [256], "input_norm": False, "activation": None, "dropout": 0.0},
+                     transformer={"N": 2, "d_ff": 1024, "h": 2, "positional_encoding": None, "dropout": 0.1},
+                     post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
 }
-SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [("approxndcg", 245760 // S, S)
+SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [(name, 245760 // S, S)
+                                                                     for name in ("approxndcg", "d128_h1", "d256_h2")
                                                                      for S in (1024, 2048, 4096)]
 
 
@@ -77,13 +86,18 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--models", default=None, help="comma-separated subset of the models (default: all)")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
+    only = set(args.models.split(",")) if args.models else set(MODELS)
+    assert only <= set(MODELS), f"unknown model in {sorted(only - set(MODELS))}"
     assert torch.cuda.is_available(), "needs a CUDA device"
     name_gpu, power = gpu_info()
     print(f"GPU: {name_gpu}; power limit, max SM clock: {power}", flush=True)
     rows = []
     for name, B, S in SHAPES:
+        if name not in only:
+            continue
         step = make_step(name)
         modes = (2, 0) if fits_unfused(name, B, S) else (2,)
         x, y = make_batch(B, S)
