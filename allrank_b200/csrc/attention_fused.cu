@@ -376,10 +376,10 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
                 tf32_round_on_load(), pool_units);
 }
 
-// attn_fwd_kernel: S <= 256 at head width 16, 32 or 64; attention_long.cu: S <= 4096 at 16, 32 and 36 ... 128 in steps
+// attn_fwd_kernel: S <= 256 at head width 16, 32 or 64; attention_long.cu: S <= 4096 at 16, 32 and 36 ... 256 in steps
 // of 4 (every width but 64 at S <= 256 runs there)
 bool attn_fused_supported(int S, int dk) {
-  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 128 && dk % 4 == 0));
+  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 256 && dk % 4 == 0));
 }
 
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {

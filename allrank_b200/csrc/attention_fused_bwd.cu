@@ -23,7 +23,8 @@ constexpr int BWD_THREADS = 32 * (BWD_WARPS + 2);     // + one load warp, one st
 
 // delta[b,h,q] = sum_e dO[b,q,h,e] * O[b,q,h,e]: one warp per row of the [B*S, d_model] activations, 128-bit loads,
 // segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32, 64, 128}: 4, 8, 16 or 32 lanes per
-// head); other widths (36 ... 124) reduce one head at a time over the whole warp.
+// head); other widths (36 ... 124) reduce one head at a time over the whole warp.  Widths above 128:
+// attn_delta_wide_kernel.
 constexpr int DELTA_RPW = 4;     // rows per warp of the delta kernel
 __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ d_o, const float* __restrict__ o,
                                                          long long pitch, int B, int S, int h, int dk,
@@ -91,6 +92,46 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
       if (item[q] >= 0 && c < width && (lane % lanes_per_head) == 0) {
         const int b = int(item[q] / S), qi = int(item[q] - (long long)b * S);
         delta[((long long)b * h + c / dk) * S + qi] = acc;
+      }
+    }
+  }
+}
+
+// delta at head widths 132 ... 256 (dense fp32 rows): one head at a time, lane l takes the head's 4-column groups l and
+// l + 32 (columns 4l ... 4l + 3 and 128 + 4l ... 128 + 4l + 3, those below dk), summed in that order, then reduced
+// over the whole warp.  Rows as attn_delta_kernel's.
+__global__ void __launch_bounds__(256) attn_delta_wide_kernel(const float* __restrict__ d_o, const float* __restrict__ o,
+                                                              long long pitch, int S, int h, int dk,
+                                                              float* __restrict__ delta, const int* __restrict__ rows_dev,
+                                                              const int* __restrict__ rowmap, long long rows_cap) {
+  arb_pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const long long row0 = ((long long)blockIdx.x * 8 + (threadIdx.x >> 5)) * DELTA_RPW;
+  const long long rows = rows_dev ? min(rows_cap, (long long)__ldg(rows_dev)) : rows_cap;
+  if (row0 >= rows) return;
+  long long item[DELTA_RPW];
+#pragma unroll
+  for (int q = 0; q < DELTA_RPW; ++q) item[q] = (row0 + q < rows) ? (rowmap ? (long long)rowmap[row0 + q] : row0 + q) : -1;
+  for (int head = 0; head < h; ++head) {
+#pragma unroll
+    for (int q = 0; q < DELTA_RPW; ++q) {
+      float acc = 0.f;
+      if (item[q] >= 0) {
+        const long long row = row0 + q;
+#pragma unroll
+        for (int grp = 0; grp < 2; ++grp) {
+          const int col = 128 * grp + 4 * lane;
+          if (col < dk) {
+            const float4 x = *reinterpret_cast<const float4*>(d_o + row * pitch + head * dk + col);
+            const float4 y = *reinterpret_cast<const float4*>(o + row * pitch + head * dk + col);
+            acc += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
+          }
+        }
+      }
+      for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(FULL, acc, off);
+      if (item[q] >= 0 && lane == 0) {
+        const int b = int(item[q] / S), qi = int(item[q] - (long long)b * S);
+        delta[((long long)b * h + head) * S + qi] = acc;
       }
     }
   }
@@ -594,6 +635,12 @@ static int launch_delta(const AttnBwdArgs& a, cudaStream_t st) {
   const double rf = packed ? arb_row_frac() : 1.0;
   ProfScope ps(ARB_PROF_SCORER_SIMT, rf * double(a.B) * a.S * (8.0 * a.h * a.dk + 4.0 * a.h), st, 0.0, "attn_delta_kernel");
   const long long rows = packed ? (long long)a.q.dim[1] : (long long)a.B * a.S;   // packed: the buffers' row count
+  if (a.dk > 128) {
+    if (a.o_bf16) { arb_set_error("attn_delta: a bf16 context needs head width <= 128"); return ARB_E_UNSUPPORTED; }
+    return launch(attn_delta_wide_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0,
+                  st, /*pdl=*/true, a.do_ptr, static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.S, a.h, a.dk,
+                  a.delta, a.rows_dev, a.rowmap, rows);
+  }
   return launch(attn_delta_kernel, dim3(unsigned((rows + 8 * DELTA_RPW - 1) / (8 * DELTA_RPW))), dim3(256), 0, st,
                 /*pdl=*/true, a.do_ptr, static_cast<const float*>(a.o_ptr), (long long)a.o_pitch, a.B, a.S, a.h,
                 a.dk, a.delta, a.o_bf16, a.rows_dev, a.rowmap, rows);
@@ -647,9 +694,9 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 
-// head widths 16 and 32, and 36 ... 128 in steps of 4 (attention_long.cu)
+// head widths 16 and 32, and 36 ... 256 in steps of 4 (attention_long.cu)
 bool attn_fused_bwd_supported(int S, int dk) {
-  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 128 && dk % 4 == 0));
+  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 256 && dk % 4 == 0));
 }
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {

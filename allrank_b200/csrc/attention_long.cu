@@ -1,14 +1,16 @@
-// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 128 (w % 4 == 0)
+// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 256 (w % 4 == 0)
 // for slates of 1 ... 4096 items, forward and backward, without the S x S matrix.  attention_fused.cu /
 // attention_fused_bwd.cu serve S <= 256 at width <= 32 (the forward also 64) by holding a whole (slate, head) in shared
-// memory; that stops fitting beyond 256 rows or 32 columns, so here a work item is one 128-row tile of a (slate, head)
-// and the other side of its products streams through a ring of shared-memory stages:
-//   attn_long_fwd_kernel   tile of 128 queries;  streams K (pass A), then K and V (pass B)          -> ctx, row stats
-//   attn_long_dkdv_kernel  tile of 128 keys;     streams Q, dO and the queries' {nm, delta}         -> dK, dV
-//   attn_long_dq_kernel    tile of 128 queries;  streams K, V                                      -> dQ
+// memory; that stops fitting beyond 256 rows or 32 columns, so here a work item is one 128-row tile (DK 192, 256: 64
+// rows) of a (slate, head) and the other side of its products streams through a ring of shared-memory stages:
+//   attn_long_fwd_kernel   tile of queries;  streams K (pass A), then K and V (pass B)              -> ctx, row stats
+//   attn_long_dkdv_kernel  tile of keys;     streams Q, dO and the queries' {nm, delta}             -> dK, dV
+//   attn_long_dq_kernel    tile of queries;  streams K, V                                          -> dQ
 // Each 16-row strip of a tile is one compute warp's and runs the short kernels' per-strip arithmetic in the same key /
 // query order (two-pass softmax, no rescaling), so a slate that the short kernels serve gets the same bits here: the
-// context, row statistics and dQ / dK / dV.  Only the QKV bias gradient is summed in another order.
+// context, row statistics and dQ / dK / dV.  Only the QKV bias gradient is summed in another order.  At DK 192 and 256
+// a strip is two warps': both compute its full score rows with the same instructions (so the same P / dS bits), and
+// each multiplies them into its own half of the output columns.
 #include <algorithm>
 #include <cstdint>
 #include <type_traits>
@@ -24,9 +26,10 @@
 
 namespace arb {
 
-constexpr int LONG_WARPS = 8;                         // compute warps: one 16-row strip of the tile each
+constexpr int LONG_WARPS = 8;                         // compute warps: one 16-row strip of the tile each (DK 192, 256:
+                                                      // warps i and i + 4 share strip i)
 constexpr int LONG_THREADS = 32 * (LONG_WARPS + 1);   // + one load warp
-constexpr int LONG_BLK = 128;                         // rows of a tile
+constexpr int LONG_BLK = 128;                         // rows of a tile (DK 192, 256: LongSmem::BLK = 64)
 
 // An operand row of DK columns is NKB slabs of 128 bytes (32 fp32 columns; TMA zero-fills the columns past the head
 // width), each slab of a buffer 128B-swizzled in its own 16-row boxes.  A buffer holds two operands, slab after slab,
@@ -37,14 +40,22 @@ constexpr int LONG_BLK = 128;                         // rows of a tile
 //             tile of 2 x 4 slabs takes 129 KB); the tile stays resident for the whole item: the dK / dV and dQ strips
 //             re-read its fragments for every k-step (they would not fit in registers beside the accumulators), and
 //             each warp stages its finished strip over its own 16 rows of the tile.
+//   DK 192, 256 (paired): 64-row tiles (48 / 64 KB per operand), 32- / 16-row streamed blocks in two stages; the two
+//             warps of a strip own NKB / 2 output slabs each (the accumulators of DK 96 / 128) and stage into their
+//             own slabs of the strip's tile rows, after both are done reading those rows.
 template <int DK>
 struct LongSmem {
   static constexpr bool WIDE = DK > 32;
+  static constexpr bool PAIR = DK > 128;              // two warps per strip, each with half the output columns
+  static constexpr int BLK = PAIR ? 64 : LONG_BLK;    // rows of a tile
+  static constexpr int STRIPS = BLK / 16;             // strips of a tile
   static constexpr int NKB = (DK + 31) / 32;          // 128-byte slabs per operand row
+  static constexpr int NKO = PAIR ? NKB / 2 : NKB;    // output slabs per warp
   static constexpr int KSB = DK / 8 / NKB;            // k8 steps per slab
-  static constexpr int SBLK = DK > 96 ? 32 : WIDE ? 64 : 128;   // rows of a streamed block
+  static constexpr int SBLK = DK > 192 ? 16 : DK > 96 ? 32 : WIDE ? 64 : 128;   // rows of a streamed block
+  static constexpr int SAUX = SBLK < 32 ? 32 : SBLK;  // rows of a streamed block's aux (whole 32-bit key words)
   static constexpr int NST = DK <= 64 ? 4 : 2;        // stages of the ring
-  static constexpr int TSLAB = LONG_BLK * 128;        // one slab of a tile operand
+  static constexpr int TSLAB = BLK * 128;             // one slab of a tile operand
   static constexpr int SSLAB = SBLK * 128;            // one slab of a streamed operand
   static constexpr int TOP = NKB * TSLAB, SOP = NKB * SSLAB;
   static constexpr int TBUF = 2 * TOP + 1024, SBUF = 2 * SOP + 1024;
@@ -85,12 +96,14 @@ __device__ __forceinline__ void attn_long_body(
     float* __restrict__ stat_sum, const float* __restrict__ delta, int S, int n_heads, float scale, DropSite drop,
     float* __restrict__ dbias, int d_model, const int* __restrict__ extent, int n_items, int rnd) {
   using L = LongSmem<DK>;
-  constexpr int NKB = L::NKB, KSB = L::KSB, SBLK = L::SBLK, NST = L::NST;
-  constexpr bool WIDE = L::WIDE;
+  constexpr int NKB = L::NKB, NKO = L::NKO, KSB = L::KSB, SBLK = L::SBLK, NST = L::NST, BLK = L::BLK;
+  constexpr int STRIPS = L::STRIPS;
+  constexpr bool WIDE = L::WIDE, PAIR = L::PAIR;
   // the tile's fragments stay in registers for the whole item (the forward's Q up to DK 96: at 128 Q's 64 registers
   // and O's 64 would spill)
   constexpr bool KEEP = !WIDE || (MODE == LONG_FWD && DK <= 96);
   constexpr int DKDV_NB = DK > 64 ? 1 : 2;      // 8-query blocks in flight in dK / dV
+  constexpr int DQ_NB = DK > 192 ? 1 : 2;       // 8-key blocks in flight in dQ
   // DK 128: dK and dV are two passes over the streamed queries (dK, then dV), one 64-register accumulator each
   constexpr bool SPLIT = MODE == LONG_DKDV && DK > 96;
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
@@ -103,7 +116,7 @@ __device__ __forceinline__ void attn_long_body(
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const float c_log2e = scale * 1.4426950408889634f;
-  const int tiles = (S + LONG_BLK - 1) / LONG_BLK;
+  const int tiles = (S + BLK - 1) / BLK;
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(tmR0); ptx::prefetch_tmap(tmR1); ptx::prefetch_tmap(tmS0); ptx::prefetch_tmap(tmS1);
@@ -127,8 +140,8 @@ __device__ __forceinline__ void attn_long_body(
     it.head = bh - it.b * n_heads;
     it.e = max(1, min(S, extent ? __ldg(extent + it.b) : S));
     it.rows16 = (it.e + 15) & ~15;
-    it.ns = min(LONG_WARPS, (S + 15) / 16 - LONG_WARPS * it.tile);       // strips of the tile below round_up(S, 16)
-    it.live = MODE == LONG_FWD ? it.ns : max(0, min(it.ns, it.rows16 / 16 - LONG_WARPS * it.tile));
+    it.ns = min(STRIPS, (S + 15) / 16 - STRIPS * it.tile);               // strips of the tile below round_up(S, 16)
+    it.live = MODE == LONG_FWD ? it.ns : max(0, min(it.ns, it.rows16 / 16 - STRIPS * it.tile));
     it.nblk = it.live > 0 ? (it.rows16 + SBLK - 1) / SBLK : 0;          // streamed blocks (keys, or queries for dK / dV)
     return it;
   };
@@ -177,13 +190,13 @@ __device__ __forceinline__ void attn_long_body(
     for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k) {
       const Item it = item_info(item);
       if (k >= 1) ptx::mbar_wait(res_empty, (k - 1) & 1);
-      fill(smem, res_full, it, LONG_BLK * it.tile, 16 * it.live, RES_OPS, L::TSLAB, LONG_BLK, tmR0, tmR1, RES_AUX);
+      fill(smem, res_full, it, BLK * it.tile, 16 * it.live, RES_OPS, L::TSLAB, BLK, tmR0, tmR1, RES_AUX);
       for (int pass = 0; pass < NPASS; ++pass) {
         for (int blk = 0; blk < it.nblk; ++blk, ++cnt) {
           const int st = cnt % NST;
           if (cnt >= NST) ptx::mbar_wait(empty + st, ((cnt / NST) - 1) & 1);
           fill(smem + L::ring + st * L::SBUF, full + st, it, SBLK * blk, min(SBLK, it.rows16 - SBLK * blk),
-               (MODE == LONG_FWD && pass == 0) ? 1 : 2, L::SSLAB, SBLK, tmS0, tmS1, STR_AUX);
+               (MODE == LONG_FWD && pass == 0) ? 1 : 2, L::SSLAB, L::SAUX, tmS0, tmS1, STR_AUX);
         }
       }
     }
@@ -193,7 +206,13 @@ __device__ __forceinline__ void attn_long_body(
   // ===== compute warps
   if constexpr (DROP) drop.seed = drop_seed(drop);
   auto rt = [&](uint32_t& x) { if (rnd) x = ptx::cvt_tf32(__uint_as_float(x)); };
-  const int r0 = 16 * warp;                                            // the warp's strip rows in the tile buffer
+  const int sw = PAIR ? warp % STRIPS : warp;                          // the warp's strip of the tile
+  const int kb0 = PAIR ? (warp / STRIPS) * NKO : 0;                    // the warp's first output slab
+  const int r0 = 16 * sw;                                              // the warp's strip rows in the tile buffer
+  // paired: both warps of the strip are done reading its tile rows, which either may now overwrite in its own slabs
+  auto pair_sync = [&]() {
+    if constexpr (PAIR) ptx::named_bar_sync(1 + sw, 64);
+  };
   const uint32_t res_s = sbase;
   // output boxes: operand o, slab kb at ob_s + o * OB_OP + kb * L::TSLAB (wide: the warp's own tile rows)
   constexpr int OB_OP = WIDE ? L::TOP : 2048;
@@ -227,8 +246,8 @@ __device__ __forceinline__ void attn_long_body(
   int cnt = 0, k = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k) {
     const Item it = item_info(item);
-    const bool has = warp < it.ns, live = warp < it.live;
-    const int strip = LONG_WARPS * it.tile + warp;
+    const bool has = sw < it.ns, live = sw < it.live;
+    const int strip = STRIPS * it.tile + sw;
     const unsigned long long dbase = (unsigned long long)(it.b * n_heads + it.head) * S;
     // the streamed blocks of this item: fn(block, buffer address) on the warps that have a live strip; every warp
     // frees every stage
@@ -245,14 +264,15 @@ __device__ __forceinline__ void attn_long_body(
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(res_empty);
     };
-    // a finished 16-row strip (rows g, g + 8 of acc, x mul) into the 128B-swizzled output box of operand o
-    auto stage_strip = [&](int o, const float (&acc)[NKB][KSB][4], float mul) {
+    // a finished 16-row strip (rows g, g + 8 of acc, x mul) into the 128B-swizzled output box of operand o (the warp's
+    // NKO slabs from kb0)
+    auto stage_strip = [&](int o, const float (&acc)[NKO][KSB][4], float mul) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = g + 8 * h;
 #pragma unroll
-        for (int kb = 0; kb < NKB; ++kb) {
-          const uint32_t b = ob_s + o * OB_OP + kb * L::TSLAB;
+        for (int kb = 0; kb < NKO; ++kb) {
+          const uint32_t b = ob_s + o * OB_OP + (kb0 + kb) * L::TSLAB;
           float v[2][KSB];      // v[0]: head columns of output column 2t, v[1]: of 2t + 1 (n-tile order)
 #pragma unroll
           for (int nt = 0; nt < KSB; ++nt) { v[0][nt] = acc[kb][nt][2 * h] * mul; v[1][nt] = acc[kb][nt][2 * h + 1] * mul; }
@@ -266,15 +286,16 @@ __device__ __forceinline__ void attn_long_body(
       }
     };
     // QKV bias gradient: the staged strip's column sums (rows in order) of the head's w real columns, added to this
-    // warp's own slot -- one slot per (CTA, warp), its items in a fixed order; DetParts sums the slots in order
+    // warp's own slot -- one slot per (CTA, warp), its items in a fixed order; DetParts sums the slots in order (paired:
+    // each warp sums only its own slabs' columns)
     auto bias_add = [&](int o, int col0) {
       if (dbias == nullptr) return;
       const int w = WIDE ? d_model / n_heads : DK;
 #pragma unroll
-      for (int kb = 0; kb < NKB; ++kb) {
-        const int c = 32 * kb + lane;
+      for (int kb = 0; kb < NKO; ++kb) {
+        const int c = 32 * (kb0 + kb) + lane;
         if (c >= w) break;
-        const uint8_t* b = ob + o * OB_OP + kb * L::TSLAB;
+        const uint8_t* b = ob + o * OB_OP + (kb0 + kb) * L::TSLAB;
         float s = 0.f;
 #pragma unroll
         for (int r = 0; r < 16; ++r) s += *reinterpret_cast<const float*>(b + ptx::sw128(r, 4 * lane));
@@ -291,8 +312,12 @@ __device__ __forceinline__ void attn_long_body(
       if (lane == 0) {
         for (int o = 0; o < nbox; ++o)
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
-            ptx::tma_store_4d(o ? tmO1 : tmO0, ob + o * OB_OP + kb * L::TSLAB, 32 * kb, 16 * strip, it.head, it.b);
+          for (int kb = 0; kb < NKO; ++kb) {
+            // paired: a slab wholly beyond the head width (e.g. columns 160 ... 191 at width 132) has nothing to store
+            if (PAIR && 32 * (kb0 + kb) >= d_model / n_heads) break;
+            ptx::tma_store_4d(o ? tmO1 : tmO0, ob + o * OB_OP + (kb0 + kb) * L::TSLAB, 32 * (kb0 + kb), 16 * strip,
+                              it.head, it.b);
+          }
         ptx::tma_store_commit();
       }
     };
@@ -346,9 +371,9 @@ __device__ __forceinline__ void attn_long_body(
       const float mxsA = mxA * c_log2e, mxsB = mxB * c_log2e;
       const bool odd = (t & 1) != 0;
       float sumA = 0.f, sumB = 0.f;
-      float o[NKB][KSB][4];
+      float o[NKO][KSB][4];
 #pragma unroll
-      for (int kb = 0; kb < NKB; ++kb)
+      for (int kb = 0; kb < NKO; ++kb)
 #pragma unroll
         for (int nt = 0; nt < KSB; ++nt) o[kb][nt][0] = o[kb][nt][1] = o[kb][nt][2] = o[kb][nt][3] = 0.f;
       consume([&](int blk, uint32_t buf) {
@@ -382,10 +407,10 @@ __device__ __forceinline__ void attn_long_body(
           const uint32_t pa[4] = {__float_as_uint(round_tf32(p[0])), __float_as_uint(round_tf32(p[2])),
                                   __float_as_uint(round_tf32(p[1])), __float_as_uint(round_tf32(p[3]))};
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb) {
+          for (int kb = 0; kb < NKO; ++kb) {
             uint32_t v0[KSB], v1[KSB];
-            ld_b_out<KSB>(v_s + kb * L::SSLAB, 8 * j + t, g, v0);
-            ld_b_out<KSB>(v_s + kb * L::SSLAB, 8 * j + t + 4, g, v1);
+            ld_b_out<KSB>(v_s + (kb0 + kb) * L::SSLAB, 8 * j + t, g, v0);
+            ld_b_out<KSB>(v_s + (kb0 + kb) * L::SSLAB, 8 * j + t + 4, g, v1);
 #pragma unroll
             for (int nt = 0; nt < KSB; ++nt) {
               rt(v0[nt]); rt(v1[nt]);
@@ -398,7 +423,7 @@ __device__ __forceinline__ void attn_long_body(
       if (has) {
         sumA += __shfl_xor_sync(FULL, sumA, 2); sumA += __shfl_xor_sync(FULL, sumA, 1);
         sumB += __shfl_xor_sync(FULL, sumB, 2); sumB += __shfl_xor_sync(FULL, sumB, 1);
-        if (t == 0) {
+        if (t == 0 && kb0 == 0) {     // (paired: both warps have the same statistics)
           const size_t so = (size_t(it.b) * n_heads + it.head) * S;
           if (qA < S) { stat_max[so + qA] = mxA; stat_sum[so + qA] = sumA; }
           if (qB < S) { stat_max[so + qB] = mxB; stat_sum[so + qB] = sumB; }
@@ -407,12 +432,13 @@ __device__ __forceinline__ void attn_long_body(
         // O / rowsum, per row (one reciprocal each, as attn_fwd_kernel)
         const float invA = 1.0f / sumA, invB = 1.0f / sumB;
 #pragma unroll
-        for (int kb = 0; kb < NKB; ++kb)
+        for (int kb = 0; kb < NKO; ++kb)
 #pragma unroll
           for (int nt = 0; nt < KSB; ++nt) {
             o[kb][nt][0] *= invA; o[kb][nt][1] *= invA;
             o[kb][nt][2] *= invB; o[kb][nt][3] *= invB;
           }
+        pair_sync();
         stage_strip(0, o, 1.0f);
         store(1);
       }
@@ -422,7 +448,7 @@ __device__ __forceinline__ void attn_long_body(
       const int kA = 16 * strip + g, kB = kA + 8;
       bool liveA = false, liveB = false;
       if (live) {
-        const uint32_t kw = reinterpret_cast<const uint32_t*>(smem + 2 * L::TOP)[warp >> 1];
+        const uint32_t kw = reinterpret_cast<const uint32_t*>(smem + 2 * L::TOP)[sw >> 1];
         liveA = (kw >> ((r0 + g) & 31)) & 1u;
         liveB = (kw >> ((r0 + g + 8) & 31)) & 1u;
         load_tile_frags(2);
@@ -432,9 +458,9 @@ __device__ __forceinline__ void attn_long_body(
       // one pass over the streamed queries that adds their dV products to dv (with_dv) and / or their dK products to dk
       // (with_dk), in the same query order either way; a dV-only pass needs neither dP nor the tile's V.  The flags are
       // constants at every call, so each call compiles to its own loop.
-      auto dkdv_pass = [&](bool with_dv, bool with_dk, float (&dv)[NKB][KSB][4], float (&dk)[NKB][KSB][4]) {
+      auto dkdv_pass = [&](bool with_dv, bool with_dk, float (&dv)[NKO][KSB][4], float (&dk)[NKO][KSB][4]) {
 #pragma unroll
-        for (int kb = 0; kb < NKB; ++kb)
+        for (int kb = 0; kb < NKO; ++kb)
 #pragma unroll
           for (int nt = 0; nt < KSB; ++nt)
 #pragma unroll
@@ -497,10 +523,11 @@ __device__ __forceinline__ void attn_long_body(
             const uint32_t pa[4] = {__float_as_uint(pu[0]), __float_as_uint(pu[2]), __float_as_uint(pu[1]), __float_as_uint(pu[3])};
             const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
 #pragma unroll
-            for (int kb = 0; kb < NKB; ++kb) {
+            for (int kb = 0; kb < NKO; ++kb) {
+              const uint32_t do_b = do_s + (kb0 + kb) * L::SSLAB, q_b = q_s + (kb0 + kb) * L::SSLAB;
               uint32_t o0[KSB], o1[KSB], q0v[KSB], q1v[KSB];
-              if (with_dv) { ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t, g, o0); ld_b_out<KSB>(do_s + kb * L::SSLAB, q0 + t + 4, g, o1); }
-              if (with_dk) { ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t, g, q0v); ld_b_out<KSB>(q_s + kb * L::SSLAB, q0 + t + 4, g, q1v); }
+              if (with_dv) { ld_b_out<KSB>(do_b, q0 + t, g, o0); ld_b_out<KSB>(do_b, q0 + t + 4, g, o1); }
+              if (with_dk) { ld_b_out<KSB>(q_b, q0 + t, g, q0v); ld_b_out<KSB>(q_b, q0 + t + 4, g, q1v); }
 #pragma unroll
               for (int nt = 0; nt < KSB; ++nt) {
                 if (with_dv) {
@@ -533,16 +560,20 @@ __device__ __forceinline__ void attn_long_body(
       };
       if constexpr (SPLIT) {
         // dK first, staged over the warp's own V rows (the dV pass reads only K), then dV over its K rows
-        float acc[NKB][KSB][4];
+        float acc[NKO][KSB][4];
         dkdv_pass(false, true, acc, acc);
         if (has) {
           store_wait();
+          pair_sync();
           stage_strip(1, acc, scale);
         }
         dkdv_pass(true, false, acc, acc);
-        if (has) stage_strip(0, acc, 1.0f);
+        if (has) {
+          pair_sync();
+          stage_strip(0, acc, 1.0f);
+        }
       } else {
-        float dv[NKB][KSB][4], dk[NKB][KSB][4];
+        float dv[NKO][KSB][4], dk[NKO][KSB][4];
         dkdv_pass(true, true, dv, dk);
         if (has) {
           store_wait();
@@ -567,9 +598,9 @@ __device__ __forceinline__ void attn_long_body(
         load_tile_frags(2);
       }
       if constexpr (!WIDE) release_tile();
-      float dq[NKB][KSB][4];
+      float dq[NKO][KSB][4];
 #pragma unroll
-      for (int kb = 0; kb < NKB; ++kb)
+      for (int kb = 0; kb < NKO; ++kb)
 #pragma unroll
         for (int nt = 0; nt < KSB; ++nt) dq[kb][nt][0] = dq[kb][nt][1] = dq[kb][nt][2] = dq[kb][nt][3] = 0.f;
       const int nk8 = (it.e + 7) & ~7;     // keys at or beyond the extent are masked
@@ -623,9 +654,10 @@ __device__ __forceinline__ void attn_long_body(
           }
           const uint32_t dsa[4] = {__float_as_uint(ds[0]), __float_as_uint(ds[2]), __float_as_uint(ds[1]), __float_as_uint(ds[3])};
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb) {
+          for (int kb = 0; kb < NKO; ++kb) {
+            const uint32_t k_b = k_s + (kb0 + kb) * L::SSLAB;
             uint32_t k0v[KSB], k1v[KSB];
-            ld_b_out<KSB>(k_s + kb * L::SSLAB, k0 + t, g, k0v); ld_b_out<KSB>(k_s + kb * L::SSLAB, k0 + t + 4, g, k1v);
+            ld_b_out<KSB>(k_b, k0 + t, g, k0v); ld_b_out<KSB>(k_b, k0 + t + 4, g, k1v);
 #pragma unroll
             for (int nt = 0; nt < KSB; ++nt) {
               rt(k0v[nt]); rt(k1v[nt]);
@@ -634,12 +666,13 @@ __device__ __forceinline__ void attn_long_body(
             }
           }
         };
+        // two blocks in flight (DK 256: one, or the fragments spill)
         int k0 = 0;
-        for (; k0 + 16 <= nk; k0 += 16) {
+        for (; k0 + 8 * DQ_NB <= nk; k0 += 8 * DQ_NB) {
           float s[2][4], dp[2][4];
-          products(std::integral_constant<int, 2>{}, k0, s, dp);
-          accumulate(k0, s[0], dp[0]);
-          accumulate(k0 + 8, s[1], dp[1]);
+          products(std::integral_constant<int, DQ_NB>{}, k0, s, dp);
+#pragma unroll
+          for (int n = 0; n < DQ_NB; ++n) accumulate(k0 + 8 * n, s[n], dp[n]);
         }
         if (k0 < nk) {
           float s[2][4], dp[2][4];
@@ -649,6 +682,7 @@ __device__ __forceinline__ void attn_long_body(
       });
       if (has) {
         store_wait();
+        pair_sync();
         stage_strip(0, dq, scale);
         __syncwarp();
         if (live) bias_add(0, 0);
@@ -680,17 +714,19 @@ using LongKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, 
                             const uint8_t*, float*, float*, const float*, int, int, float, DropSite, float*, int,
                             const int*, int, int);
 
-static int long_items(int B, int h, int S) { return B * h * ((S + LONG_BLK - 1) / LONG_BLK); }
+static int long_items(int B, int h, int S, int blk) { return B * h * ((S + blk - 1) / blk); }
 
-// Bytes the kernels request from L2 / HBM per (slate, head): the tile side once, the streamed side once per tile
-// (the ProfScope accounting; the streamed rows mostly hit L2)
-static double long_bytes(int S, int dk, int tile_ops, int stream_ops, int out_ops) {
-  const double tiles = (S + LONG_BLK - 1) / LONG_BLK;
+// Bytes the kernels request from L2 / HBM per (slate, head): the tile side once, the streamed side once per tile of
+// blk rows (the ProfScope accounting; the streamed rows mostly hit L2)
+static double long_bytes(int S, int dk, int blk, int tile_ops, int stream_ops, int out_ops) {
+  const double tiles = (S + blk - 1) / blk;
   return 4.0 * S * dk * (tile_ops + out_ops + tiles * stream_ops);
 }
 
-// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96, 128)
-static int long_dk(int dk) { return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : dk <= 96 ? 96 : 128; }
+// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96, 128), then 192 and 256
+static int long_dk(int dk) {
+  return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : dk <= 96 ? 96 : dk <= 128 ? 128 : dk <= 192 ? 192 : 256;
+}
 
 template <int DK>
 static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
@@ -702,13 +738,15 @@ static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   if ((rc = make_tmap_4d(&tV, a.v, box, 0))) return rc;
   if ((rc = make_tmap_4d(&tO, a.o, box, 0))) return rc;
   const LongKernel kern = a.drop.thresh != 0 ? attn_long_fwd_kernel<DK, true> : attn_long_fwd_kernel<DK, false>;
-  const int n_items = long_items(a.B, a.h, a.S);
+  constexpr int blk = LongSmem<DK>::BLK;
+  const int n_items = long_items(a.B, a.h, a.S, blk);
   dim3 grid(std::max(1, std::min(n_items, sm_count())));
   ProfScope ps(ARB_PROF_GEMM, (a.extent ? arb_attn_frac() : 1.0) * 4.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
-               double(a.B) * a.h * (long_bytes(a.S, a.dk, 1, 3, 1) + 8.0 * a.S), "attn_long_fwd_kernel");
+               double(a.B) * a.h * (long_bytes(a.S, a.dk, blk, 1, 3, 1) + 8.0 * a.S), "attn_long_fwd_kernel");
+  // d_model = h * dk: the paired kernels store no slab that lies wholly beyond the head width
   return launch(kern, grid, dim3(LONG_THREADS), size_t(LongSmem<DK>::total), st, /*pdl=*/true, tQ, tQ, tK, tV, tO, tO,
                 a.mask, a.stat_max, a.stat_sum, static_cast<const float*>(nullptr), a.S, a.h, a.scale, a.drop,
-                static_cast<float*>(nullptr), 0, a.extent, n_items, tf32_round_on_load());
+                static_cast<float*>(nullptr), a.h * a.dk, a.extent, n_items, tf32_round_on_load());
 }
 
 int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st) {
@@ -719,7 +757,9 @@ int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st) {
     case 32: return launch_long_fwd_t<32>(a, st);
     case 64: return launch_long_fwd_t<64>(a, st);
     case 96: return launch_long_fwd_t<96>(a, st);
-    default: return launch_long_fwd_t<128>(a, st);
+    case 128: return launch_long_fwd_t<128>(a, st);
+    case 192: return launch_long_fwd_t<192>(a, st);
+    default: return launch_long_fwd_t<256>(a, st);
   }
 }
 
@@ -739,7 +779,8 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const LongKernel kdkdv = drop ? attn_long_dkdv_kernel<DK, true> : attn_long_dkdv_kernel<DK, false>;
   const LongKernel kdq = drop ? attn_long_dq_kernel<DK, true> : attn_long_dq_kernel<DK, false>;
   constexpr size_t smem = size_t(LongSmem<DK>::total);
-  const int n_items = long_items(a.B, a.h, a.S);
+  constexpr int blk = LongSmem<DK>::BLK;
+  const int n_items = long_items(a.B, a.h, a.S, blk);
   const int n_ctas = std::max(1, std::min(n_items, sm_count()));
   // the QKV bias gradient: one slot per (CTA, compute warp), summed in order afterwards
   float* dbias = a.dbias_qkv;
@@ -751,7 +792,7 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   const double frac = a.extent ? arb_attn_frac() : 1.0;
   {
     ProfScope ps(ARB_PROF_GEMM, frac * 8.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
-                 double(a.B) * a.h * (long_bytes(a.S, a.dk, 2, 2, 2) + 8.0 * a.S), "attn_long_dkdv_kernel");
+                 double(a.B) * a.h * (long_bytes(a.S, a.dk, blk, 2, 2, 2) + 8.0 * a.S), "attn_long_dkdv_kernel");
     if ((rc = launch(kdkdv, dim3(n_ctas), dim3(LONG_THREADS), smem, st, /*pdl=*/true, tK, tV, tQ,
                      tDO, tDV, tDK, a.mask, smax, ssum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent,
                      n_items, tf32_round_on_load())))
@@ -759,7 +800,7 @@ static int launch_long_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
   }
   {
     ProfScope ps(ARB_PROF_GEMM, frac * 6.0 * double(a.S) * a.S * a.dk * a.h * a.B, st,
-                 double(a.B) * a.h * (long_bytes(a.S, a.dk, 2, 2, 1) + 12.0 * a.S), "attn_long_dq_kernel");
+                 double(a.B) * a.h * (long_bytes(a.S, a.dk, blk, 2, 2, 1) + 12.0 * a.S), "attn_long_dq_kernel");
     if ((rc = launch(kdq, dim3(n_ctas), dim3(LONG_THREADS), smem, st, /*pdl=*/true, tQ, tDO, tK,
                      tV, tDQ, tDQ, a.mask, smax, ssum, a.delta, a.S, a.h, a.scale, a.drop, dbias, a.d_model, a.extent,
                      n_items, tf32_round_on_load())))
@@ -774,7 +815,9 @@ int launch_attn_long_bwd(const AttnBwdArgs& a, cudaStream_t st) {
     case 32: return launch_long_bwd_t<32>(a, st);
     case 64: return launch_long_bwd_t<64>(a, st);
     case 96: return launch_long_bwd_t<96>(a, st);
-    default: return launch_long_bwd_t<128>(a, st);
+    case 128: return launch_long_bwd_t<128>(a, st);
+    case 192: return launch_long_bwd_t<192>(a, st);
+    default: return launch_long_bwd_t<256>(a, st);
   }
 }
 

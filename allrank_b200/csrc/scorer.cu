@@ -96,7 +96,7 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
       arb_set_error("scorer: need d_model % h == 0, (d_model/h) % 4 == 0 and d_ff % 4 == 0");
       return ARB_E_UNSUPPORTED;
     }
-    if (c.d_model / c.n_heads > 128) { arb_set_error("scorer: head width above 128 is not supported"); return ARB_E_UNSUPPORTED; }
+    if (c.d_model / c.n_heads > 256) { arb_set_error("scorer: head width above 256 is not supported"); return ARB_E_UNSUPPORTED; }
   }
   if (c.d_model > 1024) { arb_set_error("scorer: d_model above 1024 is not supported"); return ARB_E_UNSUPPORTED; }
   if (c.bf16 && c.n_layers > 0 && (c.d_model % 8 || c.d_ff % 8 || c.d_model < 64 || c.d_ff < 64)) {
@@ -956,7 +956,7 @@ static int attention_hook_check(const char* what, int B, int S, int h, float p, 
   if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
   if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
   if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
-    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 128 in steps of 4)").c_str());
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 256 in steps of 4)").c_str());
     return ARB_E_UNSUPPORTED;
   }
   return ARB_OK;

@@ -37,7 +37,8 @@ then also runs the first FC layer's input-gradient product; with every parameter
 gradient at all.  In the default packed-row layout (include/allrank_b200.h: arb_set_pack_rows) items at or beyond their
 slate's packed rows get 0 in `prepare_for_output` and in x.grad, and a gradient sent to their hidden rows is ignored --
 the same contract as their score.  Double backward is not supported (it raises).
-Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes.
+Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes, and
+attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU).
 """
 import contextlib
 import copy

@@ -1,13 +1,14 @@
 """Training steps of the shipped Transformer configurations whose heads are wider than 32 columns -- local_config
 (d 64, h 1: width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96,
-h 1: width 96) -- of a d = 256, h = 4 model (width 64), and of two width-128 models (d 128, h 1 and d 256, h 2), each
-with its own dropout and loss: the fused attention
+h 1: width 96) -- of a d = 256, h = 4 model (width 64), of two width-128 models (d 128, h 1 and d 256, h 2), and of the
+neuralNDCG-paper model widened to one head of 136, 192 or 256 columns, each with its own dropout and loss: the fused
+attention
 kernels (attention mode 2; csrc/attention_long.cu serves these widths) against the unfused sequence
 (arb_set_attention_mode(0): [B, h, S, S] probabilities in HBM) where the latter exists (S <= 1536).
 
     python tools/bench_head_widths.py [--steps 5] [--warmup 2] [--runs 3] [--models a,b] [--json out.json]
 
-Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the width-96 and width-128 models at S = 1024,
+Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the models of width 96 and above at S = 1024,
 2048, 4096
 (B = 245760 / S slates, fewer where the unfused path would not fit in memory).  Slate lengths ~ N(S/2, S/4) clamped to
 [1, S].  Step time is the host clock around `steps` training steps that end in a device synchronise, per run; the
@@ -45,9 +46,14 @@ MODELS = {
                      transformer={"N": 2, "d_ff": 1024, "h": 2, "positional_encoding": None, "dropout": 0.1},
                      post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0})),
 }
-SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [(name, 245760 // S, S)
-                                                                     for name in ("approxndcg", "d128_h1", "d256_h2")
-                                                                     for S in (1024, 2048, 4096)]
+# the neuralNDCG-paper model (approxndcg) widened to one head of 136 (the MSLR feature count), 192 and 256 columns
+for _w in (136, 192, 256):
+    MODELS[f"d{_w}_h1"] = (dict(fc_model={"sizes": [_w], "input_norm": False, "activation": None, "dropout": 0.0},
+                                transformer={"N": 2, "d_ff": 384, "h": 1, "positional_encoding": None, "dropout": 0.1},
+                                post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0}))
+SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [
+    (name, 245760 // S, S) for name in ("approxndcg", "d128_h1", "d256_h2", "d136_h1", "d192_h1", "d256_h1")
+    for S in (1024, 2048, 4096)]
 
 
 def make_batch(B, S, seed=7):
