@@ -435,7 +435,9 @@ __global__ void __launch_bounds__(256) listmle_kernel(const float* __restrict__ 
   for (int i = threadIdx.x; i < S; i += blockDim.x) {
     src[i] = __float_as_int(cc[i]);
     if (z[i] == mx) amax = min(amax, i);
-    z[i] = z[i] - mx;
+    // pads stay -inf: in an all-padded slate mx is -inf too and -inf - -inf would make them NaN, i.e. "valid"
+    // below, where the reference masks them to 0 and the slate adds nothing
+    if (z[i] != -CUDART_INF_F) z[i] = z[i] - mx;
     e[i] = expf(z[i]);
   }
   // first arg-max in sorted order (torch.max(dim) returns the first maximal index)
@@ -735,11 +737,11 @@ __global__ void __launch_bounds__(256) ranknet_kernel(const float* __restrict__ 
 }
 
 // binary_listNet (losses/binary_listNet.py:8-33), pointwise_rmse (pointwise.py:6-32), bce (bce.py:8-32):
-// O(S) per slate, one warp per slate, mode selects the formula.
+// O(S) per slate, one warp per slate, mode selects the formula.  Each pass streams the slate, item i on lane i % 32,
+// and recomputes what it needs from the inputs, so any slate length runs with a handful of registers.
 //   mode 0 binary_listNet: -sum_i (y_i / max(sum y,1 if 0)) log(softmax(s)_i + eps)           mean over batch
 //   mode 1 pointwise_rmse: sqrt( sum_valid (y_i - L s_i)^2 / n_valid )                          mean over batch
 //   mode 2 bce           : sum_valid -(y log p + (1-y) log(1-p)) (logs clamped at -100),  / #slates with a valid item
-constexpr int PW_MAX_PER_LANE = 40;
 __global__ void __launch_bounds__(128) pointwise_warp_kernel(const float* __restrict__ y_pred,
                                                              const float* __restrict__ y_true, int B, int S,
                                                              float pad, int mode, float param, float eps, float inv_B,
@@ -750,86 +752,75 @@ __global__ void __launch_bounds__(128) pointwise_warp_kernel(const float* __rest
   if (b >= B) return;
   const float* yp = y_pred + size_t(b) * S;
   const float* yt = y_true + size_t(b) * S;
-  float s[PW_MAX_PER_LANE], t[PW_MAX_PER_LANE];
-  bool ok[PW_MAX_PER_LANE];
-  float nvalid = 0.f, tsum = 0.f, ms = -CUDART_INF_F;
-#pragma unroll
-  for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-    const int i = lane + 32 * r;
-    ok[r] = false; s[r] = 0.f; t[r] = 0.f;
-    if (i < S) {
-      const float lab = yt[i];
-      ok[r] = lab != pad;
-      s[r] = yp[i];
-      t[r] = ok[r] ? lab : 0.f;
+  float* gb = grad ? grad + size_t(b) * S : nullptr;
+  float nvalid = 0.f, lossb = 0.f;
+  if (mode == 2) {
+    for (int i = lane; i < S; i += 32) {
+      const float y = yt[i];
+      float g = 0.f;
+      if (y != pad) {
+        const float p = yp[i];
+        nvalid += 1.f;
+        lossb -= y * fmaxf(logf(p), -100.0f) + (1.0f - y) * fmaxf(logf(1.0f - p), -100.0f);
+        g = (p - y) / fmaxf(p * (1.0f - p), 1e-12f);       // BCELoss backward
+      }
+      if (gb) gb[i] = g;
     }
-    if (ok[r]) { nvalid += 1.f; tsum += t[r]; ms = fmaxf(ms, s[r]); }
+    nvalid = warp_sum(nvalid);
+    lossb = warp_sum(lossb);
+    if (lane == 0) { val[b] = lossb; cnt[b] = nvalid > 0.f ? 1.f : 0.f; }
+    return;
+  }
+  float tsum = 0.f, ms = -CUDART_INF_F;
+  for (int i = lane; i < S; i += 32) {
+    const float lab = yt[i];
+    if (lab != pad) { nvalid += 1.f; tsum += lab; ms = fmaxf(ms, yp[i]); }
   }
   nvalid = warp_sum(nvalid);
   tsum = warp_sum(tsum);
-  float lossb = 0.f;
   if (mode == 0) {
     ms = warp_max(ms);
     const float norm = (tsum == 0.0f) ? 1.0f : tsum;
     float zs = 0.f;
-#pragma unroll
-    for (int r = 0; r < PW_MAX_PER_LANE; ++r) { s[r] = ok[r] ? expf(s[r] - ms) : 0.f; zs += s[r]; }
+    for (int i = lane; i < S; i += 32)
+      if (yt[i] != pad) zs += expf(yp[i] - ms);
     zs = warp_sum(zs);
+    // padded items: q = 0 and p = 0, so they add -0 to the loss and 0 to R (all-padded slate: p = 0/0, NaN)
     float R = 0.f;
-#pragma unroll
-    for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-      const float p = s[r] / zs, q = t[r] / norm;
-      if (lane + 32 * r < S) lossb -= q * logf(p + eps);   // padded items: q = 0 and p = 0 -> 0 * log(eps) = -0
-      const float rr = q * p / (p + eps);
-      R += rr;
-      s[r] = p; t[r] = rr;
+    for (int i = lane; i < S; i += 32) {
+      const float lab = yt[i];
+      const bool ok = lab != pad;
+      const float p = (ok ? expf(yp[i] - ms) : 0.f) / zs, q = (ok ? lab : 0.f) / norm;
+      lossb -= q * logf(p + eps);
+      R += q * p / (p + eps);
     }
     lossb = warp_sum(lossb);
     R = warp_sum(R);
     if (lane == 0) { val[b] = lossb * inv_B; cnt[b] = 1.f; }
-    if (grad) {
-#pragma unroll
-      for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-        const int i = lane + 32 * r;
-        if (i < S) grad[size_t(b) * S + i] = -(t[r] - s[r] * R) * inv_B;
+    if (gb) {
+      for (int i = lane; i < S; i += 32) {
+        const float lab = yt[i];
+        const bool ok = lab != pad;
+        const float p = (ok ? expf(yp[i] - ms) : 0.f) / zs, q = (ok ? lab : 0.f) / norm;
+        gb[i] = -(q * p / (p + eps) - p * R) * inv_B;
       }
     }
-  } else if (mode == 1) {
+  } else {
     float sq = 0.f;
-#pragma unroll
-    for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-      const float e = ok[r] ? t[r] - param * s[r] : 0.f;
-      t[r] = e;
-      sq += e * e;
+    for (int i = lane; i < S; i += 32) {
+      const float lab = yt[i];
+      if (lab != pad) {
+        const float e = lab - param * yp[i];
+        sq += e * e;
+      }
     }
     sq = warp_sum(sq);
     const float rmse = sqrtf(sq / nvalid);
     if (lane == 0) { val[b] = rmse * inv_B; cnt[b] = 1.f; }
-    if (grad) {
-#pragma unroll
-      for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-        const int i = lane + 32 * r;
-        if (i < S) grad[size_t(b) * S + i] = ok[r] ? (-param * t[r] / (nvalid * rmse)) * inv_B : 0.f;
-      }
-    }
-  } else {
-#pragma unroll
-    for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-      if (ok[r]) {
-        const float p = s[r], y = t[r];
-        lossb -= y * fmaxf(logf(p), -100.0f) + (1.0f - y) * fmaxf(logf(1.0f - p), -100.0f);
-        t[r] = (p - y) / fmaxf(p * (1.0f - p), 1e-12f);       // BCELoss backward
-      } else {
-        t[r] = 0.f;
-      }
-    }
-    lossb = warp_sum(lossb);
-    if (lane == 0) { val[b] = lossb; cnt[b] = nvalid > 0.f ? 1.f : 0.f; }
-    if (grad) {
-#pragma unroll
-      for (int r = 0; r < PW_MAX_PER_LANE; ++r) {
-        const int i = lane + 32 * r;
-        if (i < S) grad[size_t(b) * S + i] = t[r];
+    if (gb) {
+      for (int i = lane; i < S; i += 32) {
+        const float lab = yt[i];
+        gb[i] = lab != pad ? (-param * (lab - param * yp[i]) / (nvalid * rmse)) * inv_B : 0.f;
       }
     }
   }
@@ -1025,7 +1016,6 @@ extern "C" int32_t arb_pointwise_loss(const float* y_pred, const float* y_true, 
                                       void* stream) {
   ARB_CHECK_ARGS(y_pred && y_true && loss && scratch && B > 0 && S > 0, "arb_pointwise_loss: null pointer or bad shape");
   ARB_CHECK_ARGS(mode >= 0 && mode <= 2, "arb_pointwise_loss: mode must be 0 (binary_listNet), 1 (rmse) or 2 (bce)");
-  if (S > 32 * PW_MAX_PER_LANE) { arb_set_error("arb_pointwise_loss: slate_length above 1280 is not supported"); return ARB_E_UNSUPPORTED; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int wpb = 4;
   {

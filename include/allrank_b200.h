@@ -118,7 +118,11 @@ int32_t arb_ranknet(const float* y_pred, const float* y_true, int32_t B, int32_t
                     int32_t weight_mode, float* loss, float* grad, float* scratch, void* stream);
 /* mode 0: binary_listNet(eps)            .../losses/binary_listNet.py:8-33
  * mode 1: pointwise_rmse(no_of_levels = param)   .../losses/pointwise.py:6-32
- * mode 2: bce (y_pred are probabilities)          .../losses/bce.py:8-32 */
+ * mode 2: bce (y_pred are probabilities)          .../losses/bce.py:8-32
+ * Any slate length: one warp streams each slate and uses no shared memory.  The other losses are bounded by the
+ * shared memory of one CTA: neuralNDCG serves S <= 4096 exactly, lambdaLoss about 5570, approxNDCG (and
+ * arb_rank_metrics) about 6680, listMLE 8192, listNet and rankNet about 29 000, ordinal any length; a longer slate
+ * returns ARB_E_UNSUPPORTED without a launch. */
 int32_t arb_pointwise_loss(const float* y_pred, const float* y_true, int32_t B, int32_t S, float pad_value,
                            int32_t mode, float param, float eps, float* loss, float* grad, float* scratch,
                            void* stream);

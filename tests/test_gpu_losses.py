@@ -150,11 +150,10 @@ def test_padding_and_item_permutation_invariance(L, name, kw):
     extra = 16
     y2 = torch.cat([y, torch.full((B, extra), -1.0)], dim=1)
     yp2 = torch.cat([yp, torch.randn(B, extra)], dim=1)
-    if name != "neuralNDCG":
-        val2, grad2 = run(getattr(L, name), yp2, y2, **kw)
-        assert val2 == pytest.approx(val, rel=2e-6)
-        assert np.abs(grad2[:, :S] - grad).max() <= 2e-6 * np.abs(grad).max()
-        assert (grad2[:, S:] == 0).all()
+    val2, grad2 = run(getattr(L, name), yp2, y2, **kw)
+    assert val2 == pytest.approx(val, rel=2e-6)
+    assert np.abs(grad2[:, :S] - grad).max() <= 2e-6 * np.abs(grad).max()
+    assert (grad2[:, S:] == 0).all()
     # (2) permute the items of every slate (keeps pads as pads); NeuralSort's scaling uses positions of the
     #     valid block, so keep the valid prefix a prefix: permute only inside the valid prefix
     g = torch.Generator().manual_seed(3)

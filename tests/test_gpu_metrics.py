@@ -61,7 +61,7 @@ def test_golden_bit_exact(M, golden):
                               g[key + "_dcg_identity"]), key
 
 
-@pytest.mark.parametrize("B,S", [(64, 240), (256, 120), (4, 1251), (3, 1), (2, 2049)])
+@pytest.mark.parametrize("B,S", [(64, 240), (256, 120), (4, 1251), (3, 1), (2, 2049), (1, 4096)])
 def test_against_oracle_bit_exact(M, B, S):
     from oracle import metrics_ref
     from allrank_b200.synth import make_slates, make_scores
