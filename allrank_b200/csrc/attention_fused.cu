@@ -1,4 +1,5 @@
-// Fused self-attention core for slates of up to 256 items:  ctx = softmax(mask(Q K^T / sqrt(dk))) V
+// Fused self-attention core for slates of up to 256 items (head widths 4 ... 32 and 64):
+//   ctx = softmax(mask(Q K^T / sqrt(dk))) V
 // in ONE kernel, the [S,S] score / probability tile living only in registers.
 //
 // Reference: attention() allrank/models/transformer.py:137-156 (+ the head split / concat of
@@ -348,7 +349,8 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
   if ((rc = make_tmap_4d(&tK, a.k, box, 0))) return rc;
   if ((rc = make_tmap_4d(&tV, a.v, box, 0))) return rc;
   const bool out16 = a.o.bf16 != 0;
-  if (out16 && DK > 32) { arb_set_error("attn_fwd: a bf16 context needs head width <= 32"); return ARB_E_UNSUPPORTED; }
+  // the bfloat16 head view's head stride (2 w bytes) must be a multiple of 16 bytes for TMA
+  if (out16 && (DK > 32 || a.dk % 8)) { arb_set_error("attn_fwd: a bf16 context needs head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
   const bool packed = a.pack_off != nullptr;
   if (packed && !a.extent) { arb_set_error("attn_fwd: packed rows need the slate extents"); return ARB_E_UNSUPPORTED; }
   if ((rc = make_tmap_4d(&tO, a.o, box, out16 ? 1 : 0))) return rc;
@@ -376,20 +378,20 @@ static int launch_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
                 tf32_round_on_load(), pool_units);
 }
 
-// attn_fwd_kernel: S <= 256 at head width 16, 32 or 64; attention_long.cu: S <= 4096 at 16, 32 and 36 ... 256 in steps
-// of 4 (every width but 64 at S <= 256 runs there)
+// attn_fwd_kernel: S <= 256 at head widths 4 ... 32 in steps of 4 and at 64; attention_long.cu: S <= 4096 at 4 ... 256 in
+// steps of 4 (every width above 32 but 64 at S <= 256 runs there).  Widths below 16 run on DK 16 and widths 20 ... 28
+// on DK 32, as in attention_long.cu: the tensor maps have the real width, so TMA loads zero-fill the columns past it
+// and TMA stores clip there.
 bool attn_fused_supported(int S, int dk) {
-  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 256 && dk % 4 == 0));
+  return S >= 1 && S <= 4096 && dk >= 4 && dk <= 256 && dk % 4 == 0;
 }
 
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
   if (!attn_fused_supported(a.S, a.dk)) { arb_set_error("fused attention: unsupported shape"); return ARB_E_UNSUPPORTED; }
   if (a.S > 256 || (a.dk > 32 && a.dk != 64)) return launch_attn_long_fwd(a, st);
-  switch (a.dk) {
-    case 16: return launch_fwd_t<16>(a, st);
-    case 32: return launch_fwd_t<32>(a, st);
-    default: return launch_fwd_t<64>(a, st);
-  }
+  if (a.dk <= 16) return launch_fwd_t<16>(a, st);
+  if (a.dk <= 32) return launch_fwd_t<32>(a, st);
+  return launch_fwd_t<64>(a, st);
 }
 
 }  // namespace arb

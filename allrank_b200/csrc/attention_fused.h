@@ -21,9 +21,9 @@ struct AttnFwdArgs {
                                  // only the first round_up(extent[b], 16) rows of every slate, slate b at row pack_off[b]
 };
 
-// S <= 256 at head width 16, 32 or 64 (attention_fused.cu), or, with an fp32 context and the dense layout
-// (attention_long.cu), 256 < S <= 4096 at head width 16 or 32 and 1 <= S <= 4096 at 36 ... 256 in steps of 4 (but 64 at
-// S <= 256)
+// S <= 256 at head widths 4 ... 32 in steps of 4 and at 64 (attention_fused.cu), or, with an fp32 context and the dense
+// layout (attention_long.cu), 256 < S <= 4096 at head widths 4 ... 32 and 1 <= S <= 4096 at 36 ... 256 in steps of 4
+// (but 64 at S <= 256).  A bf16 context needs S <= 256 and head width 8, 16, 24 or 32.
 bool attn_fused_supported(int S, int dk);
 void set_attn_fwd_two_pass(int on);   // accepted for the C ABI; every setting runs the same kernel
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st);
@@ -58,8 +58,8 @@ struct AttnBwdArgs {
   const int* rowmap = nullptr;   // packed rows: item index of every packed row (for the delta kernel)
 };
 
-// S <= 4096 at head width 16, 32 and 36 ... 256 in steps of 4; beyond 256 items or 32 columns fp32 operands and the
-// dense layout only
+// S <= 4096 at head widths 4 ... 256 in steps of 4; beyond 256 items or 32 columns fp32 operands and the dense layout
+// only
 bool attn_fused_bwd_supported(int S, int dk);
 void set_attn_bwd_persistent(int on);   // 1: one CTA per SM walks the (slate, head) items; 0: one CTA per item
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st);

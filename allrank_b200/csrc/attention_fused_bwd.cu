@@ -1,4 +1,4 @@
-// Fused self-attention backward for slates of up to 256 items and head width 16 or 32 (other shapes:
+// Fused self-attention backward for slates of up to 256 items and head widths 4 ... 32 (on DK 16 or 32; other shapes:
 // attention_long.cu).
 //
 // Reference: autograd of attention() allrank/models/transformer.py:137-156.  Given d ctx it produces dQ, dK, dV
@@ -22,9 +22,9 @@ constexpr int BWD_WARPS = 8;                          // compute warps: one 16-r
 constexpr int BWD_THREADS = 32 * (BWD_WARPS + 2);     // + one load warp, one store warp
 
 // delta[b,h,q] = sum_e dO[b,q,h,e] * O[b,q,h,e]: one warp per row of the [B*S, d_model] activations, 128-bit loads,
-// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {16, 32, 64, 128}: 4, 8, 16 or 32 lanes per
-// head); other widths (36 ... 124) reduce one head at a time over the whole warp.  Widths above 128:
-// attn_delta_wide_kernel.
+// segmented shuffle reduction over the dk/4 lanes that share a head (dk in {4, 8, 16, 32, 64, 128}: 1, 2, 4, 8, 16 or
+// 32 lanes per head); other widths (12 ... 28, 36 ... 124) reduce one head at a time over the whole warp.  Widths above
+// 128: attn_delta_wide_kernel.
 constexpr int DELTA_RPW = 4;     // rows per warp of the delta kernel
 __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict__ d_o, const float* __restrict__ o,
                                                          long long pitch, int B, int S, int h, int dk,
@@ -44,8 +44,8 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
 #pragma unroll
   for (int q = 0; q < DELTA_RPW; ++q) item[q] = (row0 + q < rows) ? (rowmap ? (long long)rowmap[row0 + q] : row0 + q) : -1;
   if (dk & (dk - 1)) {
-    // a width that is not a power of two (36 ... 124, dense fp32 rows): one head at a time, lane l takes its columns
-    // 4l ... 4l + 3 (dk / 4 <= 31 lanes), reduced over the whole warp
+    // a width that is not a power of two (12 ... 28, 36 ... 124, dense rows): one head at a time, lane l takes its
+    // columns 4l ... 4l + 3 (dk / 4 <= 31 lanes), reduced over the whole warp
     for (int head = 0; head < h; ++head) {
       const int c = head * dk + lane * 4;
       const bool on = lane < lanes_per_head;
@@ -55,7 +55,14 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const float* __restrict
         if (on && item[q] >= 0) {
           const long long row = row0 + q;
           const float4 x = *reinterpret_cast<const float4*>(d_o + row * pitch + c);
-          const float4 y = *reinterpret_cast<const float4*>(o + row * pitch + c);
+          float4 y;
+          if (o_bf16) {     // bf16 mode (width 24): the saved context is bfloat16
+            const uint2 u = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(o) + row * pitch + c);
+            y = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                            __uint_as_float(u.y & 0xffff0000u));
+          } else {
+            y = *reinterpret_cast<const float4*>(o + row * pitch + c);
+          }
           acc = x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
         }
         for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(FULL, acc, off);
@@ -366,7 +373,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
       for (int r = 0; r < 16; ++r) s += v[r];
       return s;
     };
-    const bool sums = dbias_qkv != nullptr && lane < DK;
+    // lane c sums column c of the head's w real columns (w < DK: the staged columns past w are zeros, never stored)
+    const int w = d_model / n_heads;
+    const bool sums = dbias_qkv != nullptr && lane < w;
     int seq = 0;
     for (int item = next_item(blockIdx.x); item < n_items; item = next_item(item + gridDim.x)) {
       const Item it = item_info(item);
@@ -402,9 +411,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_bwd_kernel(
           }
         }
         if (sums) {
-          bias_acc[2 * d_model + it.head * DK + lane] += sv;
-          bias_acc[d_model + it.head * DK + lane] += sk;
-          bias_acc[it.head * DK + lane] += sq;
+          bias_acc[2 * d_model + it.head * w + lane] += sv;
+          bias_acc[d_model + it.head * w + lane] += sk;
+          bias_acc[it.head * w + lane] += sq;
         }
       }
     }
@@ -694,9 +703,10 @@ static int launch_bwd_t(const AttnBwdArgs& a, cudaStream_t st) {
 }
 
 
-// head widths 16 and 32, and 36 ... 256 in steps of 4 (attention_long.cu)
+// head widths 4 ... 256 in steps of 4: S <= 256 at widths up to 32 here (below 16 on DK 16, 20 ... 28 on DK 32, with
+// tensor maps of the real width), the rest in attention_long.cu
 bool attn_fused_bwd_supported(int S, int dk) {
-  return S >= 1 && S <= 4096 && (dk == 16 || dk == 32 || (dk > 32 && dk <= 256 && dk % 4 == 0));
+  return S >= 1 && S <= 4096 && dk >= 4 && dk <= 256 && dk % 4 == 0;
 }
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
@@ -705,13 +715,14 @@ int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
   // the same [B, h, S] format at width 64)
   if (a.S > 256 || a.dk > 32) {
     if (a.o_bf16 || a.dq.bf16 || a.dk_.bf16 || a.dv.bf16 || a.pack_off) {
-      arb_set_error("fused attention backward: bf16 operands and packed rows need slate_length <= 256 and head width 16 or 32");
+      arb_set_error("fused attention backward: bf16 operands and packed rows need slate_length <= 256 and head width <= 32");
       return ARB_E_UNSUPPORTED;
     }
     int rc = launch_delta(a, st);
     return rc ? rc : launch_attn_long_bwd(a, st);
   }
-  return a.dk == 16 ? launch_bwd_t<16>(a, st) : launch_bwd_t<32>(a, st);
+  // the same DK as attention_long.cu's long_dk, so a slate gets the same bits from either
+  return a.dk <= 16 ? launch_bwd_t<16>(a, st) : launch_bwd_t<32>(a, st);
 }
 
 }  // namespace arb

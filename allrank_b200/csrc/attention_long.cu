@@ -1,5 +1,5 @@
-// Fused self-attention at head width 16 or 32 for slates of 257 ... 4096 items, and at head widths 36 ... 256 (w % 4 == 0)
-// for slates of 1 ... 4096 items, forward and backward, without the S x S matrix.  attention_fused.cu /
+// Fused self-attention at head widths 4 ... 32 for slates of 257 ... 4096 items, and at head widths 36 ... 256 for slates
+// of 1 ... 4096 items (w % 4 == 0), forward and backward, without the S x S matrix.  attention_fused.cu /
 // attention_fused_bwd.cu serve S <= 256 at width <= 32 (the forward also 64) by holding a whole (slate, head) in shared
 // memory; that stops fitting beyond 256 rows or 32 columns, so here a work item is one 128-row tile (DK 192, 256: 64
 // rows) of a (slate, head) and the other side of its products streams through a ring of shared-memory stages:
@@ -290,7 +290,7 @@ __device__ __forceinline__ void attn_long_body(
     // each warp sums only its own slabs' columns)
     auto bias_add = [&](int o, int col0) {
       if (dbias == nullptr) return;
-      const int w = WIDE ? d_model / n_heads : DK;
+      const int w = d_model / n_heads;
 #pragma unroll
       for (int kb = 0; kb < NKO; ++kb) {
         const int c = 32 * (kb0 + kb) + lane;
@@ -723,7 +723,8 @@ static double long_bytes(int S, int dk, int blk, int tile_ops, int stream_ops, i
   return 4.0 * S * dk * (tile_ops + out_ops + tiles * stream_ops);
 }
 
-// the instantiation that serves head width dk: 16, 32, or the next slab multiple (64, 96, 128), then 192 and 256
+// the instantiation that serves head width dk: 16 (4 ... 16), 32 (20 ... 32), or the next slab multiple (64, 96, 128),
+// then 192 and 256
 static int long_dk(int dk) {
   return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 64 ? 64 : dk <= 96 ? 96 : dk <= 128 ? 128 : dk <= 192 ? 192 : 256;
 }
@@ -750,8 +751,8 @@ static int launch_long_fwd_t(const AttnFwdArgs& a, cudaStream_t st) {
 }
 
 int launch_attn_long_fwd(const AttnFwdArgs& a, cudaStream_t st) {
-  if (a.o.bf16) { arb_set_error("attn_fwd: a bf16 context needs slate_length <= 256 and head width 16, 32 or 64"); return ARB_E_UNSUPPORTED; }
-  if (a.pack_off) { arb_set_error("attn_fwd: packed rows need slate_length <= 256 and head width 16, 32 or 64"); return ARB_E_UNSUPPORTED; }
+  if (a.o.bf16) { arb_set_error("attn_fwd: a bf16 context needs slate_length <= 256 and head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
+  if (a.pack_off) { arb_set_error("attn_fwd: packed rows need slate_length <= 256 and head width <= 32 or 64"); return ARB_E_UNSUPPORTED; }
   switch (long_dk(a.dk)) {
     case 16: return launch_long_fwd_t<16>(a, st);
     case 32: return launch_long_fwd_t<32>(a, st);

@@ -38,8 +38,8 @@ static int g_skip_padding = ARB_DEFAULT_SKIP_PADDING;
 // computes for an all-zero feature row, which every consumer in allRank masks: DESIGN.md 4.12); 0: dense [B*S] rows
 static int g_pack_rows = ARB_DEFAULT_PACK_ROWS;
 // Beyond 256 items the fused kernels (attention_long.cu) read and write fp32 only: bf16 mode keeps the unfused path
-// there (which it does not support, so such a call fails as before).  At head widths above 32 the fused kernels refuse
-// a bf16 context, so bf16 mode fails there too.
+// there (which it does not support, so such a call fails as before).  bf16 mode needs head width 8, 16, 24 or 32
+// (bf16_head_width); other widths are refused before any launch.
 static bool use_fused(const arb_scorer_config& c, int S) {
   return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, c.d_model / c.n_heads) && !(c.bf16 && S > 256);
 }
@@ -65,12 +65,18 @@ static bool use_ffn_chain(const arb_scorer_config& c, int64_t rows) {
          rows >= int64_t(4) * 128 * sm_count();
 }
 
+// The bfloat16 context and dQ | dK | dV are read and written through per-head tensor maps whose head stride (2 w bytes)
+// TMA needs to be a multiple of 16 bytes; the short kernels stage at most 32 bfloat16 columns per row.
+static bool bf16_head_width(int w) { return w <= 32 && w % 8 == 0; }
+
 // Packed rows need both fused attention kernels of slates up to 256 items at head width 16 or 32 (they take per-slate
 // row offsets; attention_long.cu runs the dense layout, which scores padded items as the reference does) and, so far, a call
 // without dropout (its counters index the dense layout), without a positional encoding and with a single output per
-// item.
+// item.  Narrower heads run the same short kernels but keep the dense layout: packing them would change what their
+// padded items score.
 static bool pack_eligible(const arb_scorer_config& c, int S) {
-  return c.n_layers > 0 && S <= 256 && c.d_model / c.n_heads <= 32 && use_fused_bwd(c, S) && c.dropout == 0.0f &&
+  const int w = c.n_layers > 0 ? c.d_model / c.n_heads : 0;
+  return c.n_layers > 0 && S <= 256 && (w == 16 || w == 32) && use_fused_bwd(c, S) && c.dropout == 0.0f &&
          c.fc_dropout == 0.0f && c.pe_mode == 0 && n_outputs(c) == 1;
 }
 static bool use_pack(const arb_scorer_config& c, int S) { return g_pack_rows && g_skip_padding && pack_eligible(c, S); }
@@ -451,8 +457,13 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   const bool bf = c.bf16 && c.n_layers > 0;
   uint16_t* Pb = bf ? reinterpret_cast<uint16_t*>(ws + W.wb16) : nullptr;
   if (bf) {
+    if (!bf16_head_width(dk)) {
+      arb_set_error("scorer: bf16 mode needs head width 8, 16, 24 or 32 (a bfloat16 head of w columns is 2 w bytes, "
+                    "which TMA needs to be a multiple of 16)");
+      return ARB_E_UNSUPPORTED;
+    }
     if (!use_fused_bwd(c, S)) {
-      arb_set_error("scorer: bf16 mode needs the fused attention kernels (slate_length <= 256, head width 16 or 32)");
+      arb_set_error("scorer: bf16 mode needs the fused attention kernels (slate_length <= 256)");
       return ARB_E_UNSUPPORTED;
     }
     ARB_TRY(convert_to_bf16(P, Pb, L.total, st));      // refresh the GEMM-operand shadow of the master weights
@@ -704,8 +715,13 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   // workspace), the saved bf16 activations, and bf16 copies of the gradients (dy16: the residual-stream gradient as
   // the sublayer below receives it; dxn / dqkv: gradients that only feed products are bfloat16 outright)
   const bool bf = c.bf16 && c.n_layers > 0;
+  if (bf && !bf16_head_width(dk)) {
+    arb_set_error("scorer: bf16 mode needs head width 8, 16, 24 or 32 (a bfloat16 head of w columns is 2 w bytes, "
+                  "which TMA needs to be a multiple of 16)");
+    return ARB_E_UNSUPPORTED;
+  }
   if (bf && !use_fused_bwd(c, S)) {
-    arb_set_error("scorer: bf16 mode needs the fused attention kernels (slate_length <= 256, head width 16 or 32)");
+    arb_set_error("scorer: bf16 mode needs the fused attention kernels (slate_length <= 256)");
     return ARB_E_UNSUPPORTED;
   }
   const uint16_t* Pb = bf ? reinterpret_cast<const uint16_t*>(ws + W.wb16) : nullptr;
@@ -956,7 +972,7 @@ static int attention_hook_check(const char* what, int B, int S, int h, float p, 
   if (B <= 0 || h <= 0 || S <= 0) { arb_set_error((std::string(what) + ": B, S and h must be positive").c_str()); return ARB_E_INVALID_ARG; }
   if (!(p >= 0.0f && p < 1.0f)) { arb_set_error((std::string(what) + ": dropout rate must be in [0, 1)").c_str()); return ARB_E_INVALID_ARG; }
   if (!(bwd ? attn_fused_bwd_supported(S, dk) : attn_fused_supported(S, dk))) {
-    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head width 16, 32, or 36 ... 256 in steps of 4)").c_str());
+    arb_set_error((std::string(what) + ": unsupported shape (S <= 4096 at head widths 4 ... 256 in steps of 4)").c_str());
     return ARB_E_UNSUPPORTED;
   }
   return ARB_OK;
@@ -967,7 +983,7 @@ extern "C" int32_t arb_attention_forward(const float* qkv, const uint8_t* mask, 
                                          int32_t ctx_bf16, void* ctx, float* stat_max, float* stat_sum, void* stream) {
   if (!qkv || !mask || !ctx || !stat_max || !stat_sum) { arb_set_error("arb_attention_forward: null pointer"); return ARB_E_INVALID_ARG; }
   ARB_TRY(attention_hook_check("arb_attention_forward", B, S, h, p, false, dk));
-  if (ctx_bf16 && dk > 32) { arb_set_error("arb_attention_forward: a bf16 context needs head width <= 32"); return ARB_E_UNSUPPORTED; }
+  if (ctx_bf16 && !bf16_head_width(dk)) { arb_set_error("arb_attention_forward: a bf16 context needs head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
   if (ctx_bf16 && S > 256) { arb_set_error("arb_attention_forward: a bf16 context needs S <= 256"); return ARB_E_UNSUPPORTED; }
   const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
   const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
@@ -986,6 +1002,7 @@ extern "C" int32_t arb_attention_backward(const float* qkv, const void* ctx, int
     return ARB_E_INVALID_ARG;
   }
   ARB_TRY(attention_hook_check("arb_attention_backward", B, S, h, p, true, dk));
+  if (ctx_bf16 && !bf16_head_width(dk)) { arb_set_error("arb_attention_backward: a bf16 context needs head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
   const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
   const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
   return launch_attn_bwd(attn_bwd_args(z, qkv, o, d_ctx, d_qkv, mask, extent, stat_max, stat_sum, delta_scratch,

@@ -37,8 +37,11 @@ then also runs the first FC layer's input-gradient product; with every parameter
 gradient at all.  In the default packed-row layout (include/allrank_b200.h: arb_set_pack_rows) items at or beyond their
 slate's packed rows get 0 in `prepare_for_output` and in x.grad, and a gradient sent to their hidden rows is ignored --
 the same contract as their score.  Double backward is not supported (it raises).
+Attention runs on the fused kernels at every head width d_model / h that is a multiple of 4 from 4 to 256, for slates
+of up to 4096 items.
 Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes, and
-attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU).
+attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU);
+compute_dtype="bf16" at head widths other than 8, 16, 24 and 32.
 """
 import contextlib
 import copy
@@ -315,8 +318,9 @@ class LTRModel(nn.Module):
         if value not in ("tf32", "bf16"):
             raise ValueError("compute_dtype must be 'tf32' or 'bf16'")
         if value == "bf16" and self.n_layers > 0 and (self.d_model % 8 or self.d_ff % 8 or
-                                                      self.d_model // max(self.n_heads, 1) not in (16, 32)):
-            raise NotImplementedError("bf16 mode needs d_model, d_ff multiples of 8 and a head width of 16 or 32")
+                                                      self.d_model // max(self.n_heads, 1) not in (8, 16, 24, 32)):
+            raise NotImplementedError("bf16 mode needs d_model, d_ff multiples of 8 and a head width of 8, 16, 24 or 32 "
+                                      "(a bfloat16 head must span a multiple of 16 bytes)")
         self._cfg.bf16 = 1 if value == "bf16" else 0
 
     # ---- flat parameter storage -------------------------------------------------------------------

@@ -204,7 +204,8 @@ typedef struct arb_scorer_config {
                            feed products (LayerNorm outputs, attention context, FFN hidden layer) and the gradients that
                            only feed products stored as bfloat16; residual stream, LayerNorm statistics, softmax,
                            attention scores (TF32 products on fp32 Q/K/V), head, loss and parameter gradients stay fp32.
-                           Needs the fused attention kernels (slate_length <= 256, head width 16 or 32) and
+                           Needs the fused attention kernels (slate_length <= 256), head width 8, 16, 24 or 32
+                           (a bfloat16 head of w columns spans 2w bytes, which TMA needs to be a multiple of 16) and
                            d_model, d_ff multiples of 8.  0: TF32 products on fp32 data everywhere.                  */
 } arb_scorer_config;
 #define ARB_MAX_FC_LAYERS 8
@@ -275,8 +276,8 @@ int32_t arb_scorer_backward_ex_dseed(const arb_scorer_config* cfg, const float* 
 
 /* 0: unfused attention (materialised logits + generic GEMMs); 1: fused tensor-core attention forward kernel, unfused
  * backward; 2 (default): fused forward and backward kernels.  Fused kernels serve slates of <= 256 items at head width
- * 16 or 32 and, in TF32 mode, slates of 1 ... 4096 items at head width 16, 32 or 36 ... 256 (multiples of 4); other
- * shapes use the unfused path automatically (slate_length <= 1536).  Process-wide; exists for A/B tests. */
+ * 8, 16, 24 or 32 in bf16 mode and, in TF32 mode, slates of 1 ... 4096 items at every head width 4 ... 256 in steps of
+ * 4; other shapes use the unfused path automatically (slate_length <= 1536).  Process-wide; exists for A/B tests. */
 void arb_set_attention_mode(int32_t mode);
 
 /* 1 (default): the fused attention kernels stop at each slate's extent -- the 16-row strips of keys (and, where their
@@ -335,8 +336,8 @@ int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const void* aux, co
 
 /* Building blocks exposed for tests: the fused attention kernels of one encoder layer, dense layout, launched with the
  * descriptors the scorer uses (csrc/attention_fused.cu, attention_fused_bwd.cu, attention_long.cu).  Shapes: B slates
- * of S <= 256 items, h heads of width dk 16 or 32 (a bf16 context allowed), or of S <= 4096 items at dk 16, 32 or
- * 36 ... 256 in steps of 4 with an fp32 context (a bf16 context there: ARB_E_UNSUPPORTED); d = h * dk.
+ * of S <= 4096 items, h heads of width dk 4 ... 256 in steps of 4, with an fp32 context; a bf16 context needs S <= 256
+ * and dk 8, 16, 24 or 32 (otherwise ARB_E_UNSUPPORTED); d = h * dk.
  *   qkv       [B*S, 3d] fp32: the QKV linear's output, Q | K | V, head j at columns j*dk ... j*dk + dk - 1 of each
  *   mask      [B, S] uint8, 1 = padded item (a masked key)
  *   extent    nullable [B] int32: keys at or beyond extent[b] must be masked; the kernels skip their work (forward:

@@ -1,18 +1,17 @@
-"""Training steps of the shipped Transformer configurations whose heads are wider than 32 columns -- local_config
-(d 64, h 1: width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96,
-h 1: width 96) -- of a d = 256, h = 4 model (width 64), of two width-128 models (d 128, h 1 and d 256, h 2), and of the
-neuralNDCG-paper model widened to one head of 136, 192 or 256 columns, each with its own dropout and loss: the fused
-attention
-kernels (attention mode 2; csrc/attention_long.cu serves these widths) against the unfused sequence
+"""Training steps of Transformer configurations whose heads are not 16 or 32 columns wide -- local_config (d 64, h 1:
+width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96, h 1: width
+96) -- of a d = 256, h = 4 model (width 64), of two width-128 models (d 128, h 1 and d 256, h 2), of the
+neuralNDCG-paper model widened to one head of 136, 192 or 256 columns, and of the neuralNDCG-paper model at d 64, 96
+and 192 with eight heads (widths 8, 12 and 24), each with its own dropout and loss: the fused attention kernels
+(attention mode 2) against the unfused sequence
 (arb_set_attention_mode(0): [B, h, S, S] probabilities in HBM) where the latter exists (S <= 1536).
 
     python tools/bench_head_widths.py [--steps 5] [--warmup 2] [--runs 3] [--models a,b] [--json out.json]
 
-Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the models of width 96 and above at S = 1024,
-2048, 4096
-(B = 245760 / S slates, fewer where the unfused path would not fit in memory).  Slate lengths ~ N(S/2, S/4) clamped to
-[1, S].  Step time is the host clock around `steps` training steps that end in a device synchronise, per run; the
-modes alternate run by run.  Peak memory is torch.cuda.max_memory_allocated over a run.  The attention kernels' times
+Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the models of width 96 and above and the
+eight-head models at S = 1024, 2048, 4096 (B = 245760 / S slates, fewer where the unfused path would not fit in
+memory).  Slate lengths ~ N(S/2, S/4) clamped to [1, S].  Step time is the host clock around `steps` training steps
+that end in a device synchronise, per run; the modes alternate run by run.  Peak memory is torch.cuda.max_memory_allocated over a run.  The attention kernels' times
 come from torch.profiler in a separate run per shape.  The GPU's name and power limit are printed with the numbers."""
 import argparse
 import json
@@ -51,8 +50,14 @@ for _w in (136, 192, 256):
     MODELS[f"d{_w}_h1"] = (dict(fc_model={"sizes": [_w], "input_norm": False, "activation": None, "dropout": 0.0},
                                 transformer={"N": 2, "d_ff": 384, "h": 1, "positional_encoding": None, "dropout": 0.1},
                                 post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0}))
+# ... and with eight heads of 8 (d 64, the local_config width), 12 (d 96, the paper's width) and 24 (d 192) columns
+for _d in (64, 96, 192):
+    MODELS[f"d{_d}_h8"] = (dict(fc_model={"sizes": [_d], "input_norm": False, "activation": None, "dropout": 0.0},
+                                transformer={"N": 2, "d_ff": 384, "h": 8, "positional_encoding": None, "dropout": 0.1},
+                                post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0}))
 SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [
-    (name, 245760 // S, S) for name in ("approxndcg", "d128_h1", "d256_h2", "d136_h1", "d192_h1", "d256_h1")
+    (name, 245760 // S, S) for name in ("approxndcg", "d128_h1", "d256_h2", "d136_h1", "d192_h1", "d256_h1",
+                                        "d64_h8", "d96_h8", "d192_h8")
     for S in (1024, 2048, 4096)]
 
 
