@@ -1026,8 +1026,7 @@ template <int BLOCK_N, int A_MN, int B_MN>
 static int launch_bf16_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
                          const CUtensorMap& tX, const GemmParams& p, dim3 grid, cudaStream_t st) {
   constexpr bool WGRAD = (A_MN == 1 && B_MN == 1);
-  const bool drop = (p.flags & EPI_DROPOUT) != 0;
-  if (drop && (A_MN || B_MN)) { arb_set_error("gemm_bf16: dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
+  const bool drop = (p.flags & EPI_DROPOUT) != 0;   // (K-major operands only: launch_gemm_tf32)
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams) = nullptr;
   int smem = 0;
   if constexpr (WGRAD) {
@@ -1070,8 +1069,7 @@ static int launch_t(const GemmDesc& d, const CUtensorMap& tA, const CUtensorMap&
   // ring depth: 4 stages for the long split-K loops of the weight gradients (1 CTA/SM), 3 for K >= 256
   // (2 CTAs/SM), 2 for the short contractions (3-4 CTAs/SM)
   constexpr bool CAN_DROP = (A_MN == 0 && B_MN == 0);
-  const bool drop = (p.flags & EPI_DROPOUT) != 0;
-  if (drop && !CAN_DROP) { arb_set_error("gemm_tf32: dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
+  const bool drop = (p.flags & EPI_DROPOUT) != 0;   // (K-major operands only: launch_gemm_tf32)
   const bool deep = !WGRAD && d.K >= 256;
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
   int smem;
@@ -1100,6 +1098,8 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   if ((d.flags & (EPI_ADD_AUX | EPI_MASK_AUX)) && (d.Aux.bf16 != 0) != out16) { arb_set_error("gemm: the aux tile must have the output's element type"); return ARB_E_INVALID_ARG; }
   if (in16 && d.block_n < 64) { arb_set_error("gemm: bf16 operands need block_n >= 64 (a 128-byte row holds 64 elements)"); return ARB_E_INVALID_ARG; }
   if (in16 && (d.nb2 != 1 || d.nb3 != 1)) { arb_set_error("gemm: bf16 operands serve the unbatched linears only"); return ARB_E_UNSUPPORTED; }
+  // (the bf16 kernel for two MN-major operands is the weight gradients' and stages an fp32 tile only)
+  if (out16 && d.a_mn && d.b_mn) { arb_set_error("gemm: a bf16 output needs a K-major operand"); return ARB_E_UNSUPPORTED; }
   const uint32_t kel = in16 ? 64u : 32u;          // K elements per 128-byte row
   const uint32_t ocol = out16 ? 64u : 32u;        // output columns per 128-byte staging row
   alignas(64) CUtensorMap tA, tB, tC, tX;
@@ -1143,6 +1143,8 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   if (d.rows_dev && (d.nb2 != 1 || d.nb3 != 1)) { arb_set_error("gemm: a device-side row count serves unbatched launches only"); return ARB_E_INVALID_ARG; }
   if ((d.flags & EPI_COLSUM) && (!d.colsum_out || split)) { arb_set_error("gemm_tf32: EPI_COLSUM needs colsum_out and a non-split launch"); return ARB_E_INVALID_ARG; }
   if ((d.flags & EPI_DROPOUT) && d.drop.thresh == 0) p.flags &= ~EPI_DROPOUT;
+  // (checked here, before the kernel is picked: the persistent kernel would otherwise take what the one-tile one refuses)
+  if ((p.flags & EPI_DROPOUT) && (d.a_mn || d.b_mn)) { arb_set_error("gemm: the dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
   p.kb_per_split = (total_kb + splits - 1) / splits;
   const int eff_splits = split ? (total_kb + p.kb_per_split - 1) / std::max(1, p.kb_per_split) : 1;
   dim3 grid((d.N + d.block_n - 1) / d.block_n, (d.M + BLOCK_M - 1) / BLOCK_M, split ? std::max(1, eff_splits) : d.nb2 * d.nb3);
@@ -1216,5 +1218,27 @@ extern "C" int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const vo
   d.C = mat(C, N, M, out_bf16 != 0);
   if (aux) d.Aux = mat(aux, N, M, out_bf16 != 0);
   if (flags & EPI_ATOMIC) { d.atomic_out = static_cast<float*>(C); d.atomic_ld = N; }
+  return launch_gemm_tf32(d, static_cast<cudaStream_t>(stream));
+}
+
+// The whole descriptor, copied field for field: the tests launch exactly what the scorer's helpers build.
+extern "C" int32_t arb_gemm_launch(const arb_gemm_desc* in, void* stream) {
+  using namespace arb;
+  if (!in) { arb_set_error("arb_gemm_launch: null descriptor"); return ARB_E_INVALID_ARG; }
+  auto view = [](const arb_gemm_view& v) {
+    TRef t; t.ptr = v.ptr; t.bf16 = v.bf16;
+    for (int i = 0; i < 4; ++i) { t.dim[i] = v.dim[i]; t.stride[i] = v.stride[i]; }
+    return t;
+  };
+  GemmDesc d;
+  d.M = in->M; d.N = in->N; d.K = in->K;
+  d.a_mn = in->a_mn; d.b_mn = in->b_mn; d.b_tf32 = in->b_tf32; d.dgrad = in->dgrad;
+  d.A = view(in->A); d.B = view(in->B); d.C = view(in->C); d.Aux = view(in->aux);
+  d.nb2 = in->nb2; d.nb3 = in->nb3;
+  d.a_b2 = in->a_b2; d.a_b3 = in->a_b3; d.b_b2 = in->b_b2; d.b_b3 = in->b_b3; d.c_b2 = in->c_b2; d.c_b3 = in->c_b3;
+  d.block_n = in->block_n; d.split_k = in->split_k; d.flags = in->flags; d.alpha = in->alpha;
+  d.bias = in->bias; d.atomic_out = in->atomic_out; d.atomic_ld = in->atomic_ld;
+  d.drop = DropSite{in->drop_seed, in->drop_thresh, in->drop_scale, in->drop_key, in->drop_call_seed};
+  d.colsum_out = in->colsum_out; d.bits = in->bits; d.rows_dev = in->rows_dev;
   return launch_gemm_tf32(d, static_cast<cudaStream_t>(stream));
 }

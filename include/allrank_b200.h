@@ -334,6 +334,42 @@ int32_t arb_gemm_bf16(const void* A, const void* B, void* C, const void* aux, co
                       int32_t K, int32_t a_mn, int32_t b_mn, int32_t block_n, int32_t flags, float alpha,
                       int32_t split_k, int32_t out_bf16, float* colsum_out, void* stream);
 
+/* The whole launch descriptor of the GEMM (csrc/gemm_tf32.h, GemmDesc), field for field, for tests that build the
+ * launches the scorer builds: pitched and 4-D batched views, dropout, column sums, ReLU bit words and device-side row
+ * counts.  A view has up to 4 dimensions, dim[0] contiguous, strides in elements; bf16 = 1: bfloat16 elements.
+ * K-major operand: dim = (K, rows, b2, b3); MN-major: dim = (rows, K, b2, b3); C / aux: dim = (N, M, b2, b3).
+ * flags are the EPI_* values of csrc/gemm_tf32.h: 1 bias, 2 ReLU, 4 add aux, 8 mask by aux > 0, 16 split-K into
+ * atomic_out, 32 dropout, 64 column sums into colsum_out, 128 ReLU bit words written, 256 bit words read as the mask.
+ * drop_call_seed: null, or a device word from which the kernel derives the seed
+ * (drop_key as for the scorer's sites); else drop_seed is used.  rows_dev: null, or a device pointer to the live row
+ * count.  Returns 0 or ARB_E_* without launching anything when the descriptor breaks a rule of the GEMM. */
+typedef struct arb_gemm_view {
+  const void* ptr;
+  int64_t dim[4];
+  int64_t stride[4];
+  int32_t bf16;
+} arb_gemm_view;
+typedef struct arb_gemm_desc {
+  int32_t M, N, K;
+  int32_t a_mn, b_mn, b_tf32, dgrad;
+  arb_gemm_view A, B, C, aux;
+  int32_t nb2, nb3;
+  int32_t a_b2, a_b3, b_b2, b_b3, c_b2, c_b3;
+  int32_t block_n, split_k, flags;
+  float alpha;
+  const float* bias;
+  float* atomic_out;
+  int64_t atomic_ld;
+  uint32_t drop_seed, drop_thresh;
+  float drop_scale;
+  uint32_t drop_key;
+  const uint64_t* drop_call_seed;
+  float* colsum_out;
+  uint32_t* bits;
+  const int32_t* rows_dev;
+} arb_gemm_desc;
+int32_t arb_gemm_launch(const arb_gemm_desc* d, void* stream);
+
 /* Building blocks exposed for tests: the fused attention kernels of one encoder layer, dense layout, launched with the
  * descriptors the scorer uses (csrc/attention_fused.cu, attention_fused_bwd.cu, attention_long.cu).  Shapes: B slates
  * of S <= 4096 items, h heads of width dk 4 ... 256 in steps of 4, with an fp32 context; a bf16 context needs S <= 256

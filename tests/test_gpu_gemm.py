@@ -1,9 +1,12 @@
-"""The TMA + tensor-core TF32 GEMM building block against a plain PyTorch fp32 reference of the same op.
+"""The TMA + tensor-core TF32 GEMM building block against an fp64 reference of the same op.
 
-TF32 keeps 10 mantissa bits of each operand (truncation by the tensor core datapath), fp32 accumulate:
-tolerance = 2^-10 relative per operand -> |err| <= ~2e-3 * sqrt(K)-ish of the operand scale; we bound by
-4e-3 * sum_k |a||b| which is the worst-case truncation bound."""
+The kernels round each fp32 operand to tf32 (nearest even) and accumulate in fp32, one rounding per k8 step of the
+tensor core.  The reference is therefore the fp64 product of the operands rounded the same way on the host, and the
+bound is the accumulation depth's: TAU * (ceil(K / 8) + 1) * 2^-24 * sum_k |a~||b~| (+1: the epilogue's rounding);
+truncated operands, or operands rounded another way, miss it by orders of magnitude.  The epilogue and the exact
+bits of the rounding are pinned by tests/test_gpu_gemm_epilogues.py."""
 import ctypes
+import math
 
 import pytest
 import torch
@@ -29,11 +32,29 @@ def gemm():
     return call
 
 
-def ref_and_bound(A, B):
-    """A [.., M,K], B [.., N,K] logical; returns fp64 product and the TF32 truncation bound."""
-    ref = A.double() @ B.double().transpose(-1, -2)
-    bound = 4e-3 * (A.abs().double() @ B.abs().double().transpose(-1, -2)) + 1e-6
+TAU = 2.0      # as tests/test_gpu_gemm_epilogues.py
+
+
+def tf32(x):
+    """fp32 -> tf32, round to nearest even (what the kernels do to their operands)"""
+    b = x.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    b = (b + 0xFFF + ((b >> 13) & 1)) & 0xFFFFE000
+    return torch.where(b >= 2 ** 31, b - 2 ** 32, b).to(torch.int32).view(torch.float32)
+
+
+def ref_and_bound(A, B, steps=0):
+    """A [.., M,K], B [.., N,K] logical; returns the fp64 product of the tf32-rounded operands and the depth bound
+    (steps: further fp32 roundings of the result, e.g. the split-K slot sums)."""
+    Ar, Br = tf32(A).double(), tf32(B).double()
+    ref = Ar @ Br.transpose(-1, -2)
+    depth = math.ceil(A.shape[-1] / 8) + 1 + steps
+    bound = TAU * depth * 2.0 ** -24 * (Ar.abs() @ Br.abs().transpose(-1, -2)) + 1e-30
     return ref, bound
+
+
+def epi_bound(bound, want):
+    """the product's bound, plus one fp32 rounding of each epilogue addition"""
+    return bound + 2.0 ** -23 * want.abs()
 
 
 @pytest.mark.parametrize("block_n", [32, 64, 128])
@@ -61,20 +82,21 @@ def test_epilogues(gemm):
     W = torch.randn(N, K, device="cuda") / K ** 0.5
     bias = torch.randn(N, device="cuda")
     X = torch.randn(M, N, device="cuda")
-    base = A.double() @ W.double().t()
-    tol = 6e-3
+    base, bound = ref_and_bound(A, W)
     # bias + relu
     C = torch.empty(M, N, device="cuda")
     gemm(A, W, C, None, bias, M, N, K, 0, 0, 1, 0, 0, 0, 64, EPI_BIAS | EPI_RELU, 1.0)
-    assert (C.double() - torch.relu(base + bias.double())).abs().max() < tol
+    want = torch.relu(base + bias.double())
+    assert ((C.double() - want).abs() <= epi_bound(bound, want)).all()
     # bias + residual, in place (C aliases aux)
     Xc = X.clone()
     gemm(A, W, Xc, Xc, bias, M, N, K, 0, 0, 1, 0, 0, 0, 128, EPI_BIAS | EPI_ADD_AUX, 1.0)
-    assert (Xc.double() - (base + bias.double() + X.double())).abs().max() < tol
+    want = base + bias.double() + X.double()
+    assert ((Xc.double() - want).abs() <= epi_bound(2 * bound, want)).all()
     # relu-backward mask with a scale
     C = torch.empty(M, N, device="cuda")
     gemm(A, W, C, X, None, M, N, K, 0, 0, 1, 0, 0, 0, 32, EPI_MASK_AUX, 0.5)
-    assert (C.double() - 0.5 * base * (X > 0).double()).abs().max() < tol
+    assert ((C.double() - 0.5 * base * (X > 0).double()).abs() <= 0.5 * bound).all()
 
 
 def test_batched_and_broadcast(gemm):
@@ -91,8 +113,8 @@ def test_batched_and_broadcast(gemm):
     V = torch.randn(nb, N, 32, device="cuda")
     O = torch.full((nb, M, 32), float("nan"), device="cuda")
     gemm(P, V, O, None, None, M, 32, N, 0, 1, nb, M * N, N * 32, M * 32, 32, 0, 1.0)
-    ref = P.double() @ V.double()
-    assert (O.double() - ref).abs().max() < 4e-3
+    ref, bound = ref_and_bound(P, V.transpose(-1, -2))
+    assert ((O.double() - ref).abs() <= bound).all()
     # weights shared across the batch (stride 0)
     W = torch.randn(48, K, device="cuda")
     Y = torch.full((nb, M, 48), float("nan"), device="cuda")
@@ -109,8 +131,7 @@ def test_split_k_weight_gradient(gemm):
     X = torch.randn(rows, in_f, device="cuda")
     dW = torch.zeros(out_f, in_f, device="cuda")
     gemm(dY, X, dW, None, None, out_f, in_f, rows, 1, 1, 1, 0, 0, 0, 64, EPI_ATOMIC, 1.0, split_k=37)
-    ref = dY.double().t() @ X.double()
-    bound = 4e-3 * (dY.abs().double().t() @ X.abs().double()) + 1e-4
+    ref, bound = ref_and_bound(dY.t(), X.t(), steps=37)
     assert ((dW.double() - ref).abs() <= bound).all()
 
 
@@ -172,6 +193,8 @@ def test_persistent_modes_are_bit_identical_to_the_tile_kernel(gemm, mode, K, bl
     finally:
         import os
         _lib.lib().arb_set_gemm_persistent(int(os.environ.get("ARB_GEMM_PERSISTENT", 2)))
-    assert (want[1].double() - (A.double() @ W.double().t() + bias.double() + X.double())).abs().max() < 6e-3
+    base, bound = ref_and_bound(A, W)
+    ref = base + bias.double() + X.double()
+    assert ((want[1].double() - ref).abs() <= epi_bound(2 * bound, ref)).all()
     for w, g in zip(want, got):
         assert torch.equal(w, g)
