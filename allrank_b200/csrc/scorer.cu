@@ -39,12 +39,14 @@ static int g_skip_padding = ARB_DEFAULT_SKIP_PADDING;
 static int g_pack_rows = ARB_DEFAULT_PACK_ROWS;
 // Beyond 256 items the fused kernels (attention_long.cu) read and write fp32 only: bf16 mode keeps the unfused path
 // there (which it does not support, so such a call fails as before).  bf16 mode needs head width 8, 16, 24 or 32
-// (bf16_head_width); other widths are refused before any launch.
+// (bf16_head_width); other widths are refused before any launch.  The kernels run at the buffers' head width: d / h,
+// or round_up(d / h, 4) for padded heads (HeadPad).
+static int buffer_head_width(const arb_scorer_config& c) { return int(align_up(c.d_model / c.n_heads, 4)); }
 static bool use_fused(const arb_scorer_config& c, int S) {
-  return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, c.d_model / c.n_heads) && !(c.bf16 && S > 256);
+  return g_attn_mode >= 1 && c.n_layers > 0 && attn_fused_supported(S, buffer_head_width(c)) && !(c.bf16 && S > 256);
 }
 static bool use_fused_bwd(const arb_scorer_config& c, int S) {
-  return g_attn_mode >= 2 && use_fused(c, S) && attn_fused_bwd_supported(S, c.d_model / c.n_heads);
+  return g_attn_mode >= 2 && use_fused(c, S) && attn_fused_bwd_supported(S, buffer_head_width(c));
 }
 
 static inline int n_outputs(const arb_scorer_config& c) { return c.d_output > 1 ? c.d_output : 1; }
@@ -89,6 +91,8 @@ struct ParamLayout {
   struct Layer { int64_t wqkv, bqkv, wo, bo, w1, b1, w2, b2, ln1_a, ln1_b, ln2_a, ln2_b; };
   Layer layer[64];
   int64_t lnf_a, lnf_b, head_w, head_b, pe, total;
+  int hw, hs;                                // head width d_model / h and its padded width round_up(hw, 4) (0: no encoder)
+  bool padded() const { return hs != hw; }   // heads padded to hs columns (HeadPad, DESIGN.md 4.15)
 };
 
 static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
@@ -98,11 +102,17 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
     return ARB_E_UNSUPPORTED;
   }
   if (c.n_layers > 0) {
-    if (c.n_heads <= 0 || c.d_model % c.n_heads || (c.d_model / c.n_heads) % 4 || c.d_ff <= 0 || c.d_ff % 4) {
-      arb_set_error("scorer: need d_model % h == 0, (d_model/h) % 4 == 0 and d_ff % 4 == 0");
+    if (c.n_heads <= 0 || c.d_model % c.n_heads || c.d_ff <= 0 || c.d_ff % 4) {
+      arb_set_error("scorer: need d_model % h == 0 and d_ff % 4 == 0");
       return ARB_E_UNSUPPORTED;
     }
     if (c.d_model / c.n_heads > 256) { arb_set_error("scorer: head width above 256 is not supported"); return ARB_E_UNSUPPORTED; }
+    // a head width that is not a multiple of 4 is padded to one (HeadPad); the padded heads keep within the 1024
+    // columns every attention kernel and buffer is built for
+    if (int64_t(c.n_heads) * align_up(c.d_model / c.n_heads, 4) > 1024) {
+      arb_set_error("scorer: heads padded to a multiple of 4 columns must fit 1024 columns (h * round_up(d_model / h, 4))");
+      return ARB_E_UNSUPPORTED;
+    }
   }
   if (c.d_model > 1024) { arb_set_error("scorer: d_model above 1024 is not supported"); return ARB_E_UNSUPPORTED; }
   if (c.bf16 && c.n_layers > 0 && (c.d_model % 8 || c.d_ff % 8 || c.d_model < 64 || c.d_ff < 64)) {
@@ -162,7 +172,21 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
     if (c.pe_mode == 2) { o = align_up(o, 4); L.pe = o; o += int64_t(c.pe_rows) * d; }
   }
   L.total = o;
+  L.hw = c.n_layers > 0 ? c.d_model / c.n_heads : 0;
+  L.hs = int(align_up(L.hw, 4));
   return ARB_OK;
+}
+
+static HeadPad head_pad(const arb_scorer_config& c, const ParamLayout& L) {
+  HeadPad m{};
+  m.n_layers = c.n_layers; m.d = c.d_model; m.h = c.n_heads; m.w = L.hw; m.hs = L.hs;
+  if (c.n_layers > 0) {
+    const auto& y = L.layer[0];
+    m.enc0 = y.wqkv;
+    m.enc_stride = y.ln2_b + c.d_model - y.wqkv;
+    m.o_bqkv = y.bqkv - y.wqkv; m.o_wo = y.wo - y.wqkv;
+  }
+  return m;
 }
 
 struct WsLayout {
@@ -177,6 +201,7 @@ struct WsLayout {
   int64_t wb16;                     // bf16 mode: bfloat16 shadow of the whole parameter buffer (same element offsets)
   int64_t wt32, wt32t;              // TF32 mode: the parameters rounded to tf32, and every weight matrix W [out,in]
                                     // rounded and transposed to [in,out] (same element offsets; written by the forward)
+  int64_t wpad;                     // padded heads: the padded attention weights of every layer (HeadPad::size() each)
   int64_t meanf, stdf, xf, total;   // xf: final-norm output, kept only for the multi-output head
   int Sp;
   bool fused;
@@ -190,6 +215,7 @@ static int64_t buffer_rows(const arb_scorer_config& c, int B, int S) {
 
 static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, int training, WsLayout& W) {
   const int64_t R = buffer_rows(c, B, S), d = c.d_model, f = c.d_ff, h = c.n_heads;
+  const int64_t dp = h * L.hs;      // width of the attention activations: d, or the padded heads
   W.Sp = int(align_up(S, 4));
   W.fused = use_fused(c, S);
   int64_t o = 0;
@@ -214,16 +240,17 @@ static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int
   W.wb16 = op == 2 ? take((L.total + 1) / 2) : 0;
   W.wt32 = op == 1 ? take(L.total) : 0;
   W.wt32t = op == 1 ? take(L.total) : 0;
+  W.wpad = L.padded() ? take(c.n_layers * head_pad(c, L).size()) : 0;
   WsLayout::Layer shared{};
   for (int l = 0; l < c.n_layers; ++l) {
     auto& y = W.layer[l];
     if (training || l == 0) {
       y.xn1 = take(R * d / op); y.mean1 = take(R); y.std1 = take(R);
-      y.qkv = take(R * 3 * d);
+      y.qkv = take(R * 3 * dp);
       y.prob = W.fused ? 0 : take(int64_t(B) * h * S * W.Sp);
       y.smax = take(int64_t(B) * h * S);
       y.ssum = take(int64_t(B) * h * S);
-      y.ctx = take(R * d / op);
+      y.ctx = take(R * dp / op);
       y.xn2 = training ? take(R * d / op) : y.xn1;
       y.mean2 = training ? take(R) : y.mean1;
       y.std2 = training ? take(R) : y.std1;
@@ -362,9 +389,10 @@ static void batch_all(GemmDesc& g, int h, int B) {
 // the test entry points (arb_attention_forward / arb_attention_backward) both launch through these, so the tests run
 // the descriptors the scorer uses.
 struct AttnGeom {
-  int B, S, h, dk;
+  int B, S, h, dk;        // dk: the width of a head in the buffers (padded heads: hs)
   int64_t rows;
   const int* pack_off;
+  int w;                  // the real head width: the scale is 1/sqrt(w)
   TRef view(V v, int64_t pitch) const {
     return pack_off ? head_view(v, dk, int(rows), h, 1, pitch) : head_view(v, dk, S, h, B, pitch);
   }
@@ -380,7 +408,7 @@ static AttnFwdArgs attn_fwd_args(const AttnGeom& z, const float* qkv, V ctx, con
   a.o = z.view(ctx, d);
   a.pack_off = z.pack_off;
   a.mask = mask; a.stat_max = stat_max; a.stat_sum = stat_sum;
-  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.dk));
+  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.w));
   a.drop = drop;
   a.extent = extent;
   return a;
@@ -410,7 +438,7 @@ static AttnBwdArgs attn_bwd_args(const AttnGeom& z, const float* qkv, V ctx, con
   a.pack_off = z.pack_off; a.rows_dev = rows_dev; a.rowmap = rowmap;
   a.o_ptr = ctx.p; a.o_bf16 = ctx.bf16 ? 1 : 0; a.do_ptr = dctx; a.o_pitch = d;
   a.mask = mask; a.stat_max = stat_max; a.stat_sum = stat_sum; a.delta = delta;
-  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.dk));
+  a.B = z.B; a.h = z.h; a.S = z.S; a.dk = z.dk; a.scale = 1.0f / sqrtf(float(z.w));
   a.drop = drop;
   a.dbias_qkv = dbias_qkv; a.d_model = int(d);
   a.extent = extent;
@@ -448,7 +476,8 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   if (ws_floats < W.total) { arb_set_error("arb_scorer_forward: workspace too small"); return ARB_E_WORKSPACE; }
   Ctx k{c, B, S, int64_t(B) * S, st};
   const int d = c.d_model, F = c.n_features, f = c.d_ff, h = c.n_heads;
-  const int dk = c.n_layers > 0 ? d / h : 0;
+  const int dk = L.hs, dp = h * dk;   // the buffers' head width (padded heads: round_up(d / h, 4)) and attention width
+  const HeadPad hp = head_pad(c, L);
 
   // dropout follows the module's train()/eval() mode (the host zeroes these in eval); `training` only selects
   // whether activations are kept for a backward pass
@@ -457,7 +486,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   const bool bf = c.bf16 && c.n_layers > 0;
   uint16_t* Pb = bf ? reinterpret_cast<uint16_t*>(ws + W.wb16) : nullptr;
   if (bf) {
-    if (!bf16_head_width(dk)) {
+    if (!bf16_head_width(L.hw)) {
       arb_set_error("scorer: bf16 mode needs head width 8, 16, 24 or 32 (a bfloat16 head of w columns is 2 w bytes, "
                     "which TMA needs to be a multiple of 16)");
       return ARB_E_UNSUPPORTED;
@@ -471,6 +500,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     // refresh the GEMM-operand copy of the master weights (rounded once here instead of in every GEMM; the transposed
     // matrices make every input-gradient product K-major); the backward of this call reads it too
     ARB_TRY(tf32_weight_copy(P, L.total, weight_mats(c, L), tf32_round_on_load(), ws + W.wt32, ws + W.wt32t, st));
+    if (L.padded()) ARB_TRY(head_pad_copy(ws + W.wt32, P, hp, ws + W.wpad, st));
   }
   auto wt = [&](int64_t off) { return bf ? b16(Pb + off) : t32(ws + W.wt32 + off); };
   auto wfc = [&](int64_t off) { return bf ? V(P + off) : t32(ws + W.wt32 + off); };   // FC weights stay fp32 in bf16 mode
@@ -568,25 +598,29 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     if (z.count) ARB_TRY(zero_rows(z, plan, k.R, st));
   }
   // per-head views: dense (dk, S, h, B), or packed (dk, rows, h, 1) with per-slate row offsets inside the kernels
-  const AttnGeom geom{B, S, h, dk, k.R, poff};
+  const AttnGeom geom{B, S, h, dk, k.R, poff, L.hw};
   for (int l = 0; l < c.n_layers; ++l) {
     const auto& pl = L.layer[l];
     const auto& wl = W.layer[l];
     float* xn1 = ws + wl.xn1; float* qkv = ws + wl.qkv; float* prob = ws + wl.prob; float* ctx = ws + wl.ctx;
     float* xmid = ws + wl.xmid; float* xn2 = ws + wl.xn2; float* hdn = ws + wl.hdn; float* xout = ws + wl.xout;
+    // padded heads: the QKV and output linears read the padded weights, so Q | K | V and the context come out padded
+    const float* wpad = L.padded() ? ws + W.wpad + l * hp.size() : nullptr;
+    const V w_qkv = wpad ? t32(wpad + hp.wqkv()) : wt(pl.wqkv), w_o = wpad ? t32(wpad + hp.wo()) : wt(pl.wo);
+    const float* b_qkv = wpad ? wpad + hp.bqkv() : P + pl.bqkv;
     // ---- self-attention sublayer: x + O(attn(LN(x)))   (transformer.py:133, :105-106)
     ARB_TRY(ln_forward(xcur, P + pl.ln1_a, P + pl.ln1_b, c.ln_eps, k.R, d, xn1, ws + wl.mean1, ws + wl.std1, st, 0,
                        bf ? xn1 : nullptr, plan));
-    ARB_TRY(linear_fwd(k, act(xn1), d, d, wt(pl.wqkv), P + pl.bqkv, 3 * d, qkv, 3 * d, 0, nullptr, 0));
+    ARB_TRY(linear_fwd(k, act(xn1), d, d, w_qkv, b_qkv, 3 * dp, qkv, 3 * dp, 0, nullptr, 0));
     if (W.fused) {
       ARB_TRY(launch_attn_fwd(attn_fwd_args(geom, qkv, act(ctx), mask, g_skip_padding ? kext : nullptr, ws + wl.smax,
                                             ws + wl.ssum, make_drop_site(seed, l, SITE_ATTN_P, p_drop)), st));
     } else {
       {
-        GemmDesc g;   // logits = Q K^T / sqrt(dk)      (transformer.py:148)
-        g.M = S; g.N = S; g.K = dk; g.alpha = 1.0f / sqrtf(float(dk));
-        g.A = head_view(qkv, dk, S, h, B, 3 * d);
-        g.B = head_view(qkv + d, dk, S, h, B, 3 * d);
+        GemmDesc g;   // logits = Q K^T / sqrt(w)      (transformer.py:148)
+        g.M = S; g.N = S; g.K = dk; g.alpha = 1.0f / sqrtf(float(L.hw));
+        g.A = head_view(qkv, dk, S, h, B, 3 * dp);
+        g.B = head_view(qkv + dp, dk, S, h, B, 3 * dp);
         g.C = prob_view(prob, S, W.Sp, h, B);
         batch_all(g, h, B); g.block_n = 64;
         ARB_TRY(launch_gemm_tf32(g, st));
@@ -598,13 +632,13 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
         GemmDesc g;   // ctx = P V, written straight into the concatenated-heads layout (transformer.py:156, :201-202)
         g.M = S; g.N = dk; g.K = S; g.b_mn = 1;
         g.A = prob_view(prob, S, W.Sp, h, B);
-        g.B = head_view(qkv + 2 * d, dk, S, h, B, 3 * d);
-        g.C = head_view(ctx, dk, S, h, B, d);
+        g.B = head_view(qkv + 2 * dp, dk, S, h, B, 3 * dp);
+        g.C = head_view(ctx, dk, S, h, B, dp);
         batch_all(g, h, B); g.block_n = pick_block_n(dk);
         ARB_TRY(launch_gemm_tf32(g, st));
       }
     }
-    ARB_TRY(linear_fwd(k, act(ctx), d, d, wt(pl.wo), P + pl.bo, d, xmid, d, EPI_ADD_AUX, xcur, d,
+    ARB_TRY(linear_fwd(k, act(ctx), dp, dp, w_o, P + pl.bo, d, xmid, d, EPI_ADD_AUX, xcur, d,
                        make_drop_site(seed, l, SITE_ATTN_OUT, p_drop)));
     // ---- feed-forward sublayer: x + W2 relu(W1 LN(x))   (transformer.py:134, :227)
     ARB_TRY(ln_forward(xmid, P + pl.ln2_a, P + pl.ln2_b, c.ln_eps, k.R, d, xn2, ws + wl.mean2, ws + wl.std2, st, 0,
@@ -650,7 +684,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   return ARB_OK;
 }
 
-struct ScratchLayout { int64_t dxa, dxb, dxn, dxm, dqkv, dctx, dprob, prob, delta, dfa, dfb, ext, dy16, dxin, total; };
+struct ScratchLayout { int64_t dxa, dxb, dxn, dxm, dqkv, dctx, dprob, prob, delta, gpad, dfa, dfb, ext, dy16, dxin, total; };
 // want_dx: room for d loss / d x over packed rows (backward_ex), after everything the plain backward uses
 static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, ScratchLayout& Z,
                                 bool want_dx = false) {
@@ -661,13 +695,15 @@ static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L
   Z.dxa = take(R * d); Z.dxb = take(R * d); Z.dxn = take(R * d);
   Z.dxm = (c.dropout > 0.0f || c.fc_dropout > 0.0f || c.pe_mode != 0) ? take(R * d) : 0;
   if (c.n_layers > 0) {
-    Z.dqkv = take(R * 3 * d); Z.dctx = take(R * d);
+    const int64_t dp = int64_t(c.n_heads) * L.hs;
+    Z.dqkv = take(R * 3 * dp); Z.dctx = take(R * dp);
     const bool fb = use_fused_bwd(c, S);
     Z.dprob = fb ? 0 : take(int64_t(B) * c.n_heads * S * Sp);
     Z.prob = (use_fused(c, S) && !fb) ? take(int64_t(B) * c.n_heads * S * Sp) : 0;
     Z.delta = fb ? take(int64_t(B) * c.n_heads * S) : 0;
+    Z.gpad = L.padded() ? take(head_pad(c, L).gsize()) : 0;   // one layer's padded weight and bias gradients
   } else {
-    Z.dqkv = Z.dctx = Z.dprob = Z.prob = Z.delta = 0;
+    Z.dqkv = Z.dctx = Z.dprob = Z.prob = Z.delta = Z.gpad = 0;
   }
   // FC-block backward: two gradient buffers of the widest tensor it differentiates through
   int64_t widest = c.fc_input_norm ? c.n_features : 0;
@@ -699,8 +735,10 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   if (scratch_floats < Z.total) { arb_set_error("arb_scorer_backward: scratch too small"); return ARB_E_WORKSPACE; }
   Ctx k{c, B, S, int64_t(B) * S, st};
   const int d = c.d_model, F = c.n_features, f = c.d_ff, h = c.n_heads;
-  const int dk = c.n_layers > 0 ? d / h : 0;
-  const float alpha = c.n_layers > 0 ? 1.0f / sqrtf(float(dk)) : 1.0f;
+  const int dk = L.hs, dp = h * dk;   // the buffers' head width (padded heads: round_up(d / h, 4)) and attention width
+  const float alpha = c.n_layers > 0 ? 1.0f / sqrtf(float(L.hw)) : 1.0f;
+  const HeadPad hp = head_pad(c, L);
+  float* gpad = L.padded() && G ? scratch + Z.gpad : nullptr;   // padded heads: this layer's padded gradients
   auto g = [&](int64_t off) { return G ? G + off : nullptr; };   // a parameter's gradient, or null
   float* dx = scratch + Z.dxa;      // gradient w.r.t. the residual stream at the current depth
   float* dx_alt = scratch + Z.dxb;
@@ -715,7 +753,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   // workspace), the saved bf16 activations, and bf16 copies of the gradients (dy16: the residual-stream gradient as
   // the sublayer below receives it; dxn / dqkv: gradients that only feed products are bfloat16 outright)
   const bool bf = c.bf16 && c.n_layers > 0;
-  if (bf && !bf16_head_width(dk)) {
+  if (bf && !bf16_head_width(L.hw)) {
     arb_set_error("scorer: bf16 mode needs head width 8, 16, 24 or 32 (a bfloat16 head of w columns is 2 w bytes, "
                   "which TMA needs to be a multiple of 16)");
     return ARB_E_UNSUPPORTED;
@@ -752,7 +790,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   const int* poff = pack ? reinterpret_cast<const int*>(ws + W.poff) : nullptr;
   if (pack) { k.rows_dev = plan; k.R = buffer_rows(c, B, S); x = ws + W.xc; gext = reinterpret_cast<int*>(ws + W.kext); }
   else if (skip) ARB_TRY(slate_extents(mask, dhidden ? dhidden : dscores, dhidden ? d : n_outputs(c), B, S, gext, st));
-  const AttnGeom geom{B, S, h, dk, k.R, poff};
+  const AttnGeom geom{B, S, h, dk, k.R, poff, L.hw};
   if (pack) {
     // 256 finite rows of d ctx behind the packed rows (the attention backward's boxes overrun the last slates), and
     // zero dQ | dK | dV in the alignment rows no slate writes (the QKV weight gradient sums over them): both buffers
@@ -828,13 +866,23 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     // dx_alt = d loss / d xmid ; dy = the same through the dropout on the attention sublayer output
     dy = site_ao.thresh ? dxm : dx_alt;
     // ---- attention sublayer backward:  xmid = xin + Wo ctx + bo
+    // padded heads: the products read the padded weights (W^T from the forward's copy) and write the weight and
+    // bias gradients padded into gpad, whose real rows and columns are added to G at the end of the layer
+    const float* wpad = L.padded() ? ws + W.wpad + l * hp.size() : nullptr;
+    const V wt_qkv = wpad ? t32(wpad + hp.wqkvt()) : wt(pl.wqkv), wt_o = wpad ? t32(wpad + hp.wot()) : wt(pl.wo);
+    float* const gw_qkv = gpad ? gpad + hp.gwqkv() : g(pl.wqkv);
+    float* const gb_qkv = gpad ? gpad + hp.gbqkv() : g(pl.bqkv);
+    float* const gw_o = gpad ? gpad + hp.gwo() : g(pl.wo);
+    if (gpad && cudaMemsetAsync(gpad, 0, size_t(hp.gsize()) * sizeof(float), st) != cudaSuccess) {
+      arb_set_error("scorer: memset failed"); return ARB_E_CUDA;
+    }
     const V dyo = bf ? b16(dy16) : V(dy);
-    if (G) ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), d, d, G + pl.wo));   // (bo gradient: fused into the LayerNorm backward above)
-    ARB_TRY(linear_bwd_input(k, dyo, d, d, wt(pl.wo), d, dctx, d, 0, nullptr, 0));
+    if (G) ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), dp, dp, gw_o));   // (bo gradient: fused into the LayerNorm backward above)
+    ARB_TRY(linear_bwd_input(k, dyo, d, d, wt_o, dp, dctx, dp, 0, nullptr, 0));
     if (use_fused_bwd(c, S)) {
       // dQ | dK | dV into one [R, 3d] buffer (bfloat16 in bf16 mode); the QKV bias gradient is fused
       ARB_TRY(launch_attn_bwd(attn_bwd_args(geom, qkv, act(ctx), dctx, dqkv, mask, (skip || pack) ? gext : nullptr,
-                                            ws + wl.smax, ws + wl.ssum, scratch + Z.delta, g(pl.bqkv),
+                                            ws + wl.smax, ws + wl.ssum, scratch + Z.delta, gb_qkv,
                                             make_drop_site(seed, l, SITE_ATTN_P, p_drop), plan, rowmap), st));
     } else {
       const DropSite site_p = make_drop_site(seed, l, SITE_ATTN_P, p_drop);
@@ -843,8 +891,8 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         // the dropped ones): recompute P = softmax(mask(alpha Q K^T))
         GemmDesc g;
         g.M = S; g.N = S; g.K = dk; g.alpha = alpha;
-        g.A = head_view(qkv, dk, S, h, B, 3 * d);
-        g.B = head_view(qkv + d, dk, S, h, B, 3 * d);
+        g.A = head_view(qkv, dk, S, h, B, 3 * dp);
+        g.B = head_view(qkv + dp, dk, S, h, B, 3 * dp);
         g.C = prob_view(prob, S, W.Sp, h, B);
         batch_all(g, h, B); g.block_n = 64;
         ARB_TRY(launch_gemm_tf32(g, st));
@@ -853,8 +901,8 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
       {
         GemmDesc g;   // dP~ = dctx V^T   (gradient w.r.t. the dropped probabilities)
         g.M = S; g.N = S; g.K = dk;
-        g.A = head_view(dctx, dk, S, h, B, d);
-        g.B = head_view(qkv + 2 * d, dk, S, h, B, 3 * d);
+        g.A = head_view(dctx, dk, S, h, B, dp);
+        g.B = head_view(qkv + 2 * dp, dk, S, h, B, 3 * dp);
         g.C = prob_view(dprob, S, W.Sp, h, B);
         batch_all(g, h, B); g.block_n = 64;
         ARB_TRY(launch_gemm_tf32(g, st));
@@ -865,8 +913,8 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         GemmDesc g;   // dV = P~^T dctx     (P~ read as an MN-major A operand, dctx as an MN-major B operand)
         g.M = S; g.N = dk; g.K = S; g.a_mn = 1; g.b_mn = 1;
         g.A = prob_view(prob, S, W.Sp, h, B);
-        g.B = head_view(dctx, dk, S, h, B, d);
-        g.C = head_view(dqkv + 2 * d, dk, S, h, B, 3 * d);
+        g.B = head_view(dctx, dk, S, h, B, dp);
+        g.C = head_view(dqkv + 2 * dp, dk, S, h, B, 3 * dp);
         batch_all(g, h, B); g.block_n = pick_block_n(dk);
         ARB_TRY(launch_gemm_tf32(g, st));
       }
@@ -874,8 +922,8 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         GemmDesc g;   // dQ = alpha dS K
         g.M = S; g.N = dk; g.K = S; g.b_mn = 1; g.alpha = alpha;
         g.A = prob_view(dprob, S, W.Sp, h, B);
-        g.B = head_view(qkv + d, dk, S, h, B, 3 * d);
-        g.C = head_view(dqkv, dk, S, h, B, 3 * d);
+        g.B = head_view(qkv + dp, dk, S, h, B, 3 * dp);
+        g.C = head_view(dqkv, dk, S, h, B, 3 * dp);
         batch_all(g, h, B); g.block_n = pick_block_n(dk);
         ARB_TRY(launch_gemm_tf32(g, st));
       }
@@ -883,15 +931,16 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         GemmDesc g;   // dK = alpha dS^T Q
         g.M = S; g.N = dk; g.K = S; g.a_mn = 1; g.b_mn = 1; g.alpha = alpha;
         g.A = prob_view(dprob, S, W.Sp, h, B);
-        g.B = head_view(qkv, dk, S, h, B, 3 * d);
-        g.C = head_view(dqkv + d, dk, S, h, B, 3 * d);
+        g.B = head_view(qkv, dk, S, h, B, 3 * dp);
+        g.C = head_view(dqkv + dp, dk, S, h, B, 3 * dp);
         batch_all(g, h, B); g.block_n = pick_block_n(dk);
         ARB_TRY(launch_gemm_tf32(g, st));
       }
     }
-    if (G) ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * d, 3 * d, act(xn1), d, d, G + pl.wqkv));
-    if (G && !use_fused_bwd(c, S)) ARB_TRY(colsum_accumulate(dqkv, k.R, 3 * d, 3 * d, G + pl.bqkv, st));
-    ARB_TRY(linear_bwd_input(k, act(dqkv), 3 * d, 3 * d, wt(pl.wqkv), d, act(dxn), d, 0, nullptr, 0));
+    if (G) ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * dp, 3 * dp, act(xn1), d, d, gw_qkv));
+    if (G && !use_fused_bwd(c, S)) ARB_TRY(colsum_accumulate(dqkv, k.R, 3 * dp, 3 * dp, gb_qkv, st));
+    ARB_TRY(linear_bwd_input(k, act(dqkv), 3 * dp, 3 * dp, wt_qkv, d, act(dxn), d, 0, nullptr, 0));
+    if (gpad) ARB_TRY(head_pad_grads(gpad, hp, l, G, st));
     DropSite site_below = l > 0 ? make_drop_site(seed, l - 1, SITE_FFN_OUT, p_drop) : (fc_act ? none_site : fc_site);
     // with a positional encoding the encoder input is sqrt(d) * fc_out + pe: the gradient that reaches the FC
     // (through its dropout mask, if any) carries the extra sqrt(d)
@@ -985,7 +1034,7 @@ extern "C" int32_t arb_attention_forward(const float* qkv, const uint8_t* mask, 
   ARB_TRY(attention_hook_check("arb_attention_forward", B, S, h, p, false, dk));
   if (ctx_bf16 && !bf16_head_width(dk)) { arb_set_error("arb_attention_forward: a bf16 context needs head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
   if (ctx_bf16 && S > 256) { arb_set_error("arb_attention_forward: a bf16 context needs S <= 256"); return ARB_E_UNSUPPORTED; }
-  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
+  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr, dk};
   const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
   return launch_attn_fwd(attn_fwd_args(z, qkv, o, mask, extent, stat_max, stat_sum,
                                        make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p)),
@@ -1003,9 +1052,47 @@ extern "C" int32_t arb_attention_backward(const float* qkv, const void* ctx, int
   }
   ARB_TRY(attention_hook_check("arb_attention_backward", B, S, h, p, true, dk));
   if (ctx_bf16 && !bf16_head_width(dk)) { arb_set_error("arb_attention_backward: a bf16 context needs head width 8, 16, 24 or 32"); return ARB_E_UNSUPPORTED; }
-  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr};
+  const AttnGeom z{B, S, h, dk, int64_t(B) * S, nullptr, dk};
   const V o = ctx_bf16 ? b16(ctx) : V(static_cast<const float*>(ctx));
   return launch_attn_bwd(attn_bwd_args(z, qkv, o, d_ctx, d_qkv, mask, extent, stat_max, stat_sum, delta_scratch,
+                                       dbias_qkv, make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p),
+                                       nullptr, nullptr),
+                         static_cast<cudaStream_t>(stream));
+}
+
+// The same kernels over padded heads (include/allrank_b200.h): heads of w columns, each taking round_up(w, 4) columns
+// of the buffers, with the scale 1/sqrt(w) -- the scorer's launches at such widths.  fp32 context only.
+static int padded_geom(const char* what, int B, int S, int h, int w, float p, bool bwd, AttnGeom& z) {
+  if (w < 1 || w > 256) { arb_set_error((std::string(what) + ": head width must be in [1, 256]").c_str()); return ARB_E_UNSUPPORTED; }
+  const int hs = int(align_up(w, 4));
+  ARB_TRY(attention_hook_check(what, B, S, h, p, bwd, hs));
+  z = AttnGeom{B, S, h, hs, int64_t(B) * S, nullptr, w};
+  return ARB_OK;
+}
+
+extern "C" int32_t arb_attention_padded_forward(const float* qkv, const uint8_t* mask, const int32_t* extent, int32_t B,
+                                                int32_t S, int32_t h, int32_t w, float p, uint64_t seed, int32_t layer,
+                                                float* ctx, float* stat_max, float* stat_sum, void* stream) {
+  if (!qkv || !mask || !ctx || !stat_max || !stat_sum) { arb_set_error("arb_attention_padded_forward: null pointer"); return ARB_E_INVALID_ARG; }
+  AttnGeom z;
+  ARB_TRY(padded_geom("arb_attention_padded_forward", B, S, h, w, p, false, z));
+  return launch_attn_fwd(attn_fwd_args(z, qkv, V(ctx), mask, extent, stat_max, stat_sum,
+                                       make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p)),
+                         static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int32_t arb_attention_padded_backward(const float* qkv, const float* ctx, const float* d_ctx,
+                                                 const uint8_t* mask, const int32_t* extent, const float* stat_max,
+                                                 const float* stat_sum, int32_t B, int32_t S, int32_t h, int32_t w,
+                                                 float p, uint64_t seed, int32_t layer, float* d_qkv, float* dbias_qkv,
+                                                 float* delta_scratch, void* stream) {
+  if (!qkv || !ctx || !d_ctx || !mask || !stat_max || !stat_sum || !d_qkv || !delta_scratch) {
+    arb_set_error("arb_attention_padded_backward: null pointer");
+    return ARB_E_INVALID_ARG;
+  }
+  AttnGeom z;
+  ARB_TRY(padded_geom("arb_attention_padded_backward", B, S, h, w, p, true, z));
+  return launch_attn_bwd(attn_bwd_args(z, qkv, V(ctx), d_ctx, d_qkv, mask, extent, stat_max, stat_sum, delta_scratch,
                                        dbias_qkv, make_drop_site(CallSeed{seed, nullptr}, layer, SITE_ATTN_P, p),
                                        nullptr, nullptr),
                          static_cast<cudaStream_t>(stream));

@@ -439,6 +439,58 @@ __global__ void __launch_bounds__(256) tf32_weight_copy_kernel(const float* __re
   }
 }
 
+// Padded heads: the padded copies of W_qkv, its transpose, b_qkv, W_o and its transpose (HeadPad), every element
+// written, the pads as +0.  Padded row (column) g * hs + t holds the real row (column) g * w + t when t < w.
+__global__ void __launch_bounds__(256) head_pad_copy_kernel(const float* __restrict__ pr, const float* __restrict__ P,
+                                                            HeadPad m, float* __restrict__ out) {
+  arb_pdl_wait();
+  const long long d = m.d, dp = m.dp(), size = m.size(), n = size * m.n_layers;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long l = i / size, j = i - l * size, base = m.enc0 + l * m.enc_stride;
+    long long src;      // offset of the real element in the flat parameters, or -1 for a pad
+    const float* from = pr;
+    auto real = [&](long long padded) { const long long g = padded / m.hs, t = padded - g * m.hs; return t < m.w ? g * m.w + t : -1; };
+    if (j < m.wqkvt()) {                     // wqkv [3 dp, d]
+      const long long r = real(j / d);
+      src = r < 0 ? -1 : base + r * d + j % d;
+    } else if (j < m.bqkv()) {               // wqkvt [d, 3 dp]
+      const long long e = j - m.wqkvt(), r = real(e % (3 * dp));
+      src = r < 0 ? -1 : base + r * d + e / (3 * dp);
+    } else if (j < m.wo()) {                 // bqkv [3 dp]: the fp32 bias, as the unpadded QKV linear reads it
+      const long long r = real(j - m.bqkv());
+      src = r < 0 ? -1 : base + m.o_bqkv + r;
+      from = P;
+    } else if (j < m.wot()) {                // wo [d, dp]
+      const long long e = j - m.wo(), c = real(e % dp);
+      src = c < 0 ? -1 : base + m.o_wo + e / dp * d + c;
+    } else {                                 // wot [dp, d]
+      const long long e = j - m.wot(), c = real(e / d);
+      src = c < 0 ? -1 : base + m.o_wo + e % d * d + c;
+    }
+    out[i] = src < 0 ? 0.0f : from[src];
+  }
+}
+
+// Padded heads: G += the real rows / columns of one layer's padded weight and bias gradients (HeadPad::g*), one
+// thread per real element.
+__global__ void __launch_bounds__(256) head_pad_grads_kernel(const float* __restrict__ gp, HeadPad m, long long base,
+                                                             float* __restrict__ G) {
+  arb_pdl_wait();
+  const long long d = m.d, dp = m.dp(), n_w = 3 * d * d, n_b = 3 * d, n = n_w + n_b + d * d;
+  auto padded = [&](long long real) { const long long g = real / m.w; return g * m.hs + (real - g * m.w); };
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (i < n_w) {                           // W_qkv [3d, d]
+      G[base + i] += gp[m.gwqkv() + padded(i / d) * d + i % d];
+    } else if (i < n_w + n_b) {              // b_qkv [3d]
+      const long long e = i - n_w;
+      G[base + m.o_bqkv + e] += gp[m.gbqkv() + padded(e)];
+    } else {                                 // W_o [d, d]
+      const long long e = i - n_w - n_b;
+      G[base + m.o_wo + e] += gp[m.gwo() + e / d * dp + padded(e % d)];
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ slate extents
 __global__ void __launch_bounds__(256) slate_extent_kernel(const uint8_t* __restrict__ mask,
                                                            const float* __restrict__ dscores, int n_out, int B, int S,
@@ -1208,6 +1260,20 @@ int tf32_weight_copy(const float* P, long long n, const WeightMats& m, int rnd, 
   ProfScope ps(ARB_PROF_SCORER_SIMT, 12.0 * double(n), st);
   return launch(tf32_weight_copy_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 8)))),
                 dim3(256), 0, st, /*pdl=*/true, P, n, m, rnd, pr, pt);
+}
+
+int head_pad_copy(const float* pr, const float* P, const HeadPad& m, float* out, cudaStream_t st) {
+  const long long n = m.size() * m.n_layers;
+  ProfScope ps(ARB_PROF_SCORER_SIMT, 8.0 * double(n), st);
+  return launch(head_pad_copy_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 8)))),
+                dim3(256), 0, st, /*pdl=*/true, pr, P, m, out);
+}
+
+int head_pad_grads(const float* gp, const HeadPad& m, int l, float* G, cudaStream_t st) {
+  const long long n = 4LL * m.d * m.d + 3LL * m.d;
+  ProfScope ps(ARB_PROF_SCORER_SIMT, 12.0 * double(n), st);
+  return launch(head_pad_grads_kernel, dim3(unsigned(std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 8)))),
+                dim3(256), 0, st, /*pdl=*/true, gp, m, m.enc0 + l * m.enc_stride, G);
 }
 
 int colsum_accumulate(const float* in, long long rows, int width, long long ld, float* out, cudaStream_t st) {

@@ -60,6 +60,33 @@ struct WeightMats {
 // W [out, in] at offset o, pt[o + c * out + r] = W[r][c] (W^T, the K-major B operand of the input gradient); values
 // rounded to tf32 (nearest even) when rnd != 0, else copied as they are (the tensor core then truncates them).
 int tf32_weight_copy(const float* P, long long n, const WeightMats& m, int rnd, float* pr, float* pt, cudaStream_t st);
+// Padded heads (DESIGN.md 4.15): when the head width w = d / h is not a multiple of 4, every head of Q | K | V, the
+// context and their gradients takes hs = round_up(w, 4) columns, the last hs - w of them exact zeros, so that the
+// per-head tensor maps get a head stride of a multiple of 16 bytes.  The attention linears then read padded copies of
+// their weights, one block of size() floats per layer (dp = h * hs):
+//   wqkv [3 dp, d] (zero rows in the pads), wqkvt = wqkv^T [d, 3 dp], bqkv [3 dp], wo [d, dp] (zero columns in the
+//   pads), wot = wo^T [dp, d]
+// and write their weight and bias gradients to a padded block of gsize() floats: gwqkv [3 dp, d], gbqkv [3 dp],
+// gwo [d, dp].  Every offset is a multiple of 4 floats (16 bytes, as TMA needs).
+struct HeadPad {
+  int n_layers, d, h, w, hs;
+  long long enc0, enc_stride, o_bqkv, o_wo;   // flat parameters: layer l at enc0 + l * enc_stride; b_qkv, W_o inside it
+  __host__ __device__ long long dp() const { return (long long)h * hs; }
+  __host__ __device__ long long wqkv() const { return 0; }
+  __host__ __device__ long long wqkvt() const { return 3 * dp() * d; }
+  __host__ __device__ long long bqkv() const { return 6 * dp() * d; }
+  __host__ __device__ long long wo() const { return 6 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long wot() const { return 7 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long size() const { return 8 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long gwqkv() const { return 0; }
+  __host__ __device__ long long gbqkv() const { return 3 * dp() * d; }
+  __host__ __device__ long long gwo() const { return 3 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long gsize() const { return 4 * dp() * d + 3 * dp(); }
+};
+// out[l * m.size() + ...] = the padded copies of every layer: weights from pr (the TF32 copy), the bias from P
+int head_pad_copy(const float* pr, const float* P, const HeadPad& m, float* out, cudaStream_t st);
+// G += the real rows and columns of layer l's padded gradient block gp (each element one addition: no atomics)
+int head_pad_grads(const float* gp, const HeadPad& m, int l, float* G, cudaStream_t st);
 int colsum_accumulate(const float* in, long long rows, int width, long long ld, float* out, cudaStream_t st);
 int head_forward(const float* x, const float* a, const float* b, float eps, const float* w, const float* wb,
                  int has_norm, int act, long long rows, int width, float* score, float* mean, float* sd,

@@ -37,11 +37,14 @@ then also runs the first FC layer's input-gradient product; with every parameter
 gradient at all.  In the default packed-row layout (include/allrank_b200.h: arb_set_pack_rows) items at or beyond their
 slate's packed rows get 0 in `prepare_for_output` and in x.grad, and a gradient sent to their hidden rows is ignored --
 the same contract as their score.  Double backward is not supported (it raises).
-Attention runs on the fused kernels at every head width d_model / h that is a multiple of 4 from 4 to 256, for slates
-of up to 4096 items.
-Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes, and
-attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU);
-compute_dtype="bf16" at head widths other than 8, 16, 24 and 32.
+Attention runs on the fused kernels at every head width d_model / h from 1 to 256, for slates of up to 4096 items.  A
+width that is not a multiple of 4 (d_model 144 with h = 8: 18 columns) runs on heads padded with zero columns to the
+next multiple of 4 inside the CUDA scorer (DESIGN.md 4.15); the parameters and the state_dict keep the reference's
+shapes.
+Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes,
+attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU) and
+padded heads beyond 1024 columns in all (h * round_up(d_model / h, 4)); compute_dtype="bf16" at head widths other than
+8, 16, 24 and 32.
 """
 import contextlib
 import copy

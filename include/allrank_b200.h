@@ -395,6 +395,21 @@ int32_t arb_attention_backward(const float* qkv, const void* ctx, int32_t ctx_bf
                                const float* stat_sum, int32_t B, int32_t S, int32_t h, int32_t dk, float p,
                                uint64_t seed, int32_t layer, void* d_qkv, float* dbias_qkv, float* delta_scratch,
                                void* stream);
+/* The same kernels over padded heads, as the scorer runs a head width w = d_model / h that is not a multiple of 4:
+ * every head takes hs = round_up(w, 4) columns of the buffers (any w from 1 to 256; hs = w when w is a multiple of 4),
+ * and the probabilities are softmax(Q K^T / sqrt(w)).  dp = h * hs; fp32 context only.
+ *   qkv    [B*S, 3 dp]: Q | K | V, head j at columns j*hs ... j*hs + hs - 1 of each; columns w ... hs - 1 of every
+ *          head must be zero (the scorer's padded QKV weights and bias give exact zeros there)
+ *   ctx, d_ctx [B*S, dp]; d_qkv [B*S, 3 dp]; dbias_qkv nullable [3 dp]
+ * The pad columns of ctx and d_qkv come out as +0 (a zero column adds exact zeros to every product) and the pad
+ * entries of dbias_qkv receive +0.  Everything else as arb_attention_forward / arb_attention_backward. */
+int32_t arb_attention_padded_forward(const float* qkv, const uint8_t* mask, const int32_t* extent, int32_t B, int32_t S,
+                                     int32_t h, int32_t w, float p, uint64_t seed, int32_t layer, float* ctx,
+                                     float* stat_max, float* stat_sum, void* stream);
+int32_t arb_attention_padded_backward(const float* qkv, const float* ctx, const float* d_ctx, const uint8_t* mask,
+                                      const int32_t* extent, const float* stat_max, const float* stat_sum, int32_t B,
+                                      int32_t S, int32_t h, int32_t w, float p, uint64_t seed, int32_t layer,
+                                      float* d_qkv, float* dbias_qkv, float* delta_scratch, void* stream);
 
 /* Building blocks exposed for tests: the encoder's feed-forward sublayer as the scorer runs it in TF32 mode without
  * dropout, both linears chained in one kernel per direction (csrc/ffn_chain.cu).  All matrices are dense row-major

@@ -2,7 +2,10 @@
 width 64), contextaware ordinal (d 144, h 2: width 72, four outputs), neuralNDCG-paper approxNDCG (d 96, h 1: width
 96) -- of a d = 256, h = 4 model (width 64), of two width-128 models (d 128, h 1 and d 256, h 2), of the
 neuralNDCG-paper model widened to one head of 136, 192 or 256 columns, and of the neuralNDCG-paper model at d 64, 96
-and 192 with eight heads (widths 8, 12 and 24), each with its own dropout and loss: the fused attention kernels
+and 192 with eight heads (widths 8, 12 and 24), and models whose head width is not a multiple of 4 (padded heads,
+DESIGN.md 4.15: d 144 / h 8, width 18; d 96 / h 32, width 3; d 200 / h 8, width 25) beside the nearest multiple-of-4
+width at the same d_model (d 144 / h 9, width 16; d 96 / h 24, width 4; d 200 / h 10, width 20), each with its own
+dropout and loss: the fused attention kernels
 (attention mode 2) against the unfused sequence
 (arb_set_attention_mode(0): [B, h, S, S] probabilities in HBM) where the latter exists (S <= 1536).
 
@@ -10,7 +13,8 @@ and 192 with eight heads (widths 8, 12 and 24), each with its own dropout and lo
 
 Shapes: every model at B = 64 and B = 1024 slates of S = 240 items, and the models of width 96 and above and the
 eight-head models at S = 1024, 2048, 4096 (B = 245760 / S slates, fewer where the unfused path would not fit in
-memory).  Slate lengths ~ N(S/2, S/4) clamped to [1, S].  Step time is the host clock around `steps` training steps
+memory), and the padded-head models and their comparisons at S = 1024 (B = 240).  --fused-only skips the unfused
+arm.  Slate lengths ~ N(S/2, S/4) clamped to [1, S].  Step time is the host clock around `steps` training steps
 that end in a device synchronise, per run; the modes alternate run by run.  Peak memory is torch.cuda.max_memory_allocated over a run.  The attention kernels' times
 come from torch.profiler in a separate run per shape.  The GPU's name and power limit are printed with the numbers."""
 import argparse
@@ -55,10 +59,18 @@ for _d in (64, 96, 192):
     MODELS[f"d{_d}_h8"] = (dict(fc_model={"sizes": [_d], "input_norm": False, "activation": None, "dropout": 0.0},
                                 transformer={"N": 2, "d_ff": 384, "h": 8, "positional_encoding": None, "dropout": 0.1},
                                 post_model={"output_activation": None, "d_output": 1}), ("approxNDCGLoss", {"alpha": 1.0}))
+# ... and padded heads (widths 18, 3, 25) next to the nearest multiple-of-4 width at the same d_model (16, 4, 20)
+for _d, _h in ((144, 8), (144, 9), (96, 32), (96, 24), (200, 8), (200, 10)):
+    MODELS[f"d{_d}_h{_h}"] = (dict(fc_model={"sizes": [_d], "input_norm": False, "activation": None, "dropout": 0.0},
+                                   transformer={"N": 2, "d_ff": 384, "h": _h, "positional_encoding": None,
+                                                "dropout": 0.1},
+                                   post_model={"output_activation": None, "d_output": 1}),
+                              ("approxNDCGLoss", {"alpha": 1.0}))
+ODD = ("d144_h8", "d144_h9", "d96_h32", "d96_h24", "d200_h8", "d200_h10")
 SHAPES = [(name, B, 240) for name in MODELS for B in (64, 1024)] + [
     (name, 245760 // S, S) for name in ("approxndcg", "d128_h1", "d256_h2", "d136_h1", "d192_h1", "d256_h1",
                                         "d64_h8", "d96_h8", "d192_h8")
-    for S in (1024, 2048, 4096)]
+    for S in (1024, 2048, 4096)] + [(name, 240, 1024) for name in ODD]
 
 
 def make_batch(B, S, seed=7):
@@ -99,6 +111,7 @@ def main():
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--models", default=None, help="comma-separated subset of the models (default: all)")
     ap.add_argument("--json", default=None)
+    ap.add_argument("--fused-only", action="store_true", help="skip the unfused arm")
     args = ap.parse_args()
     only = set(args.models.split(",")) if args.models else set(MODELS)
     assert only <= set(MODELS), f"unknown model in {sorted(only - set(MODELS))}"
@@ -110,7 +123,7 @@ def main():
         if name not in only:
             continue
         step = make_step(name)
-        modes = (2, 0) if fits_unfused(name, B, S) else (2,)
+        modes = (2, 0) if fits_unfused(name, B, S) and not args.fused_only else (2,)
         x, y = make_batch(B, S)
         res = {m: [] for m in modes}
         for _ in range(args.runs):
