@@ -57,7 +57,8 @@ struct GemmParams {
   int rnd;            // round fp32 operands to tf32 (nearest) before the MMA; else the tensor core truncates them
   int rnd_b;          // wgmma path: round the B stages in place (rnd, unless B arrives rounded already)
   float alpha;
-  int atomic_ld;
+  int atomic_ld;         // EPI_ATOMIC: the row pitch of atomic_out; EPI_DROPOUT (never with EPI_ATOMIC): the row
+                         // width of the dropout counter (GemmDesc::drop_n) -- one field keeps GemmParams in 128 bytes
   const float* bias;
   float* atomic_out;     // split-K: the splits' slots [split][M][atomic_ld] (DetParts), summed in order afterwards
   DropSite drop;
@@ -557,7 +558,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
             if (p.flags & EPI_BIAS) x += bias_s[32 * c + j];
             if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
             if constexpr (DROP) {
-              const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
+              const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.atomic_ld + (n0 + 32 * c + j);
               x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
             }
             o[e] = x;
@@ -597,7 +598,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tf32_kernel(const __grid_co
           if (p.flags & EPI_BIAS) x += bias_s[32 * c + j];
           if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
           if constexpr (DROP) {
-            const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
+            const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.atomic_ld + (n0 + 32 * c + j);
             x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
           }
           o[e] = x;
@@ -863,7 +864,7 @@ __global__ void __launch_bounds__(PERSIST_THREADS, 1) gemm_tf32_persistent(const
               if (p.flags & EPI_BIAS) x += bias_s[32 * c + j];
               if (p.flags & EPI_RELU) x = fmaxf(x, 0.0f);
               if (p.flags & EPI_DROPOUT) {
-                const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.N + (n0 + 32 * c + j);
+                const unsigned long long idx = (unsigned long long)(m0 + row) * (unsigned long long)p.atomic_ld + (n0 + 32 * c + j);
                 x = drop_keep(idx, drop_s, p.drop.thresh) ? x * p.drop.scale : 0.0f;
               }
               o[e] = x;
@@ -1145,6 +1146,12 @@ int launch_gemm_tf32(const GemmDesc& d, cudaStream_t st) {
   if ((d.flags & EPI_DROPOUT) && d.drop.thresh == 0) p.flags &= ~EPI_DROPOUT;
   // (checked here, before the kernel is picked: the persistent kernel would otherwise take what the one-tile one refuses)
   if ((p.flags & EPI_DROPOUT) && (d.a_mn || d.b_mn)) { arb_set_error("gemm: the dropout epilogue needs K-major operands"); return ARB_E_UNSUPPORTED; }
+  if (p.flags & EPI_DROPOUT) {
+    if ((p.flags & EPI_ATOMIC) || d.drop_n < 0 || d.drop_n > d.N) {
+      arb_set_error("gemm: the dropout epilogue needs a plain output and 0 <= drop_n <= N"); return ARB_E_INVALID_ARG;
+    }
+    p.atomic_ld = d.drop_n ? d.drop_n : d.N;
+  }
   p.kb_per_split = (total_kb + splits - 1) / splits;
   const int eff_splits = split ? (total_kb + p.kb_per_split - 1) / std::max(1, p.kb_per_split) : 1;
   dim3 grid((d.N + d.block_n - 1) / d.block_n, (d.M + BLOCK_M - 1) / BLOCK_M, split ? std::max(1, eff_splits) : d.nb2 * d.nb3);

@@ -45,7 +45,9 @@ struct GemmDesc {
   const float* bias = nullptr;  // [N]
   float* atomic_out = nullptr;  // row-major [M, atomic_ld]
   int64_t atomic_ld = 0;
-  DropSite drop{0u, 0u, 1.0f};  // EPI_DROPOUT: element index = m * N + n (unbatched problems only)
+  DropSite drop{0u, 0u, 1.0f};  // EPI_DROPOUT: element index = m * drop_n + n (unbatched problems only)
+  int drop_n = 0;               // EPI_DROPOUT: row width of the counter layout (0: N); a layer of n real columns stored
+                                // at N = round_up(n, 4) counts over its real columns (DESIGN.md 4.16)
   float* colsum_out = nullptr;  // EPI_COLSUM: [N], += column sums (per-tile slots summed in order)
   uint32_t* bits = nullptr;     // EPI_RELU_BITS (written) / EPI_MASK_BITS (read): [M, N / 32] words, row-major
   const int* rows_dev = nullptr;   // packed rows (unbatched launches): device pointer to the live row count, a

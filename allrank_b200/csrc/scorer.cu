@@ -26,6 +26,11 @@
 namespace arb {
 
 static inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
+// Layers of any width (DESIGN.md 4.16): a layer of n columns (FC, d_model, d_ff) is stored with pad4(n) columns --
+// activations, weights [pad4(out), pad4(in)], biases, LayerNorm gains -- whose last pad4(n) - n columns are exact
+// zeros, so every product and row kernel runs at a multiple of 4 columns (TMA strides are multiples of 16 bytes) and
+// the zeros add nothing to a real column
+static inline int pad4(int n) { return (n + 3) & ~3; }
 
 // 0: unfused attention (materialised [B,h,S,S] logits, generic GEMMs)   1: fused forward kernel, unfused backward
 // 2 (default): fused forward and fused backward kernels
@@ -86,7 +91,7 @@ static bool use_pack(const arb_scorer_config& c, int S) { return g_pack_rows && 
 struct ParamLayout {
   int n_fc;                                  // FC layers (>= 1)
   int fc_size[ARB_MAX_FC_LAYERS];            // output width of FC layer i; fc_size[n_fc-1] = d_model
-  int64_t fc_w[ARB_MAX_FC_LAYERS], fc_b[ARB_MAX_FC_LAYERS];
+  int64_t fc_w[ARB_MAX_FC_LAYERS], fc_b[ARB_MAX_FC_LAYERS];   // [pad4(out), pad4(in)] and [pad4(out)], zero-padded
   int64_t in_a, in_b;                        // nn.LayerNorm(F) of fc_model.input_norm (-1: none)
   struct Layer { int64_t wqkv, bqkv, wo, bo, w1, b1, w2, b2, ln1_a, ln1_b, ln2_a, ln2_b; };
   Layer layer[64];
@@ -97,13 +102,13 @@ struct ParamLayout {
 
 static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
   if (c.n_layers < 0 || c.n_layers > 64) { arb_set_error("scorer: n_layers must be in [0,64]"); return ARB_E_UNSUPPORTED; }
-  if (c.d_model <= 0 || c.d_model % 4 || c.n_features <= 0 || c.n_features % 4) {
-    arb_set_error("scorer: d_model and (padded) n_features must be positive multiples of 4");
+  if (c.d_model <= 0 || c.n_features <= 0 || c.n_features % 4) {
+    arb_set_error("scorer: d_model must be positive and (padded) n_features a positive multiple of 4");
     return ARB_E_UNSUPPORTED;
   }
   if (c.n_layers > 0) {
-    if (c.n_heads <= 0 || c.d_model % c.n_heads || c.d_ff <= 0 || c.d_ff % 4) {
-      arb_set_error("scorer: need d_model % h == 0 and d_ff % 4 == 0");
+    if (c.n_heads <= 0 || c.d_model % c.n_heads || c.d_ff <= 0) {
+      arb_set_error("scorer: need d_model % h == 0 and d_ff >= 1");
       return ARB_E_UNSUPPORTED;
     }
     if (c.d_model / c.n_heads > 256) { arb_set_error("scorer: head width above 256 is not supported"); return ARB_E_UNSUPPORTED; }
@@ -119,13 +124,13 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
     arb_set_error("scorer: bf16 mode needs d_model and d_ff to be multiples of 8, at least 64");
     return ARB_E_UNSUPPORTED;
   }
-  const int64_t d = c.d_model, F = c.n_features, f = c.d_ff;
+  const int64_t d = c.d_model, F = c.n_features, dw = pad4(c.d_model), fw = pad4(c.d_ff);
   L.n_fc = c.n_fc_layers > 0 ? c.n_fc_layers : 1;
   if (L.n_fc > ARB_MAX_FC_LAYERS) { arb_set_error("scorer: at most 8 FC layers"); return ARB_E_UNSUPPORTED; }
   for (int i = 0; i < L.n_fc; ++i) {
     L.fc_size[i] = c.n_fc_layers > 0 ? c.fc_sizes[i] : c.d_model;
-    if (L.fc_size[i] <= 0 || L.fc_size[i] % 4 || L.fc_size[i] > 8192) {
-      arb_set_error("scorer: FC layer widths must be positive multiples of 4, at most 8192");
+    if (L.fc_size[i] <= 0 || L.fc_size[i] > 8192) {
+      arb_set_error("scorer: FC layer widths must be in [1, 8192]");
       return ARB_E_UNSUPPORTED;
     }
   }
@@ -134,34 +139,38 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
   if (c.fc_input_norm && F > 1024) { arb_set_error("scorer: input_norm supports up to 1024 features"); return ARB_E_UNSUPPORTED; }
   int64_t o = 0;
   for (int i = 0; i < L.n_fc; ++i) {
-    const int64_t in = i == 0 ? F : L.fc_size[i - 1];
-    L.fc_w[i] = o; o += int64_t(L.fc_size[i]) * in;
-    L.fc_b[i] = o; o += L.fc_size[i];
+    const int64_t in = i == 0 ? F : pad4(L.fc_size[i - 1]);
+    L.fc_w[i] = o; o += int64_t(pad4(L.fc_size[i])) * in;
+    L.fc_b[i] = o; o += pad4(L.fc_size[i]);
   }
   L.in_a = L.in_b = -1;
   if (c.fc_input_norm) { L.in_a = o; o += F; L.in_b = o; o += F; }
   // the encoder's parameters start on a 32-byte boundary (8 elements): their bfloat16 shadow (bf16 mode) is read by TMA,
   // which needs 16-byte aligned bases; every size inside the encoder section is then a multiple of 8 elements
   if (c.n_layers > 0) o = align_up(o, 8);
+  // the attention linears keep the reference's layout (their heads are interior blocks; HeadPad builds padded copies);
+  // everything from b_o on is stored at the padded widths dw = pad4(d), fw = pad4(d_ff), starting on a 16-byte
+  // boundary (the alignment is empty when d is a multiple of 4)
   for (int l = 0; l < c.n_layers; ++l) {
     auto& y = L.layer[l];
     y.wqkv = o; o += 3 * d * d;
     y.bqkv = o; o += 3 * d;
     y.wo = o; o += d * d;
-    y.bo = o; o += d;
-    y.w1 = o; o += f * d;
-    y.b1 = o; o += f;
-    y.w2 = o; o += d * f;
-    y.b2 = o; o += d;
-    y.ln1_a = o; o += d;
-    y.ln1_b = o; o += d;
-    y.ln2_a = o; o += d;
-    y.ln2_b = o; o += d;
+    o = align_up(o, 4);
+    y.bo = o; o += dw;
+    y.w1 = o; o += fw * dw;
+    y.b1 = o; o += fw;
+    y.w2 = o; o += dw * fw;
+    y.b2 = o; o += dw;
+    y.ln1_a = o; o += dw;
+    y.ln1_b = o; o += dw;
+    y.ln2_a = o; o += dw;
+    y.ln2_b = o; o += dw;
   }
-  if (c.n_layers > 0) { L.lnf_a = o; o += d; L.lnf_b = o; o += d; } else { L.lnf_a = L.lnf_b = -1; }
+  if (c.n_layers > 0) { L.lnf_a = o; o += dw; L.lnf_b = o; o += dw; } else { L.lnf_a = L.lnf_b = -1; }
   if (c.d_output < 0 || c.d_output > 64) { arb_set_error("scorer: d_output must be in [1,64]"); return ARB_E_UNSUPPORTED; }
   const int64_t n_out = n_outputs(c);
-  L.head_w = o; o += n_out * d;      // nn.Linear(d, d_output).weight, row-major [d_output, d]
+  L.head_w = o; o += n_out * pad4(c.d_model);   // nn.Linear(d, d_output).weight, row-major [d_output, pad4(d)]
   L.head_b = o; o += n_out;
   L.pe = -1;
   if (c.pe_mode != 0) {
@@ -169,7 +178,7 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
       arb_set_error("scorer: positional encoding needs a transformer and a table of >= 2 rows");
       return ARB_E_UNSUPPORTED;
     }
-    if (c.pe_mode == 2) { o = align_up(o, 4); L.pe = o; o += int64_t(c.pe_rows) * d; }
+    if (c.pe_mode == 2) { o = align_up(o, 4); L.pe = o; o += int64_t(c.pe_rows) * dw; }
   }
   L.total = o;
   L.hw = c.n_layers > 0 ? c.d_model / c.n_heads : 0;
@@ -179,11 +188,11 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
 
 static HeadPad head_pad(const arb_scorer_config& c, const ParamLayout& L) {
   HeadPad m{};
-  m.n_layers = c.n_layers; m.d = c.d_model; m.h = c.n_heads; m.w = L.hw; m.hs = L.hs;
+  m.n_layers = c.n_layers; m.d = c.d_model; m.h = c.n_heads; m.w = L.hw; m.hs = L.hs; m.dw = pad4(c.d_model);
   if (c.n_layers > 0) {
     const auto& y = L.layer[0];
     m.enc0 = y.wqkv;
-    m.enc_stride = y.ln2_b + c.d_model - y.wqkv;
+    m.enc_stride = y.ln2_b + pad4(c.d_model) - y.wqkv;
     m.o_bqkv = y.bqkv - y.wqkv; m.o_wo = y.wo - y.wqkv;
   }
   return m;
@@ -214,7 +223,7 @@ static int64_t buffer_rows(const arb_scorer_config& c, int B, int S) {
 }
 
 static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, int training, WsLayout& W) {
-  const int64_t R = buffer_rows(c, B, S), d = c.d_model, f = c.d_ff, h = c.n_heads;
+  const int64_t R = buffer_rows(c, B, S), d = pad4(c.d_model), f = pad4(c.d_ff), h = c.n_heads;
   const int64_t dp = h * L.hs;      // width of the attention activations: d, or the padded heads
   W.Sp = int(align_up(S, 4));
   W.fused = use_fused(c, S);
@@ -225,12 +234,12 @@ static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int
     int64_t ping[2] = {0, 0};
     if (!training && L.n_fc > 1) {   // eval: two buffers of the widest hidden layer, used alternately
       int64_t widest = 0;
-      for (int i = 0; i + 1 < L.n_fc; ++i) widest = std::max<int64_t>(widest, L.fc_size[i]);
+      for (int i = 0; i + 1 < L.n_fc; ++i) widest = std::max<int64_t>(widest, pad4(L.fc_size[i]));
       ping[0] = take(R * widest);
       ping[1] = L.n_fc > 2 ? take(R * widest) : ping[0];
     }
     for (int i = 0; i < ARB_MAX_FC_LAYERS; ++i)
-      W.fch[i] = (i + 1 < L.n_fc) ? (training ? take(R * L.fc_size[i]) : ping[i & 1]) : 0;
+      W.fch[i] = (i + 1 < L.n_fc) ? (training ? take(R * pad4(L.fc_size[i])) : ping[i & 1]) : 0;
   }
   W.fc_last = (training && c.fc_act != ARB_ACT_NONE && c.pe_mode != 0) ? take(R * d) : 0;
   W.xnorm = W.in_mean = W.in_std = 0;
@@ -268,7 +277,8 @@ static void make_ws_layout(const arb_scorer_config& c, const ParamLayout& L, int
   if (pack_eligible(c, S)) { W.xc = take(R * c.n_features); W.poff = take(B + 1); W.plan = take(2); W.rowmap = take(R); }
   W.meanf = take(R);
   W.stdf = take(R);
-  W.xf = (n_outputs(c) > 1 && c.n_layers > 0) ? take(R * d) : 0;
+  // (a padded d_model runs the final norm on its own too, DESIGN.md 4.16)
+  W.xf = ((n_outputs(c) > 1 || d != c.d_model) && c.n_layers > 0) ? take(R * d) : 0;
   W.total = o;
 }
 
@@ -300,10 +310,10 @@ static int pick_block_n(int n) { return n <= 32 ? 32 : (n < 128 ? 64 : 128); }
 // Y[R,out] = epi( X[R,in] W[out,in]^T + bias )
 static int linear_fwd(const Ctx& k, V X, int64_t x_pitch, int in, V Wt, const float* bias, int out,
                       V Y, int64_t y_pitch, int flags, V aux, int64_t aux_pitch,
-                      DropSite drop = DropSite{0u, 0u, 1.0f}, uint32_t* relu_bits_out = nullptr) {
+                      DropSite drop = DropSite{0u, 0u, 1.0f}, uint32_t* relu_bits_out = nullptr, int drop_n = 0) {
   GemmDesc g;
   g.M = int(k.R); g.N = out; g.K = in;
-  g.drop = drop;
+  g.drop = drop; g.drop_n = drop_n;     // (a padded output: the dropout counter runs over the drop_n real columns)
   if (drop.thresh != 0) flags |= EPI_DROPOUT;
   g.A = rows_view(X, in, k.R, x_pitch);
   g.B = rows_view(Wt, in, out, in);
@@ -449,13 +459,13 @@ static WeightMats weight_mats(const arb_scorer_config& c, const ParamLayout& L) 
   WeightMats m{};
   m.n_fc = L.n_fc;
   for (int i = 0; i < L.n_fc; ++i) {
-    m.fc_w[i] = L.fc_w[i]; m.fc_out[i] = L.fc_size[i]; m.fc_in[i] = i == 0 ? c.n_features : L.fc_size[i - 1];
+    m.fc_w[i] = L.fc_w[i]; m.fc_out[i] = pad4(L.fc_size[i]); m.fc_in[i] = i == 0 ? c.n_features : pad4(L.fc_size[i - 1]);
   }
-  m.n_layers = c.n_layers; m.d = c.d_model; m.f = c.d_ff;
+  m.n_layers = c.n_layers; m.d = c.d_model; m.f = c.d_ff; m.dw = pad4(c.d_model); m.fw = pad4(c.d_ff);
   if (c.n_layers > 0) {
     const auto& y = L.layer[0];
     m.enc0 = y.wqkv;
-    m.enc_stride = y.ln2_b + c.d_model - y.wqkv;     // the layers follow each other with the same layout
+    m.enc_stride = y.ln2_b + pad4(c.d_model) - y.wqkv;     // the layers follow each other with the same layout
     m.o_wo = y.wo - y.wqkv; m.o_w1 = y.w1 - y.wqkv; m.o_w2 = y.w2 - y.wqkv;
   }
   return m;
@@ -476,6 +486,7 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   if (ws_floats < W.total) { arb_set_error("arb_scorer_forward: workspace too small"); return ARB_E_WORKSPACE; }
   Ctx k{c, B, S, int64_t(B) * S, st};
   const int d = c.d_model, F = c.n_features, f = c.d_ff, h = c.n_heads;
+  const int dw = pad4(d), fw = pad4(f);   // the buffers' widths of the residual stream and the FFN hidden layer
   const int dk = L.hs, dp = h * dk;   // the buffers' head width (padded heads: round_up(d / h, 4)) and attention width
   const HeadPad hp = head_pad(c, L);
 
@@ -558,21 +569,27 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
       hin = ws + W.xnorm;
     }
     for (int i = 0; i < L.n_fc; ++i) {
-      const int out = L.fc_size[i];
+      const int n = L.fc_size[i], out = pad4(n);   // real and stored width
       const bool last = i + 1 == L.n_fc;
       float* hout = last ? (W.fc_last ? ws + W.fc_last : xcur) : ws + W.fch[i];
       const DropSite site = make_drop_site(seed, i, SITE_FC, p_fc);
-      if (c.fc_act == ARB_ACT_NONE || c.fc_act == ARB_ACT_RELU) {
+      // the GEMM epilogue's dropout counter is row * out + column: a padded layer applies its dropout in act_forward,
+      // which counts over the real columns (with the same kept values: the epilogue drops after bias and ReLU too)
+      if ((c.fc_act == ARB_ACT_NONE || c.fc_act == ARB_ACT_RELU) && (n == out || site.thresh == 0)) {
         ARB_TRY(linear_fwd(k, hin, in, in, wfc(L.fc_w[i]), P + L.fc_b[i], out, hout, out,
                            c.fc_act == ARB_ACT_RELU ? EPI_RELU : 0, nullptr, 0, site));
+      } else if (c.fc_act == ARB_ACT_NONE || c.fc_act == ARB_ACT_RELU) {
+        ARB_TRY(linear_fwd(k, hin, in, in, wfc(L.fc_w[i]), P + L.fc_b[i], out, hout, out,
+                           c.fc_act == ARB_ACT_RELU ? EPI_RELU : 0, nullptr, 0));
+        ARB_TRY(act_forward(hout, k.R, out, ARB_ACT_NONE, site, st, plan, n));
       } else {
         ARB_TRY(linear_fwd(k, hin, in, in, wfc(L.fc_w[i]), P + L.fc_b[i], out, hout, out, 0, nullptr, 0));
-        ARB_TRY(act_forward(hout, k.R, out, c.fc_act, site, st, plan));
+        ARB_TRY(act_forward(hout, k.R, out, c.fc_act, site, st, plan, n));
       }
       hin = hout; in = out;
     }
     if (W.fc_last) {   // keep the activated FC output for backward: the positional encoding rewrites x0 in place
-      if (cudaMemcpyAsync(xcur, ws + W.fc_last, size_t(k.R) * d * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+      if (cudaMemcpyAsync(xcur, ws + W.fc_last, size_t(k.R) * dw * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
         arb_set_error("scorer: device copy failed"); return ARB_E_CUDA;
       }
     }
@@ -580,7 +597,8 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   if (c.pe_mode != 0) {   // x = sqrt(d) x + pe[indices]   (transformer.py:51-52, positional.py)
     const float* table = c.pe_mode == 2 ? P + L.pe : pe_table;
     if (!indices || !table) { arb_set_error("scorer: positional encoding needs indices and a table"); return ARB_E_INVALID_ARG; }
-    ARB_TRY(pos_forward(xcur, reinterpret_cast<const long long*>(indices), mask, table, c.pe_rows, sqrtf(float(d)), k.R, d, st));
+    // (at a padded d the table is stored at the pitch dw too, zero pads: the learned one in P, the fixed one by the host)
+    ARB_TRY(pos_forward(xcur, reinterpret_cast<const long long*>(indices), mask, table, c.pe_rows, sqrtf(float(d)), k.R, dw, st));
   }
   if (pack) {
     // The context of the alignment rows (no slate writes them) feeds the output projection: zero.  Nothing else
@@ -609,9 +627,9 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
     const V w_qkv = wpad ? t32(wpad + hp.wqkv()) : wt(pl.wqkv), w_o = wpad ? t32(wpad + hp.wo()) : wt(pl.wo);
     const float* b_qkv = wpad ? wpad + hp.bqkv() : P + pl.bqkv;
     // ---- self-attention sublayer: x + O(attn(LN(x)))   (transformer.py:133, :105-106)
-    ARB_TRY(ln_forward(xcur, P + pl.ln1_a, P + pl.ln1_b, c.ln_eps, k.R, d, xn1, ws + wl.mean1, ws + wl.std1, st, 0,
-                       bf ? xn1 : nullptr, plan));
-    ARB_TRY(linear_fwd(k, act(xn1), d, d, w_qkv, b_qkv, 3 * dp, qkv, 3 * dp, 0, nullptr, 0));
+    ARB_TRY(ln_forward(xcur, P + pl.ln1_a, P + pl.ln1_b, c.ln_eps, k.R, dw, xn1, ws + wl.mean1, ws + wl.std1, st, 0,
+                       bf ? xn1 : nullptr, plan, nullptr, d));
+    ARB_TRY(linear_fwd(k, act(xn1), dw, dw, w_qkv, b_qkv, 3 * dp, qkv, 3 * dp, 0, nullptr, 0));
     if (W.fused) {
       ARB_TRY(launch_attn_fwd(attn_fwd_args(geom, qkv, act(ctx), mask, g_skip_padding ? kext : nullptr, ws + wl.smax,
                                             ws + wl.ssum, make_drop_site(seed, l, SITE_ATTN_P, p_drop)), st));
@@ -638,11 +656,11 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
         ARB_TRY(launch_gemm_tf32(g, st));
       }
     }
-    ARB_TRY(linear_fwd(k, act(ctx), dp, dp, w_o, P + pl.bo, d, xmid, d, EPI_ADD_AUX, xcur, d,
-                       make_drop_site(seed, l, SITE_ATTN_OUT, p_drop)));
+    ARB_TRY(linear_fwd(k, act(ctx), dp, dp, w_o, P + pl.bo, dw, xmid, dw, EPI_ADD_AUX, xcur, dw,
+                       make_drop_site(seed, l, SITE_ATTN_OUT, p_drop), nullptr, d));
     // ---- feed-forward sublayer: x + W2 relu(W1 LN(x))   (transformer.py:134, :227)
-    ARB_TRY(ln_forward(xmid, P + pl.ln2_a, P + pl.ln2_b, c.ln_eps, k.R, d, xn2, ws + wl.mean2, ws + wl.std2, st, 0,
-                       bf ? xn2 : nullptr, plan));
+    ARB_TRY(ln_forward(xmid, P + pl.ln2_a, P + pl.ln2_b, c.ln_eps, k.R, dw, xn2, ws + wl.mean2, ws + wl.std2, st, 0,
+                       bf ? xn2 : nullptr, plan, nullptr, d));
     if (use_ffn_chain(c, k.R)) {      // both linears in one kernel; H is kept for the backward only
       FfnChain fc;
       fc.rows = int(k.R); fc.d = d; fc.f = f; fc.rows_dev = k.rows_dev;
@@ -652,21 +670,28 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
       fc.bits = wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr;
       ARB_TRY(launch_ffn_chain(fc, st));
     } else {
-      ARB_TRY(linear_fwd(k, act(xn2), d, d, wt(pl.w1), P + pl.b1, f, act(hdn), f, EPI_RELU, nullptr, 0,
+      ARB_TRY(linear_fwd(k, act(xn2), dw, dw, wt(pl.w1), P + pl.b1, fw, act(hdn), fw, EPI_RELU, nullptr, 0,
                          make_drop_site(seed, l, SITE_FFN_HID, p_drop),
-                         wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr));
-      ARB_TRY(linear_fwd(k, act(hdn), f, f, wt(pl.w2), P + pl.b2, d, xout, d, EPI_ADD_AUX, xmid, d,
-                         make_drop_site(seed, l, SITE_FFN_OUT, p_drop)));
+                         wl.hbits ? reinterpret_cast<uint32_t*>(ws + wl.hbits) : nullptr, f));
+      ARB_TRY(linear_fwd(k, act(hdn), fw, fw, wt(pl.w2), P + pl.b2, dw, xout, dw, EPI_ADD_AUX, xmid, dw,
+                         make_drop_site(seed, l, SITE_FFN_OUT, p_drop), nullptr, d));
     }
     xcur = xout;
   }
   const int has_norm = c.n_layers > 0;
   if (hidden) {   // encoder output (model.py:62-70): the final norm's output, written at the items' places
-    if (has_norm)
+    if (has_norm && dw == d)
       return ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, d, hidden, ws + W.meanf, ws + W.stdf, st, 0,
                         nullptr, plan, rowmap);
-    // no encoder: the reference's encoder is the identity (model.py:59), so this is the activated FC output
-    if (cudaMemcpyAsync(hidden, xcur, size_t(k.R) * d * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+    if (has_norm) {   // padded d: normed into xf, then its real columns copied out below
+      ARB_TRY(ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, dw, ws + W.xf, ws + W.meanf, ws + W.stdf, st, 0,
+                         nullptr, nullptr, nullptr, d));
+      xcur = ws + W.xf;
+    }
+    // (no encoder: the reference's encoder is the identity, model.py:59, so this is the activated FC output) the real
+    // columns of the stored rows: hidden is [B, S, d]
+    if (cudaMemcpy2DAsync(hidden, size_t(d) * sizeof(float), xcur, size_t(dw) * sizeof(float), size_t(d) * sizeof(float),
+                          size_t(k.R), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
       arb_set_error("scorer: device copy failed"); return ARB_E_CUDA;
     }
     return ARB_OK;
@@ -674,13 +699,22 @@ static int forward_impl(const arb_scorer_config& c, const float* P, const float*
   if (n_outputs(c) > 1) {   // d_output > 1: final norm as its own kernel, then one dot product per output (model.py:116)
     const float* xf = xcur;
     if (has_norm) {
-      ARB_TRY(ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, d, ws + W.xf, ws + W.meanf, ws + W.stdf, st));
+      ARB_TRY(ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, dw, ws + W.xf, ws + W.meanf, ws + W.stdf, st, 0,
+                         nullptr, nullptr, nullptr, d));
       xf = ws + W.xf;
     }
-    return head_multi_forward(xf, P + L.head_w, P + L.head_b, c.out_act, k.R, d, n_outputs(c), scores, st);
+    return head_multi_forward(xf, P + L.head_w, P + L.head_b, c.out_act, k.R, dw, n_outputs(c), scores, st);
   }
+  if (has_norm && dw != d) {   // padded d: the final norm over the real columns on its own, then the plain head
+    ARB_TRY(ln_forward(xcur, P + L.lnf_a, P + L.lnf_b, c.ln_eps, k.R, dw, ws + W.xf, ws + W.meanf, ws + W.stdf, st, 0,
+                       nullptr, nullptr, nullptr, d));
+    return head_forward(ws + W.xf, nullptr, nullptr, c.ln_eps, P + L.head_w, P + L.head_b, 0, c.out_act, k.R, dw, scores,
+                        nullptr, nullptr, st, nullptr, nullptr);
+  }
+  // (an FC-only model of a width that is not a multiple of 4 runs the head at the stored width: the pads of x and of
+  // the head's weight are zeros, which add exact zeros to the dot product)
   ARB_TRY(head_forward(xcur, has_norm ? P + L.lnf_a : nullptr, has_norm ? P + L.lnf_b : nullptr, c.ln_eps, P + L.head_w,
-                       P + L.head_b, has_norm, c.out_act, k.R, d, scores, ws + W.meanf, ws + W.stdf, st, plan, rowmap));
+                       P + L.head_b, has_norm, c.out_act, k.R, dw, scores, ws + W.meanf, ws + W.stdf, st, plan, rowmap));
   return ARB_OK;
 }
 
@@ -688,7 +722,7 @@ struct ScratchLayout { int64_t dxa, dxb, dxn, dxm, dqkv, dctx, dprob, prob, delt
 // want_dx: room for d loss / d x over packed rows (backward_ex), after everything the plain backward uses
 static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L, int B, int S, ScratchLayout& Z,
                                 bool want_dx = false) {
-  const int64_t R = buffer_rows(c, B, S), d = c.d_model;
+  const int64_t R = buffer_rows(c, B, S), d = pad4(c.d_model);
   const int Sp = int(align_up(S, 4));
   int64_t o = 0;
   auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
@@ -707,7 +741,7 @@ static void make_scratch_layout(const arb_scorer_config& c, const ParamLayout& L
   }
   // FC-block backward: two gradient buffers of the widest tensor it differentiates through
   int64_t widest = c.fc_input_norm ? c.n_features : 0;
-  for (int i = 0; i + 1 < L.n_fc; ++i) widest = std::max<int64_t>(widest, L.fc_size[i]);
+  for (int i = 0; i + 1 < L.n_fc; ++i) widest = std::max<int64_t>(widest, pad4(L.fc_size[i]));
   if (c.fc_act != ARB_ACT_NONE) widest = std::max<int64_t>(widest, d);
   Z.dfa = widest ? take(R * widest) : 0;
   Z.dfb = widest ? take(R * widest) : 0;
@@ -735,6 +769,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   if (scratch_floats < Z.total) { arb_set_error("arb_scorer_backward: scratch too small"); return ARB_E_WORKSPACE; }
   Ctx k{c, B, S, int64_t(B) * S, st};
   const int d = c.d_model, F = c.n_features, f = c.d_ff, h = c.n_heads;
+  const int dw = pad4(d), fw = pad4(f);   // the buffers' widths of the residual stream and the FFN hidden layer
   const int dk = L.hs, dp = h * dk;   // the buffers' head width (padded heads: round_up(d / h, 4)) and attention width
   const float alpha = c.n_layers > 0 ? 1.0f / sqrtf(float(L.hw)) : 1.0f;
   const HeadPad hp = head_pad(c, L);
@@ -801,34 +836,57 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     ARB_TRY(zero_rows(z, plan, k.R, st));
   }
   const int has_norm = c.n_layers > 0;
+  if (dhidden && dw != d) {
+    // a d_model that is not a multiple of 4: d hidden [B, S, d] widened to the stored width, pads +0 (into dxn, which
+    // the layers below only write after the final norm's backward has read it)
+    if (cudaMemsetAsync(dxn, 0, size_t(k.R) * dw * sizeof(float), st) != cudaSuccess ||
+        cudaMemcpy2DAsync(dxn, size_t(dw) * sizeof(float), dhidden, size_t(d) * sizeof(float), size_t(d) * sizeof(float),
+                          size_t(k.R), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+      arb_set_error("scorer: device copy failed"); return ARB_E_CUDA;
+    }
+    dhidden = dxn;
+  }
+  // The head kernels apply the dropout mask of the layer below with the counter row * width + column: at a padded width
+  // (FC-only) they emit the unmasked gradient and act_backward masks it over the real columns (and sums the bias
+  // gradient).
+  const bool split_drop = c.n_layers == 0 && dw != d && top_site.thresh != 0;
   const float* xlast = c.n_layers > 0 ? ws + W.layer[c.n_layers - 1].xout : ws + W.x0;
   float* top_bias_grad = c.n_layers > 0 ? g(L.layer[c.n_layers - 1].b2) : fc_bias_grad;
   const float* dy = top_site.thresh ? dxm : dx;   // gradient w.r.t. the output of the linear below the dropout
   if (dhidden) {
     if (has_norm) {   // the final norm's backward from the given gradient (packed rows: read at the items' places)
-      ARB_TRY(ln_backward(dhidden, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, d, dx,
-                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16, plan, rowmap));
+      ARB_TRY(ln_backward(dhidden, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, dw, dx,
+                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16, plan, rowmap, d));
     } else if (!fc_act) {   // FC-only model: d hidden through the FC dropout; the FC bias gradient is its column sums
       if (fc_site.thresh || fc_bias_grad)
-        ARB_TRY(act_backward(dhidden, ws + W.x0, dx, k.R, d, ARB_ACT_NONE, fc_site, 1.0f, fc_bias_grad, st));
+        ARB_TRY(act_backward(dhidden, ws + W.x0, dx, k.R, dw, ARB_ACT_NONE, fc_site, 1.0f, fc_bias_grad, st, nullptr, d));
       dy = (fc_site.thresh || fc_bias_grad) ? dx : dhidden;
     }   // (FC-only with an activation: act_backward below reads dhidden)
-  } else if (n_outputs(c) > 1) {
+  } else if (n_outputs(c) > 1 || (has_norm && dw != d)) {
     if (has_norm) {   // d xf into dxn, then the final norm's backward emits dx (+ its masked copy and the b2 gradient)
-      ARB_TRY(head_multi_backward(dscores, scores, ws + W.xf, P + L.head_w, c.out_act, k.R, d, n_outputs(c), dxn,
-                                  g(L.head_w), g(L.head_b), st));
-      ARB_TRY(ln_backward(dxn, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, d, dx,
-                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16));
+      if (n_outputs(c) > 1)
+        ARB_TRY(head_multi_backward(dscores, scores, ws + W.xf, P + L.head_w, c.out_act, k.R, dw, n_outputs(c), dxn,
+                                    g(L.head_w), g(L.head_b), st));
+      else    // padded d: the plain head over xf, as the forward ran it
+        ARB_TRY(head_backward(dscores, scores, ws + W.xf, nullptr, nullptr, nullptr, nullptr, c.ln_eps, P + L.head_w,
+                              P + L.head_b, 0, c.out_act, k.R, dw, dxn, nullptr, nullptr, g(L.head_w), g(L.head_b), st));
+      ARB_TRY(ln_backward(dxn, xlast, P + L.lnf_a, ws + W.meanf, ws + W.stdf, c.ln_eps, nullptr, k.R, dw, dx,
+                          g(L.lnf_a), g(L.lnf_b), st, dxm, top_site, top_bias_grad, 0, nullptr, dy16, nullptr, nullptr,
+                          d));
     } else {
-      ARB_TRY(head_multi_backward(dscores, scores, xlast, P + L.head_w, c.out_act, k.R, d, n_outputs(c), dx,
-                                  g(L.head_w), g(L.head_b), st, dxm, top_site, top_bias_grad));
+      ARB_TRY(head_multi_backward(dscores, scores, xlast, P + L.head_w, c.out_act, k.R, dw, n_outputs(c), dx,
+                                  g(L.head_w), g(L.head_b), st, split_drop ? nullptr : dxm,
+                                  split_drop ? none_site : top_site, split_drop ? nullptr : top_bias_grad));
     }
   } else {
     ARB_TRY(head_backward(dscores, scores, xlast, has_norm ? P + L.lnf_a : nullptr, has_norm ? P + L.lnf_b : nullptr,
-                          ws + W.meanf, ws + W.stdf, c.ln_eps, P + L.head_w, P + L.head_b, has_norm, c.out_act, k.R, d,
+                          ws + W.meanf, ws + W.stdf, c.ln_eps, P + L.head_w, P + L.head_b, has_norm, c.out_act, k.R, dw,
                           dx, has_norm ? g(L.lnf_a) : nullptr, has_norm ? g(L.lnf_b) : nullptr, g(L.head_w),
-                          g(L.head_b), st, dxm, top_site, top_bias_grad, dy16, plan, rowmap));
+                          g(L.head_b), st, split_drop ? nullptr : dxm, split_drop ? none_site : top_site,
+                          split_drop ? nullptr : top_bias_grad, dy16, plan, rowmap));
   }
+  if (split_drop && !dhidden)
+    ARB_TRY(act_backward(dx, xlast, dxm, k.R, dw, ARB_ACT_NONE, top_site, 1.0f, top_bias_grad, st, plan, d));
   for (int l = c.n_layers - 1; l >= 0; --l) {
     const auto& pl = L.layer[l];
     const auto& wl = W.layer[l];
@@ -838,7 +896,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
     float* xmid = ws + wl.xmid; float* xn2 = ws + wl.xn2; float* hdn = ws + wl.hdn;
     // ---- feed-forward sublayer backward:  xout = xmid + W2 relu(W1 xn2 + b1) + b2
     const V dyv = bf ? b16(dy16) : V(dy);      // what the sublayer's products read as the incoming gradient
-    if (G) ARB_TRY(linear_bwd_weight(k, dyv, d, d, act(hdn), f, f, G + pl.w2));   // (b2 gradient: fused into the kernel that emitted dy)
+    if (G) ARB_TRY(linear_bwd_weight(k, dyv, dw, dw, act(hdn), fw, fw, G + pl.w2));   // (b2 gradient: fused into the kernel that emitted dy)
     // hdn <- d hdn in place; hdn > 0 <=> ReLU active AND kept by the hidden dropout, so the mask tile also carries
     // the dropout mask and only the 1/(1-p) scale is needed
     if (use_ffn_chain(c, k.R)) {
@@ -852,17 +910,18 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
       if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
     } else {
       if (wl.hbits)    // ReLU mask from the forward's bit mask (1 bit per unit) instead of the fp32 activation tile
-        ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_COLSUM, nullptr, 0, 1.0f, g(pl.b1),
+        ARB_TRY(linear_bwd_input(k, dyv, dw, dw, wt(pl.w2), fw, act(hdn), fw, EPI_COLSUM, nullptr, 0, 1.0f, g(pl.b1),
                                  reinterpret_cast<const uint32_t*>(ws + wl.hbits)));
       else
-        ARB_TRY(linear_bwd_input(k, dyv, d, d, wt(pl.w2), f, act(hdn), f, EPI_MASK_AUX | EPI_COLSUM, act(hdn), f,
+        ARB_TRY(linear_bwd_input(k, dyv, dw, dw, wt(pl.w2), fw, act(hdn), fw, EPI_MASK_AUX | EPI_COLSUM, act(hdn), fw,
                                  drop_on ? 1.0f / (1.0f - p_drop) : 1.0f, g(pl.b1)));   // b1 gradient in the epilogue
-      if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), f, f, act(xn2), d, d, G + pl.w1));
-      ARB_TRY(linear_bwd_input(k, act(hdn), f, f, wt(pl.w1), d, act(dxn), d, 0, nullptr, 0));
+      if (G) ARB_TRY(linear_bwd_weight(k, act(hdn), fw, fw, act(xn2), dw, dw, G + pl.w1));
+      ARB_TRY(linear_bwd_input(k, act(hdn), fw, fw, wt(pl.w1), dw, act(dxn), dw, 0, nullptr, 0));
     }
     const DropSite site_ao = make_drop_site(seed, l, SITE_ATTN_OUT, p_drop);
-    ARB_TRY(ln_backward(dxn, xmid, P + pl.ln2_a, ws + wl.mean2, ws + wl.std2, c.ln_eps, dx, k.R, d, dx_alt,
-                        g(pl.ln2_a), g(pl.ln2_b), st, dxm, site_ao, g(pl.bo), 0, bf ? dxn : nullptr, dy16, plan));
+    ARB_TRY(ln_backward(dxn, xmid, P + pl.ln2_a, ws + wl.mean2, ws + wl.std2, c.ln_eps, dx, k.R, dw, dx_alt,
+                        g(pl.ln2_a), g(pl.ln2_b), st, dxm, site_ao, g(pl.bo), 0, bf ? dxn : nullptr, dy16, plan, nullptr,
+                        d));
     // dx_alt = d loss / d xmid ; dy = the same through the dropout on the attention sublayer output
     dy = site_ao.thresh ? dxm : dx_alt;
     // ---- attention sublayer backward:  xmid = xin + Wo ctx + bo
@@ -877,8 +936,8 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
       arb_set_error("scorer: memset failed"); return ARB_E_CUDA;
     }
     const V dyo = bf ? b16(dy16) : V(dy);
-    if (G) ARB_TRY(linear_bwd_weight(k, dyo, d, d, act(ctx), dp, dp, gw_o));   // (bo gradient: fused into the LayerNorm backward above)
-    ARB_TRY(linear_bwd_input(k, dyo, d, d, wt_o, dp, dctx, dp, 0, nullptr, 0));
+    if (G) ARB_TRY(linear_bwd_weight(k, dyo, dw, dw, act(ctx), dp, dp, gw_o));   // (bo gradient: fused into the LayerNorm backward above)
+    ARB_TRY(linear_bwd_input(k, dyo, dw, dw, wt_o, dp, dctx, dp, 0, nullptr, 0));
     if (use_fused_bwd(c, S)) {
       // dQ | dK | dV into one [R, 3d] buffer (bfloat16 in bf16 mode); the QKV bias gradient is fused
       ARB_TRY(launch_attn_bwd(attn_bwd_args(geom, qkv, act(ctx), dctx, dqkv, mask, (skip || pack) ? gext : nullptr,
@@ -937,23 +996,23 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         ARB_TRY(launch_gemm_tf32(g, st));
       }
     }
-    if (G) ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * dp, 3 * dp, act(xn1), d, d, gw_qkv));
+    if (G) ARB_TRY(linear_bwd_weight(k, act(dqkv), 3 * dp, 3 * dp, act(xn1), dw, dw, gw_qkv));
     if (G && !use_fused_bwd(c, S)) ARB_TRY(colsum_accumulate(dqkv, k.R, 3 * dp, 3 * dp, gb_qkv, st));
-    ARB_TRY(linear_bwd_input(k, act(dqkv), 3 * dp, 3 * dp, wt_qkv, d, act(dxn), d, 0, nullptr, 0));
+    ARB_TRY(linear_bwd_input(k, act(dqkv), 3 * dp, 3 * dp, wt_qkv, dw, act(dxn), dw, 0, nullptr, 0));
     if (gpad) ARB_TRY(head_pad_grads(gpad, hp, l, G, st));
     DropSite site_below = l > 0 ? make_drop_site(seed, l - 1, SITE_FFN_OUT, p_drop) : (fc_act ? none_site : fc_site);
     // with a positional encoding the encoder input is sqrt(d) * fc_out + pe: the gradient that reaches the FC
     // (through its dropout mask, if any) carries the extra sqrt(d)
     if (l == 0 && c.pe_mode != 0 && !fc_act) site_below.scale *= sqrtf(float(d));
-    ARB_TRY(ln_backward(dxn, xin, P + pl.ln1_a, ws + wl.mean1, ws + wl.std1, c.ln_eps, dx_alt, k.R, d, dx,
+    ARB_TRY(ln_backward(dxn, xin, P + pl.ln1_a, ws + wl.mean1, ws + wl.std1, c.ln_eps, dx_alt, k.R, dw, dx,
                         g(pl.ln1_a), g(pl.ln1_b), st, dxm, site_below, l > 0 ? g(L.layer[l - 1].b2) : fc_bias_grad,
-                        0, bf ? dxn : nullptr, l > 0 ? dy16 : nullptr, plan));   // (the FC block below layer 0 stays TF32)
+                        0, bf ? dxn : nullptr, l > 0 ? dy16 : nullptr, plan, nullptr, d));   // (the FC block below layer 0 stays TF32)
     // dx = d loss / d xin ; dy = the same through the dropout that produced xin's last summand
     dy = (site_below.thresh || site_below.scale != 1.0f) ? dxm : dx;
   }
   if (c.pe_mode == 2 && G) {   // learned table: d pe[idx] += d x0
     if (!indices) { arb_set_error("scorer: positional encoding needs indices"); return ARB_E_INVALID_ARG; }
-    ARB_TRY(pos_backward(dx, reinterpret_cast<const long long*>(indices), mask, G + L.pe, c.pe_rows, k.R, d, st));
+    ARB_TRY(pos_backward(dx, reinterpret_cast<const long long*>(indices), mask, G + L.pe, c.pe_rows, k.R, dw, st));
   }
   // ---- FC-block backward (model.py:35-44), last layer first.  dz = gradient w.r.t. the linear's output.
   const float* dz = dy;            // identity activation: mask + bias gradient were fused into the kernel that emitted dy
@@ -962,13 +1021,13 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
   if (fc_act) {
     const float* h_last = W.fc_last ? ws + W.fc_last : ws + W.x0;
     const float* dh = (dhidden && c.n_layers == 0) ? dhidden : dx;   // d loss / d (activated FC output)
-    ARB_TRY(act_backward(dh, h_last, dfa, k.R, d, c.fc_act, fc_site, c.pe_mode != 0 ? sqrtf(float(d)) : 1.0f,
-                         g(L.fc_b[L.n_fc - 1]), st, plan));
+    ARB_TRY(act_backward(dh, h_last, dfa, k.R, dw, c.fc_act, fc_site, c.pe_mode != 0 ? sqrtf(float(d)) : 1.0f,
+                         g(L.fc_b[L.n_fc - 1]), st, plan, d));
     dz = dfa; std::swap(dfa, dfb);
   }
   for (int i = L.n_fc - 1; i >= 0; --i) {
-    const int out = L.fc_size[i];
-    const int in = i > 0 ? L.fc_size[i - 1] : F;
+    const int out = pad4(L.fc_size[i]);       // the stored widths (the products run over the zero pads)
+    const int in = i > 0 ? pad4(L.fc_size[i - 1]) : F;
     const float* hin = i > 0 ? ws + W.fch[i - 1] : (c.fc_input_norm ? ws + W.xnorm : x);
     if (G) ARB_TRY(linear_bwd_weight(k, dz, out, out, hin, in, in, G + L.fc_w[i]));
     if (i > 0) {
@@ -980,7 +1039,7 @@ static int backward_impl(const arb_scorer_config& c, const float* P, const float
         ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[i]), in, dfa, in, EPI_COLSUM, nullptr, 0, 1.0f, g(L.fc_b[i - 1])));
       } else {
         ARB_TRY(linear_bwd_input(k, dz, out, out, wfc(L.fc_w[i]), in, dfa, in, 0, nullptr, 0));
-        ARB_TRY(act_backward(dfa, hin, dfa, k.R, in, c.fc_act, site, 1.0f, g(L.fc_b[i - 1]), st, plan));
+        ARB_TRY(act_backward(dfa, hin, dfa, k.R, in, c.fc_act, site, 1.0f, g(L.fc_b[i - 1]), st, plan, L.fc_size[i - 1]));
       }
       dz = dfa; std::swap(dfa, dfb);
       continue;

@@ -137,7 +137,10 @@ __device__ __forceinline__ void r_reduce_columns(float4 (&acc)[NJ], float (*sh)[
 // (Little's law), and a warp that retires after a single step spends a third of its life waiting for its first loads
 // and for a new block to be scheduled.
 // MAP: packed rows with a row-mapped output (rowmap_out); a template flag so that the plain kernels compile unchanged
-template <int LPR, int NJ, bool FILLED, bool MAP>
+// PAD: a row of n real columns stored at the pitch width = round_up(n, 4) with zero pads (DESIGN.md 4.16): the
+// statistics run over the n real columns (the zero pads add nothing to the sum; the squares are masked per element)
+// and the zero pads of the gain and bias write +0 into the pads of y; also a template flag
+template <int LPR, int NJ, bool FILLED, bool MAP, bool PAD = false>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float* __restrict__ x,
                                                                     const float* __restrict__ a,
                                                                     const float* __restrict__ b, float eps,
@@ -146,8 +149,9 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
                                                                     float* __restrict__ std_o, int torch_mode,
                                                                     uint16_t* __restrict__ y16,
                                                                     const int* __restrict__ rows_dev, int steps,
-                                                                    const int* __restrict__ rowmap_out) {
+                                                                    const int* __restrict__ rowmap_out, int n) {
   if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
+  if (!PAD) n = width;
   arb_pdl_wait();
   constexpr int RW = 32 / LPR;
   const int lane = threadIdx.x & 31, rg = lane / LPR;
@@ -166,19 +170,21 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
     float sum = 0.f;
 #pragma unroll
     for (int j = 0; j < NJ; ++j) sum += cur[j].x + cur[j].y + cur[j].z + cur[j].w;
-    const float m = r_sum<LPR>(sum) / float(width);
+    const float m = r_sum<LPR>(sum) / float(n);
     float ss = 0.f;
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
-      if (r_col<LPR>(lane, j) < width) {
-        const float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
+      const int c = r_col<LPR>(lane, j);
+      if (c < width) {
+        float d0 = cur[j].x - m, d1 = cur[j].y - m, d2 = cur[j].z - m, d3 = cur[j].w - m;
+        if (PAD) { if (c >= n) d0 = 0.f; if (c + 1 >= n) d1 = 0.f; if (c + 2 >= n) d2 = 0.f; if (c + 3 >= n) d3 = 0.f; }
         ss += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
       }
     }
     ss = r_sum<LPR>(ss);
     // torch_mode: nn.LayerNorm (biased variance, eps inside the root; FCModel's input_norm, model.py:27) -- the saved
     // "std" is then sqrt(var + eps) and the backward is called with eps = 0
-    const float sdq = torch_mode ? sqrtf(ss / float(width) + eps) : sqrtf(ss / float(width - 1));
+    const float sdq = torch_mode ? sqrtf(ss / float(n) + eps) : sqrtf(ss / float(n - 1));
     // one reciprocal per row instead of a division per element: the kernel is bound by instruction issue as much as
     // by HBM (an IEEE division is ~10 instructions), and a * (x - mean) * (1 / (std + eps)) differs from the
     // reference's a * (x - mean) / (std + eps) by one rounding (6e-8 relative)
@@ -207,15 +213,18 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) ln_fwd_kernel(const float
 // dx = [dres +] r (dxh - mean(dxh)) - r^2 (sum_k dxh_k c_k) / ((d-1) std) * c,   dxh = dy * a, c = x - mean,
 // r = 1/(std+eps).   grad_a += sum_rows dy * xhat,  grad_b += sum_rows dy  (block partials -> DetParts slots).
 // MAP: packed rows reading a row-mapped gradient (rowmap_in); a template flag as in ln_fwd_kernel
-template <int LPR, int NJ, bool FILLED, bool MAP>
+// PAD: n real columns at the pitch width as in ln_fwd_kernel: c = x - mean and the outputs are +0 in the pads, and the
+// dropout counter of dx_masked is row * n + column
+template <int LPR, int NJ, bool FILLED, bool MAP, bool PAD = false>
 __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) ln_bwd_kernel(
     const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ a,
     const float* __restrict__ mean_i, const float* __restrict__ std_i, float eps, const float* __restrict__ dres,
     long long rows, int width, int steps, float* __restrict__ dx, float* __restrict__ grad_a,
     float* __restrict__ grad_b, float* __restrict__ dx_masked, DropSite site, float* __restrict__ colsum_out,
     int torch_mode, const uint16_t* __restrict__ dy16_in, uint16_t* __restrict__ dy16_out,
-    const int* __restrict__ rows_dev, const int* __restrict__ rowmap_in) {
+    const int* __restrict__ rows_dev, const int* __restrict__ rowmap_in, int n) {
   if (FILLED) width = 4 * LPR * NJ;   // (see with_row_layout)
+  if (!PAD) n = width;
   arb_pdl_wait();
   site.seed = drop_seed(site);
   constexpr int RW = 32 / LPR;
@@ -257,7 +266,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) ln_bwd_k
       float* ab = &acc_b[j].x;
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
-        const float cc = in ? xv[t] - mean : 0.f;
+        const float cc = in && (!PAD || r_col<LPR>(lane, j) + t < n) ? xv[t] - mean : 0.f;
         const float dyv = gv[t];
         aa[t] += dyv * cc * r;     // dy * xhat
         ab[t] += dyv;
@@ -270,9 +279,9 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) ln_bwd_k
     }
     s1 = r_sum<LPR>(s1);
     s2 = r_sum<LPR>(s2);
-    const float m1 = s1 / float(width);
-    const float coef = torch_mode ? r * r * r * s2 / float(width)
-                                  : ((sd > 0.f) ? r * r * s2 / (float(width - 1) * sd) : 0.f);
+    const float m1 = s1 / float(n);
+    const float coef = torch_mode ? r * r * r * s2 / float(n)
+                                  : ((sd > 0.f) ? r * r * s2 / (float(n - 1) * sd) : 0.f);
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       float* gv = &g[j].x;
@@ -282,13 +291,14 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) ln_bwd_k
       for (int t = 0; t < 4; ++t) {
         float o = r * (gv[t] - m1) - coef * xv[t];
         if (dres) o += rv[t];
+        if (PAD && r_col<LPR>(lane, j) + t >= n) o = 0.f;   // (r (0 - m1) is not 0)
         gv[t] = o;
       }
     }
     if (ok) {
       r_store<LPR>(dx + row * width, width, lane, g);
       if (dx_masked) {   // the same gradient through the dropout of the sublayer below (mask regenerated)
-        r_drop<LPR>(g, row, width, lane, site);
+        r_drop<LPR>(g, row, n, lane, site);
         r_store<LPR>(dx_masked + row * width, width, lane, g);
       }
       // bf16 mode: the copy the weight / input-gradient GEMMs of the sublayer below read (after its dropout mask)
@@ -426,11 +436,11 @@ __global__ void __launch_bounds__(256) tf32_weight_copy_kernel(const float* __re
       if (i >= m.fc_w[j] && i < m.fc_w[j] + (long long)m.fc_out[j] * m.fc_in[j]) { o = m.fc_w[j]; rows = m.fc_out[j]; cols = m.fc_in[j]; }
     if (o < 0 && m.n_layers > 0 && i >= m.enc0 && i < m.enc0 + m.n_layers * m.enc_stride) {
       const long long base = m.enc0 + (i - m.enc0) / m.enc_stride * m.enc_stride, j = i - base;
-      const long long d = m.d, f = m.f;
+      const long long d = m.d, dw = m.dw, fw = m.fw;
       if (j < 3 * d * d) { o = base; rows = int(3 * d); cols = int(d); }
       else if (j >= m.o_wo && j < m.o_wo + d * d) { o = base + m.o_wo; rows = int(d); cols = int(d); }
-      else if (j >= m.o_w1 && j < m.o_w1 + f * d) { o = base + m.o_w1; rows = int(f); cols = int(d); }
-      else if (j >= m.o_w2 && j < m.o_w2 + d * f) { o = base + m.o_w2; rows = int(d); cols = int(f); }
+      else if (j >= m.o_w1 && j < m.o_w1 + fw * dw) { o = base + m.o_w1; rows = int(fw); cols = int(dw); }
+      else if (j >= m.o_w2 && j < m.o_w2 + dw * fw) { o = base + m.o_w2; rows = int(dw); cols = int(fw); }
     }
     if (o >= 0) {
       const long long e = i - o, r = e / cols, c = e % cols;
@@ -440,32 +450,33 @@ __global__ void __launch_bounds__(256) tf32_weight_copy_kernel(const float* __re
 }
 
 // Padded heads: the padded copies of W_qkv, its transpose, b_qkv, W_o and its transpose (HeadPad), every element
-// written, the pads as +0.  Padded row (column) g * hs + t holds the real row (column) g * w + t when t < w.
+// written, the pads as +0.  Padded row (column) g * hs + t holds the real row (column) g * w + t when t < w; rows
+// (columns) of the residual stream from d to dw are pads too.
 __global__ void __launch_bounds__(256) head_pad_copy_kernel(const float* __restrict__ pr, const float* __restrict__ P,
                                                             HeadPad m, float* __restrict__ out) {
   arb_pdl_wait();
-  const long long d = m.d, dp = m.dp(), size = m.size(), n = size * m.n_layers;
+  const long long d = m.d, dw = m.dw, dp = m.dp(), size = m.size(), n = size * m.n_layers;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const long long l = i / size, j = i - l * size, base = m.enc0 + l * m.enc_stride;
     long long src;      // offset of the real element in the flat parameters, or -1 for a pad
     const float* from = pr;
     auto real = [&](long long padded) { const long long g = padded / m.hs, t = padded - g * m.hs; return t < m.w ? g * m.w + t : -1; };
-    if (j < m.wqkvt()) {                     // wqkv [3 dp, d]
-      const long long r = real(j / d);
-      src = r < 0 ? -1 : base + r * d + j % d;
-    } else if (j < m.bqkv()) {               // wqkvt [d, 3 dp]
-      const long long e = j - m.wqkvt(), r = real(e % (3 * dp));
-      src = r < 0 ? -1 : base + r * d + e / (3 * dp);
+    if (j < m.wqkvt()) {                     // wqkv [3 dp, dw]
+      const long long r = real(j / dw), c = j % dw;
+      src = r < 0 || c >= d ? -1 : base + r * d + c;
+    } else if (j < m.bqkv()) {               // wqkvt [dw, 3 dp]
+      const long long e = j - m.wqkvt(), r = real(e % (3 * dp)), c = e / (3 * dp);
+      src = r < 0 || c >= d ? -1 : base + r * d + c;
     } else if (j < m.wo()) {                 // bqkv [3 dp]: the fp32 bias, as the unpadded QKV linear reads it
       const long long r = real(j - m.bqkv());
       src = r < 0 ? -1 : base + m.o_bqkv + r;
       from = P;
-    } else if (j < m.wot()) {                // wo [d, dp]
-      const long long e = j - m.wo(), c = real(e % dp);
-      src = c < 0 ? -1 : base + m.o_wo + e / dp * d + c;
-    } else {                                 // wot [dp, d]
-      const long long e = j - m.wot(), c = real(e / d);
-      src = c < 0 ? -1 : base + m.o_wo + e % d * d + c;
+    } else if (j < m.wot()) {                // wo [dw, dp]
+      const long long e = j - m.wo(), c = real(e % dp), r = e / dp;
+      src = c < 0 || r >= d ? -1 : base + m.o_wo + r * d + c;
+    } else {                                 // wot [dp, dw]
+      const long long e = j - m.wot(), c = real(e / dw), r = e % dw;
+      src = c < 0 || r >= d ? -1 : base + m.o_wo + r * d + c;
     }
     out[i] = src < 0 ? 0.0f : from[src];
   }
@@ -479,8 +490,8 @@ __global__ void __launch_bounds__(256) head_pad_grads_kernel(const float* __rest
   const long long d = m.d, dp = m.dp(), n_w = 3 * d * d, n_b = 3 * d, n = n_w + n_b + d * d;
   auto padded = [&](long long real) { const long long g = real / m.w; return g * m.hs + (real - g * m.w); };
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    if (i < n_w) {                           // W_qkv [3d, d]
-      G[base + i] += gp[m.gwqkv() + padded(i / d) * d + i % d];
+    if (i < n_w) {                           // W_qkv [3d, d] (padded: [3 dp, dw])
+      G[base + i] += gp[m.gwqkv() + padded(i / d) * m.dw + i % d];
     } else if (i < n_w + n_b) {              // b_qkv [3d]
       const long long e = i - n_w;
       G[base + m.o_bqkv + e] += gp[m.gbqkv() + padded(e)];
@@ -910,28 +921,43 @@ __global__ void __launch_bounds__(256) pos_bwd_kernel(const float* __restrict__ 
 // FCModel applies dropout(activation(linear(x))) per layer (model.py:41-43).  ReLU / identity run inside the GEMM
 // epilogue; the kernels below serve the other activations and the backward of every activation under dropout.
 // Element index of the dropout counter = row * width + column (the same as the GEMM epilogue's).
+// A layer of n columns that is not a multiple of 4 is stored at the pitch width = round_up(n, 4) (DESIGN.md 4.16): the
+// counter then keeps the real layout, row * n + column, and the pad columns are written +0 (sigmoid(0) is not 0).
 __global__ void __launch_bounds__(256) act_fwd_kernel(float* __restrict__ h, long long n4, int act, DropSite site,
-                                                      const int* __restrict__ rows_dev, int width4) {
+                                                      const int* __restrict__ rows_dev, int width4, int n) {
   site.seed = drop_seed(site);
   if (rows_dev) n4 = min(n4, (long long)__ldg(rows_dev) * width4);
+  const bool padded = n != 4 * width4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = reinterpret_cast<float4*>(h)[i];
     float* e = &v.x;
+    if (padded) {
+      const long long r = i / width4;
+      const int c0 = int(i - r * width4) * 4;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float y = act_fwd(e[j], act);
-      e[j] = drop_keep((unsigned long long)i * 4 + j, site.seed, site.thresh) ? y * site.scale : 0.0f;
+      for (int j = 0; j < 4; ++j) {
+        const float y = act_fwd(e[j], act);
+        const bool real = c0 + j < n;
+        e[j] = real && drop_keep((unsigned long long)r * n + c0 + j, site.seed, site.thresh) ? y * site.scale : 0.0f;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float y = act_fwd(e[j], act);
+        e[j] = drop_keep((unsigned long long)i * 4 + j, site.seed, site.thresh) ? y * site.scale : 0.0f;
+      }
     }
     reinterpret_cast<float4*>(h)[i] = v;
   }
 }
 
 // dz = mul * dh * m/(1-p) * act'(y)  with y = act(z) recovered from the stored h = m y/(1-p); colsum_out += column sums
-// of dz (the bias gradient of the linear that produced z).  dz may alias dh.
+// of dz (the bias gradient of the linear that produced z).  dz may alias dh.  n < width: a padded layer as in
+// act_fwd_kernel (dropout counter row * n + column; pad columns of dz +0).
 __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const float* __restrict__ h, float* dz,
                                                       long long rows, int width, int act, DropSite site, float mul,
                                                       int tx_n, int rows_per_block, float* __restrict__ colsum_out,
-                                                      const int* __restrict__ rows_dev) {
+                                                      const int* __restrict__ rows_dev, int n) {
   extern __shared__ float sh_cols[];     // [ty_n][width]: one row of column partials per row group
   site.seed = drop_seed(site);
   const int tx = threadIdx.x % tx_n, ty = threadIdx.x / tx_n, ty_n = blockDim.x / tx_n;
@@ -954,7 +980,9 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
       float* ge = &gv.x;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const bool keep = drop_keep((unsigned long long)at + j, site.seed, site.thresh);
+        const bool keep = n == width ? drop_keep((unsigned long long)at + j, site.seed, site.thresh)
+                                     : g * 4 + j < n && drop_keep((unsigned long long)r * n + g * 4 + j, site.seed,
+                                                                  site.thresh);
         const float y = he[j] * inv_scale;
         ge[j] = keep ? ge[j] * mul * site.scale * act_bwd(y, y, act) : 0.0f;   // ReLU: y > 0 <=> z > 0
       }
@@ -1153,24 +1181,35 @@ int zero_rows(const ZeroRegions& z, const int* plan, long long cap_rows, cudaStr
 
 int ln_forward(const float* x, const float* a, const float* b, float eps, long long rows, int width, float* y,
                float* mean, float* sd, cudaStream_t st, int torch_mode, void* y16, const int* rows_dev,
-               const int* rowmap_out) {
+               const int* rowmap_out, int n) {
   if (rowmap_out && y16) { arb_set_error("ln_forward: a row-mapped output is fp32 only"); return ARB_E_INVALID_ARG; }
   if (width % 4) { arb_set_error("LayerNorm width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
+  if (n < 0) n = width;
+  if (n > width || n <= width - 4 || (n != width && (rowmap_out || y16 || torch_mode))) {
+    arb_set_error("ln_forward: a padded row needs n <= width < n + 4, fp32 dense rows and the reference's norm");
+    return ARB_E_UNSUPPORTED;
+  }
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * ((y16 ? 6.0 : 8.0) * width + 8), st);
   return with_row_layout(width, [&](auto LPR, auto NJ, auto FILLED) {
     const int steps = r_fwd_steps(rows), per_block = ROWS_PER_BLOCK * (32 / LPR) * steps;
     const unsigned nblk = unsigned((rows + per_block - 1) / per_block);
-    return launch(rowmap_out ? ln_fwd_kernel<LPR, NJ, FILLED, true> : ln_fwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
+    return launch(n != width ? ln_fwd_kernel<LPR, NJ, false, false, true>
+                  : rowmap_out ? ln_fwd_kernel<LPR, NJ, FILLED, true> : ln_fwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
                   dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, x, a, b, eps, rows, width, y, mean, sd, torch_mode,
-                  static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out);
+                  static_cast<uint16_t*>(y16), rows_dev, steps, rowmap_out, n);
   });
 }
 
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
                 const float* dres, long long rows, int width, float* dx, float* grad_a, float* grad_b,
                 cudaStream_t st, float* dx_masked, DropSite site, float* colsum_out, int torch_mode,
-                const void* dy16_in, void* dy16_out, const int* rows_dev, const int* rowmap_in) {
+                const void* dy16_in, void* dy16_out, const int* rows_dev, const int* rowmap_in, int n) {
   if (rowmap_in && dy16_in) { arb_set_error("ln_backward: a row-mapped gradient is fp32 only"); return ARB_E_INVALID_ARG; }
+  if (n < 0) n = width;
+  if (n > width || n <= width - 4 || (n != width && (rowmap_in || dy16_in || dy16_out || torch_mode))) {
+    arb_set_error("ln_backward: a padded row needs n <= width < n + 4, fp32 dense rows and the reference's norm");
+    return ARB_E_UNSUPPORTED;
+  }
   if (site.thresh == 0 && site.scale == 1.0f) dx_masked = nullptr;
   if (dy16_out && dx_masked == nullptr && (site.thresh != 0 || site.scale != 1.0f)) {
     arb_set_error("ln_backward: a masked bf16 copy needs the masked fp32 buffer too"); return ARB_E_INVALID_ARG;
@@ -1182,10 +1221,11 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
     DetParts dp;
     dp.add(grad_a, nblk, 1, width, width); dp.add(grad_b, nblk, 1, width, width); dp.add(colsum_out, nblk, 1, width, width);
     if (int rc = dp.begin(st)) return rc;
-    if (int rc = launch(rowmap_in ? ln_bwd_kernel<LPR, NJ, FILLED, true> : ln_bwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
+    if (int rc = launch(n != width ? ln_bwd_kernel<LPR, NJ, false, false, true>
+                        : rowmap_in ? ln_bwd_kernel<LPR, NJ, FILLED, true> : ln_bwd_kernel<LPR, NJ, FILLED, false>, dim3(nblk),
                         dim3(ROWS_PER_BLOCK * 32), 0, st, /*pdl=*/true, dy, x, a, mean, sd, eps, dres, rows, width,
                         steps, dx, grad_a, grad_b, dx_masked, site, colsum_out, torch_mode,
-                        static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in))
+                        static_cast<const uint16_t*>(dy16_in), static_cast<uint16_t*>(dy16_out), rows_dev, rowmap_in, n))
       return rc;
     return dp.finish(st);
   });
@@ -1219,17 +1259,21 @@ int pos_backward(const float* dx, const long long* indices, const uint8_t* mask,
   return dp.finish(st);
 }
 
-int act_forward(float* h, long long rows, int width, int act, DropSite site, cudaStream_t st, const int* rows_dev) {
-  if (width % 4) { arb_set_error("activation: width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
+int act_forward(float* h, long long rows, int width, int act, DropSite site, cudaStream_t st, const int* rows_dev,
+                int n) {
+  if (n < 0) n = width;
+  if (width % 4 || n > width || n <= width - 4) { arb_set_error("activation: width must be a multiple of 4"); return ARB_E_UNSUPPORTED; }
   const long long n4 = rows * width / 4;
   ProfScope ps(ARB_PROF_SCORER_SIMT, live_rows(rows, rows_dev) * 8.0 * width, st);
   const unsigned blocks = unsigned(std::min<long long>((n4 + 255) / 256, 132 * 16));
-  return launch(act_fwd_kernel, dim3(blocks), dim3(256), 0, st, /*pdl=*/false, h, n4, act, site, rows_dev, width / 4);
+  return launch(act_fwd_kernel, dim3(blocks), dim3(256), 0, st, /*pdl=*/false, h, n4, act, site, rows_dev, width / 4,
+                n);
 }
 
 int act_backward(const float* dh, const float* h, float* dz, long long rows, int width, int act, DropSite site, float mul,
-                 float* colsum_out, cudaStream_t st, const int* rows_dev) {
-  if (width % 4 || width > 8192) { arb_set_error("activation: width must be a multiple of 4 and <= 8192"); return ARB_E_UNSUPPORTED; }
+                 float* colsum_out, cudaStream_t st, const int* rows_dev, int n) {
+  if (n < 0) n = width;
+  if (width % 4 || width > 8192 || n > width || n <= width - 4) { arb_set_error("activation: width must be a multiple of 4 and <= 8192"); return ARB_E_UNSUPPORTED; }
   int tx_n = 1;
   while (tx_n < width / 4 && tx_n < 256) tx_n *= 2;
   const int rpb = 64 * (256 / tx_n);
@@ -1239,7 +1283,7 @@ int act_backward(const float* dh, const float* h, float* dz, long long rows, int
   dp.add(colsum_out, blocks, 1, width, width);
   if (int rc = dp.begin(st)) return rc;
   if (int rc = launch(act_bwd_kernel, dim3(blocks), dim3(256), size_t(256 / tx_n) * width * 4, st, /*pdl=*/false, dh, h,
-                      dz, rows, width, act, site, mul, tx_n, rpb, colsum_out, rows_dev))
+                      dz, rows, width, act, site, mul, tx_n, rpb, colsum_out, rows_dev, n))
     return rc;
   return dp.finish(st);
 }

@@ -14,7 +14,9 @@ int ln_forward(const float* x, const float* a, const float* b, float eps, long l
                float* mean, float* sd, cudaStream_t st, int torch_mode = 0,
                void* y16 = nullptr,    // y16 != nullptr: write the output as bfloat16 there INSTEAD of y (bf16 mode)
                const int* rows_dev = nullptr,    // packed rows: device pointer to the live row count (<= rows)
-               const int* rowmap_out = nullptr); // packed rows: write row r to y[rowmap_out[r]] (< 0: not at all); fp32
+               const int* rowmap_out = nullptr,  // packed rows: write row r to y[rowmap_out[r]] (< 0: not at all); fp32
+               int n = -1);    // n < width: n real columns at the pitch width = round_up(n, 4), zero pads (DESIGN.md
+                               // 4.16): statistics over the real columns, +0 in the pads; fp32 dense rows only
 // dx = (dres ? dres : 0) + LayerNormBackward(dy); grad_a / grad_b (null: not computed) are accumulated
 int ln_backward(const float* dy, const float* x, const float* a, const float* mean, const float* sd, float eps,
                 const float* dres, long long rows, int width, float* dx, float* grad_a, float* grad_b,
@@ -24,7 +26,8 @@ int ln_backward(const float* dy, const float* x, const float* a, const float* me
                 const void* dy16_in = nullptr,  // bf16 mode: dy is read from this bfloat16 buffer instead
                 void* dy16_out = nullptr,       // bf16 mode: bfloat16 copy of the emitted (masked) gradient
                 const int* rows_dev = nullptr,
-                const int* rowmap_in = nullptr);  // packed rows: dy of row r is dy[rowmap_in[r]] (< 0: zero); fp32
+                const int* rowmap_in = nullptr,  // packed rows: dy of row r is dy[rowmap_in[r]] (< 0: zero); fp32
+                int n = -1);    // as in ln_forward; the pads of every output are +0, the dropout counter row * n + column
 int pos_forward(float* x, const long long* indices, const uint8_t* mask, const float* pe, int pe_rows, float scale,
                 long long rows, int width, cudaStream_t st);
 int pos_backward(const float* dx, const long long* indices, const uint8_t* mask, float* dpe, int pe_rows, long long rows,
@@ -33,10 +36,12 @@ int pos_backward(const float* dx, const long long* indices, const uint8_t* mask,
 // the backward then expects `prob` = the UNDROPPED probabilities and overwrites it with the dropped ones
 // FC-block activations (model.py:41-43): h <- dropout(act(h)) in place; backward: dz = mul * dh * mask/(1-p) * act'
 // from the stored output h, colsum_out[c] += column sums of dz.  act: ARB_ACT_*
+// n (default: width): the real width of a layer stored at the pitch width = round_up(n, 4) -- the dropout counter is
+// row * n + column and the pad columns are written +0 (DESIGN.md 4.16)
 int act_forward(float* h, long long rows, int width, int act, DropSite site, cudaStream_t st,
-                const int* rows_dev = nullptr);
+                const int* rows_dev = nullptr, int n = -1);
 int act_backward(const float* dh, const float* h, float* dz, long long rows, int width, int act, DropSite site, float mul,
-                 float* colsum_out, cudaStream_t st, const int* rows_dev = nullptr);
+                 float* colsum_out, cudaStream_t st, const int* rows_dev = nullptr, int n = -1);
 int softmax_forward(float* sc, const uint8_t* mask, int B, int h, int S, int pitch, cudaStream_t st,
                     DropSite site = DropSite{0u, 0u, 1.0f});
 int softmax_backward(float* dp, float* prob, long long rows, int S, int pitch, cudaStream_t st,
@@ -48,12 +53,13 @@ int slate_extents(const uint8_t* mask, const float* dscores, int n_out, int B, i
 // flat fp32 -> bfloat16 copy (the GEMM-operand shadow of the parameter buffer in bf16 mode); n multiple of 4
 int convert_to_bf16(const float* src, void* dst, long long n, cudaStream_t st);
 // The weight matrices inside the flat parameter buffer: FC layer i at fc_w[i] ([fc_out[i], fc_in[i]] row-major) and the
-// four of encoder layer l at enc0 + l * enc_stride + {0, o_wo, o_w1, o_w2} ([3d, d], [d, d], [f, d], [d, f]).
+// four of encoder layer l at enc0 + l * enc_stride + {0, o_wo, o_w1, o_w2} ([3d, d], [d, d], [fw, dw], [dw, fw]:
+// the feed-forward weights are stored zero-padded to dw = round_up(d, 4), fw = round_up(f, 4), DESIGN.md 4.16).
 struct WeightMats {
   int n_fc;
   long long fc_w[8];
   int fc_out[8], fc_in[8];
-  int n_layers, d, f;
+  int n_layers, d, f, dw, fw;
   long long enc0, enc_stride, o_wo, o_w1, o_w2;
 };
 // The GEMM-operand copy of the parameter buffer in TF32 mode, one launch: pr[i] = P[i] and, for every weight matrix
@@ -63,25 +69,26 @@ int tf32_weight_copy(const float* P, long long n, const WeightMats& m, int rnd, 
 // Padded heads (DESIGN.md 4.15): when the head width w = d / h is not a multiple of 4, every head of Q | K | V, the
 // context and their gradients takes hs = round_up(w, 4) columns, the last hs - w of them exact zeros, so that the
 // per-head tensor maps get a head stride of a multiple of 16 bytes.  The attention linears then read padded copies of
-// their weights, one block of size() floats per layer (dp = h * hs):
-//   wqkv [3 dp, d] (zero rows in the pads), wqkvt = wqkv^T [d, 3 dp], bqkv [3 dp], wo [d, dp] (zero columns in the
-//   pads), wot = wo^T [dp, d]
-// and write their weight and bias gradients to a padded block of gsize() floats: gwqkv [3 dp, d], gbqkv [3 dp],
-// gwo [d, dp].  Every offset is a multiple of 4 floats (16 bytes, as TMA needs).
+// their weights, one block of size() floats per layer (dp = h * hs; dw = round_up(d, 4), the residual stream's stored
+// width, DESIGN.md 4.16: a d_model that is not a multiple of 4 always has padded heads):
+//   wqkv [3 dp, dw] (zero rows in the head pads, zero columns from d on), wqkvt = wqkv^T [dw, 3 dp], bqkv [3 dp],
+//   wo [dw, dp] (zero columns in the head pads, zero rows from d on), wot = wo^T [dp, dw]
+// and write their weight and bias gradients to a padded block of gsize() floats: gwqkv [3 dp, dw], gbqkv [3 dp],
+// gwo [dw, dp].  Every offset is a multiple of 4 floats (16 bytes, as TMA needs).
 struct HeadPad {
-  int n_layers, d, h, w, hs;
+  int n_layers, d, h, w, hs, dw;
   long long enc0, enc_stride, o_bqkv, o_wo;   // flat parameters: layer l at enc0 + l * enc_stride; b_qkv, W_o inside it
   __host__ __device__ long long dp() const { return (long long)h * hs; }
   __host__ __device__ long long wqkv() const { return 0; }
-  __host__ __device__ long long wqkvt() const { return 3 * dp() * d; }
-  __host__ __device__ long long bqkv() const { return 6 * dp() * d; }
-  __host__ __device__ long long wo() const { return 6 * dp() * d + 3 * dp(); }
-  __host__ __device__ long long wot() const { return 7 * dp() * d + 3 * dp(); }
-  __host__ __device__ long long size() const { return 8 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long wqkvt() const { return 3 * dp() * dw; }
+  __host__ __device__ long long bqkv() const { return 6 * dp() * dw; }
+  __host__ __device__ long long wo() const { return 6 * dp() * dw + 3 * dp(); }
+  __host__ __device__ long long wot() const { return 7 * dp() * dw + 3 * dp(); }
+  __host__ __device__ long long size() const { return 8 * dp() * dw + 3 * dp(); }
   __host__ __device__ long long gwqkv() const { return 0; }
-  __host__ __device__ long long gbqkv() const { return 3 * dp() * d; }
-  __host__ __device__ long long gwo() const { return 3 * dp() * d + 3 * dp(); }
-  __host__ __device__ long long gsize() const { return 4 * dp() * d + 3 * dp(); }
+  __host__ __device__ long long gbqkv() const { return 3 * dp() * dw; }
+  __host__ __device__ long long gwo() const { return 3 * dp() * dw + 3 * dp(); }
+  __host__ __device__ long long gsize() const { return 4 * dp() * dw + 3 * dp(); }
 };
 // out[l * m.size() + ...] = the padded copies of every layer: weights from pr (the TF32 copy), the bias from P
 int head_pad_copy(const float* pr, const float* P, const HeadPad& m, float* out, cudaStream_t st);

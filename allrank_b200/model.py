@@ -41,6 +41,13 @@ Attention runs on the fused kernels at every head width d_model / h from 1 to 25
 width that is not a multiple of 4 (d_model 144 with h = 8: 18 columns) runs on heads padded with zero columns to the
 next multiple of 4 inside the CUDA scorer (DESIGN.md 4.15); the parameters and the state_dict keep the reference's
 shapes.
+Layers may have any width: FC sizes from 1 to 8192, d_model up to 1024 (d_model % h == 0), any d_ff.  A layer of n
+columns is stored in the flat buffer with round_up(n, 4) columns whose pads are exact zeros (FC and feed-forward
+weights as zero-padded [round_up(out, 4), round_up(in, 4)] blocks, biases, LayerNorm vectors and learned positional
+rows padded, the head's weight as [d_output, round_up(d_model, 4)]; the attention linears keep the reference's
+layout), and LayerNorm runs its statistics over the real columns; the parameters are views of the real part, so
+state_dict keys, shapes and the seeded initialisation are the reference's (DESIGN.md 4.16).  A fixed sinusoidal
+encoding at an odd d_model fails in its constructor, as the reference's does.
 Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes,
 attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU) and
 padded heads beyond 1024 columns in all (h * round_up(d_model / h, 4)); compute_dtype="bf16" at head widths other than
@@ -56,6 +63,11 @@ import torch.nn as nn
 from . import _lib
 
 _ACTS = {None: 0, "Tanh": 1, "Sigmoid": 2, "ReLU": 3}
+
+
+def _pad4(n):
+    """The stored width of a layer of n columns (csrc/scorer.cu: pad4)."""
+    return (int(n) + 3) // 4 * 4
 
 
 class ScorerConfig(ctypes.Structure):
@@ -328,39 +340,47 @@ class LTRModel(nn.Module):
 
     # ---- flat parameter storage -------------------------------------------------------------------
     def _ordered(self):
-        """(parameter, flat shape) in the C ABI's layout order (include/allrank_b200.h)."""
-        Fp = self._Fp
+        """(parameter, flat shape) in the C ABI's layout order (include/allrank_b200.h).  A flat shape other than the
+        parameter's own is its zero-padded block: FC weights are [pad4(out), pad4(in)] (layer 0: in = _Fp features)
+        and FC biases [pad4(out)]; the head's weight of an FC-only model is [d_output, pad4(d_model)]."""
         out = []
-        for i, lin in enumerate(self.input_layer.layers):   # layer 0's weight rows are padded to Fp features
-            out += [(lin.weight, (lin.out_features, Fp) if i == 0 else None), (lin.bias, None)]
+        for i, lin in enumerate(self.input_layer.layers):
+            pin = self._Fp if i == 0 else _pad4(lin.in_features)
+            out += [(lin.weight, (_pad4(lin.out_features), pin)), (lin.bias, (_pad4(lin.out_features),))]
         if self.input_norm_on:
             out += [(self.input_layer.input_norm.weight, None), (self.input_layer.input_norm.bias, None)]
         if self.encoder is not None:
             out += [(None, "align8")]      # the encoder section starts on a 32-byte boundary (include/allrank_b200.h)
         if self.encoder is not None:
+            dw, fw = _pad4(self.d_model), _pad4(self.d_ff)
             for lyr in self.encoder.layers:
                 lin = lyr.self_attn.linears
+                # the attention linears keep the reference's layout; from b_o on the widths are padded, starting on a
+                # 16-byte boundary
                 out += [(lin[0].weight, None), (lin[1].weight, None), (lin[2].weight, None),
                         (lin[0].bias, None), (lin[1].bias, None), (lin[2].bias, None),
-                        (lin[3].weight, None), (lin[3].bias, None),
-                        (lyr.feed_forward.w_1.weight, None), (lyr.feed_forward.w_1.bias, None),
-                        (lyr.feed_forward.w_2.weight, None), (lyr.feed_forward.w_2.bias, None),
-                        (lyr.sublayer[0].norm.a_2, None), (lyr.sublayer[0].norm.b_2, None),
-                        (lyr.sublayer[1].norm.a_2, None), (lyr.sublayer[1].norm.b_2, None)]
-            out += [(self.encoder.norm.a_2, None), (self.encoder.norm.b_2, None)]
-        out += [(self.output_layer.w_1.weight, None), (self.output_layer.w_1.bias, None)]
+                        (lin[3].weight, None), (None, "align4"), (lin[3].bias, (dw,)),
+                        (lyr.feed_forward.w_1.weight, (fw, dw)), (lyr.feed_forward.w_1.bias, (fw,)),
+                        (lyr.feed_forward.w_2.weight, (dw, fw)), (lyr.feed_forward.w_2.bias, (dw,)),
+                        (lyr.sublayer[0].norm.a_2, (dw,)), (lyr.sublayer[0].norm.b_2, (dw,)),
+                        (lyr.sublayer[1].norm.a_2, (dw,)), (lyr.sublayer[1].norm.b_2, (dw,))]
+            out += [(self.encoder.norm.a_2, (dw,)), (self.encoder.norm.b_2, (dw,))]
+        out += [(self.output_layer.w_1.weight, (self.d_output, _pad4(self.d_model))), (self.output_layer.w_1.bias, None)]
         if self.encoder is not None and isinstance(self.encoder.position, _LearnedPE):
-            out += [(self.encoder.position.pe.weight, "align4")]
+            out += [(None, "align4"), (self.encoder.position.pe.weight, (self.encoder.position.pe.weight.shape[0],
+                                                                         _pad4(self.d_model)))]
         return out
 
     def _view_of(self, flat, offset, p, flat_shape):
+        """The view of p's real part in its flat block (the leading corner of a zero-padded block) and the block's
+        length."""
         if flat_shape is None or tuple(flat_shape) == tuple(p.shape):
             return flat[offset:offset + p.numel()].view(p.shape), p.numel()
         n = 1
         for s in flat_shape:
             n *= s
         full = flat[offset:offset + n].view(flat_shape)
-        return full[..., :p.shape[-1]], n
+        return full[tuple(slice(0, s) for s in p.shape)], n
 
     def _pack(self, device):
         total = int(_lib.lib().arb_scorer_param_count(ctypes.byref(self._cfg)))
@@ -370,12 +390,10 @@ class LTRModel(nn.Module):
         grad = torch.zeros(total, dtype=torch.float32, device=device)
         views, off = [], 0
         for p, shape in self._ordered():
-            if shape == "align8":          # padding only
-                off = (off + 7) // 8 * 8
+            if shape in ("align4", "align8"):   # padding only
+                a = int(shape[-1])
+                off = (off + a - 1) // a * a
                 continue
-            if shape == "align4":          # the learned positional table starts on a 16-byte boundary
-                off = (off + 3) // 4 * 4
-                shape = None
             v, n = self._view_of(flat, off, p, shape)
             gv, _ = self._view_of(grad, off, p, shape)
             with torch.no_grad():
@@ -422,11 +440,15 @@ class LTRModel(nn.Module):
         pos = self.encoder.position if self.encoder is not None else None
         if not isinstance(pos, _FixedPE):
             return None
-        if pos.pe.device == device and pos.pe.dtype == torch.float32 and pos.pe.is_contiguous():
+        padded = _pad4(self.d_model) != self.d_model   # stored with zero pad columns like the activations (DESIGN.md 4.16)
+        if pos.pe.device == device and pos.pe.dtype == torch.float32 and pos.pe.is_contiguous() and not padded:
             return pos.pe
         cached = getattr(self, "_pe_dev", None)
         if cached is None or cached[0].device != device or cached[1] != pos.pe._version:
-            cached = (pos.pe.detach().to(device=device, dtype=torch.float32).contiguous(), pos.pe._version)
+            table = pos.pe.detach().to(device=device, dtype=torch.float32)
+            if padded:
+                table = torch.nn.functional.pad(table, (0, _pad4(self.d_model) - self.d_model))
+            cached = (table.contiguous(), pos.pe._version)
             self._pe_dev = cached
         return cached[0]
 

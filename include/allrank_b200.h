@@ -166,9 +166,12 @@ int32_t arb_neural_sort_debug(const float* y_pred, const float* y_true, int32_t 
  * (csrc/dropout.cuh); `seed` must be the same in the forward and the backward call of a step.
  *
  *  Parameters live in ONE flat fp32 buffer (the host layer makes the nn.Parameters views of it), laid out as
- *   per FC layer i: fc_w[s_i, s_{i-1}] fc_b[s_i] (s_{-1} = F) | in_norm_w[F] in_norm_b[F] if fc_input_norm |
- *   (pad to a multiple of 8 elements) | per layer: wq wk wv [3d,d] bq bk bv [3d] wo[d,d] bo[d] w1[dff,d] b1[dff] w2[d,dff] b2[d]
- *   ln1_a ln1_b ln2_a ln2_b [d each] | lnf_a lnf_b [d] head_w[d] head_b[1] (pad to 4) | pe[pe_rows,d] if pe_mode == 2
+ *   per FC layer i: fc_w[p(s_i), p(s_{i-1})] fc_b[p(s_i)] (s_{-1} = F; p(n) = round_up(n, 4), the last p(n) - n rows /
+ *   columns of each block zero) | in_norm_w[F] in_norm_b[F] if fc_input_norm |
+ *   (pad to a multiple of 8 elements) | per layer: wq wk wv [3d,d] bq bk bv [3d] wo[d,d] (pad to 4) bo[p(d)]
+ *   w1[p(dff),p(d)] b1[p(dff)] w2[p(d),p(dff)] b2[p(d)] ln1_a ln1_b ln2_a ln2_b [p(d) each] | lnf_a lnf_b [p(d)]
+ *   head_w[d_output, p(d)] head_b[d_output] (pad to 4) | pe[pe_rows,p(d)] if pe_mode == 2
+ *   (a fixed table, pe_mode == 1, is passed with p(d) columns too, zero pads)
  * (a fixed sinusoidal table, pe_mode == 1, is a buffer, not a parameter: it is passed separately as `pe_table`)
  * arb_scorer_param_count() gives the total; gradients use the same layout and are ACCUMULATED into `grads`.
  */
@@ -194,7 +197,8 @@ typedef struct arb_scorer_config {
                            > 1 (ordinal loss): scores are [B,S,d_output], head weight [d_output,d_model]           */
   /* --- ABI v3: the general FCModel input block (model.py:16-44): [nn.LayerNorm(F)] -> n x dropout(act(Linear)) */
   int32_t n_fc_layers;  /* len(fc_model.sizes), 1..ARB_MAX_FC_LAYERS; 0 = one layer of width d_model (v2 behaviour)  */
-  int32_t fc_sizes[8];  /* fc_model.sizes (multiples of 4, <= 8192); fc_sizes[n_fc_layers-1] must equal d_model       */
+  int32_t fc_sizes[8];  /* fc_model.sizes (1 ... 8192; stored padded to multiples of 4, see the parameter layout);
+                           fc_sizes[n_fc_layers-1] must equal d_model                                                */
   int32_t fc_act;       /* ARB_ACT_*: fc_model.activation applied after every FC linear, before its dropout          */
   int32_t fc_input_norm;/* fc_model.input_norm: nn.LayerNorm(n_features) (eps 1e-5, biased variance) on x first;
                            needs n_features % 4 == 0 (no feature padding)                                             */
