@@ -18,6 +18,8 @@ The callers either side of the path (SURVEY.md 8(f) ranks 3-4) are rebound the s
 allrank/rank_and_click.py imports make_model, CustomDataParallel, rank_slates, metrics_on_clicked_slates and
 click_on_slates by name (rank_and_click.py:11-18); those bindings are rebound too.
 """
+import functools
+
 from . import click_models as _click_models
 from . import data as _data
 from . import inference as _inference
@@ -62,10 +64,14 @@ def _import_rank_and_click():
         return False
 
 
-def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_clicks=False):
+def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_clicks=False, data_parser="sklearn"):
     """Rebind allrank.models.{losses,metrics}.<name> (and make_model, the epoch-metric helpers, rank_slates,
     metrics_on_clicked_slates and -- opt-in -- the slate loaders and click_on_slates) to the CUDA implementations.
+    data_parser: how the patched loaders read LibSVM files -- "sklearn" (the reference's parser on the host) or
+    "device" (the CUDA parser of allrank_b200.data, same arrays bit for bit).
     Returns the dict of original callables so the caller can restore them."""
+    if data_parser not in _data.PARSERS:
+        raise ValueError("data_parser must be one of {}, got {!r}".format(_data.PARSERS, data_parser))
     import allrank.models.losses as ref_losses
     import allrank.models.metrics as ref_metrics
     import allrank.models.model as ref_model
@@ -107,10 +113,15 @@ def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_cli
         if have_rac:
             _rebind(saved, "rank_and_click", "click_on_slates", _click_models.click_on_slates)
     if patch_data:
-        for name in ("load_libsvm_dataset", "load_libsvm_dataset_role", "load_libsvm_role", "create_data_loaders"):
-            _rebind(saved, "dataset_loading", name, getattr(_data, name))
+        loaders = {name: getattr(_data, name) for name in ("load_libsvm_dataset", "load_libsvm_dataset_role",
+                                                           "load_libsvm_role", "create_data_loaders")}
+        if data_parser != "sklearn":
+            for name in ("load_libsvm_dataset", "load_libsvm_dataset_role", "load_libsvm_role"):
+                loaders[name] = functools.partial(loaders[name], parser=data_parser)
+        for name, fn in loaders.items():
+            _rebind(saved, "dataset_loading", name, fn)
         try:
-            _rebind(saved, "main", "load_libsvm_dataset", _data.load_libsvm_dataset)
+            _rebind(saved, "main", "load_libsvm_dataset", loaders["load_libsvm_dataset"])
             _rebind(saved, "main", "create_data_loaders", _data.create_data_loaders)
         except Exception:
             pass

@@ -632,6 +632,58 @@ int32_t arb_click_slates(const arb_click_node* nodes_host, int32_t n_nodes, cons
                          float pad, int64_t slate_offset, uint64_t seed, float* clicks, int32_t* status,
                          void* workspace, size_t ws_bytes, void* stream);
 
+/* ---------------------------------------------------------------- LibSVM parsing (DESIGN.md section 11)
+ * Replaces sklearn.datasets.load_svmlight_file(f, query_id=True) + the densification of SlateStore
+ * (allrank/data/dataset_loading.py:100-107) with the file's bytes already in device memory.  The output is bit for
+ * bit what that path stores.  Grammar (libsvm_numeral.cuh states it in full): lines end at '\n'; a line is cut at its
+ * first '#'; tokens are separated by space \t \r \v \f; the first token is the label (Python float()); a second token
+ * that starts with "qid" is the query id (numpy.int64 of what follows its first ':'); every other token is
+ * index:value with index an int() that fits a C int and value a float().  A line without tokens is not a row.
+ * Limits: n_bytes >= 1 (64-bit offsets throughout, at most 2^31 - 1 chunks of 64 KB); the text pointer is 16-byte
+ * aligned; n_features <= ARB_LIBSVM_MAX_FEATURES = 2^31 (indices are C ints, so index INT32_MAX with a 0 index present
+ * gives the largest width).  A NUL byte before the first '#' of a line keeps the line uncut, as sklearn's strchr.
+ * Sequence (every step enqueues on `stream` and returns without synchronising):
+ *   1. arb_libsvm_count_lines: chunk_counts [arb_libsvm_chunks(n_bytes) + 1] int64 receives the exclusive scan of
+ *      the newlines per 64 KB chunk, and the total newline count in its last word.
+ *   2. arb_libsvm_index_lines: line_end [newlines] int64 receives each newline's byte position.  The text has
+ *      n_lines = newlines + (last byte != '\n') lines.
+ *   3. arb_libsvm_pass1: validates every line.  line_row [n_lines] int64 receives the row number of each line
+ *      (exclusive scan of "the line has tokens"), line_qid [n_lines] int64 each line's qid (0 without one), and
+ *      summary [8] int64: [0] (1-based line << 8) | ARB_LIBSVM_E_* of the first failing line, or -1; [1] the smallest
+ *      feature index (INT32_MAX without features); [2] the largest (-1 without); [3] the row count; [4] rows without
+ *      a qid.  The host reads the summary and refuses the file before step 4 when [0] != -1.
+ *   4. arb_libsvm_pass2: writes docs_x [n_rows, n_features] (every element), docs_y [n_rows] and qids [n_rows].
+ *      shift is 1 when [1] > 0 and a feature exists (sklearn's zero_based="auto"), else 0; n_features is
+ *      [2] - shift + 1, or 1 without features.
+ * Every entry point checks its arguments first and returns ARB_E_INVALID_ARG (or ARB_E_UNSUPPORTED for a text with
+ * more than 2^31 - 1 chunks) without a launch.  No allocation. */
+#define ARB_LIBSVM_E_LABEL 1           /* label: not a float()                        -> ValueError */
+#define ARB_LIBSVM_E_QID 2             /* qid token without ':' or not an int()       -> ValueError */
+#define ARB_LIBSVM_E_QID_OVERFLOW 3    /* qid outside int64                           -> OverflowError */
+#define ARB_LIBSVM_E_NO_COLON 4        /* feature token without ':'                   -> ValueError */
+#define ARB_LIBSVM_E_INDEX 5           /* index not an int()                          -> ValueError */
+#define ARB_LIBSVM_E_INDEX_OVERFLOW 6  /* index outside a C int                       -> OverflowError */
+#define ARB_LIBSVM_E_NEGATIVE 7        /* index < 0                                   -> ValueError */
+#define ARB_LIBSVM_E_NOT_SORTED 8      /* index <= the previous index of the line     -> ValueError */
+#define ARB_LIBSVM_E_VALUE 9           /* value not a float()                         -> ValueError */
+#define ARB_LIBSVM_E_UNSUPPORTED 10    /* value beyond the exact path's big integers (not reachable by the grammar) */
+int64_t arb_libsvm_chunks(int64_t n_bytes);
+int32_t arb_libsvm_count_lines(const uint8_t* text, int64_t n_bytes, int64_t* chunk_counts, void* stream);
+int32_t arb_libsvm_index_lines(const uint8_t* text, int64_t n_bytes, const int64_t* chunk_counts, int64_t* line_end,
+                               void* stream);
+int32_t arb_libsvm_pass1(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
+                         int64_t n_lines, int64_t* line_row, int64_t* line_qid, int64_t* summary, void* stream);
+#define ARB_LIBSVM_MAX_FEATURES 2147483648LL
+int32_t arb_libsvm_pass2(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
+                         int64_t n_lines, const int64_t* line_row, const int64_t* line_qid, int64_t n_rows,
+                         int32_t shift, int64_t n_features, float* docs_x, float* docs_y, int64_t* qids, void* stream);
+/* Host-side test hook: the numeral conversion of the kernels, run on the CPU over n tokens
+ * text_host[offsets_host[i], offsets_host[i + 1]).  kind 0: float() -> float64 bits; 1: float32(float(token)) bits
+ * (as the labels are stored); 2: int() into a C int; 3: numpy.int64().  status_host[i]: 0 ok, 1 refused (ValueError),
+ * 2 out of range (OverflowError).  Launches nothing. */
+int32_t arb_libsvm_parse_numerals_host(const uint8_t* text_host, const int64_t* offsets_host, int64_t n, int32_t kind,
+                                       uint64_t* out_host, int32_t* status_host);
+
 /* Per-launch device timing for bench.py's roofline: enable, run steps, collect per kernel class
  * (0 = tensor-core GEMM [work = flops], 1 = scorer SIMT, 2 = losses, 3 = metrics, 4 = optimiser, 5 = slate assembly /
  * gather [work = bytes]). */
