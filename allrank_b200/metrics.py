@@ -63,16 +63,40 @@ def _prep(y_pred, y_true):
     return y_pred.detach().float().contiguous(), y_true.detach().float().contiguous()
 
 
+def dcg_cutoffs(ats, S):
+    """The cut-offs the reference's dcg evaluates for `ats` on slates of S items (metrics.py:58-75), each in [1, S].
+
+    Every `at` is clipped to S.  The reference then keeps the first max(clipped) cumulative columns (a Python slice, so
+    a negative maximum keeps all but that many) and reads column `at - 1` of them, so a cut-off <= 0 counts from the
+    end: 0 is the last kept column, -1 the one before.  An index before the first column raises IndexError, and an
+    empty list ValueError (the reference's np.max), like the reference.
+    """
+    clipped = [min(int(a), S) for a in ats]
+    if not clipped:
+        raise ValueError("ats must name at least one cut-off")
+    kept = len(range(S)[:max(clipped)])
+    out = []
+    for a in clipped:
+        at = a if a > 0 else kept + a
+        if at < 1:
+            raise IndexError(f"cut-off {a} reads before the first of {kept} cumulative DCG columns")
+        out.append(at)
+    return out
+
+
 def _ats_array(ats):
+    if ats is None:
+        return None
     if len(ats) > 32:
         raise ValueError("at most 32 evaluation ranks per call")
     return (ctypes.c_int32 * len(ats))(*[int(a) for a in ats])
 
 
 def _launch(y_pred, y_true, ats_dcg, ats_mrr, gain_mode, pad, filler, want):
+    """ats_dcg: cut-offs in [1, S] (None when no DCG output is wanted); ats_mrr: raw cut-offs (None likewise)."""
     B, S = y_pred.shape
     dev = y_pred.device
-    n = len(ats_dcg)
+    n = len(ats_dcg if ats_dcg is not None else ats_mrr)
     outs = {k: torch.empty((B, n), dtype=torch.float32, device=dev) for k in want if k != "order"}
     if "order" in want:
         outs["order"] = torch.empty((B, S), dtype=torch.int32, device=dev)
@@ -95,19 +119,16 @@ def dcg(y_pred, y_true, ats=None, gain_function=pow2_gain, padding_indicator=PAD
     """Discounted Cumulative Gain at k -- metrics.py:41-77."""
     yp, yt = _prep(y_pred, y_true)
     S = yt.shape[1]
-    ats = [S] if ats is None else list(ats)
-    clipped = [min(int(a), S) for a in ats]
-    return _launch(yp, yt, clipped, clipped, _gain_mode(gain_function), padding_indicator, 0.0, ("dcg",))["dcg"]
+    cut = dcg_cutoffs([S] if ats is None else list(ats), S)
+    return _launch(yp, yt, cut, None, _gain_mode(gain_function), padding_indicator, 0.0, ("dcg",))["dcg"]
 
 
 def ndcg(y_pred, y_true, ats=None, gain_function=pow2_gain, padding_indicator=PADDED_Y_VALUE, filler_value=1.0):
     """Normalized DCG at k; slates whose ideal DCG is 0 get `filler_value` -- metrics.py:7-28."""
     yp, yt = _prep(y_pred, y_true)
     S = yt.shape[1]
-    ats = [S] if ats is None else list(ats)
-    clipped = [min(int(a), S) for a in ats]
-    return _launch(yp, yt, clipped, clipped, _gain_mode(gain_function), padding_indicator, filler_value,
-                   ("ndcg",))["ndcg"]
+    cut = dcg_cutoffs([S] if ats is None else list(ats), S)
+    return _launch(yp, yt, cut, None, _gain_mode(gain_function), padding_indicator, filler_value, ("ndcg",))["ndcg"]
 
 
 def mrr(y_pred, y_true, ats=None, padding_indicator=PADDED_Y_VALUE):
@@ -115,8 +136,7 @@ def mrr(y_pred, y_true, ats=None, padding_indicator=PADDED_Y_VALUE):
     yp, yt = _prep(y_pred, y_true)
     S = yt.shape[1]
     ats = [S] if ats is None else list(ats)
-    clipped = [min(int(a), S) for a in ats]
-    return _launch(yp, yt, clipped, [int(a) for a in ats], GAIN_POW2, padding_indicator, 0.0, ("mrr",))["mrr"]
+    return _launch(yp, yt, None, [int(a) for a in ats], GAIN_POW2, padding_indicator, 0.0, ("mrr",))["mrr"]
 
 
 def ranking(y_pred, y_true, padding_indicator=PADDED_Y_VALUE):
@@ -130,6 +150,5 @@ def all_metrics(y_pred, y_true, ats, padding_indicator=PADDED_Y_VALUE, filler_va
     """One launch for dcg + ndcg + mrr (what a fused eval step wants); returns a dict of [B,len(ats)] tensors."""
     yp, yt = _prep(y_pred, y_true)
     S = yt.shape[1]
-    clipped = [min(int(a), S) for a in ats]
-    return _launch(yp, yt, clipped, [int(a) for a in ats], GAIN_POW2, padding_indicator, filler_value,
+    return _launch(yp, yt, dcg_cutoffs(ats, S), [int(a) for a in ats], GAIN_POW2, padding_indicator, filler_value,
                    ("dcg", "idcg", "ndcg", "mrr"))
