@@ -135,7 +135,8 @@ static int make_param_layout(const arb_scorer_config& c, ParamLayout& L) {
     }
   }
   if (L.fc_size[L.n_fc - 1] != c.d_model) { arb_set_error("scorer: the last FC width must equal d_model"); return ARB_E_INVALID_ARG; }
-  if (c.fc_act < ARB_ACT_NONE || c.fc_act > ARB_ACT_RELU) { arb_set_error("scorer: unknown FC activation"); return ARB_E_UNSUPPORTED; }
+  if (!act_known(c.fc_act)) { arb_set_error("scorer: unknown FC activation"); return ARB_E_UNSUPPORTED; }
+  if (!act_known(c.out_act)) { arb_set_error("scorer: unknown output activation"); return ARB_E_UNSUPPORTED; }
   if (c.fc_input_norm && F > 1024) { arb_set_error("scorer: input_norm supports up to 1024 features"); return ARB_E_UNSUPPORTED; }
   int64_t o = 0;
   for (int i = 0; i < L.n_fc; ++i) {

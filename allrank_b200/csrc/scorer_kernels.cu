@@ -563,17 +563,48 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ i
 
 // ------------------------------------------------------------------------------------------------ head fwd
 // score = act( w . LN(x) + bias )  (final encoder LayerNorm fused; has_norm = 0 for FC-only models)
+// The activations (ARB_ACT_*) in torch's fp32 formulas at its default arguments (aten/src/ATen/native/cuda: the ELU
+// family with expm1, Softplus with log1p(exp(z)) up to its threshold, LogSigmoid as min(z, 0) - log1p(exp(-|z|)),
+// Hardsigmoid as clamp(z + 3, 0, 6) * (1 / 6)).
+constexpr float SELU_SCALE = 1.0507009873554805f;
+constexpr float SELU_NEG = 1.6732632423543772f * SELU_SCALE;   // alpha * lambda, multiplied in fp32 as torch does
 __device__ __forceinline__ float act_fwd(float z, int act) {
-  if (act == ARB_ACT_TANH) return tanhf(z);
-  if (act == ARB_ACT_SIGMOID) return 1.0f / (1.0f + expf(-z));
-  if (act == ARB_ACT_RELU) return fmaxf(z, 0.f);
-  return z;
+  switch (act) {
+    case ARB_ACT_TANH: return tanhf(z);
+    case ARB_ACT_SIGMOID: return 1.0f / (1.0f + expf(-z));
+    case ARB_ACT_RELU: return fmaxf(z, 0.f);
+    case ARB_ACT_LEAKY_RELU: return z > 0.f ? z : z * 0.01f;
+    case ARB_ACT_ELU: case ARB_ACT_CELU: return z > 0.f ? z : expm1f(z);
+    case ARB_ACT_SELU: return z > 0.f ? z * SELU_SCALE : expm1f(z) * SELU_NEG;
+    case ARB_ACT_SOFTPLUS: return z > 20.f ? z : log1pf(expf(z));
+    case ARB_ACT_SOFTSIGN: return z / (fabsf(z) + 1.0f);
+    case ARB_ACT_HARDTANH: return fminf(fmaxf(z, -1.f), 1.f);
+    case ARB_ACT_RELU6: return fminf(fmaxf(z, 0.f), 6.f);
+    case ARB_ACT_HARDSIGMOID: return fminf(fmaxf(z + 3.f, 0.f), 6.f) * (1.0f / 6.0f);
+    case ARB_ACT_LOGSIGMOID: return fminf(z, 0.f) - log1pf(expf(-fabsf(z)));
+    case ARB_ACT_HARDSHRINK: return z >= -0.5f && z <= 0.5f ? 0.f : z;
+    case ARB_ACT_SOFTSHRINK: return z > 0.5f ? z - 0.5f : (z < -0.5f ? z + 0.5f : 0.f);
+    default: return z;
+  }
 }
-__device__ __forceinline__ float act_bwd(float out, float z, int act) {
-  if (act == ARB_ACT_TANH) return 1.0f - out * out;
-  if (act == ARB_ACT_SIGMOID) return out * (1.0f - out);
-  if (act == ARB_ACT_RELU) return z > 0.f ? 1.0f : 0.0f;
-  return 1.0f;
+// act'(z) from the output y = act(z) (include/allrank_b200.h, ARB_ACT_*)
+__device__ __forceinline__ float act_bwd(float y, int act) {
+  switch (act) {
+    case ARB_ACT_TANH: return 1.0f - y * y;
+    case ARB_ACT_SIGMOID: return y * (1.0f - y);
+    case ARB_ACT_RELU: return y > 0.f ? 1.0f : 0.0f;   // y > 0 <=> z > 0
+    case ARB_ACT_LEAKY_RELU: return y > 0.f ? 1.0f : 0.01f;
+    case ARB_ACT_ELU: case ARB_ACT_CELU: return y > 0.f ? 1.0f : y + 1.0f;
+    case ARB_ACT_SELU: return y > 0.f ? SELU_SCALE : y + SELU_NEG;
+    case ARB_ACT_SOFTPLUS: return y > 20.f ? 1.0f : -expm1f(-y);   // sigmoid(z) = 1 - exp(-softplus(z))
+    case ARB_ACT_SOFTSIGN: { const float t = 1.0f - fabsf(y); return t * t; }
+    case ARB_ACT_HARDTANH: return y > -1.f && y < 1.f ? 1.0f : 0.0f;
+    case ARB_ACT_RELU6: return y > 0.f && y < 6.f ? 1.0f : 0.0f;
+    case ARB_ACT_HARDSIGMOID: return y > 0.f && y < 1.f ? 1.0f / 6.0f : 0.0f;
+    case ARB_ACT_LOGSIGMOID: return -expm1f(y);                    // sigmoid(-z) = 1 - exp(logsigmoid(z))
+    case ARB_ACT_HARDSHRINK: case ARB_ACT_SOFTSHRINK: return y != 0.f ? 1.0f : 0.0f;
+    default: return 1.0f;
+  }
 }
 
 template <int LPR, int NJ, bool FILLED>
@@ -696,9 +727,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32, NJ <= 4 ? 2 : 1) head_bwd
       if (has_norm) { mean = mean_i[row]; sd = std_i[row]; }
     }
     const float out = at >= 0 ? score[at] : 0.f;
-    float z = 0.f;
-    if (act == ARB_ACT_RELU) z = out;   // relu: out > 0 <=> z > 0
-    const float dz = at >= 0 ? dscore[at] * act_bwd(out, z, act) : 0.f;
+    const float dz = at >= 0 ? dscore[at] * act_bwd(out, act) : 0.f;
     if (lane % LPR == 0) acc_wb += dz;
     if (!has_norm) {
 #pragma unroll
@@ -824,7 +853,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
     r_zero(g);
     for (int j = 0; j < n; ++j) {
       const float out = score[row * n + j];
-      const float dz = dscore[row * n + j] * act_bwd(out, out, act);   // relu: out > 0 <=> z > 0
+      const float dz = dscore[row * n + j] * act_bwd(out, act);
       r_load<32>(w + (long long)j * width, width, lane, gw);
 #pragma unroll
       for (int k = 0; k < NV; ++k) {
@@ -849,7 +878,7 @@ __global__ void __launch_bounds__(ROWS_PER_BLOCK * 32) head_multi_bwd_kernel(
         const long long row = first + it;
         if (row >= rows) break;
         const float out = score[row * n + j];
-        const float dz = dscore[row * n + j] * act_bwd(out, out, act);
+        const float dz = dscore[row * n + j] * act_bwd(out, act);
         r_load<32>(xf + row * width, width, lane, gw);
         acc_b += dz;
 #pragma unroll
@@ -951,6 +980,18 @@ __global__ void __launch_bounds__(256) act_fwd_kernel(float* __restrict__ h, lon
   }
 }
 
+// act'(z) of a kept element from its stored h = fl(y * scale).  The round trip y = h * (1 / scale) can land a saturated
+// output (exactly 1 or 6) one ulp inside its bound, so the clamping activations compare h with fl(bound * scale),
+// the very product the forward stored for a saturated y; lower bounds at 0 are decided by sign.
+__device__ __forceinline__ float act_bwd_stored(float h, float inv_scale, float scale, int act) {
+  switch (act) {
+    case ARB_ACT_HARDTANH: return h > -scale && h < scale ? 1.0f : 0.0f;
+    case ARB_ACT_RELU6: return h > 0.f && h < 6.0f * scale ? 1.0f : 0.0f;
+    case ARB_ACT_HARDSIGMOID: return h > 0.f && h < scale ? 1.0f / 6.0f : 0.0f;
+    default: return act_bwd(h * inv_scale, act);
+  }
+}
+
 // dz = mul * dh * m/(1-p) * act'(y)  with y = act(z) recovered from the stored h = m y/(1-p); colsum_out += column sums
 // of dz (the bias gradient of the linear that produced z).  dz may alias dh.  n < width: a padded layer as in
 // act_fwd_kernel (dropout counter row * n + column; pad columns of dz +0).
@@ -983,8 +1024,7 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* dh, const flo
         const bool keep = n == width ? drop_keep((unsigned long long)at + j, site.seed, site.thresh)
                                      : g * 4 + j < n && drop_keep((unsigned long long)r * n + g * 4 + j, site.seed,
                                                                   site.thresh);
-        const float y = he[j] * inv_scale;
-        ge[j] = keep ? ge[j] * mul * site.scale * act_bwd(y, y, act) : 0.0f;   // ReLU: y > 0 <=> z > 0
+        ge[j] = keep ? ge[j] * mul * site.scale * act_bwd_stored(he[j], inv_scale, site.scale, act) : 0.0f;
       }
       *reinterpret_cast<float4*>(dz + at) = gv;
       acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
@@ -1460,7 +1500,7 @@ extern "C" int32_t arb_head_forward(const float* x, const float* a, const float*
                                     const float* wb, int32_t has_norm, int32_t act, int64_t rows, int32_t width,
                                     float* score, float* mean, float* sd, const int32_t* rows_dev,
                                     const int32_t* rowmap, void* stream) {
-  ARB_ROW_ARGS("arb_head_forward", x && w && wb && score && (!has_norm || (a && b)) && !mean == !sd, rows, width, 0.0f);
+  ARB_ROW_ARGS("arb_head_forward", act_known(act) && x && w && wb && score && (!has_norm || (a && b)) && !mean == !sd, rows, width, 0.0f);
   return head_forward(x, a, b, eps, w, wb, has_norm, act, rows, width, score, mean, sd,
                       static_cast<cudaStream_t>(stream), rows_dev, rowmap);
 }
@@ -1472,7 +1512,7 @@ extern "C" int32_t arb_head_backward(const float* dscore, const float* score, co
                                      void* dy16_out, float* colsum_out, float p, uint64_t seed, int32_t layer,
                                      int32_t site, const int32_t* rows_dev, const int32_t* rowmap, void* stream) {
   ARB_ROW_ARGS("arb_head_backward",
-               dscore && score && x && w && dx && (!has_norm || (a && b && mean && sd)),
+               act_known(act) && dscore && score && x && w && dx && (!has_norm || (a && b && mean && sd)),
                rows, width, p);
   return head_backward(dscore, score, x, a, b, mean, sd, eps, w, nullptr, has_norm, act, rows, width, dx, grad_a,
                        grad_b, grad_w, grad_wb, static_cast<cudaStream_t>(stream), dx_masked,
@@ -1481,7 +1521,7 @@ extern "C" int32_t arb_head_backward(const float* dscore, const float* score, co
 
 extern "C" int32_t arb_head_multi_forward(const float* xf, const float* w, const float* wb, int32_t act, int64_t rows,
                                           int32_t width, int32_t n, float* score, void* stream) {
-  ARB_ROW_ARGS("arb_head_multi_forward", xf && w && wb && score && n >= 1, rows, width, 0.0f);
+  ARB_ROW_ARGS("arb_head_multi_forward", act_known(act) && xf && w && wb && score && n >= 1, rows, width, 0.0f);
   return head_multi_forward(xf, w, wb, act, rows, width, n, score, static_cast<cudaStream_t>(stream));
 }
 
@@ -1490,7 +1530,7 @@ extern "C" int32_t arb_head_multi_backward(const float* dscore, const float* sco
                                            float* grad_w, float* grad_wb, float* dx_masked, float* colsum_out, float p,
                                            uint64_t seed, int32_t layer, int32_t site, void* stream) {
   ARB_ROW_ARGS("arb_head_multi_backward",
-               dscore && score && xf && w && dxf && n >= 1 && !grad_w == !grad_wb, rows, width, p);
+               act_known(act) && dscore && score && xf && w && dxf && n >= 1 && !grad_w == !grad_wb, rows, width, p);
   return head_multi_backward(dscore, score, xf, w, act, rows, width, n, dxf, grad_w, grad_wb,
                              static_cast<cudaStream_t>(stream), dx_masked, test_site(seed, layer, site, p), colsum_out);
 }
@@ -1526,7 +1566,7 @@ extern "C" int32_t arb_softmax_backward(float* dprob, float* prob, int64_t rows,
 // scorer's launchers.
 extern "C" int32_t arb_activation_forward(float* h, int64_t rows, int32_t width, int32_t act, float p, uint64_t seed,
                                           int32_t layer, const int32_t* rows_dev, void* stream) {
-  if (!h || rows < 0 || width <= 0 || act < ARB_ACT_NONE || act > ARB_ACT_RELU || !(p >= 0.0f && p < 1.0f)) {
+  if (!h || rows < 0 || width <= 0 || !act_known(act) || !(p >= 0.0f && p < 1.0f)) {
     arb_set_error("arb_activation_forward: null pointer or bad argument"); return ARB_E_INVALID_ARG;
   }
   if (rows == 0) return width % 4 ? ARB_E_UNSUPPORTED : ARB_OK;
@@ -1536,7 +1576,7 @@ extern "C" int32_t arb_activation_forward(float* h, int64_t rows, int32_t width,
 extern "C" int32_t arb_activation_backward(const float* dh, const float* h, float* dz, int64_t rows, int32_t width,
                                            int32_t act, float p, uint64_t seed, int32_t layer, float mul,
                                            float* colsum_out, const int32_t* rows_dev, void* stream) {
-  if (!dh || !h || !dz || dz == h || rows < 0 || width <= 0 || act < ARB_ACT_NONE || act > ARB_ACT_RELU ||
+  if (!dh || !h || !dz || dz == h || rows < 0 || width <= 0 || !act_known(act) ||
       !(p >= 0.0f && p < 1.0f)) {
     arb_set_error("arb_activation_backward: null pointer, dz aliasing h, or bad argument"); return ARB_E_INVALID_ARG;
   }

@@ -34,6 +34,10 @@ int pos_backward(const float* dx, const long long* indices, const uint8_t* mask,
                  int width, cudaStream_t st);
 // site.thresh != 0: inverted dropout on the probabilities (index ((b*h+head)*S+q)*S+key, as in the fused kernels);
 // the backward then expects `prob` = the UNDROPPED probabilities and overwrites it with the dropped ones
+// an ARB_ACT_* id the activation kernels implement
+inline bool act_known(int act) {
+  return (act >= ARB_ACT_NONE && act <= ARB_ACT_RELU) || (act >= ARB_ACT_LEAKY_RELU && act <= ARB_ACT_LAST);
+}
 // FC-block activations (model.py:41-43): h <- dropout(act(h)) in place; backward: dz = mul * dh * mask/(1-p) * act'
 // from the stored output h, colsum_out[c] += column sums of dz.  act: ARB_ACT_*
 // n (default: width): the real width of a layer stored at the pitch width = round_up(n, 4) -- the dropout counter is

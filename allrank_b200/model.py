@@ -30,7 +30,11 @@ padding row for padded items) are applied by a SIMT kernel after the input FC; t
 parameter buffer.
 
 The input block is the reference's general FCModel (model.py:16-44): optional nn.LayerNorm on the features, then any
-number of Linear layers each followed by the activation (None / ReLU / Tanh / Sigmoid) and dropout.  With
+number of Linear layers each followed by the activation and dropout.  The activation of the FC block and the output
+activation may be None or any of ReLU, Tanh, Sigmoid, LeakyReLU, ELU, CELU, SELU, Softplus, Softsign, Hardtanh, ReLU6,
+Hardsigmoid, LogSigmoid, Hardshrink and Softshrink at torch's default arguments: the classes of
+torch.nn.modules.activation without parameters whose derivative is a function of their output, which is all the
+backward keeps.  With
 `transformer=None` the model is that MLP plus the output head (the `*_mlp.json` configurations of the paper).
 Autograd reaches `x` as well as the parameters: x.grad (in x's dtype and shape) comes from the CUDA backward, which
 then also runs the first FC layer's input-gradient product; with every parameter frozen it computes no parameter
@@ -48,7 +52,9 @@ rows padded, the head's weight as [d_output, round_up(d_model, 4)]; the attentio
 layout), and LayerNorm runs its statistics over the real columns; the parameters are views of the real part, so
 state_dict keys, shapes and the seeded initialisation are the reference's (DESIGN.md 4.16).  A fixed sinusoidal
 encoding at an odd d_model fails in its constructor, as the reference's does.
-Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes,
+Not supported (raise NotImplementedError rather than fall back): `fc_model=None`, other activation classes (GELU,
+SiLU, Mish, Hardswish and Tanhshrink need the pre-activation in the backward, PReLU has a weight, RReLU a random slope,
+GLU and the softmax family are not elementwise),
 attention heads wider than 256 columns (d_model / h; raised when the parameters are first packed on the GPU) and
 padded heads beyond 1024 columns in all (h * round_up(d_model / h, 4)); compute_dtype="bf16" at head widths other than
 8, 16, 24 and 32.
@@ -62,7 +68,15 @@ import torch.nn as nn
 
 from . import _lib
 
-_ACTS = {None: 0, "Tanh": 1, "Sigmoid": 2, "ReLU": 3}
+# torch.nn.modules.activation class name -> ARB_ACT_* (include/allrank_b200.h): the parameter-free elementwise
+# activations whose derivative follows from their output, at torch's default arguments (the reference builds them by
+# name with none).  Id 4 is not assigned.
+_ACTS = {None: 0, "Tanh": 1, "Sigmoid": 2, "ReLU": 3, "LeakyReLU": 5, "ELU": 6, "CELU": 7, "SELU": 8, "Softplus": 9,
+         "Softsign": 10, "Hardtanh": 11, "ReLU6": 12, "Hardsigmoid": 13, "LogSigmoid": 14, "Hardshrink": 15,
+         "Softshrink": 16}
+_ACTS_REFUSED = ("the kernels take an activation's derivative from its output, so classes whose derivative needs the "
+                 "pre-activation (GELU, SiLU, Mish, Hardswish, Tanhshrink), learned or random ones (PReLU, RReLU) and "
+                 "non-elementwise ones (GLU, Softmax, ...) are not implemented")
 
 
 def _pad4(n):
@@ -264,7 +278,8 @@ class LTRModel(nn.Module):
         if not 1 <= len(fc_sizes) <= 8:
             raise NotImplementedError("fc_model.sizes must list 1 to 8 layers")
         if fc_activation not in _ACTS:
-            raise NotImplementedError(f"fc_model.activation {fc_activation!r}: supported {sorted(map(str, _ACTS))}")
+            raise NotImplementedError(f"fc_model.activation {fc_activation!r}: supported {sorted(map(str, _ACTS))}; "
+                                      f"{_ACTS_REFUSED}")
         if input_norm and n_features % 4:
             raise NotImplementedError("fc_model.input_norm needs n_features % 4 == 0 (no feature padding under the norm)")
         self.fc_sizes, self.fc_activation, self.input_norm_on = fc_sizes, fc_activation, bool(input_norm)
@@ -272,7 +287,8 @@ class LTRModel(nn.Module):
         if not 1 <= self.d_output <= 64:
             raise NotImplementedError("d_output must be in [1, 64]")
         if output_activation not in _ACTS:
-            raise NotImplementedError(f"output activation {output_activation!r}: supported {sorted(map(str, _ACTS))}")
+            raise NotImplementedError(f"output activation {output_activation!r}: supported {sorted(map(str, _ACTS))}; "
+                                      f"{_ACTS_REFUSED}")
         self.n_features, self.d_model, self.n_layers = int(n_features), int(d_model), int(n_layers)
         self.n_heads, self.d_ff, self.dropout_p = int(n_heads), int(d_ff), float(dropout or 0.0)
         self.fc_dropout_p = float(fc_dropout or 0.0)

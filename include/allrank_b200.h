@@ -175,10 +175,32 @@ int32_t arb_neural_sort_debug(const float* y_pred, const float* y_true, int32_t 
  * (a fixed sinusoidal table, pe_mode == 1, is a buffer, not a parameter: it is passed separately as `pe_table`)
  * arb_scorer_param_count() gives the total; gradients use the same layout and are ACCUMULATED into `grads`.
  */
+/* Activations: the parameter-free elementwise classes of torch.nn.modules.activation whose derivative is a function of
+ * their output, each at torch's default constructor arguments (allRank builds them by name without arguments).  The
+ * backward computes act'(z) from the stored output y = act(z) -- no pre-activation is kept:
+ *   None 1 | Tanh 1 - y^2 | Sigmoid y (1 - y) | ReLU [y > 0] | LeakyReLU (slope 0.01) y > 0 ? 1 : 0.01 |
+ *   ELU, CELU (alpha 1) y > 0 ? 1 : y + 1 | SELU y > 0 ? lambda : y + lambda alpha |
+ *   Softplus (beta 1, threshold 20) y > 20 ? 1 : -expm1(-y) | Softsign (1 - |y|)^2 | Hardtanh [-1 < y < 1] |
+ *   ReLU6 [0 < y < 6] | Hardsigmoid [0 < y < 1] / 6 | LogSigmoid -expm1(y) | Hardshrink, Softshrink (0.5) [y != 0].
+ * At the kinks these give torch's backward conventions (elu_backward, hardtanh_backward, softplus_backward, ...).
+ * Id 4 is not assigned: it stays an unknown id, refused like any id above ARB_ACT_LAST. */
 #define ARB_ACT_NONE 0
 #define ARB_ACT_TANH 1
 #define ARB_ACT_SIGMOID 2
 #define ARB_ACT_RELU 3
+#define ARB_ACT_LEAKY_RELU 5
+#define ARB_ACT_ELU 6
+#define ARB_ACT_CELU 7
+#define ARB_ACT_SELU 8
+#define ARB_ACT_SOFTPLUS 9
+#define ARB_ACT_SOFTSIGN 10
+#define ARB_ACT_HARDTANH 11
+#define ARB_ACT_RELU6 12
+#define ARB_ACT_HARDSIGMOID 13
+#define ARB_ACT_LOGSIGMOID 14
+#define ARB_ACT_HARDSHRINK 15
+#define ARB_ACT_SOFTSHRINK 16
+#define ARB_ACT_LAST ARB_ACT_SOFTSHRINK
 
 typedef struct arb_scorer_config {
   int32_t n_features;   /* F (row pitch of x; must be a multiple of 4 -- the host layer pads)            */
@@ -186,7 +208,8 @@ typedef struct arb_scorer_config {
   int32_t n_layers;     /* transformer N; 0 = FC-only model (no encoder, no final LayerNorm)              */
   int32_t n_heads;      /* h                                                                             */
   int32_t d_ff;         /* PositionwiseFeedForward hidden width                                           */
-  int32_t out_act;      /* ARB_ACT_*: post_model.output_activation (model.py:105-107)                     */
+  int32_t out_act;      /* ARB_ACT_*: post_model.output_activation (model.py:105-107); its derivative is taken from
+                           the stored scores                                                                  */
   float ln_eps;         /* 1e-6 (transformer.py:63)                                                       */
   float dropout;        /* transformer.dropout: on attention probabilities, both sublayer outputs and the FFN
                            hidden layer (transformer.py:105,155,227); applied only when training != 0          */
@@ -199,7 +222,8 @@ typedef struct arb_scorer_config {
   int32_t n_fc_layers;  /* len(fc_model.sizes), 1..ARB_MAX_FC_LAYERS; 0 = one layer of width d_model (v2 behaviour)  */
   int32_t fc_sizes[8];  /* fc_model.sizes (1 ... 8192; stored padded to multiples of 4, see the parameter layout);
                            fc_sizes[n_fc_layers-1] must equal d_model                                                */
-  int32_t fc_act;       /* ARB_ACT_*: fc_model.activation applied after every FC linear, before its dropout          */
+  int32_t fc_act;       /* ARB_ACT_*: fc_model.activation applied after every FC linear, before its dropout; its
+                           derivative is taken from the stored (dropped, scaled) layer output                        */
   int32_t fc_input_norm;/* fc_model.input_norm: nn.LayerNorm(n_features) (eps 1e-5, biased variance) on x first;
                            needs n_features % 4 == 0 (no feature padding)                                             */
   int32_t bf16;         /* 1: bf16 mode of the encoder (BASELINE config 3): every encoder linear runs as a tensor-core
@@ -450,7 +474,8 @@ int32_t arb_ffn_backward_input(const float* dy, const float* w2t, const float* w
  *   - torch_mode: nn.LayerNorm (biased variance, eps under the root); sd receives sqrt(var + eps), and the backward is
  *     then called with eps = 0 as the scorer calls it.  Otherwise the reference's LayerNorm (unbiased std, eps added to
  *     the std).  A row with sd = 0 (a constant row) gets y = b, and in the backward the std term of dx is 0.
- *   - act: ARB_ACT_*; has_norm = 0 is the FC-only head score = act(w . x + wb[0]).
+ *   - act: ARB_ACT_* (an unknown id is ARB_E_INVALID_ARG); has_norm = 0 is the FC-only head score =
+ *     act(w . x + wb[0]).  The backward reads act'(z) off the stored score (see ARB_ACT_*).
  *   - the multi-output head: score [rows, n] = act(xf w^T + wb), w [n, width]; grad_w and grad_wb both or neither.
  * Softmax: in place on scores [B, h, S] rows of `pitch` >= S floats (S <= 1536, else ARB_E_UNSUPPORTED), keys with
  * mask [B, S] = 1 get probability 0, an all-masked slate gets NaN rows.  Dropout on the probabilities with the
@@ -491,9 +516,11 @@ int32_t arb_softmax_backward(float* dprob, float* prob, int64_t rows, int32_t S,
  *   activation forward: h [rows, width] <- dropout(act(h)) in place, act ARB_ACT_*, width a multiple of 4; dropout
  *     with rate p at the FC site of `layer` under `seed`, element counter row * width + column, kept values times
  *     1 / (1 - p), dropped ones +0.
- *   activation backward: dz = ((dh * mul) * scale) * act'(h / scale) where kept, else 0 (scale = 1 / (1 - p), h the
- *     stored forward output); dz may alias dh but not h; width a multiple of 4 up to 8192 (else ARB_E_UNSUPPORTED);
- *     colsum_out (nullable) += the column sums of dz.
+ *   activation backward: dz = ((dh * mul) * scale) * act'(h * (1 / scale)) where kept, else 0 (scale = 1 / (1 - p),
+ *     h the stored forward output, act' from the output as listed at ARB_ACT_*); Hardtanh, ReLU6 and Hardsigmoid
+ *     instead decide saturation on h itself, against bound * scale (the product the forward stored for a saturated
+ *     output), so every saturated element gets exactly 0; dz may alias dh but not h; width a multiple of 4 up to 8192
+ *     (else ARB_E_UNSUPPORTED); colsum_out (nullable) += the column sums of dz.
  *   rows_dev (nullable, device int32): rows at or beyond *rows_dev are neither read nor written.
  *   positional forward: x [rows, width] = scale * x + pe[idx] with idx = the last table row (the padding row) for a
  *     masked row, else indices[row] with values above the last row clamped to it, -pe_rows ... -1 counted from the
