@@ -11,7 +11,8 @@
 //                           kernel's out_order).
 //
 // Sampling uses a counter-based hash (seed, slate, attempt, item) instead of numpy's Mersenne stream, so sampled
-// slates agree with the reference in distribution; padded slates are bit-identical.
+// slates agree with the reference in distribution; padded slates are bit-identical.  oracle/slates_ref.py restates
+// the hash on the host (HashSource) and drives the reference's _sample rules with it: every slate equals that model.
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -22,7 +23,8 @@
 namespace arb {
 
 constexpr int ASM_THREADS = 256;
-constexpr int ASM_MAX_ATTEMPTS = 1024;   // the reference recurses without bound (dataset_loading.py:69-70)
+constexpr int ASM_MAX_ATTEMPTS = 1024;   // the reference recurses without bound (dataset_loading.py:69-70); the
+                                         // 1024th draw is kept even if it holds no relevant item
 
 __device__ __forceinline__ uint32_t sample_hash(uint64_t seed, uint32_t slate, uint32_t attempt, uint32_t item) {
   uint32_t h = mix32(uint32_t(seed) ^ (slate * 0x9e3779b1u));
@@ -76,18 +78,22 @@ __global__ void __launch_bounds__(ASM_THREADS) assemble_slates_kernel(
       float got = 0.f;
       for (int r = threadIdx.x; r < S; r += blockDim.x) got += y[uint32_t(keys[r])];
       got = block_sum(got, red);
-      if (got != 0.f || tot == 0.f || attempt + 1 >= ASM_MAX_ATTEMPTS) break;   // has a relevant item / none exists
-      if (tot == 1.0f) break;             // single relevant item: patched in below (:66-68)
-      __syncthreads();                    // tot > 0: draw again (:69-70)
+      // draw again only while the sample sums to 0 and the query to more than 0 but not 1 (:69-70); a query sum
+      // of 0, below 0 or NaN keeps the sample, a sum of 1 is patched below (:66-68)
+      if (!(got == 0.f && tot > 0.f && tot != 1.0f) || attempt + 1 >= ASM_MAX_ATTEMPTS) break;
+      __syncthreads();
     }
     float got = 0.f;
     for (int r = threadIdx.x; r < S; r += blockDim.x) { sel[r] = int(uint32_t(keys[r])); got += y[sel[r]]; }
     got = block_sum(got, red);
-    if (got == 0.f && tot == 1.0f) {      // keep S-1 of the sample, append the relevant item (np.argmax: first maximum)
+    if (got == 0.f && tot == 1.0f) {      // keep S-1 of the sample, append np.argmax(y): the first maximum
+      float m = -CUDART_INF_F;
+      for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, y[i]);
+      m = block_max(m, red);
       if (threadIdx.x == 0) s_first_max = n;
       __syncthreads();
       for (int i = threadIdx.x; i < n; i += blockDim.x)
-        if (y[i] > 0.f) atomicMin(&s_first_max, i);
+        if (y[i] == m) atomicMin(&s_first_max, i);
       __syncthreads();
       if (threadIdx.x == 0) sel[S - 1] = s_first_max;
     }
