@@ -17,13 +17,13 @@
 
 #include "common.h"
 #include "libsvm_numeral.cuh"
+#include "libsvm_scan.cuh"
 
 namespace arb {
 
 constexpr int LF_CHUNK = 1 << 16;       // bytes per block of the newline kernels
 constexpr int LF_THREADS = 256;         // x 16 bytes = 4 KB per block step
 constexpr int SVM_WARPS = 8;            // warps per block of the line kernels
-constexpr int SCAN_THREADS = 1024;
 
 // summary words (int64) of pass 1
 enum { SUM_ERROR = 0, SUM_MIN_INDEX = 1, SUM_MAX_INDEX = 2, SUM_ROWS = 3, SUM_NO_QID = 4, SUM_WORDS = 8 };
@@ -95,32 +95,6 @@ __global__ void __launch_bounds__(LF_THREADS) lf_write_kernel(const uint8_t* __r
     base += total;
     __syncthreads();
   }
-}
-
-// In-place exclusive scan of a[0, n) by one block; *total = the sum.
-__global__ void __launch_bounds__(SCAN_THREADS) exclusive_scan_kernel(long long* __restrict__ a, long long n,
-                                                                      long long* __restrict__ total) {
-  __shared__ long long warp_tot[SCAN_THREADS / 32];
-  const long long seg = (n + SCAN_THREADS - 1) / SCAN_THREADS;
-  const long long lo = threadIdx.x * seg, hi = lo + seg < n ? lo + seg : n;
-  long long s = 0;
-  for (long long i = lo; i < hi; ++i) s += a[i];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long incl = s;
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) warp_tot[wid] = incl;
-  __syncthreads();
-  long long run = incl - s;
-  for (int w = 0; w < wid; ++w) run += warp_tot[w];
-  for (long long i = lo; i < hi; ++i) {
-    const long long v = a[i];
-    a[i] = run;
-    run += v;
-  }
-  if (threadIdx.x == SCAN_THREADS - 1) *total = run;
 }
 
 // What one line holds (pass 1) -- or, in pass 2, the writes it makes.

@@ -255,7 +255,8 @@ __host__ __device__ __forceinline__ int cmp_halfway(const uint8_t* s, const Deci
 }
 
 // exact rounding starting from the candidate bit pattern b (magnitude); returns the correctly rounded pattern
-__host__ __device__ ARB_SVM_NOINLINE uint64_t exact_round(const uint8_t* s, const Decimal& dec, uint64_t b, bool* bad) {
+static __host__ __device__ ARB_SVM_NOINLINE uint64_t exact_round(const uint8_t* s, const Decimal& dec, uint64_t b,
+                                                                 bool* bad) {
   for (int iter = 0; iter < 64; ++iter) {
     uint64_t H;
     int64_t F;

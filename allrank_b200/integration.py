@@ -15,8 +15,10 @@ The callers either side of the path (SURVEY.md 8(f) ranks 3-4) are rebound the s
     click metrics : allrank.inference.inference_utils.metrics_on_clicked_slates                inference_utils.py:63-82
     clicks        : allrank.click_models.click_utils.click_on_slates -- opt-in (`patch_clicks=True`): random
                     click models then draw from a counter hash instead of numpy's stream.
-allrank/rank_and_click.py imports make_model, CustomDataParallel, rank_slates, metrics_on_clicked_slates and
-click_on_slates by name (rank_and_click.py:11-18); those bindings are rebound too.
+    LibSVM saving : allrank.data.dataset_saving.write_to_libsvm_without_masked -- opt-in (`patch_write=True`): the
+                    click-through files are formatted on the device, byte for byte what sklearn writes.
+allrank/rank_and_click.py imports make_model, CustomDataParallel, rank_slates, metrics_on_clicked_slates,
+click_on_slates and write_to_libsvm_without_masked by name (rank_and_click.py:11-18); those bindings are rebound too.
 """
 import functools
 
@@ -27,6 +29,7 @@ from . import losses as _losses
 from . import metrics as _metrics
 from . import model as _model
 from . import training as _training
+from . import writer as _writer
 
 LOSS_NAMES = ("listNet", "listMLE", "approxNDCGLoss", "lambdaLoss", "neuralNDCG", "neuralNDCG_transposed", "rankNet",
               "rankNet_weightByGTDiff", "rankNet_weightByGTDiff_pow", "binary_listNet", "pointwise_rmse", "bce",
@@ -37,7 +40,8 @@ METRIC_NAMES = ("ndcg", "dcg", "mrr")
 _MODULES = {"losses": "allrank.models.losses", "metrics": "allrank.models.metrics", "model": "allrank.models.model",
             "main": "allrank.main", "train_utils": "allrank.training.train_utils",
             "inference_utils": "allrank.inference.inference_utils", "dataset_loading": "allrank.data.dataset_loading",
-            "rank_and_click": "allrank.rank_and_click", "click_utils": "allrank.click_models.click_utils"}
+            "rank_and_click": "allrank.rank_and_click", "click_utils": "allrank.click_models.click_utils",
+            "dataset_saving": "allrank.data.dataset_saving"}
 
 
 def single_process_model(model):
@@ -64,9 +68,11 @@ def _import_rank_and_click():
         return False
 
 
-def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_clicks=False, data_parser="sklearn"):
+def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_clicks=False, data_parser="sklearn",
+                  patch_write=False):
     """Rebind allrank.models.{losses,metrics}.<name> (and make_model, the epoch-metric helpers, rank_slates,
-    metrics_on_clicked_slates and -- opt-in -- the slate loaders and click_on_slates) to the CUDA implementations.
+    metrics_on_clicked_slates and -- opt-in -- the slate loaders, click_on_slates and write_to_libsvm_without_masked)
+    to the CUDA implementations.
     data_parser: how the patched loaders read LibSVM files -- "sklearn" (the reference's parser on the host) or
     "device" (the CUDA parser of allrank_b200.data, same arrays bit for bit).
     Returns the dict of original callables so the caller can restore them."""
@@ -112,6 +118,10 @@ def patch_allrank(patch_model=True, patch_eval=True, patch_data=False, patch_cli
         _rebind(saved, "click_utils", "click_on_slates", _click_models.click_on_slates)
         if have_rac:
             _rebind(saved, "rank_and_click", "click_on_slates", _click_models.click_on_slates)
+    if patch_write:
+        _rebind(saved, "dataset_saving", "write_to_libsvm_without_masked", _writer.write_to_libsvm_without_masked)
+        if have_rac:
+            _rebind(saved, "rank_and_click", "write_to_libsvm_without_masked", _writer.write_to_libsvm_without_masked)
     if patch_data:
         loaders = {name: getattr(_data, name) for name in ("load_libsvm_dataset", "load_libsvm_dataset_role",
                                                            "load_libsvm_role", "create_data_loaders")}

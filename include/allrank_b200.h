@@ -724,6 +724,31 @@ double arb_prof_last_bytes(int32_t cls);
  * cap - 1 bytes + NUL into buf and returns the count; buf == NULL returns the size needed. */
 int64_t arb_prof_report(char* buf, int64_t cap);
 
+/* ---------------------------------------------------------------- LibSVM writing (DESIGN.md section 12)
+ * The bytes sklearn.datasets.dump_svmlight_file(X, y, f, zero_based, query_id) writes for a dense X [rows, F]:
+ * per row  label[ qid:Q] j:v ...\n  with one space after the label (or qid) even without tokens; a token for every
+ * x != 0 (-0.0 is skipped), j = column + one_based.  Values and float labels are Python's "%.16g" of the value widened
+ * to double, int64 values, labels and qids "%d".  Dtypes: X ARB_SVMW_F32 / F64 / I64, y ARB_SVMW_F64 / I64.
+ *   arb_svm_write_check: *bad (int32, device) = 1 when X [n_x] or y [n_y] holds a NaN or +-inf, else 0.
+ *   arb_svm_write_chunk with text == NULL: offsets [r1 - r0 + 1] int64 receives each row's byte offset inside the
+ *     chunk of rows [r0, r1) and the chunk's byte total in its last word; with text: writes the chunk's bytes at those
+ *     offsets (the caller sizes text from the total, or from the worst case: 24 bytes per value, the index, 24 for
+ *     the label, 25 for the qid and 2).  Run the first call before the second on the same offsets.
+ * qid [rows] int64 may be NULL (no qid column).  Nothing synchronises; no allocation; every entry point checks its
+ * arguments first and returns ARB_E_INVALID_ARG without a launch. */
+#define ARB_SVMW_F32 0
+#define ARB_SVMW_F64 1
+#define ARB_SVMW_I64 2
+int32_t arb_svm_write_check(const void* X, int32_t x_kind, int64_t n_x, const void* y, int32_t y_kind, int64_t n_y,
+                            int32_t* bad, void* stream);
+int32_t arb_svm_write_chunk(const void* X, int32_t x_kind, int64_t n_features, const void* y, int32_t y_kind,
+                            const int64_t* qid, int32_t one_based, int64_t r0, int64_t r1, int64_t* offsets,
+                            uint8_t* text, void* stream);
+/* Test entry points: Python's "%.16g" % values[i] into the 24-byte slot slots[24 i], NUL-padded.  arb_format_g16
+ * takes device pointers and enqueues one launch (n >= 1); arb_format_g16_host runs the same code on the CPU. */
+int32_t arb_format_g16(const double* values, int64_t n, char* slots, void* stream);
+int32_t arb_format_g16_host(const double* values, int64_t n, char* slots);
+
 #ifdef __cplusplus
 }
 #endif
