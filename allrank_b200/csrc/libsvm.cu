@@ -8,11 +8,13 @@
 //                                       (min / max / add: the same result in any order).  The row flags are then
 //                                       scanned into row numbers.
 //   pass2_kernel                        one warp per row line: writes the whole dense row docs_x[r, :] (zeros first,
-//                                       then the values), docs_y[r] and the row's qid.
+//                                       then the values), docs_y[r] and the row's qid; float32 as SlateStore keeps
+//                                       them, or float64 as load_svmlight_file(...).toarray() returns them.
 // Lines are split at '\n' only, as Python iterates over a binary file; a line is cut at its first '#' unless a NUL
 // byte comes before it (sklearn's strchr stops there); tokens are
 // separated by ASCII whitespace (space \t \r \v \f), as bytes.split() does.  A line with no token is not a row.
 #include <cstdint>
+#include <cstdio>
 #include <cuda_runtime.h>
 
 #include "common.h"
@@ -111,11 +113,22 @@ __device__ __forceinline__ long long token_end(const uint8_t* text, long long t,
   return t;
 }
 
+// What pass 2 stores for a numeral: float32 as SlateStore keeps it (sklearn_f32_bits), or float64 as
+// load_svmlight_file(...).toarray() gives it -- float(token), with a feature's -0.0 added into the zeroed array (+0.0).
+__device__ __forceinline__ void store_feature(float* p, double v) {
+  *p = __uint_as_float(svm::sklearn_f32_bits(v, true));
+}
+__device__ __forceinline__ void store_feature(double* p, double v) { *p = v == 0.0 ? 0.0 : v; }
+__device__ __forceinline__ void store_label(float* p, double v) {
+  *p = __uint_as_float(svm::sklearn_f32_bits(v, false));
+}
+__device__ __forceinline__ void store_label(double* p, double v) { *p = v; }
+
 // Walks line [beg, end) in 32-byte windows.  Token starts come from ballots over whitespace; each start lane parses
 // its own token.  WRITE (pass 2): feature values go to xrow[idx - shift], the label to *y_out.
-template <bool WRITE>
+template <bool WRITE, typename T = float>
 __device__ LineScan scan_line(const uint8_t* __restrict__ text, long long beg, long long end, int shift,
-                              float* __restrict__ xrow, float* __restrict__ y_out) {
+                              T* __restrict__ xrow, T* __restrict__ y_out) {
   const int lane = threadIdx.x & 31;
   const unsigned lt = (1u << lane) - 1u;
   LineScan r{0, 0, 0x7fffffff, -1, false, 0};
@@ -153,7 +166,7 @@ __device__ LineScan scan_line(const uint8_t* __restrict__ text, long long beg, l
       double v;
       if (ord == 0) {                                            // the label: float(target)
         if (svm::parse_py_float(tok, len, &v) != svm::NUM_OK) code = ARB_LIBSVM_E_LABEL;
-        else if (WRITE) *y_out = __uint_as_float(svm::sklearn_f32_bits(v, false));
+        else if (WRITE) store_label(y_out, v);
       } else if (ord == 1 && len >= 3 && tok[0] == 'q' && tok[1] == 'i' && tok[2] == 'd') {
         is_qid = true;                                           // features[0].startswith(b'qid'): split(b':', 1)
         long long k = 3;
@@ -182,7 +195,7 @@ __device__ LineScan scan_line(const uint8_t* __restrict__ text, long long beg, l
             const int pst = svm::parse_py_float(tok + k + 1, len - k - 1, &v);
             if (pst == svm::NUM_SYNTAX) code = ARB_LIBSVM_E_VALUE;
             else if (pst != svm::NUM_OK) code = ARB_LIBSVM_E_UNSUPPORTED;
-            else if (WRITE) xrow[idx - shift] = __uint_as_float(svm::sklearn_f32_bits(v, true));
+            else if (WRITE) store_feature(xrow + (idx - shift), v);
           }
         }
       }
@@ -236,7 +249,7 @@ __global__ void __launch_bounds__(SVM_WARPS * 32) pass1_kernel(const uint8_t* __
   for (long long line = (long long)blockIdx.x * SVM_WARPS + (threadIdx.x >> 5); line < n_lines; line += warps) {
     long long beg, end;
     line_span(line_end, n_nl, n_bytes, line, &beg, &end);
-    const LineScan r = scan_line<false>(text, beg, end, 0, nullptr, nullptr);
+    const LineScan r = scan_line<false, float>(text, beg, end, 0, nullptr, nullptr);
     if (lane == 0) {
       line_row[line] = r.ntok > 0 && !r.status;
       line_qid[line] = r.qid;
@@ -265,25 +278,25 @@ __global__ void summary_init_kernel(long long* summary) {
   }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(SVM_WARPS * 32) pass2_kernel(const uint8_t* __restrict__ text, long long n_bytes,
                                                                const long long* __restrict__ line_end, long long n_nl,
                                                                long long n_lines, const long long* __restrict__ line_row,
                                                                const long long* __restrict__ line_qid, long long n_rows,
-                                                               int shift, long long F, float* __restrict__ docs_x,
-                                                               float* __restrict__ docs_y,
-                                                               long long* __restrict__ qids) {
+                                                               int shift, long long F, T* __restrict__ docs_x,
+                                                               T* __restrict__ docs_y, long long* __restrict__ qids) {
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * SVM_WARPS;
   for (long long line = (long long)blockIdx.x * SVM_WARPS + (threadIdx.x >> 5); line < n_lines; line += warps) {
     const long long row = line_row[line];
     const long long next = line + 1 < n_lines ? line_row[line + 1] : n_rows;
     if (next == row) continue;                       // not a row
-    float* xrow = docs_x + (size_t)row * F;
-    for (long long c = lane; c < F; c += 32) xrow[c] = 0.f;
+    T* xrow = docs_x + (size_t)row * F;
+    for (long long c = lane; c < F; c += 32) xrow[c] = T(0);
     __syncwarp();
     long long beg, end;
     line_span(line_end, n_nl, n_bytes, line, &beg, &end);
-    scan_line<true>(text, beg, end, shift, xrow, docs_y + row);
+    scan_line<true, T>(text, beg, end, shift, xrow, docs_y + row);
     if (lane == 0) qids[row] = line_qid[line];
   }
 }
@@ -354,22 +367,41 @@ extern "C" int32_t arb_libsvm_pass1(const uint8_t* text, int64_t n_bytes, const 
                 sm + SUM_ROWS);
 }
 
-extern "C" int32_t arb_libsvm_pass2(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
-                                    int64_t n_lines, const int64_t* line_row, const int64_t* line_qid, int64_t n_rows,
-                                    int32_t shift, int64_t n_features, float* docs_x, float* docs_y, int64_t* qids,
-                                    void* stream) {
+template <typename T>
+static int32_t pass2(const char* name, const uint8_t* text, int64_t n_bytes, const int64_t* line_end,
+                     int64_t n_newlines, int64_t n_lines, const int64_t* line_row, const int64_t* line_qid,
+                     int64_t n_rows, int32_t shift, int64_t n_features, T* docs_x, T* docs_y, int64_t* qids,
+                     void* stream) {
   if (!text || !line_row || !line_qid || !docs_x || !docs_y || !qids || n_bytes <= 0 || n_newlines < 0 ||
       (n_newlines > 0 && !line_end) || n_lines < n_newlines || n_lines > n_newlines + 1 || n_lines <= 0 ||
       n_rows <= 0 || n_rows > n_lines || (shift != 0 && shift != 1) || n_features <= 0 ||
       n_features > ARB_LIBSVM_MAX_FEATURES) {
-    arb_set_error("arb_libsvm_pass2: null pointer or inconsistent sizes");
+    char msg[96];
+    snprintf(msg, sizeof msg, "%s: null pointer or inconsistent sizes", name);
+    arb_set_error(msg);
     return ARB_E_INVALID_ARG;
   }
-  return launch(pass2_kernel, dim3(line_grid(n_lines)), dim3(SVM_WARPS * 32), 0, static_cast<cudaStream_t>(stream),
+  return launch(pass2_kernel<T>, dim3(line_grid(n_lines)), dim3(SVM_WARPS * 32), 0, static_cast<cudaStream_t>(stream),
                 false, text, (long long)n_bytes, reinterpret_cast<const long long*>(line_end), (long long)n_newlines,
                 (long long)n_lines, reinterpret_cast<const long long*>(line_row),
                 reinterpret_cast<const long long*>(line_qid), (long long)n_rows, (int)shift, (long long)n_features, docs_x,
                 docs_y, reinterpret_cast<long long*>(qids));
+}
+
+extern "C" int32_t arb_libsvm_pass2(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
+                                    int64_t n_lines, const int64_t* line_row, const int64_t* line_qid, int64_t n_rows,
+                                    int32_t shift, int64_t n_features, float* docs_x, float* docs_y, int64_t* qids,
+                                    void* stream) {
+  return pass2("arb_libsvm_pass2", text, n_bytes, line_end, n_newlines, n_lines, line_row, line_qid, n_rows, shift,
+               n_features, docs_x, docs_y, qids, stream);
+}
+
+extern "C" int32_t arb_libsvm_pass2_f64(const uint8_t* text, int64_t n_bytes, const int64_t* line_end,
+                                        int64_t n_newlines, int64_t n_lines, const int64_t* line_row,
+                                        const int64_t* line_qid, int64_t n_rows, int32_t shift, int64_t n_features,
+                                        double* docs_x, double* docs_y, int64_t* qids, void* stream) {
+  return pass2("arb_libsvm_pass2_f64", text, n_bytes, line_end, n_newlines, n_lines, line_row, line_qid, n_rows,
+               shift, n_features, docs_x, docs_y, qids, stream);
 }
 
 extern "C" int32_t arb_libsvm_parse_numerals_host(const uint8_t* text_host, const int64_t* offsets_host, int64_t n,

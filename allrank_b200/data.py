@@ -41,6 +41,8 @@ _lib.register("arb_libsvm_count_lines", c_i, [c_p, c_i64, c_p, c_p])
 _lib.register("arb_libsvm_index_lines", c_i, [c_p, c_i64, c_p, c_p, c_p])
 _lib.register("arb_libsvm_pass1", c_i, [c_p, c_i64, c_p, c_i64, c_i64, c_p, c_p, c_p, c_p])
 _lib.register("arb_libsvm_pass2", c_i, [c_p, c_i64, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i, c_i64, c_p, c_p, c_p, c_p])
+_lib.register("arb_libsvm_pass2_f64", c_i, [c_p, c_i64, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i, c_i64, c_p, c_p, c_p,
+                                            c_p])
 _lib.register("arb_libsvm_parse_numerals_host", c_i, [c_p, c_p, c_i64, c_i, c_p, c_p])
 
 PARSERS = ("sklearn", "device")
@@ -252,15 +254,18 @@ def read_svm_to_device(svm_file, device=None):
 class LibSVMPlan:
     """Pass 1 of the device parser over LibSVM text in device memory (include/allrank_b200.h, arb_libsvm_*): the line
     index, validation and the output shape.  Raises what load_svmlight_file + SlateStore raise for the same text
-    (ValueError / OverflowError naming the first failing line) before anything is written.  `write` is pass 2."""
+    (ValueError / OverflowError naming the first failing line) before anything is written.  `write` is pass 2.
+    require_qids=False keeps rows without a qid (load_svmlight_file accepts them; only their use fails) and counts
+    them in `rows_without_qid`."""
 
-    def __init__(self, text):
+    def __init__(self, text, require_qids=True):
         if not (isinstance(text, torch.Tensor) and text.is_cuda and text.dtype == torch.uint8 and text.dim() == 1
                 and text.is_contiguous()):
             raise _lib.ArbError("LibSVM text must be a contiguous 1-D uint8 CUDA tensor")
         self.text = text
         self.n_bytes = n = int(text.numel())
         self.n_rows, self.n_features, self.shift = 0, 1, 0     # sklearn's shape for a file without rows: (0, 1)
+        self.rows_without_qid = 0
         if n == 0:
             return
         lib, dev = _lib.lib(), text.device
@@ -290,36 +295,40 @@ class LibSVMPlan:
         if err != -1:
             exc, why = _LIBSVM_ERRORS[err & 0xFF]
             raise exc("LibSVM line {}: {}".format(err >> 8, why))
-        if no_qid:     # load_svmlight_file returns fewer qids than rows; SlateStore refuses that
+        self.rows_without_qid = no_qid
+        if no_qid and require_qids:     # load_svmlight_file returns fewer qids than rows; SlateStore refuses that
             raise ValueError("X, y and query_ids must have one row per document "
                              "({} of {} rows have no qid)".format(no_qid, rows))
         self.n_rows = rows
         if hi >= 0:
             self.shift = int(lo > 0)
             self.n_features = hi - self.shift + 1
-        need = rows * (4 * self.n_features + 12)
+        need = rows * (4 * self.n_features + 12)     # (the float32 outputs; float64 callers check their own)
         free = torch.cuda.mem_get_info(text.device)[0]
         if need > free:
             raise _lib.ArbError("the dense output ({} rows x {} features) does not fit the free device memory "
                                 "({} bytes)".format(rows, self.n_features, free))
 
     def write(self, docs_x, docs_y, qids):
-        """Pass 2: every element of docs_x [n_rows, n_features] fp32, docs_y [n_rows] fp32 and qids [n_rows] int64."""
-        shapes = ((docs_x, (self.n_rows, self.n_features), torch.float32), (docs_y, (self.n_rows,), torch.float32),
+        """Pass 2: every element of docs_x [n_rows, n_features], docs_y [n_rows] and qids [n_rows] int64.  docs_x and
+        docs_y are both fp32 (what SlateStore keeps) or both float64 (load_svmlight_file's X.toarray() and y)."""
+        dtype = torch.float64 if docs_x.dtype == torch.float64 else torch.float32
+        shapes = ((docs_x, (self.n_rows, self.n_features), dtype), (docs_y, (self.n_rows,), dtype),
                   (qids, (self.n_rows,), torch.int64))
-        for t, shape, dtype in shapes:
-            if tuple(t.shape) != shape or t.dtype != dtype or t.device != self.text.device or not t.is_contiguous():
+        for t, shape, want in shapes:
+            if tuple(t.shape) != shape or t.dtype != want or t.device != self.text.device or not t.is_contiguous():
                 raise ValueError("pass 2 outputs must be contiguous {} {} tensors on {}".format(
-                    shape, dtype, self.text.device))
+                    shape, want, self.text.device))
         if self.n_rows == 0:
             return
+        name = "arb_libsvm_pass2_f64" if dtype == torch.float64 else "arb_libsvm_pass2"
         with torch.cuda.device(self.text.device):
-            rc = _lib.lib().arb_libsvm_pass2(_lib.ptr(self.text), self.n_bytes, _lib.ptr(self.line_end),
-                                             self.n_newlines, self.n_lines, _lib.ptr(self.line_row),
-                                             _lib.ptr(self.line_qid), self.n_rows, self.shift, self.n_features,
-                                             _lib.ptr(docs_x), _lib.ptr(docs_y), _lib.ptr(qids),
-                                             _lib.stream_ptr(self.text.device))
-        _lib.check(rc, "arb_libsvm_pass2")
+            rc = getattr(_lib.lib(), name)(_lib.ptr(self.text), self.n_bytes, _lib.ptr(self.line_end),
+                                           self.n_newlines, self.n_lines, _lib.ptr(self.line_row),
+                                           _lib.ptr(self.line_qid), self.n_rows, self.shift, self.n_features,
+                                           _lib.ptr(docs_x), _lib.ptr(docs_y), _lib.ptr(qids),
+                                           _lib.stream_ptr(self.text.device))
+        _lib.check(rc, name)
 
 
 class DeviceSlateLoader:

@@ -704,6 +704,12 @@ int32_t arb_libsvm_pass1(const uint8_t* text, int64_t n_bytes, const int64_t* li
 int32_t arb_libsvm_pass2(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
                          int64_t n_lines, const int64_t* line_row, const int64_t* line_qid, int64_t n_rows,
                          int32_t shift, int64_t n_features, float* docs_x, float* docs_y, int64_t* qids, void* stream);
+/* Pass 2 with float64 outputs: docs_x and docs_y hold load_svmlight_file(f, query_id=True)'s X.toarray() and y --
+ * Python's float() of each numeral, with a feature's -0.0 stored as +0.0 -- and no float32 rounding. */
+int32_t arb_libsvm_pass2_f64(const uint8_t* text, int64_t n_bytes, const int64_t* line_end, int64_t n_newlines,
+                             int64_t n_lines, const int64_t* line_row, const int64_t* line_qid, int64_t n_rows,
+                             int32_t shift, int64_t n_features, double* docs_x, double* docs_y, int64_t* qids,
+                             void* stream);
 /* Host-side test hook: the numeral conversion of the kernels, run on the CPU over n tokens
  * text_host[offsets_host[i], offsets_host[i + 1]).  kind 0: float() -> float64 bits; 1: float32(float(token)) bits
  * (as the labels are stored); 2: int() into a C int; 3: numpy.int64().  status_host[i]: 0 ok, 1 refused (ValueError),
@@ -748,6 +754,35 @@ int32_t arb_svm_write_chunk(const void* X, int32_t x_kind, int64_t n_features, c
  * takes device pointers and enqueues one launch (n >= 1); arb_format_g16_host runs the same code on the CPU. */
 int32_t arb_format_g16(const double* values, int64_t n, char* slots, void* stream);
 int32_t arb_format_g16_host(const double* values, int64_t n, char* slots);
+
+/* ---------------------------------------------------------------- feature normalisation (DESIGN.md section 13)
+ * reproducibility/normalize_features.py on dense row-major float64 roles x [rows, n_features], in place.  Only the
+ * first n_cols columns (the train role's width) are transformed.
+ *   arb_norm_sign_flags: flags [n_cols] int32 = 1 where some value, negated when negate[c] != 0, is not >= 0 (NaN).
+ *   arb_norm_transform_a: negate where negate[c], then v = log(v + 0.01) correctly rounded where log_mask[c].
+ *   arb_norm_column_stats: mean [n_features] and std [n_features] of every column as np.mean / np.std compute them:
+ *     numpy's pairwise summation tree, given as leaves (rows [leaf_start[i], leaf_start[i + 1]), leaf_start has
+ *     n_leaves + 1 entries) and internal nodes numbered from n_leaves, level by level (level_counts: HOST array of
+ *     n_levels counts), children [2 * internal nodes] their (left, right) node numbers; the last node is the root.
+ *     node_vals [nodes * n_features] is scratch.
+ *   arb_norm_transform_b: (v - mean[c]) / (std[c] + 1e-6) for c < n_cols, 0 beyond.
+ * status [2] int64 (device; the caller sets {0, -1}): [0] += values that took the log's accurate phase; [1] = the
+ * smallest bit pattern of an argument whose rounding the accurate phase could not decide (stays -1: none). */
+int32_t arb_norm_sign_flags(const double* x, int64_t rows, int64_t n_features, int64_t n_cols, const uint8_t* negate,
+                            int32_t* flags, void* stream);
+int32_t arb_norm_transform_a(double* x, int64_t rows, int64_t n_features, int64_t n_cols, const uint8_t* negate,
+                             const uint8_t* log_mask, int64_t* status, void* stream);
+int32_t arb_norm_column_stats(const double* x, int64_t rows, int64_t n_features, const int64_t* leaf_start,
+                              int64_t n_leaves, const int64_t* children, const int64_t* level_counts, int64_t n_levels,
+                              double* node_vals, double* mean, double* std, void* stream);
+int32_t arb_norm_transform_b(double* x, int64_t rows, int64_t n_features, int64_t n_cols, const double* mean,
+                             const double* std, void* stream);
+/* Test entry points.  arb_log_cr: y[i] = log(x[i]) correctly rounded (log_cr.cuh), status as above, with
+ * force_accurate != 0 taking the accurate phase for every value; arb_log_cr_host: the same code on the CPU (host
+ * pointers).  arb_pairwise_sum_host: np.add.reduce of x[0], x[stride], ..., x[(n - 1) stride]. */
+int32_t arb_log_cr(const double* x, int64_t n, double* y, int32_t force_accurate, int64_t* status, void* stream);
+int32_t arb_log_cr_host(const double* x, int64_t n, double* y, int32_t force_accurate, int64_t* status);
+int32_t arb_pairwise_sum_host(const double* x, int64_t n, int64_t stride, double* out);
 
 #ifdef __cplusplus
 }
